@@ -2,14 +2,16 @@
 """bench.py -- video-frames/s of OmniTokenizer_VQGAN encode -> codes -> decode (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg3|cfg2|cfg4|cfg5]
-                    [--math f16x3|3xtf32|fp32]
+                    [--math f16x3|3xtf32|fp32] [--dump-outputs DIR]
 
 Workload (config.workload): cfg3 = batch of 8 synthetic videos 17x256x256 (the configuration the
 metric is quoted on, BASELINE.json configs[2]); under torchrun the batch is split over ranks
 (strong scaling), each rank encodes its shard, ONE all-gather of code indices, decode of the shard.
 cfg2 (64 images), cfg4 (4 videos 33x512x512: ranks beyond the batch idle, "replicas only beyond B") and
 cfg5 (cfg3 in VAE mode: no codes, hence no collective) are BASELINE.json's other configurations.
-A "step" is one pass of that path over the batch.  Prints ONE JSON line (rank 0).
+A "step" is one pass of that path over the batch; --steps K sets the number of timed steps.  Prints ONE JSON line (rank 0).
+--dump-outputs DIR writes what the last timed step returned (rank 0's shard) as .npy files: the code indices (or VAE
+latents) in full and a fixed, seeded sample of the reconstruction, so that two builds can be compared output for output.
 
 --impl reference: the CPU baseline arm -- the oracle port of the reference's PyTorch path
 (oracle/omni_oracle.py; the reference tree itself does not travel to the GPU box) on the host
@@ -42,11 +44,11 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -95,7 +97,7 @@ def make_model(dev, vae=False):
 
 def pick_cpu_threads(sd, x_small, vae=False):
     """The oracle's many small torch ops do not scale to every core of a 100+-core host (128 threads is
-    ~30x SLOWER than 16 on the B200 box), so take the best of a short sweep; `cores` reports that count."""
+    much slower than 16), so take the best of a short sweep; `cores` reports that count."""
     cores = os.cpu_count() or 1
     best, best_t = None, None
     for nt in sorted({min(c, cores) for c in (8, 16, 32, 64)}):
@@ -238,6 +240,28 @@ def run_reference(args):
     }))
 
 
+DUMP_SAMPLE = 1 << 22        # elements of a larger output kept by --dump-outputs (16 MiB as float32)
+
+
+def dump_outputs(out_dir, outputs):
+    """--dump-outputs: each output of the last timed step as <name>.npy, float32 (float64 where float32 would round).
+    Outputs of at most DUMP_SAMPLE elements are written whole; a larger one (the reconstruction) as a sample at fixed,
+    seeded flat positions, written next to it as <name>_index.npy, so the files stay well under 64 MB."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in sorted(outputs.items()):
+        if t is None:
+            continue
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_SAMPLE].sort().values
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.numpy().astype(np.float64))
+            flat = flat[idx.to(flat.device)]
+        dtype = np.float64 if flat.dtype in (torch.int64, torch.float64) else np.float32
+        np.save(os.path.join(out_dir, f"{name}.npy"), flat.cpu().numpy().astype(dtype).reshape(
+            t.shape if flat.numel() == t.numel() else (-1,)))
+
+
 def _event_time(fn, flush, reps=10):
     """median CUDA-event time of fn() in ms, L2 flushed before every repetition"""
     evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(reps)]
@@ -302,6 +326,8 @@ def main():
     ap.add_argument("--workload", default="cfg3", choices=sorted(WORKLOADS))
     ap.add_argument("--math", default=None, help="f16x3 | 3xtf32 | fp32 (default: OMT_MATH or the engine default)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -336,8 +362,9 @@ def main():
     x_dev = x_host.to(dev)
     m = make_model(dev, vae)
     m.prepare()
-    flush = torch.zeros(64 * 1024 * 1024, device=dev)      # 256 MiB > 126 MB L2
+    flush = torch.zeros(64 * 1024 * 1024, device=dev)      # 256 MiB >> 50 MB L2
     gathered = {}
+    outputs = {}      # what the most recent step returned (read by --dump-outputs after the timed steps)
 
     def step(x, u8=False):
         """u8: the reconstruction leaves as uint8 frames (vqgan_eval.py's clamp / 255 / byte conversion fused into the last kernel)"""
@@ -346,7 +373,9 @@ def main():
             if x.shape[0] == 0:
                 return None
             z = m.encode(x, is_image)
-            return dec(z if is_image else z.permute(0, 2, 3, 4, 1))
+            rec = dec(z if is_image else z.permute(0, 2, 3, 4, 1))
+            outputs.update(latents=z, recon=rec)
+            return rec
         codes = m.encode(x, is_image)                       # an empty shard (B < world) returns an empty, right-shaped tensor
         pending = None
         if world > 1 and not os.environ.get("OMT_BENCH_NO_GATHER"):
@@ -354,6 +383,7 @@ def main():
         rec = None if x.shape[0] == 0 else dec(codes)
         if pending is not None:
             gathered["codes"] = pending.wait()              # every rank now holds the full (B,T',h,w) index tensor
+        outputs.update(codes=codes, recon=rec)
         return rec
 
     def barrier():
@@ -379,6 +409,8 @@ def main():
     barrier()
     launches = _cabi.launch_count - n0
     t_ms = sum(a.elapsed_time(b) for a, b in evs)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, outputs)
     # the gathered codes of the last step must be the single-GPU codes of the full batch (checked once, untimed)
     gather_ok = None
     if world > 1 and not vae and "codes" in gathered:
@@ -395,7 +427,7 @@ def main():
     out_host = [torch.empty((e - s,) + shape[1:], dtype=torch.float32).pin_memory() for _ in range(2)]
     out_host_u8 = [torch.empty((e - s, 1 if is_image else shape[2], shape[-2], shape[-1], shape[1]), dtype=torch.uint8).pin_memory()
                    for _ in range(2)]
-    e2e_steps = max(3, args.steps)
+    e2e_steps = args.steps
     main = torch.cuda.current_stream()
     s_in, s_out = torch.cuda.Stream(), torch.cuda.Stream()
     xd = [torch.empty_like(x_dev) for _ in range(2)]
@@ -479,23 +511,16 @@ def main():
         math = default_math()
         tf32_peak = pk["bf16_tflops"] / 2.0
         achieved = k_flops / (k_ms * 1e-3) / 1e12
-        traffic = None
-        try:      # dram__bytes_read+write of this launch from the committed `ncu --set full` capture (cfg-3, N=1)
-            tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_ff1_traffic.json")))
-            if world == 1 and args.workload in ("cfg3", "cfg5") and not os.environ.get("OMT_BENCH_BATCH") and math in tj:
-                traffic = tj[math]["dram_bytes"]
-        except Exception:
-            pass
         kname = {"3xtf32": "gemm_tc2_kernel", "f16x3": "gemm_f16_kernel", "fp32": "gemm_fp32_kernel"}[math]
         own = {"3xtf32": "3xTF32 issues 3 tf32 MMAs per product: its own ceiling is 1/3 of this",
-               "f16x3": "f16x3 issues 3 kind::f16 MMAs (2x the tf32 rate) per product: its own ceiling is 2/3 of this",
+               "f16x3": "f16x3 issues 3 f16 wgmmas (2x the tf32 rate) per product: its own ceiling is 2/3 of this",
                "fp32": "CUDA-core FFMA kernel: bounded by the fp32 pipe, not the tensor pipe"}[math]
         roof = {"bound": "tensor", "kernel": f"{kname}[{math}] FF1+GEGLU M={M_local} N=2730 K=512",
                 "achieved": round(achieved, 2), "peak": round(tf32_peak, 1), "unit": "TFLOP/s",
-                "frac": round(achieved / tf32_peak, 4), "traffic": traffic,
+                "frac": round(achieved / tf32_peak, 4),
                 "algorithmic_bytes": int(M_local * 512 * 4 + 2 * 2730 * 512 * 4 + M_local * 1365 * 4),
                 "ms_per_launch": round(k_ms, 4),
-                "peak_note": f"tf32 dense = 0.5 x {pk_src} bf16 burst {pk['bf16_tflops']} TF/s; FLOPs are algorithmic fp32 "
+                "peak_note": f"tf32 dense = 0.5 x bf16 dense {pk['bf16_tflops']} TF/s ({pk_src}); FLOPs are algorithmic fp32 "
                              f"(2MNK); {own}",
                 "whole_path": {"tflop_per_batch": TFLOP[args.workload],
                                "achieved_tflops": round(TFLOP[args.workload] * args.steps / (t_ms / 1e3), 2)}}

@@ -1,5 +1,5 @@
 /*
- * omnitok_b200 -- C ABI of the B200 (sm_100a) kernels behind OmniTokenizer_VQGAN.encode/decode.
+ * omnitok_b200 -- C ABI of the H100 (sm_90a) kernels behind OmniTokenizer_VQGAN.encode/decode.
  *
  * The reference (FoundationVision/OmniTokenizer) has no FFI of its own: its boundary is the
  * Python module API of OmniTokenizer_VQGAN (OmniTokenizer/omnitokenizer.py:63-413).  Each entry
@@ -11,7 +11,7 @@
  *     allocated or retained; outputs may not alias inputs unless stated.
  *   - every call is asynchronous on `stream` (a cudaStream_t passed as void*).
  *   - return 0 on success, negative on error (OMT_E_*); omt_last_error() gives the message
- *     (thread-local).  There is NO CPU fallback: a non-sm_100 device returns OMT_E_ARCH.
+ *     (thread-local).  There is NO CPU fallback: a non-sm_90 device returns OMT_E_ARCH.
  *   - activations live in ONE canonical layout  X[B][T'][N][C]  (C fastest; identical to the
  *     reference's "(b t) (h w) d" tensor).  "rows" are (b,t',n) triples, M = B*T'*N.
  *   - a "row map" (seg, seg_stride, seg_off) maps logical GEMM row r to physical row
@@ -31,7 +31,7 @@ extern "C" {
 
 #define OMT_OK 0
 #define OMT_E_ARG (-1)    /* bad shape / alignment / null pointer */
-#define OMT_E_ARCH (-2)   /* device is not sm_100 */
+#define OMT_E_ARCH (-2)   /* device is not sm_90 */
 #define OMT_E_CUDA (-3)   /* a CUDA runtime call failed */
 #define OMT_E_UNSUPPORTED (-4)
 
@@ -50,14 +50,14 @@ int omt_device_info(int* sm_count, int* cc_major, int* cc_minor);
 
 /* GEMM math selectors */
 #define OMT_MATH_FP32 0      /* CUDA-core FFMA, exact fp32 (parity anchor) */
-#define OMT_MATH_3XTF32 1    /* tcgen05 kind::tf32, error-compensated hi/lo split, fp32 accumulate in TMEM */
-#define OMT_MATH_F16X3 3     /* tcgen05 kind::f16 on pre-split fp16 hi / lo operand planes (omt_linear_h) */
+#define OMT_MATH_3XTF32 1    /* wgmma tf32, error-compensated hi/lo split, fp32 accumulate in registers */
+#define OMT_MATH_F16X3 3     /* wgmma f16 on pre-split fp16 hi / lo operand planes (omt_linear_h) */
 
 /* C[M, N] = A[M, K] . W[N, K]^T (+ bias[N]) (+ residual[M, N]); nn.Linear everywhere on the path:
  * attention.py:411 (to_q / to_kv), :486 (to_out), :271/:288 (window qkv / proj), :164/:167 (FF),
  * omnitokenizer.py:809,819 (patch embed), :1007,1013 (to_pixels).
  * W must be allocated with rows padded up to a multiple of 128 (zero rows); K % 8 == 0 (fp32 path)
- * or K % 32 == 0 (tcgen05 paths).  With OMT_EPI_GEGLU, N counts packed columns and C has N/2 columns.
+ * or K % 32 == 0 (tensor-core paths).  With OMT_EPI_GEGLU, N counts packed columns and C has N/2 columns.
  * residual may alias C (same ld): out-of-place is not required.  For OMT_MATH_3XTF32 `W` must be the
  * tf32-rounded (round-to-nearest, low 13 mantissa bits zero) high part of the weight and `W_lo` the
  * exact remainder (same shape); W_lo is ignored (may be NULL) for FP32. */
@@ -137,8 +137,8 @@ int omt_attn_spatial(const float* q, int ldq, const float* k, int ldk, const flo
                      float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo, int n_seq, int N, int heads, float scale,
                      omt_stream_t stream);
 
-/* omt_attn_spatial on the operand planes written by omt_linear_h(OMT_EPI_QKV_PLANES): tcgen05 kind::f16 core, Q / P in
- * tensor memory, K / V tiles straight from TMA (V as an MN-major operand: no transpose), N % 128 == 0.
+/* omt_attn_spatial on the operand planes written by omt_linear_h(OMT_EPI_QKV_PLANES): wgmma f16 core, Q / K / V tiles
+ * straight from TMA (V as an MN-major operand: no transpose), N % 128 == 0.
  * qk_plane_scale = q_plane_scale * k_plane_scale; vinv [heads][n_seq * N]. */
 int omt_attn_spatial_h(const uint16_t* q_hi, const uint16_t* q_lo, int ldq, const uint16_t* k_hi, const uint16_t* k_lo, int ldk,
                        const uint16_t* v_hi, const uint16_t* v_lo, int ldv, const float* vinv, float qk_plane_scale,
@@ -235,11 +235,9 @@ int omt_layernorm_h(const float* x, int ldx, float* y, int ldy, uint16_t* y_hi, 
 /* Tuning knobs (process-wide): "pdl" = 0 (default; measured 2-4 % slower when on) | 1 programmatic dependent launch;
  * "peg_kernel" = 4 (default: cp.async zero-fill halo gather + packed f32x2 FMAs) | 3 (register-staged gather; also the
  * fallback for T > 64 or w > 254); identical bits;
- * "attn_kernel" = 3 (default: tcgen05 spatial attention core when N % 128 == 0) | 1 (CUDA-core fp32);
- * "f16_bn" = 0 (default: by shape) | 256 (256 x 256 tiles, one TMEM buffer released as soon as the epilogue has drained
- * it into registers) | 128 (256 x 128 tiles, double-buffered accumulators): tile width of omt_linear_h's two-accumulator form;
- * "attn_f16_ctas" = 2 (default: single S / P buffers, 256 TMEM columns, two CTAs per SM) | 1 (double-buffered S / P, one CTA per SM):
- * shape of omt_attn_spatial_h's kernel; identical results. */
+ * "attn_kernel" = 3 (default: wgmma 3xTF32 spatial attention core when N % 128 == 0) | 1 (CUDA-core fp32);
+ * "f16_bn" = 0 (default) | 128 | 256: accepted for compatibility; omt_linear_h always runs 128 x 128 tiles on sm_90;
+ * "attn_f16_ctas" = 2 (default) | 1: accepted for compatibility; omt_attn_spatial_h has one kernel shape on sm_90. */
 int omt_set_option(const char* name, int value);
 
 #ifdef __cplusplus

@@ -1,4 +1,4 @@
-"""omnitokenizer_b200: B200 (sm_100a) implementation of OmniTokenizer_VQGAN.encode/decode.
+"""omnitokenizer_b200: H100 (sm_90a) implementation of OmniTokenizer_VQGAN.encode/decode.
 
 Drop-in for the reference's ``from OmniTokenizer import OmniTokenizer_VQGAN``
 (/root/reference/OmniTokenizer/__init__.py:7); see INTEGRATION.md.

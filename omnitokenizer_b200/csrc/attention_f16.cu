@@ -1,57 +1,38 @@
-// Attention v4: spatial (full, non-causal) attention core on tcgen05 kind::f16 with row-scaled fp16 operand planes.
+// Attention v4: spatial (full, non-causal) attention core on sm_90a wgmma (f16) with row-scaled fp16 operand planes.
 //   O = softmax(scale * Q K^T) V  per (sequence, head), head dim 64, N % 128 == 0
 //   (F.scaled_dot_product_attention at modules/attention.py:451).
 //
-// Operands come from the QKV GEMM epilogue (gemm_f16.cu, OMT_EPI_QKV_PLANES) already in tensor-core form:
+// Operands come from the QKV GEMM epilogue (gemm_wgmma.cuh, OMT_EPI_QKV_PLANES) already in tensor-core form:
 //   q, k : after rope + l2norm + per-dim scale every component is bounded by max|q_scale| / max|k_scale|, so ONE static
 //          power of two per layer puts them in fp16 range: planes hi = fp16(x * 2^e), lo = fp16(x * 2^e - hi)
-//   v    : unbounded, scaled per (row, head) (the epilogue thread holds the whole 64-wide head of its row);
-//          the inverse scales live in vinv[head][row]
-// so S = Q K^T and O_j = P_j V_j each take THREE kind::f16 MMAs per 16-deep k-step into ONE fp32 accumulator
-// (hi.hi + hi.lo + lo.hi) -- half the MMAs of the 3xTF32 core, 16-deep instead of 8-deep.
-//   * Q and P are TENSOR-MEMORY A operands (two fp16 per 32-bit column): only the K / V B tiles come from shared
-//     memory, straight from TMA -- no transform warps at all.
-//   * V is consumed as an MN-MAJOR B operand: the token-major tile [64 keys][64 dims] the TMA lands is exactly the
-//     canonical SWIZZLE_128B MN-major layout, so nothing is transposed anywhere.
+//   v    : unbounded, scaled per (row, head); the inverse scales live in vinv[head][row]
+// so S = Q K^T and O_j = P_j V_j each take THREE f16 wgmmas per 16-deep k-step into ONE fp32 accumulator
+// (hi.hi + hi.lo + lo.hi).
+//   * Q, K and V tiles come straight from TMA; V is consumed as an MN-MAJOR B operand (the token-major [64 keys][64 dims]
+//     tile the TMA lands is the canonical SWIZZLE_128B MN-major layout), so nothing is transposed anywhere.
 //   * the per-key inverse V scale is folded into P: P'' = p * vinv_j * 2^ep with ONE power of two per CTA taken from the
 //     largest vinv of the sequence, so p'' stays in fp16 range; 2^-ep comes off with the final 1 / row-sum.
-//   TMEM columns (NB = 2): S[2] 0-127 | O 128-191 (accumulates over the key tiles) | P[2] x (hi 32 | lo 32) 192-319 | Q (hi 32 | lo 32) 320-383
-//                (NB = 1): S 0-63 | O 64-127 | P 128-191 | Q 192-255
-//   smem stage  : K_hi | K_lo | V_hi | V_lo (8 KiB each) | vinv (256 B), 4 (NB = 2) or 2 (NB = 1) stages, every tile one TMA transaction set
-// Measured alternatives (same box, same process, `scripts/bench_attn.py`, cfg-3 shape, two CTAs per SM): Q as a shared-memory
-// operand (SS-form S MMAs) 299 us vs 288 us for this form; P_hi.[V_hi | V_lo] as one N = 128 MMA: no gain with one CTA per SM and
-// 2.7x slower with two.  The tile loop is bound by the serial chain S read-back -> max -> exp -> P write of the softmax threads,
-// not by tensor-pipe or tensor-memory throughput (ncu: tensor pipe 30 %, issue slots 38 %), hence two CTAs per SM.
-// Roles: warp 0 TMA, warp 1 MMA issue + TMEM alloc, warps 2-9 softmax: TWO threads per query row (32 keys / 32 output
-//        dims each; they only exchange the row max), S from TMEM, P back to TMEM, O read back once at the end.
+// One CTA = two warpgroups, 64 query rows each (S and O in registers, online softmax); P'' goes through a per-warpgroup
+// shared-memory tile as the A operand of the P.V wgmmas.  K / V tiles are double-buffered; thread 0 issues the TMA loads.
 #include "omt_common.cuh"
 #include "tc_ptx.cuh"
 #include <cuda.h>
 
 namespace omt {
-int g_attn_f16_ctas = 2;      // omt_set_option("attn_f16_ctas", 1 | 2): CTAs per SM of the f16 attention core (2 = default)
+int g_attn_f16_ctas = 2;      // omt_set_option("attn_f16_ctas", 1 | 2): accepted for compatibility (one kernel shape on sm_90)
 namespace af16 {
 using namespace omt::ptx;
 
 constexpr int QT = 128, KT = 64, D = 64;
 constexpr int TILE = KT * D * 2;                    // 8 KiB: one 64 x 64 fp16 plane tile
-constexpr int STAGE_BYTES = 4 * TILE + 1024;        // K_hi, K_lo, V_hi, V_lo + vinv (256 B, padded to keep 1024-B alignment)
-// Two shapes of the same kernel.  NB = 2: S and P double-buffered, 4 K/V stages, all 512 TMEM columns, one CTA per SM.
-// NB = 1: single S / P buffers, 2 stages, 256 TMEM columns, 95 registers -> TWO CTAs per SM: the softmax threads of one
-// CTA cover the tensor-memory round trips and barriers of the other (the tile loop is latency-bound, not issue-bound).
-template <int NB> struct Cfg {
-  static constexpr int STAGES = NB == 2 ? 4 : 2;
-  static constexpr int OFF_CTRL = STAGES * STAGE_BYTES;
-  static constexpr int SMEM = OFF_CTRL + 3072 + 1024;      // barriers / exchange + alignment slack
-  static constexpr int TM_S = 0, TM_O = 64 * NB, TM_P = TM_O + 64, TM_Q = TM_P + 64 * NB;
-  static constexpr int TM_COLS = NB == 2 ? 512 : 256;
-};
-constexpr int THREADS = 64 + 256;                   // TMA, MMA, 8 softmax warps
-constexpr uint32_t IDESC_S = idesc_f16(128, 64, false, false);                      // A: TMEM, B: K-major smem
-constexpr uint32_t IDESC_PV = idesc_f16(128, 64, false, false) | (1u << 16);        // B (= V tile) is MN-major
+constexpr int OFF_Q = 0;                            // Q_hi [2 warpgroups] | Q_lo [2]
+constexpr int OFF_KV = 4 * TILE;                    // [2 stages] x (K_hi | K_lo | V_hi | V_lo)
+constexpr int OFF_P = OFF_KV + 8 * TILE;            // [2 warpgroups] x (P_hi | P_lo)
+constexpr int OFF_CTRL = OFF_P + 4 * TILE;
+constexpr int SMEM = OFF_CTRL + 1024 + 1024;        // barriers / reduction + alignment slack
+constexpr int THREADS = 256;
 
 struct Args {
-  const uint16_t* q_hi; const uint16_t* q_lo; int ldq;     // q planes (token-major, head h at columns 64 h)
   const float* vinv;                                       // [heads][rows] inverse scales of the v rows
   long long rows;                                          // n_seq * N
   float* o; uint16_t* o_hi; uint16_t* o_lo; int ldo;
@@ -59,283 +40,166 @@ struct Args {
   float scale_log2;                                        // scale * log2(e) / (q plane scale * k plane scale)
 };
 
-// 1-D bulk copy global -> shared with mbarrier completion (the vinv slice of a key tile)
-__device__ __forceinline__ void bulk_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-// UMMA shared-memory descriptor, MN-major SWIZZLE_128B: 64 MN elements (128 B) per row, k rows 128 B apart, 8-row groups
-// 1024 B apart (SBO); LBO (stride between 64-element MN groups) is unused for N = 64
-__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3fff);
-  d |= (uint64_t)(8192 >> 4) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* u) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(u[0]), "r"(u[1]), "r"(u[2]), "r"(u[3]), "r"(u[4]), "r"(u[5]), "r"(u[6]), "r"(u[7]),
-        "r"(u[8]), "r"(u[9]), "r"(u[10]), "r"(u[11]), "r"(u[12]), "r"(u[13]), "r"(u[14]), "r"(u[15]) : "memory");
-}
-
-template <int NB>
-__global__ void __launch_bounds__(THREADS, 3 - NB)
-attn_f16_kernel(const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
+__global__ void __launch_bounds__(THREADS, 1)
+attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
+                const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
                 const __grid_constant__ CUtensorMap tmVh, const __grid_constant__ CUtensorMap tmVl, const Args a) {
-  constexpr int STAGES = Cfg<NB>::STAGES, OFF_CTRL = Cfg<NB>::OFF_CTRL;
-  constexpr int TM_S = Cfg<NB>::TM_S, TM_O = Cfg<NB>::TM_O, TM_P = Cfg<NB>::TM_P, TM_Q = Cfg<NB>::TM_Q;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_CTRL);
-  uint64_t* full = bars;            // [STAGES] K / V planes + vinv of a key tile landed
-  uint64_t* empty = bars + 4;       // [STAGES] P.V of the tile retired (commit) and the 8 softmax warps are done with vinv
-  uint64_t* s_full = bars + 8;  uint64_t* s_empty = bars + 10;
-  uint64_t* o_full = bars + 12;     // [2] P.V of a tile retired (per P buffer)
-  uint64_t* p_full = bars + 16;
-  uint64_t& q_ready = bars[18];
-  uint32_t& tmem_base_s = *reinterpret_cast<uint32_t*>(bars + 20);
-  float* xch = reinterpret_cast<float*>(smem + OFF_CTRL + 256);        // [2 tile parities][2 key halves][128 rows] row-max / row-sum exchange
-  float* red = reinterpret_cast<float*>(smem + OFF_CTRL + 256 + 2048); // [8] per-warp maxima of vinv
+  uint64_t& q_full = bars[0];
+  uint64_t* full = bars + 1;                                          // [2] K / V planes of a key tile landed
+  float* red = reinterpret_cast<float*>(smem + OFF_CTRL + 64);        // [8] per-warp maxima of vinv
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2, qd = lane & 3;
   const int qt = blockIdx.x, head = blockIdx.y, seq = blockIdx.z;
   const int ntiles = a.N / KT;
   const int row_q0 = seq * a.N + qt * QT;
   const int row_k0 = seq * a.N;
   const int col0 = head * D;
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmKh)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmKl)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmVh)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmVl)) : "memory");
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1 + 8); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 8);
-      mbar_init(&o_full[i], 1);
-      mbar_init(&p_full[i], 8);
-    }
-    mbar_init(&q_ready, 8);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  if (tid == 0) {
+    prefetch_map(&tmQh); prefetch_map(&tmQl); prefetch_map(&tmKh); prefetch_map(&tmKl); prefetch_map(&tmVh); prefetch_map(&tmVl);
+    mbar_init(&q_full, 1); mbar_init(&full[0], 1); mbar_init(&full[1], 1);
+    fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(Cfg<NB>::TM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
   pdl_sync();
 
-  if (warp == 0) {
-    // ================= TMA producer =================
-    if (lane == 0) {
-      for (int j = 0; j < ntiles; ++j) {
-        const int s = j % STAGES;
-        const uint32_t ph = (j / STAGES) & 1;
-        mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
-        mbar_expect_tx(&full[s], 4 * TILE + KT * 4);
-        const int kr = row_k0 + j * KT;
-        tma_load_2d(&tmKh, &full[s], sp, col0, kr);
-        tma_load_2d(&tmKl, &full[s], sp + TILE, col0, kr);
-        tma_load_2d(&tmVh, &full[s], sp + 2 * TILE, col0, kr);
-        tma_load_2d(&tmVl, &full[s], sp + 3 * TILE, col0, kr);
-        bulk_load_1d(sp + 4 * TILE, a.vinv + (size_t)head * a.rows + kr, KT * 4, &full[s]);
-      }
+  auto issue_kv = [&](int j) {
+    const int s = j & 1;
+    uint8_t* sp = smem + OFF_KV + s * 4 * TILE;
+    const int kr = row_k0 + j * KT;
+    mbar_expect_tx(&full[s], 4 * TILE);
+    tma_load_2d(&tmKh, &full[s], sp, col0, kr);
+    tma_load_2d(&tmKl, &full[s], sp + TILE, col0, kr);
+    tma_load_2d(&tmVh, &full[s], sp + 2 * TILE, col0, kr);
+    tma_load_2d(&tmVl, &full[s], sp + 3 * TILE, col0, kr);
+  };
+  if (tid == 0) {
+    mbar_expect_tx(&q_full, 4 * TILE);
+    for (int w = 0; w < 2; ++w) {
+      tma_load_2d(&tmQh, &q_full, smem + OFF_Q + w * TILE, col0, row_q0 + w * 64);
+      tma_load_2d(&tmQl, &q_full, smem + OFF_Q + (2 + w) * TILE, col0, row_q0 + w * 64);
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ================= MMA issuer (whole warp converged; one elected lane issues) =================
-    const uint32_t sb = smem_u32(smem);
-    const uint32_t tq_hi = tmem_base + TM_Q, tq_lo = tmem_base + TM_Q + 32;
-    auto issue_s = [&](int j) {
-      const int s = j % STAGES, b = j % NB;
-      mbar_wait(&full[s], (j / STAGES) & 1);
-      mbar_wait(&s_empty[b], ((j / NB) & 1) ^ 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t d = tmem_base + TM_S + b * 64;
-        const uint64_t kh = desc_kmajor(sb + s * STAGE_BYTES), kl = desc_kmajor(sb + s * STAGE_BYTES + TILE);
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {           // 16 of the 64 head dims per MMA (8 TMEM columns of packed fp16 pairs)
-          const uint64_t adv = (uint64_t)(kk * 32 >> 4);
-          mma_f16_ts(d, tq_lo + kk * 8, kh + adv, IDESC_S, kk != 0);
-          mma_f16_ts(d, tq_hi + kk * 8, kl + adv, IDESC_S, 1);
-          mma_f16_ts(d, tq_hi + kk * 8, kh + adv, IDESC_S, 1);
-        }
-        tc_commit(&s_full[b]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(&q_ready, 0);
-    issue_s(0);
-    for (int j = 0; j < ntiles; ++j) {
-      if (j + 1 < ntiles) issue_s(j + 1);
-      const int s = j % STAGES, b = j % NB;
-      const uint32_t ph2 = (j / NB) & 1;
-      mbar_wait(&p_full[b], ph2);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t d = tmem_base + TM_O;         // O accumulates in place over the key tiles (the softmax threads rescale it)
-        const uint32_t p_hi = tmem_base + TM_P + b * 64, p_lo = p_hi + 32;
-        const uint32_t vh = sb + s * STAGE_BYTES + 2 * TILE, vl = vh + TILE;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {           // 16 keys per MMA: 16 rows of the MN-major V tile = 2 KiB
-          const uint64_t dvh = desc_mnmajor(vh + kk * 2048), dvl = desc_mnmajor(vl + kk * 2048);
-          mma_f16_ts(d, p_lo + kk * 8, dvh, IDESC_PV, (j | kk) != 0);
-          mma_f16_ts(d, p_hi + kk * 8, dvl, IDESC_PV, 1);
-          mma_f16_ts(d, p_hi + kk * 8, dvh, IDESC_PV, 1);
-        }
-        tc_commit(&o_full[b]);
-        tc_commit(&empty[s]);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ================= softmax + output accumulation =================
-    // thread (q, lane, half): query row r = 32q + lane, keys [32*half, +32) of every tile and output dims
-    // [32*half, +32).  The pair of a row sits in warps w and w+4 (same TMEM lane quarter).
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int r = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const int bar_id = 2 + q;                        // named barrier of this warp pair (64 threads)
-    const int st = threadIdx.x - 64;                 // 0..255 among the softmax threads
-    // ---- Q planes of this row half -> tensor memory (two fp16 per column), straight from global memory
-    {
-      const size_t off = (size_t)(row_q0 + r) * a.ldq + col0 + half * 32;
-      uint32_t h[16], l[16];
-      const uint4* ph = reinterpret_cast<const uint4*>(a.q_hi + off);
-      const uint4* pl = reinterpret_cast<const uint4*>(a.q_lo + off);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint4 x = __ldg(ph + i), y = __ldg(pl + i);
-        h[4 * i] = x.x; h[4 * i + 1] = x.y; h[4 * i + 2] = x.z; h[4 * i + 3] = x.w;
-        l[4 * i] = y.x; l[4 * i + 1] = y.y; l[4 * i + 2] = y.z; l[4 * i + 3] = y.w;
-      }
-      tmem_st16(tmem_base + lane_addr + TM_Q + half * 16, h);
-      tmem_st16(tmem_base + lane_addr + TM_Q + 32 + half * 16, l);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&q_ready);
-    }
-    // ---- one power of two for P'' = p * vinv_j: the largest inverse V scale of this sequence and head
-    float vmx = 0.f;
-    for (int i = st; i < a.N; i += 256) vmx = fmaxf(vmx, __ldg(a.vinv + (size_t)head * a.rows + row_k0 + i));
-    vmx = warp_max(vmx);
-    if (lane == 0) red[warp - 2] = vmx;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) vmx = fmaxf(vmx, red[i]);
-    float p_scale, p_inv;
-    row_scale(vmx, p_scale, p_inv);                  // p * vinv_j * p_scale <= 2^15 for every key
-
-    // Lazy running maximum: the reference point m_used of a row only moves when a tile's maximum exceeds it by more than
-    // 2^TAU (in the exponent); until then p = 2^((s - m_used) c) <= 2^TAU, which the P'' scale leaves room for.  O therefore
-    // accumulates IN tensor memory across the key tiles (no per-tile read-back: TMEM reads run at 64 B/clk/SM and were half of
-    // the softmax threads' tile time); on the rare move the owning threads rescale their O rows in place.
-    constexpr float TAU = 8.f;
-    const float p_scale_l = p_scale * 0x1p-8f, p_inv_l = p_inv * 0x1p8f;
-    float m_used = -INFINITY, l_run = 0.f;
-    const uint32_t o_addr = tmem_base + TM_O + lane_addr + half * 32;
-    for (int j = 0; j < ntiles; ++j) {
-      const int b = j % NB, xb = j & 1, s = j % STAGES;
-      float sv[32];
-      mbar_wait(&full[s], (j / STAGES) & 1);         // the tile's vinv slice (read below) has landed
-      mbar_wait(&s_full[b], (j / NB) & 1);
-      tc_fence_after();
-      tmem_ld32(tmem_base + TM_S + lane_addr + b * 64 + half * 32, sv);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[b]);
-      float mx = sv[0];
-#pragma unroll
-      for (int i = 1; i < 32; ++i) mx = fmaxf(mx, sv[i]);
-      // the slot alternates with the tile parity: the partner passes the NEXT tile's barrier only after this read, and
-      // that barrier comes before anyone writes this slot again -- one barrier per tile is enough
-      xch[(xb * 2 + half) * QT + r] = mx;
-      asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");
-      mx = fmaxf(mx, xch[(xb * 2 + (half ^ 1)) * QT + r]);
-      const bool grow = (mx - m_used) * a.scale_log2 > TAU;          // always true on the first tile (m_used = -inf)
-      float alpha = 1.f;
-      if (grow) { alpha = ex2_fast((m_used - mx) * a.scale_log2); m_used = mx; }
-      if (j >= NB) mbar_wait(&o_full[b], ((j - NB) / NB) & 1);       // P.V of tile j-NB no longer reads this P buffer
-      if (j > 0 && __any_sync(0xffffffffu, grow)) {
-        // rescale this warp's O rows in place: every P.V issued so far (tile j-1 is the last) must have retired, and P.V(j)
-        // is not issued before all eight warps have arrived on p_full below
-        mbar_wait(&o_full[(j - 1) % NB], ((j - 1) / NB) & 1);
-        tc_fence_after();
-        float ov[32];
-        tmem_ld32(o_addr, ov);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) ov[i] *= alpha;
-        tmem_st32(o_addr, ov);
-        tmem_st_wait();
-        tc_fence_before();
-      }
-      // p = 2^((s - m_used) * c) on packed key pairs, P'' = p * (vinv_j * 2^ep) as unscaled fp16 hi / lo planes, two
-      // keys per 32-bit TMEM column.  The K / V tile's full barrier (waited on above) covers the vinv slice.
-      {
-        const float2 c2 = make_float2(a.scale_log2, a.scale_log2);
-        const float2 nm2 = make_float2(-m_used, -m_used);
-        const float2 ps2 = make_float2(p_scale_l, p_scale_l);
-        const float4* vi = reinterpret_cast<const float4*>(smem + (size_t)s * STAGE_BYTES + 4 * TILE) + half * 8;
-        float2 ps = make_float2(0.f, 0.f);
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 w = vi[i];
-          float2 e0 = fmul2(fadd2(make_float2(sv[4 * i], sv[4 * i + 1]), nm2), c2);       // (s - m) * c: the reference point maps to exactly 0
-          float2 e1 = fmul2(fadd2(make_float2(sv[4 * i + 2], sv[4 * i + 3]), nm2), c2);
-          e0.x = ex2_fast(e0.x); e0.y = ex2_fast(e0.y);
-          e1.x = ex2_fast(e1.x); e1.y = ex2_fast(e1.y);
-          ps = fadd2(ps, fadd2(e0, e1));
-          split2u_pk(fmul2(e0, fmul2(make_float2(w.x, w.y), ps2)), hi[2 * i], lo[2 * i]);
-          split2u_pk(fmul2(e1, fmul2(make_float2(w.z, w.w), ps2)), hi[2 * i + 1], lo[2 * i + 1]);
-        }
-        l_run = fmaf(l_run, alpha, ps.x + ps.y);     // partial row sum over this thread's keys
-        const uint32_t pbase = tmem_base + lane_addr + TM_P + b * 64 + half * 16;
-        tmem_st16(pbase, hi);
-        tmem_st16(pbase + 32, lo);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(&p_full[b]); mbar_arrive(&empty[s]); }
-    }
-    float o_acc[32];
-    {
-      const int jp = ntiles - 1;
-      mbar_wait(&o_full[jp % NB], (jp / NB) & 1);
-      tc_fence_after();
-      tmem_ld32(o_addr, o_acc);
-      tc_fence_before();
-    }
-    // total row sum = the two partial sums (same running max on both sides); 2^-ep undoes the P'' scale
-    const int fb = ntiles & 1;                       // the parity the last tile did not use
-    xch[(fb * 2 + half) * QT + r] = l_run;
-    asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");
-    const float inv = p_inv_l / (l_run + xch[(fb * 2 + (half ^ 1)) * QT + r]);
-    const size_t ooff = (size_t)(row_q0 + r) * a.ldo + col0 + half * 32;
-#pragma unroll
-    for (int i = 0; i < 32; i += 4) {
-      const float4 ov = make_float4(o_acc[i] * inv, o_acc[i + 1] * inv, o_acc[i + 2] * inv, o_acc[i + 3] * inv);
-      if (a.o_hi != nullptr) store_split4(a.o_hi, a.o_lo, ooff + i, ov);
-      else *reinterpret_cast<float4*>(a.o + ooff + i) = ov;
-    }
+    issue_kv(0);
+    if (ntiles > 1) issue_kv(1);
   }
-  tc_fence_before();
+
+  // ---- one power of two for P'' = p * vinv_j: the largest inverse V scale of this sequence and head
+  const float* vinv_h = a.vinv + (size_t)head * a.rows + row_k0;
+  float vmx = 0.f;
+  for (int i = tid; i < a.N; i += THREADS) vmx = fmaxf(vmx, __ldg(vinv_h + i));
+  vmx = warp_max(vmx);
+  if (lane == 0) red[warp] = vmx;
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(Cfg<NB>::TM_COLS) : "memory");
+#pragma unroll
+  for (int i = 0; i < 8; ++i) vmx = fmaxf(vmx, red[i]);
+  float p_scale, p_inv;
+  row_scale(vmx, p_scale, p_inv);                  // p * vinv_j * p_scale <= 2^15 for every key (p <= 1)
+
+  const uint32_t sb = smem_u32(smem);
+  const uint64_t dq_hi = desc_sw128(sb + OFF_Q + wg * TILE), dq_lo = desc_sw128(sb + OFF_Q + (2 + wg) * TILE);
+  const uint32_t p_hi = sb + OFF_P + wg * 2 * TILE, p_lo = p_hi + TILE;
+  const uint64_t dp_hi = desc_sw128(p_hi), dp_lo = desc_sw128(p_lo);
+  const int rl0 = (warp & 3) * 16 + (lane >> 2);   // this thread's rows (rl0, rl0 + 8) inside the warpgroup's 64
+  float o_acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  mbar_wait(&q_full, 0);
+
+  for (int j = 0; j < ntiles; ++j) {
+    const int s = j & 1;
+    const uint32_t kv = sb + OFF_KV + s * 4 * TILE;
+    mbar_wait(&full[s], (j >> 1) & 1);
+    float sv[32];
+    {
+      const uint64_t dk_hi = desc_sw128(kv), dk_lo = desc_sw128(kv + TILE);
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {             // 16 of the 64 head dims per MMA
+        const uint64_t adv = (uint64_t)(kk * 2);
+        wgmma_f16_n64(sv, dq_lo + adv, dk_hi + adv, kk != 0);
+        wgmma_f16_n64(sv, dq_hi + adv, dk_lo + adv, 1);
+        wgmma_f16_n64(sv, dq_hi + adv, dk_hi + adv, 1);
+      }
+      wg_commit();
+      wg_wait<0>();
+    }
+    // online softmax over this tile: a row's 64 keys sit in the 4 lanes of a quad (16 each)
+    float alpha[2], nm[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sv[4 * jj + 2 * h], sv[4 * jj + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx);
+      alpha[h] = ex2_fast((m_run[h] - m_new) * a.scale_log2);
+      m_run[h] = m_new;
+      nm[h] = -m_new;
+    }
+    const float* vi = vinv_h + j * KT;
+    float ps[2] = {0.f, 0.f};
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int key = 8 * jj + 2 * qd;
+      const float2 w = __ldg(reinterpret_cast<const float2*>(vi + key));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float e0 = ex2_fast((sv[4 * jj + 2 * h] + nm[h]) * a.scale_log2);      // the row maximum maps to exactly 1
+        const float e1 = ex2_fast((sv[4 * jj + 2 * h + 1] + nm[h]) * a.scale_log2);
+        ps[h] += e0 + e1;
+        uint32_t hw, lw;
+        split2u(e0 * (w.x * p_scale), e1 * (w.y * p_scale), hw, lw);
+        const int r = rl0 + 8 * h;
+        const uint32_t off = (uint32_t)r * 128u + (uint32_t)((jj ^ (r & 7)) << 4) + (uint32_t)(qd * 4);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(p_hi + off), "r"(hw) : "memory");
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(p_lo + off), "r"(lw) : "memory");
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      l_run[h] = fmaf(l_run[h], alpha[h], ps[h]);  // partial row sum over this lane's keys
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) { o_acc[4 * jj + 2 * h] *= alpha[h]; o_acc[4 * jj + 2 * h + 1] *= alpha[h]; }
+    }
+    fence_async_smem();
+    wg_bar(1 + wg);
+    {
+      const uint32_t vh = kv + 2 * TILE, vl = kv + 3 * TILE;
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {             // 16 keys per MMA: 16 rows of the MN-major V tile = 2 KiB
+        const uint64_t adv = (uint64_t)(kk * 2);
+        const uint64_t dvh = desc_sw128(vh + kk * 2048), dvl = desc_sw128(vl + kk * 2048);
+        wgmma_f16_n64_tb(o_acc, dp_lo + adv, dvh, 1);
+        wgmma_f16_n64_tb(o_acc, dp_hi + adv, dvl, 1);
+        wgmma_f16_n64_tb(o_acc, dp_hi + adv, dvh, 1);
+      }
+      wg_commit();
+      wg_wait<0>();
+    }
+    __syncthreads();                               // both warpgroups are done with K / V stage s and their P tiles
+    if (tid == 0 && j + 2 < ntiles) issue_kv(j + 2);
+  }
+  // total row sum over the quad; 2^-ep undoes the P'' scale
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = p_inv / l;
+    const size_t ooff = (size_t)(row_q0 + wg * 64 + rl0 + 8 * h) * a.ldo + col0 + 2 * qd;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const float2 ov = make_float2(o_acc[4 * jj + 2 * h] * inv, o_acc[4 * jj + 2 * h + 1] * inv);
+      if (a.o_hi != nullptr) store_split2(a.o_hi, a.o_lo, ooff + 8 * jj, ov);
+      else *reinterpret_cast<float2*>(a.o + ooff + 8 * jj) = ov;
+    }
   }
 }
 
@@ -384,8 +248,10 @@ extern "C" int omt_attn_spatial_h(const uint16_t* q_hi, const uint16_t* q_lo, in
   OMT_REQUIRE(heads > 0 && heads <= 65535 && n_seq <= 65535 && qk_plane_scale > 0.f, "omt_attn_spatial_h: bad arguments");
   if (n_seq == 0) return OMT_OK;
   const long long rows = (long long)n_seq * N;
-  CUtensorMap tmKh, tmKl, tmVh, tmVl;
+  CUtensorMap tmQh, tmQl, tmKh, tmKl, tmVh, tmVl;
   int rc;
+  if ((rc = encode2d(&tmQh, q_hi, heads * D, rows, ldq))) return rc;
+  if ((rc = encode2d(&tmQl, q_lo, heads * D, rows, ldq))) return rc;
   if ((rc = encode2d(&tmKh, k_hi, heads * D, rows, ldk))) return rc;
   if ((rc = encode2d(&tmKl, k_lo, heads * D, rows, ldk))) return rc;
   if ((rc = encode2d(&tmVh, v_hi, heads * D, rows, ldv))) return rc;
@@ -394,16 +260,12 @@ extern "C" int omt_attn_spatial_h(const uint16_t* q_hi, const uint16_t* q_lo, in
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev >= 0 && dev < 64 && !attr[dev]) {
-    OMT_CUDA(cudaFuncSetAttribute(attn_f16_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<1>::SMEM));
-    OMT_CUDA(cudaFuncSetAttribute(attn_f16_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<2>::SMEM));
+    OMT_CUDA(cudaFuncSetAttribute(attn_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     attr[dev] = true;
   }
-  Args a{q_hi, q_lo, ldq, vinv, rows, o, o_hi, o_lo, ldo, N, scale * 1.4426950408889634f / qk_plane_scale};
+  Args a{vinv, rows, o, o_hi, o_lo, ldo, N, scale * 1.4426950408889634f / qk_plane_scale};
   dim3 grid(N / QT, heads, n_seq);
-  if (g_attn_f16_ctas == 2)
-    OMT_CUDA(launch_k(attn_f16_kernel<1>, grid, dim3(THREADS), Cfg<1>::SMEM, (cudaStream_t)stream, tmKh, tmKl, tmVh, tmVl, a));
-  else
-    OMT_CUDA(launch_k(attn_f16_kernel<2>, grid, dim3(THREADS), Cfg<2>::SMEM, (cudaStream_t)stream, tmKh, tmKl, tmVh, tmVl, a));
+  OMT_CUDA(launch_k(attn_f16_kernel, grid, dim3(THREADS), SMEM, (cudaStream_t)stream, tmQh, tmQl, tmKh, tmKl, tmVh, tmVl, a));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

@@ -249,7 +249,7 @@ static int launch_temporal(const float* q, int ldq, const float* k, int ldk, con
 
 int launch_attn_tc3(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* o, uint16_t* o_hi,
                     uint16_t* o_lo, int ldo, int n_seq, int N, int heads, float scale, cudaStream_t st);
-int g_attn_kernel = 3;   // N % 128 == 0: 3 = tcgen05 3xTF32, Q / P as TMEM operands (attention_tc3.cu); 1 = CUDA-core fp32
+int g_attn_kernel = 3;   // N % 128 == 0: 3 = wgmma 3xTF32 core (attention_tc3.cu); 1 = CUDA-core fp32
 
 static int set_flash_smem() {
   static bool done[64];      // the attribute is per device

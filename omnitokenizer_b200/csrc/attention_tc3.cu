@@ -1,21 +1,13 @@
-// Attention v3: spatial (full, non-causal) attention core on tcgen05 with 3xTF32 compensation and
-// TMEM-resident A operands (tcgen05.mma "TS" form).  Same contract as attention_tc.cu:
+// Attention v3: spatial (full, non-causal) attention core on sm_90a wgmma with 3xTF32 compensation.
 //   O = softmax(scale * Q K^T) V  per (sequence, head), head dim 64, N % 128 == 0
 //   (F.scaled_dot_product_attention at modules/attention.py:451).
 //
-// Why: with A = Q / P in shared memory every N=64 MMA re-reads a 4 KiB A tile, so the MMAs are
-// shared-memory-bandwidth bound (6 KiB per ~32-cycle instruction; measured 814 us per layer).  Here Q
-// (once per CTA) and P (every key tile) live in TENSOR MEMORY as tf32 hi / lo column blocks and are
-// consumed as the TMEM A operand; only the K / V^T B tiles (2 KiB per MMA) come from shared memory, and
-// the freed shared memory double-buffers them.
-//   TMEM columns: S[2] 0-127 | O[2] 128-255 | P[2] x (hi | lo) 256-511  -- P is double-buffered so that the
-//                 softmax of tile j+1 never waits for P.V of tile j (the measured ~430 us of pure hand-off latency)
-//   smem bytes  : K_hi[2] | K_lo[2] | V^T_hi[2] | V^T_lo[2] | V_raw[2] | Q_hi | Q_lo
-//                 K tiles land directly in their K_hi stage (split in place); every TMA load is issued a full
-//                 tile ahead of its consumer, so the load latency is off the per-tile critical path
-// Roles: warp 0 TMA, warp 1 MMA issue + TMEM alloc, warps 2-5 transform (Q -> TMEM, K split, V transpose+split),
-//        warps 6-13 softmax: TWO threads per query row (32 keys / 32 output dims each; they only exchange the
-//        row max through smem), S from TMEM, P hi/lo back to TMEM, O accumulated in registers.
+// One CTA = two warpgroups, 64 query rows each; S and O live in registers (online softmax).  Every operand is split into
+// tf32 hi / lo in shared memory by the CTA (Q once, K in place per key tile, V transposed into the K-major V^T tile the
+// tf32 wgmma needs as its B operand), and every product takes three tf32 wgmmas (lo.hi + hi.lo + hi.hi).  P goes through a
+// per-warpgroup shared-memory tile (tf32 hi / lo) as the A operand of the P.V wgmmas.
+//   smem: Q_hi | Q_lo (32 KiB each) | K_hi | K_lo | V_raw | V^T_hi | V^T_lo (16 KiB each) | P[2 warpgroups] x (hi | lo) (16 KiB each)
+// Every fp32 tile is stored as 32-column halves of 128-byte rows (SWIZZLE_128B, the layout the TMA lands).
 #include "omt_common.cuh"
 #include "tc_ptx.cuh"
 #include <cuda.h>
@@ -25,17 +17,16 @@ namespace atc3 {
 using namespace omt::ptx;
 
 constexpr int QT = 128, KT = 64, D = 64;
-constexpr int Q_BYTES = QT * D * 4;     // 32 KiB
-constexpr int K_BYTES = KT * D * 4;     // 16 KiB
-constexpr int OFF_KH = 0, OFF_KL = 2 * K_BYTES, OFF_VH = 4 * K_BYTES, OFF_VL = 6 * K_BYTES;
-constexpr int OFF_VR = 8 * K_BYTES;                                  // V_raw[2]: TMA landing, two tiles deep
-constexpr int OFF_QH = 10 * K_BYTES, OFF_QL = OFF_QH + Q_BYTES;      // Q lands in OFF_QH, split in place
-constexpr int OFF_CTRL = OFF_QL + Q_BYTES;                           // barriers, TMEM pointer, row-max exchange
-constexpr int SMEM = OFF_CTRL + 2048;                                // 226 KiB: no static shared memory, no slack
-constexpr int TM_S = 0, TM_O = 128, TM_P = 256;                      // S[2] | O[2] | P[2] x (hi 64 | lo 64)
-constexpr int THREADS = 448;   // TMA, MMA, 4 transform warps, 8 softmax warps (two per TMEM lane quarter)
-// tf32 x tf32 -> f32, M=128, N=64; bit 16 = B is MN-major (used for V)
-constexpr uint32_t IDESC_KK = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+constexpr int HALF = 64 * 32 * 4;       // 8 KiB: 64 rows x 32 fp32 (one TMA box)
+constexpr int Q_BYTES = QT * D * 4;     // 32 KiB: [column half][128 rows]
+constexpr int K_BYTES = KT * D * 4;     // 16 KiB: [column half][64 rows]
+constexpr int OFF_QH = 0, OFF_QL = Q_BYTES;
+constexpr int OFF_KH = 2 * Q_BYTES, OFF_KL = OFF_KH + K_BYTES, OFF_VR = OFF_KL + K_BYTES;
+constexpr int OFF_VH = OFF_VR + K_BYTES, OFF_VL = OFF_VH + K_BYTES;
+constexpr int OFF_P = OFF_VL + K_BYTES;                              // [2 warpgroups] x (hi | lo), [key half][64 rows] each
+constexpr int OFF_CTRL = OFF_P + 4 * K_BYTES;
+constexpr int SMEM = OFF_CTRL + 64 + 1024;                           // barriers + alignment slack
+constexpr int THREADS = 256;
 
 struct Args {
   float* o; int ldo;
@@ -44,287 +35,165 @@ struct Args {
   float scale_log2;
 };
 
+__device__ __forceinline__ void split_inplace(float4* h, float4* l, int idx) {
+  const float4 v = h[idx];
+  float4 hi, lo;
+  hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
+  lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
+  h[idx] = hi;
+  l[idx] = lo;
+}
+// byte offset of element (row, col) of a [col half][rows] SWIZZLE_128B fp32 tile (half_bytes apart)
+__device__ __forceinline__ uint32_t sw_off(int row, int col, int half_bytes) {
+  return (uint32_t)((col >> 5) * half_bytes + row * 128 + ((((col & 31) >> 2) ^ (row & 7)) << 4) + (col & 3) * 4);
+}
+
 __global__ void __launch_bounds__(THREADS, 1)
 attn_tc3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const Args a) {
-  // All shared memory is dynamic (the kernel needs 226 of the 227 KiB): with no static allocation the dynamic
-  // window starts 1024-byte aligned, which the SW128 operand tiles require -- checked, not assumed.
-  extern __shared__ __align__(1024) uint8_t smem[];
-  if ((smem_u32(smem) & 1023u) != 0) __trap();
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_CTRL);
-  uint64_t& q_full = bars[0]; uint64_t& q_ready = bars[1];
-  uint64_t* k_full = bars + 2; uint64_t* v_full = bars + 4; uint64_t* vr_free = bars + 26;
-  uint64_t* k_ready = bars + 6;  uint64_t* k_empty = bars + 8;  uint64_t* v_ready = bars + 10; uint64_t* v_empty = bars + 12;
-  uint64_t* s_full = bars + 14;  uint64_t* s_empty = bars + 16; uint64_t* o_full = bars + 18;  uint64_t* o_empty = bars + 20;
-  uint64_t* p_full = bars + 22;
-  uint32_t& tmem_base_s = *reinterpret_cast<uint32_t*>(bars + 28);
-  float (*xch)[QT] = reinterpret_cast<float (*)[QT]>(smem + OFF_CTRL + 256);   // [2 key halves][row] row-max exchange
+  uint64_t& q_full = bars[0];
+  uint64_t& kv_full = bars[1];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2, qd = lane & 3;
   const int qt = blockIdx.x, head = blockIdx.y, seq = blockIdx.z;
   const int ntiles = a.N / KT;
   const int row_q0 = seq * a.N + qt * QT;
   const int row_k0 = seq * a.N;
   const int col0 = head * D;
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmQ)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmK)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmV)) : "memory");
-    mbar_init(&q_full, 1); mbar_init(&q_ready, 4);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&k_full[i], 1); mbar_init(&v_full[i], 1); mbar_init(&vr_free[i], 4);
-      mbar_init(&k_ready[i], 4); mbar_init(&k_empty[i], 1);
-      mbar_init(&v_ready[i], 4); mbar_init(&v_empty[i], 1);
-      mbar_init(&p_full[i], 8);      // per P stage: softmax warps may run one tile ahead of the tensor pipe
-      mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 8);
-      mbar_init(&o_full[i], 1); mbar_init(&o_empty[i], 8);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  if (tid == 0) {
+    prefetch_map(&tmQ); prefetch_map(&tmK); prefetch_map(&tmV);
+    mbar_init(&q_full, 1); mbar_init(&kv_full, 1);
+    fence_barrier_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
-  pdl_sync();      // everything above (barrier init, TMEM alloc, descriptor prefetch) overlapped the previous kernel's tail
+  pdl_sync();
 
-  if (warp == 0) {
-    // ================= TMA producer =================
-    if (lane == 0) {
-      mbar_expect_tx(&q_full, Q_BYTES);
-      tma_load_2d(&tmQ, &q_full, smem + OFF_QH, col0, row_q0);
-      tma_load_2d(&tmQ, &q_full, smem + OFF_QH + Q_BYTES / 2, col0 + 32, row_q0);
-      for (int j = 0; j < ntiles; ++j) {
-        const int st = j & 1;
-        const uint32_t ph2 = (j >> 1) & 1;
-        mbar_wait(&k_empty[st], ph2 ^ 1);        // S of tile j-2 retired: its K stage is free -> K_j lands one tile early
-        mbar_expect_tx(&k_full[st], K_BYTES);
-        tma_load_2d(&tmK, &k_full[st], smem + OFF_KH + st * K_BYTES, col0, row_k0 + j * KT);
-        tma_load_2d(&tmK, &k_full[st], smem + OFF_KH + st * K_BYTES + K_BYTES / 2, col0 + 32, row_k0 + j * KT);
-        mbar_wait(&vr_free[st], ph2 ^ 1);
-        mbar_expect_tx(&v_full[st], K_BYTES);
-        tma_load_2d(&tmV, &v_full[st], smem + OFF_VR + st * K_BYTES, col0, row_k0 + j * KT);
-        tma_load_2d(&tmV, &v_full[st], smem + OFF_VR + st * K_BYTES + K_BYTES / 2, col0 + 32, row_k0 + j * KT);
+  auto issue_kv = [&](int j) {
+    const int kr = row_k0 + j * KT;
+    mbar_expect_tx(&kv_full, 2 * K_BYTES);
+    for (int c = 0; c < 2; ++c) {
+      tma_load_2d(&tmK, &kv_full, smem + OFF_KH + c * HALF, col0 + 32 * c, kr);
+      tma_load_2d(&tmV, &kv_full, smem + OFF_VR + c * HALF, col0 + 32 * c, kr);
+    }
+  };
+  if (tid == 0) {
+    mbar_expect_tx(&q_full, Q_BYTES);
+    for (int c = 0; c < 2; ++c)
+      for (int w = 0; w < 2; ++w) tma_load_2d(&tmQ, &q_full, smem + OFF_QH + c * (Q_BYTES / 2) + w * HALF, col0 + 32 * c, row_q0 + 64 * w);
+    issue_kv(0);
+  }
+  // ---- Q: tf32 hi (in place) / lo
+  mbar_wait(&q_full, 0);
+#pragma unroll
+  for (int i = 0; i < Q_BYTES / 16 / THREADS; ++i)
+    split_inplace(reinterpret_cast<float4*>(smem + OFF_QH), reinterpret_cast<float4*>(smem + OFF_QL), tid + i * THREADS);
+
+  const uint32_t sb = smem_u32(smem);
+  const uint32_t p_hi = sb + OFF_P + wg * 2 * K_BYTES, p_lo = p_hi + K_BYTES;
+  const int rl0 = (warp & 3) * 16 + (lane >> 2);   // this thread's rows (rl0, rl0 + 8) inside the warpgroup's 64
+  float o_acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+  for (int j = 0; j < ntiles; ++j) {
+    mbar_wait(&kv_full, j & 1);
+    // ---- K split in place, V transposed into V^T [dim][key] and split
+#pragma unroll
+    for (int i = 0; i < K_BYTES / 16 / THREADS; ++i)
+      split_inplace(reinterpret_cast<float4*>(smem + OFF_KH), reinterpret_cast<float4*>(smem + OFF_KL), tid + i * THREADS);
+#pragma unroll
+    for (int it = 0; it < K_BYTES / 16 / THREADS; ++it) {
+      const int idx = it * THREADS + tid;
+      const int key = idx & 63, d4 = idx >> 6;
+      const float4 v = *reinterpret_cast<const float4*>(smem + OFF_VR + sw_off(key, d4 * 4, HALF));
+      const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint32_t off = sw_off(d4 * 4 + i, key, HALF);
+        const float hi = tf32_rn(e[i]);
+        *reinterpret_cast<float*>(smem + OFF_VH + off) = hi;
+        *reinterpret_cast<float*>(smem + OFF_VL + off) = e[i] - hi;
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ================= MMA issuer (whole warp converged; one elected lane issues) =================
-    {
-      const uint32_t sb = smem_u32(smem);
-      auto issue_s = [&](int j) {
-        const int st = j & 1;
-        const uint32_t ph2 = (j >> 1) & 1;
-        mbar_wait(&k_ready[st], ph2);
-        mbar_wait(&s_empty[st], ph2 ^ 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t d = tmem_base + TM_S + st * 64;
-          const uint64_t kh0 = desc_kmajor(sb + OFF_KH + st * K_BYTES), kl0 = desc_kmajor(sb + OFF_KL + st * K_BYTES);
-          const uint64_t qh0 = desc_kmajor(sb + OFF_QH), ql0 = desc_kmajor(sb + OFF_QL);
+    fence_async_smem();
+    __syncthreads();                               // split tiles (and, on the first tile, Q) are complete
+    // ---- S = Q K^T
+    float sv[32];
+    wg_fence();
 #pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {          // 8 tf32 of the head dim per MMA
-            const uint64_t adv = (uint64_t)(((kk >> 2) * (K_BYTES / 2) + (kk & 3) * 32) >> 4);
-            const uint64_t qadv = (uint64_t)(((kk >> 2) * (Q_BYTES / 2) + (kk & 3) * 32) >> 4);
-            mma_tf32(d, ql0 + qadv, kh0 + adv, IDESC_KK, kk != 0);
-            mma_tf32(d, qh0 + qadv, kl0 + adv, IDESC_KK, 1);
-            mma_tf32(d, qh0 + qadv, kh0 + adv, IDESC_KK, 1);
-          }
-          tc_commit(&s_full[st]);
-          tc_commit(&k_empty[st]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(&q_ready, 0);
-      issue_s(0);
-      for (int j = 0; j < ntiles; ++j) {
-        if (j + 1 < ntiles) issue_s(j + 1);
-        const int st = j & 1;
-        const uint32_t ph2 = (j >> 1) & 1;
-        mbar_wait(&p_full[st], ph2);
-        mbar_wait(&v_ready[st], ph2);
-        mbar_wait(&o_empty[st], ph2 ^ 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t d = tmem_base + TM_O + st * 64;
-          const uint64_t vh0 = desc_kmajor(sb + OFF_VH + st * K_BYTES), vl0 = desc_kmajor(sb + OFF_VL + st * K_BYTES);
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {          // 8 keys per MMA
-            const uint64_t adv = (uint64_t)(((kk >> 2) * (K_BYTES / 2) + (kk & 3) * 32) >> 4);
-            const uint32_t pbase = tmem_base + TM_P + st * 128;
-            mma_tf32_ts(d, pbase + 64 + kk * 8, vh0 + adv, IDESC_KK, kk != 0);
-            mma_tf32_ts(d, pbase + kk * 8, vl0 + adv, IDESC_KK, 1);
-            mma_tf32_ts(d, pbase + kk * 8, vh0 + adv, IDESC_KK, 1);
-          }
-          tc_commit(&o_full[st]);
-          tc_commit(&v_empty[st]);
-        }
-        __syncwarp();
-      }
+    for (int kk = 0; kk < 8; ++kk) {               // 8 tf32 of the head dim per MMA
+      const uint32_t qo = (kk >> 2) * (Q_BYTES / 2) + wg * HALF + (kk & 3) * 32;
+      const uint32_t ko = (kk >> 2) * HALF + (kk & 3) * 32;
+      wgmma_tf32_n64(sv, desc_sw128(sb + OFF_QL + qo), desc_sw128(sb + OFF_KH + ko), kk != 0);
+      wgmma_tf32_n64(sv, desc_sw128(sb + OFF_QH + qo), desc_sw128(sb + OFF_KL + ko), 1);
+      wgmma_tf32_n64(sv, desc_sw128(sb + OFF_QH + qo), desc_sw128(sb + OFF_KH + ko), 1);
     }
-  } else if (warp < 6) {
-    // ================= transform =================
-    const int t = threadIdx.x - 64;
-    // ---- Q: tf32 hi (in place) / lo in shared memory
-    mbar_wait(&q_full, 0);
-    {
-      float4* h = reinterpret_cast<float4*>(smem + OFF_QH);
-      float4* l = reinterpret_cast<float4*>(smem + OFF_QL);
+    wg_commit();
+    wg_wait<0>();
+    // ---- online softmax: a row's 64 keys sit in the 4 lanes of a quad (16 each)
 #pragma unroll
-      for (int i = 0; i < Q_BYTES / 16 / 128; ++i) {
-        const int idx = t + i * 128;
-        const float4 v = h[idx];
-        float4 hi, lo;
-        hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
-        lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
-        h[idx] = hi;
-        l[idx] = lo;
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&q_ready);
-    }
-    auto split_k = [&](int jj) {
-      const int st = jj & 1;
-      mbar_wait(&k_full[st], (jj >> 1) & 1);
-      float4* h = reinterpret_cast<float4*>(smem + OFF_KH + st * K_BYTES);
-      const float4* src = h;                     // split in place
-      float4* l = reinterpret_cast<float4*>(smem + OFF_KL + st * K_BYTES);
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
 #pragma unroll
-      for (int i = 0; i < K_BYTES / 16 / 128; ++i) {
-        const int idx = t + i * 128;
-        const float4 v = src[idx];
-        float4 hi, lo;
-        hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
-        lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
-        h[idx] = hi;
-        l[idx] = lo;
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&k_ready[st]);
-    };
-    split_k(0);
-    for (int j = 0; j < ntiles; ++j) {
-      if (j + 1 < ntiles) split_k(j + 1);
-      const int st = j & 1;
-      mbar_wait(&v_full[st], (j >> 1) & 1);
-      mbar_wait(&v_empty[st], ((j >> 1) & 1) ^ 1);
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int idx = it * 128 + t;
-        const int key = idx & 63, d4 = idx >> 6;
-        const float4 v = *reinterpret_cast<const float4*>(smem + OFF_VR + st * K_BYTES + (d4 >> 3) * (K_BYTES / 2) + key * 128 +
-                                                          (((d4 & 7) ^ (key & 7)) << 4));
-        const float e[4] = {v.x, v.y, v.z, v.w};
-        const int c = key >> 5, kk = key & 31;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int d = d4 * 4 + i;
-          const int off = st * K_BYTES + c * (K_BYTES / 2) + d * 128 + ((((kk >> 2) ^ (d & 7)) << 4) | ((kk & 3) << 2));
-          const float hi = tf32_rn(e[i]);
-          *reinterpret_cast<float*>(smem + OFF_VH + off) = hi;
-          *reinterpret_cast<float*>(smem + OFF_VL + off) = e[i] - hi;
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(&v_ready[st]); mbar_arrive(&vr_free[st]); }
-    }
-  } else {
-    // ================= softmax + output accumulation =================
-    // thread (q, lane, half): query row r = 32q + lane, keys [32*half, +32) of every tile and output dims
-    // [32*half, +32).  The pair of a row sits in warps w and w+4 (same TMEM lane quarter).
-    const int q = warp & 3;
-    const int half = (warp - 6) >> 2;
-    const int r = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const int bar_id = 2 + q;                        // named barrier of this warp pair (64 threads)
-    float o_acc[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
-    float m_run = -INFINITY, l_run = 0.f, alpha_prev = 1.f;
-    for (int j = 0; j < ntiles; ++j) {
-      float s[32];
-      mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-      tc_fence_after();
-      tmem_ld32(tmem_base + TM_S + lane_addr + (j & 1) * 64 + half * 32, s);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[j & 1]);
-      float mx = s[0];
-#pragma unroll
-      for (int i = 1; i < 32; ++i) mx = fmaxf(mx, s[i]);
-      xch[half][r] = mx;
-      asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");
-      mx = fmaxf(mx, xch[half ^ 1][r]);
-      asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");   // partner has read before the slot is reused
-      const float m_new = fmaxf(m_run, mx);
-      const float alpha = exp2f((m_run - m_new) * a.scale_log2);
+      for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sv[4 * jj + 2 * h], sv[4 * jj + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx);
+      const float alpha = exp2f((m_run[h] - m_new) * a.scale_log2);
+      m_run[h] = m_new;
+      const int r = rl0 + 8 * h;
       float psum = 0.f;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) { s[i] = exp2f((s[i] - m_new) * a.scale_log2); psum += s[i]; }
-      l_run = l_run * alpha + psum;                  // partial row sum over this thread's keys
-      m_run = m_new;
-      // publish P_j first (its TMEM stage was released when tile j-2 was folded), then fold O_{j-1}:
-      // the tensor pipe starts P_j.V_j while this thread is still accumulating the previous tile
-      {
-        float hi[32], lo[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) { hi[i] = tf32_rn(s[i]); lo[i] = s[i] - hi[i]; }
-        const uint32_t pbase = tmem_base + lane_addr + TM_P + (j & 1) * 128 + half * 32;
-        tmem_st32(pbase, hi);
-        tmem_st32(pbase + 64, lo);
+      for (int jj = 0; jj < 8; ++jj) {
+        const int key = 8 * jj + 2 * qd;
+        const float e0 = exp2f((sv[4 * jj + 2 * h] - m_new) * a.scale_log2);
+        const float e1 = exp2f((sv[4 * jj + 2 * h + 1] - m_new) * a.scale_log2);
+        psum += e0 + e1;
+        const float h0 = tf32_rn(e0), h1 = tf32_rn(e1);
+        const uint32_t off = sw_off(r, key, K_BYTES / 2);
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(p_hi + off), "f"(h0), "f"(h1) : "memory");
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(p_lo + off), "f"(e0 - h0), "f"(e1 - h1) : "memory");
+        o_acc[4 * jj + 2 * h] *= alpha;
+        o_acc[4 * jj + 2 * h + 1] *= alpha;
       }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[j & 1]);
-      if (j > 0) {
-        const int jp = j - 1;
-        mbar_wait(&o_full[jp & 1], (jp >> 1) & 1);
-        tc_fence_after();
-        float oj[32];
-        tmem_ld32(tmem_base + TM_O + lane_addr + (jp & 1) * 64 + half * 32, oj);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o_acc[i] = fmaf(o_acc[i], alpha_prev, oj[i]);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&o_empty[jp & 1]);
-      }
-      alpha_prev = alpha;
+      l_run[h] = l_run[h] * alpha + psum;          // partial row sum over this lane's keys
     }
-    {
-      const int jp = ntiles - 1;
-      mbar_wait(&o_full[jp & 1], (jp >> 1) & 1);
-      tc_fence_after();
-      float oj[32];
-      tmem_ld32(tmem_base + TM_O + lane_addr + (jp & 1) * 64 + half * 32, oj);
+    fence_async_smem();
+    wg_bar(1 + wg);
+    // ---- O += P V
+    wg_fence();
 #pragma unroll
-      for (int i = 0; i < 32; ++i) o_acc[i] = fmaf(o_acc[i], alpha_prev, oj[i]);
-      tc_fence_before();
+    for (int kk = 0; kk < 8; ++kk) {               // 8 keys per MMA
+      const uint32_t ko = (kk >> 2) * (K_BYTES / 2) + (kk & 3) * 32;
+      wgmma_tf32_n64(o_acc, desc_sw128(p_lo + ko), desc_sw128(sb + OFF_VH + ko), 1);
+      wgmma_tf32_n64(o_acc, desc_sw128(p_hi + ko), desc_sw128(sb + OFF_VL + ko), 1);
+      wgmma_tf32_n64(o_acc, desc_sw128(p_hi + ko), desc_sw128(sb + OFF_VH + ko), 1);
     }
-    // total row sum = the two partial sums (same running max on both sides)
-    xch[half][r] = l_run;
-    asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");
-    const float inv = 1.0f / (l_run + xch[half ^ 1][r]);
-    const size_t ooff = (size_t)(row_q0 + r) * a.ldo + col0 + half * 32;
-#pragma unroll
-    for (int i = 0; i < 32; i += 4) {
-      const float4 ov = make_float4(o_acc[i] * inv, o_acc[i + 1] * inv, o_acc[i + 2] * inv, o_acc[i + 3] * inv);
-      if (a.o_hi != nullptr) store_split4(a.o_hi, a.o_lo, ooff + i, ov);
-      else *reinterpret_cast<float4*>(a.o + ooff + i) = ov;
-    }
+    wg_commit();
+    wg_wait<0>();
+    __syncthreads();                               // every K / V / P tile of this key tile has been read
+    if (tid == 0 && j + 1 < ntiles) issue_kv(j + 1);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+  // total row sum over the quad
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.0f / l;
+    const size_t ooff = (size_t)(row_q0 + wg * 64 + rl0 + 8 * h) * a.ldo + col0 + 2 * qd;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const float2 ov = make_float2(o_acc[4 * jj + 2 * h] * inv, o_acc[4 * jj + 2 * h + 1] * inv);
+      if (a.o_hi != nullptr) store_split2(a.o_hi, a.o_lo, ooff + 8 * jj, ov);
+      else *reinterpret_cast<float2*>(a.o + ooff + 8 * jj) = ov;
+    }
   }
 }
 
@@ -360,7 +229,7 @@ int launch_attn_tc3(const float* q, int ldq, const float* k, int ldk, const floa
   using namespace atc3;
   CUtensorMap tmQ, tmK, tmV;
   const long long rows = (long long)n_seq * N;
-  int rc = encode2d(&tmQ, q, heads * D, rows, ldq, QT);
+  int rc = encode2d(&tmQ, q, heads * D, rows, ldq, 64);
   if (rc) return rc;
   rc = encode2d(&tmK, k, heads * D, rows, ldk, KT);
   if (rc) return rc;

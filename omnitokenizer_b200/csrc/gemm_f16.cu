@@ -1,4 +1,4 @@
-// GEMM v3 ("f16x3"): persistent 2-CTA (cta_group::2) tcgen05 kind::f16 GEMM on pre-split 16-bit operands.
+// GEMM v3 ("f16x3"): wgmma f16 GEMM on pre-split 16-bit operands (the kernel lives in gemm_wgmma.cuh).
 //
 //   C[M,N] = A[M,K] . W[N,K]^T (+bias)(+residual) | GEGLU | rope+l2norm+scale,   fp32-grade accuracy.
 //
@@ -6,560 +6,26 @@
 // 11 + 11 significant bits, error <= 2^-23 |x|), written ONCE by whatever kernel produced x (LayerNorm, the attention
 // cores, the GEGLU epilogue of this kernel; weights at pack time).  The product is
 //       A.W ~= A_hi.W_hi + 2^-11 (A_hi.W_lo + A_lo.W_hi)
-// three kind::f16 MMAs per k-step: the first into the MAIN fp32 TMEM accumulator, the two cross products into a second
-// one that the epilogue folds in with an exact power-of-two scale.  Against the 3xTF32 kernel (gemm_tc2.cu):
+// three f16 wgmmas per k-step: the first into the MAIN fp32 accumulator, the two cross products into a second one that
+// the epilogue folds in with an exact power-of-two scale.  Against the 3xTF32 kernel (gemm_tc2.cu):
 //   * 16-bit MMAs run at twice the tf32 rate -> the exactness tax drops from 3 to 1.5 tf32-equivalents per product;
-//   * the operands arrive in their final shared-memory form by TMA: no transform warps, no generic-proxy round trip
-//     between the TMA landing and the MMA (the k-block critical path is TMA -> mbarrier -> tcgen05.mma);
+//   * the operands arrive in their final shared-memory form by TMA: no split in shared memory;
 //   * W_hi / W_lo are half the bytes, A_hi + A_lo the same bytes as the fp32 activation.
-//
-// Per CTA (320 threads), a CTA pair owns a 256(M) x BN(N) tile (UMMA M = 256):
-//   warp 0     TMA producer: its 128 rows of A_hi / A_lo and its BN/2 rows of W_hi / W_lo per 64-wide k-block, every load
-//              credited to the LEADER's full[s] (cp.async.bulk.tensor .cta_group::2)
-//   warp 1     TMEM alloc; in the leader: tcgen05.mma issue (elect.sync), multicast tcgen05.commit -> empty[s] /
-//              tmem_full[acc] of both CTAs
-//   warps 2-9  epilogue, lane = accumulator row (the tcgen05.ld layout is never transposed through registers): each warp
-//              DRAINS its 32 x BN/2 slice of both accumulators into registers, releases the TMEM buffer at once, and only
-//              then does the bias / residual / GELU / rope work and the stores -- fp32 outputs are staged as SWIZZLE_128B
-//              32 x 32 boxes in a warp-private slab and leave by TMA STORE; GEGLU writes the planes of U directly.
-// TMEM budget (512 columns, two accumulators per tile): BN = 256 -> one buffer (the early release keeps the tensor pipe
-// idle only for the drain, 128 lanes x 512 columns at the TMEM read rate); BN = 128 -> two buffers (epilogue fully
-// overlapped, but twice the A traffic from L2).  omt_set_option("f16_bn", 128 | 256) selects; profiles/ has the A/B.
 //
 // NACC = 1, the ROW-SCALED form (omt_common.cuh): when the A planes come from a producer that saw whole rows (LayerNorm,
 // patch gather) they carry a per-row power-of-two scale and an UNSCALED lo plane, the weights a per-matrix one; all three
-// products then share ONE accumulator -> 256-wide tiles AND double buffering, half the drain.  The epilogue multiplies by
-// the exact inverse scales (a_rs[row] * w_scale).
-#include "omt_common.cuh"
-#include "tc_ptx.cuh"
-#include <cuda.h>
+// products then share ONE accumulator.  The epilogue multiplies by the exact inverse scales (a_rs[row] * w_scale).
+#include "gemm_wgmma.cuh"
 
 namespace omt {
-namespace f16g {
-using namespace omt::ptx;
 
-constexpr int BM = 128;                       // rows per CTA (tile M = 256 per pair)
-constexpr int BK = 64;                        // 16-bit elements per k-block = one 128-byte swizzle row
-constexpr int A_BYTES = BM * BK * 2;          // 16 KiB per plane
-constexpr int EPI_WARPS = 8;
-constexpr int SLAB_BYTES = 4096;              // one 32 x 32 fp32 box per epilogue warp
-constexpr int THREADS = 64 + EPI_WARPS * 32;  // TMA, MMA, 8 epilogue warps
+int g_f16_bn = 0;   // omt_set_option("f16_bn", 0|128|256): accepted for compatibility; the wgmma kernel always uses 128-wide tiles
 
-template <int BN, int NACC> struct Cfg {
-  static constexpr int W_BYTES = (BN / 2) * BK * 2;                 // per plane, per CTA
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;     // A_hi, A_lo, W_hi, W_lo
-  static constexpr int STAGES = (BN == 256) ? 3 : 4;                // 192 KiB either way
-  static constexpr int NBUF = 512 / (NACC * BN) >= 2 ? 2 : 1;       // TMEM accumulator buffers (NACC accumulators each)
-  static constexpr int SMEM = STAGES * STAGE_BYTES + EPI_WARPS * SLAB_BYTES + 1024;
-};
-
-struct HArgs {
-  int M, N, K;
-  int num_m_blk, num_n_blk, n_split;
-  int a_seg, a_seg_stride, a_seg_off;         // A row map (the TMA strides live in the tensor maps; the epilogue needs it for a_rs)
-  const float* a_rs; const float* a2_rs;      // NACC == 1: inverse row scales of the A planes (second: dual-A columns >= n_split)
-  float a_rs_uniform;                         // NACC == 1 with a_rs == NULL: one inverse scale for every row (statically bounded A)
-  float w_scale;                              // NACC == 1: inverse scale of the W planes
-  float u_scale;                              // GEGLU: > 0 -> U planes in the static-scaled form (unscaled lo), else 2^11-scaled lo
-  int c_seg, c_seg_stride, c_seg_off;         // C / residual row map
-  const float* bias;
-  const float* residual; int ldr;
-  uint16_t* u_hi; uint16_t* u_lo; int ldu;    // GEGLU: split planes of U[M, N/2]
-  const float* rope_cos; const float* rope_sin; const float* q_scale; const float* k_scale;
-  int qk_cols; int tokens;
-  // OMT_EPI_QKV_PLANES: q / k / v leave as fp16 operand planes for the attention core (attention_f16.cu)
-  float q_ps, k_ps;                           // static plane scales of the q and k heads (powers of two)
-  float* vinv;                                // [v heads][M]: inverse per-(row, head) scale of the v planes
-};
-
-// Tile raster: clusters walk the tiles in groups of G = num_clusters m-blocks; inside a group all clusters take the
-// same n-block at the same time, so a group's slice of A and the W tile stay L2-resident across the n sweep.
-__device__ __forceinline__ void decode_tile(int linear, int num_m_blk, int num_n_blk, int G, int& m_blk, int& n_blk) {
-  const int per_group = G * num_n_blk;
-  const int g = linear / per_group;
-  const int m_lo = g * G;
-  const int gm = min(G, num_m_blk - m_lo);
-  const int r = linear - g * per_group;
-  n_blk = r / gm;
-  m_blk = m_lo + r % gm;
-}
-
-// byte offset of 16-byte chunk c4 of row `row` inside a SWIZZLE_128B box (rows of 128 B, 1024-byte aligned base)
-__device__ __forceinline__ uint32_t sw128(int row, int c4) { return (uint32_t)row * 128u + (uint32_t)((c4 ^ (row & 7)) << 4); }
-
-__device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c, float d) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
-template <int BN, int NACC, int EPI>
-__global__ void __launch_bounds__(THREADS, 1)
-gemm_f16_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
-                const __grid_constant__ CUtensorMap tmA2h, const __grid_constant__ CUtensorMap tmA2l,
-                const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl,
-                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmPh,
-                const __grid_constant__ CUtensorMap tmPl, const HArgs g) {
-  using C_ = Cfg<BN, NACC>;
-  constexpr int W_BYTES = C_::W_BYTES, STAGE_BYTES = C_::STAGE_BYTES, STAGES = C_::STAGES, NBUF = C_::NBUF;
-  static_assert(NBUF * NACC * BN <= 512, "TMEM: NACC accumulators of BN columns, NBUF buffers");
-  constexpr uint32_t IDESC = idesc_f16(256, BN, false, false);          // fp16 x fp16 -> fp32, UMMA 256 x BN x 16
-
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment (SW128 tiles) by POINTER OFFSET so the pointer keeps the shared address space
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t full[STAGES];        // used in the leader: A and W planes of BOTH CTAs landed
-  __shared__ __align__(8) uint64_t empty[STAGES];       // local: MMAs reading this stage retired (multicast commit)
-  __shared__ __align__(8) uint64_t tmem_full[2];        // local: accumulator complete (multicast commit)
-  __shared__ __align__(8) uint64_t tmem_empty[2];       // used in the leader: both CTAs' epilogues drained the accumulator
-  __shared__ uint32_t tmem_base_s;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_rank();
-  const bool leader = rank == 0;
-  const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-  const int num_kb = g.K / BK;
-  const int num_tiles = g.num_m_blk * g.num_n_blk;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAh)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAl)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA2h)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA2l)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmWh)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmWl)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmC)) : "memory");
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 2 * EPI_WARPS);   // epilogue warps of both CTAs
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();                     // peer barriers are initialised before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
-  pdl_sync();
-
-  if (warp == 0) {
-    // ================= TMA producer =================
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        int m_blk, n_blk;
-        decode_tile(tile, g.num_m_blk, g.num_n_blk, num_clusters, m_blk, n_blk);
-        const int m0 = m_blk * (2 * BM) + (int)rank * BM;
-        const int n0 = n_blk * BN + (int)rank * (BN / 2);
-        const bool second = n_blk * BN >= g.n_split;          // dual-A: columns >= n_split read the second matrix
-        const CUtensorMap* mah = second ? &tmA2h : &tmAh;
-        const CUtensorMap* mal = second ? &tmA2l : &tmAl;
-        int c1[2], c2[2];
-        for (int hf = 0; hf < 2; ++hf) {
-          const int r = m0 + hf * 64;
-          if (g.a_seg > 0) { c1[hf] = r % g.a_seg; c2[hf] = r / g.a_seg; }
-          else { c1[hf] = r; c2[hf] = 0; }
-        }
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&empty[s], ph ^ 1);
-          uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
-          if (leader) mbar_expect_tx(&full[s], 2 * STAGE_BYTES);       // both CTAs' planes
-          tma_load_3d_pair(mah, &full[s], sp, kb * BK, c1[0], c2[0]);
-          tma_load_3d_pair(mah, &full[s], sp + A_BYTES / 2, kb * BK, c1[1], c2[1]);
-          tma_load_3d_pair(mal, &full[s], sp + A_BYTES, kb * BK, c1[0], c2[0]);
-          tma_load_3d_pair(mal, &full[s], sp + A_BYTES + A_BYTES / 2, kb * BK, c1[1], c2[1]);
-          tma_load_2d_pair(&tmWh, &full[s], sp + 2 * A_BYTES, kb * BK, n0);
-          tma_load_2d_pair(&tmWl, &full[s], sp + 2 * A_BYTES + W_BYTES, kb * BK, n0);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ================= MMA issuer (leader CTA; the warp stays converged, one elected lane issues) =================
-    if (leader) {
-      uint32_t it = 0, tcount = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tcount) {
-        const uint32_t acc = tcount % NBUF, acc_ph = (tcount / NBUF) & 1;
-        mbar_wait(&tmem_empty[acc], acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_main = tmem_base + acc * (NACC * BN);
-        const uint32_t d_cross = d_main + (NACC - 1) * BN;              // == d_main in the row-scaled (single accumulator) form
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t sa = smem_u32(smem + (size_t)s * STAGE_BYTES);
-            const uint64_t d_ahi = desc_kmajor(sa), d_alo = desc_kmajor(sa + A_BYTES);
-            const uint64_t d_whi = desc_kmajor(sa + 2 * A_BYTES), d_wlo = desc_kmajor(sa + 2 * A_BYTES + W_BYTES);
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              const uint64_t adv = (uint64_t)(k * 32 >> 4);             // 16 elements = 32 bytes inside the swizzle row
-              mma_f16_pair(d_cross, d_alo + adv, d_whi + adv, IDESC, (kb | k) != 0);
-              mma_f16_pair(d_cross, d_ahi + adv, d_wlo + adv, IDESC, 1);
-              mma_f16_pair(d_main, d_ahi + adv, d_whi + adv, IDESC, NACC == 1 ? 1u : (uint32_t)((kb | k) != 0));
-            }
-            tc_commit_pair(&empty[s]);
-            if (kb == num_kb - 1) tc_commit_pair(&tmem_full[acc]);
-          }
-          __syncwarp();
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ================= epilogue =================
-    const int q = warp & 3;                            // TMEM lane quarter this warp may read
-    const int hf = (warp - 2) >> 2;                    // which half of the tile's columns
-    constexpr int CH = BN / 64;                        // 32-column chunks per warp and tile
-    const uint32_t slab = smem_u32(smem + (size_t)STAGES * STAGE_BYTES) + (uint32_t)(warp - 2) * SLAB_BYTES;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    uint32_t tcount = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tcount) {
-      const uint32_t acc = tcount % NBUF, acc_ph = (tcount / NBUF) & 1;
-      int m_blk, n_blk;
-      decode_tile(tile, g.num_m_blk, g.num_n_blk, num_clusters, m_blk, n_blk);
-      const int mw = m_blk * (2 * BM) + (int)rank * BM + q * 32;     // first row of this warp
-      const int m = mw + lane;                                        // this lane's row
-      const int n0 = n_blk * BN + hf * (BN / 2);                      // first column of this warp
-      const bool row_ok = m < g.M;
-      const long long prow = map_row(row_ok ? m : 0, g.c_seg, g.c_seg_stride, g.c_seg_off);
-      // TMA store coordinates of the warp's 32 rows (a row-map segment is a multiple of 32 rows)
-      int cm1 = mw, cm2 = 0;
-      if (g.c_seg > 0) { cm1 = mw % g.c_seg; cm2 = mw / g.c_seg; }
-      const uint32_t t_main = tmem_base + lane_addr + acc * (NACC * BN) + (uint32_t)(hf * (BN / 2));
-      float out_scale = 1.0f;                                          // row-scaled form: exact inverse of the operand scales
-      if (NACC == 1) {
-        const float* rs = (n_blk * BN >= g.n_split) ? g.a2_rs : g.a_rs;
-        out_scale = g.w_scale * (rs == nullptr ? g.a_rs_uniform : (row_ok ? __ldg(rs + map_row(m, g.a_seg, g.a_seg_stride, g.a_seg_off)) : 1.0f));
-      }
-
-      // residual row segments (8 x 16 bytes per lane and chunk) ride in ONE register buffer: the next chunk's loads are
-      // issued right after the current chunk's adds, so their latency hides behind the box store
-      const float* rrow = (EPI == OMT_EPI_NONE && g.residual != nullptr) ? g.residual + (size_t)prow * g.ldr : nullptr;
-      float4 res[8];
-      auto load_res = [&](int c) {
-        const int n = n0 + c * 32;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          res[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (rrow != nullptr && row_ok && n < g.N) res[i] = *reinterpret_cast<const float4*>(rrow + n + 4 * i);
-        }
-      };
-      if (EPI == OMT_EPI_NONE && BN == 128) load_res(0);      // 64 accumulator registers: room to prefetch
-
-      // ---- drain: this lane's row of both accumulators -> registers (main + cross * 2^-11), then release the buffer.
-      //      The q / k / v epilogues drain one 64-column head at a time (their shared-memory / TMA stores are ordered with
-      //      the release, so draining everything first keeps all 128 values of the row live and spills); the others drain
-      //      all chunks, release, and let the compiler interleave the arithmetic.
-      float v[CH][32];
-      mbar_wait(&tmem_full[acc], acc_ph);
-      tc_fence_after();
-      auto drain = [&](int c) {
-        if (NACC == 2) {
-          float x[32];
-          tmem_ld32(t_main + (uint32_t)(BN + c * 32), x);
-          tmem_ld32(t_main + (uint32_t)(c * 32), v[c]);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[c][j] = fmaf(x[j], 1.0f / F16X3_LO_SCALE, v[c][j]);
-        } else {
-          tmem_ld32(t_main + (uint32_t)(c * 32), v[c]);
-          const float2 os2 = make_float2(out_scale, out_scale);
-#pragma unroll
-          for (int j = 0; j < 32; j += 2) {
-            const float2 t = fmul2(make_float2(v[c][j], v[c][j + 1]), os2);
-            v[c][j] = t.x; v[c][j + 1] = t.y;
-          }
-        }
-      };
-      auto release = [&]() {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_remote(mapa(smem_u32(&tmem_empty[acc]), 0));
-      };
-      constexpr bool PER_HEAD = (EPI == OMT_EPI_QKV || EPI == OMT_EPI_QKV_PLANES);
-      // plain epilogue with two accumulator buffers: the release is not urgent, drain chunk by chunk (no spills)
-      constexpr bool PER_CHUNK = (EPI == OMT_EPI_NONE && NBUF == 2 && BN == 256);
-      if constexpr (!PER_HEAD && !PER_CHUNK) {
-#pragma unroll
-        for (int c = 0; c < CH; ++c) drain(c);
-        release();
-      }
-
-      // stage a finished 32 x 32 fp32 box in the slab (swizzled, conflict-free 16-byte stores) and hand it to the TMA
-      auto store_box = [&](int n, const float (&t)[32]) {
-        if (lane == 0) bulk_wait_read<0>();           // the previous box has left the slab
-        __syncwarp();
-#pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) sts128(slab + sw128(lane, c4), t[4 * c4], t[4 * c4 + 1], t[4 * c4 + 2], t[4 * c4 + 3]);
-        fence_async_smem();
-        __syncwarp();
-        if (lane == 0 && mw < g.M) {
-          tma_store_3d(&tmC, slab, n, cm1, cm2);
-          bulk_commit();
-        }
-      };
-
-      // a 32-row x 64-column fp16 plane tile (one head of this warp's rows): words w[32] of this lane's row -> slab -> TMA
-      auto store_plane = [&](const CUtensorMap* map, int n, const uint32_t (&w)[32]) {
-        if (lane == 0) bulk_wait_read<0>();
-        __syncwarp();
-#pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4)
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(slab + sw128(lane, c4)), "r"(w[4 * c4]), "r"(w[4 * c4 + 1]),
-                       "r"(w[4 * c4 + 2]), "r"(w[4 * c4 + 3]) : "memory");
-        fence_async_smem();
-        __syncwarp();
-        if (lane == 0 && mw < g.M) {
-          tma_store_2d(map, slab, n, mw);
-          bulk_commit();
-        }
-      };
-
-      if constexpr (EPI == OMT_EPI_QKV || EPI == OMT_EPI_QKV_PLANES) {
-        // ---- q / k heads: rope + l2norm + per-dim scale (attention.py:417-421, 435-437); a head = two chunks, all
-        //      64 values of a row live in one lane, so the norm is thread-local
-#pragma unroll
-        for (int hd = 0; hd < CH / 2; ++hd) {
-          const int nh = n0 + hd * 64;
-          drain(2 * hd);
-          drain(2 * hd + 1);
-          if (hd == CH / 2 - 1) release();
-          if (nh < g.N) {
-            float (&va)[32] = v[2 * hd];
-            float (&vb)[32] = v[2 * hd + 1];
-            if (nh < g.qk_cols) {
-              if (g.rope_cos != nullptr) {
-                const int pos = (row_ok ? m : 0) % g.tokens;
-                const float4* ct = reinterpret_cast<const float4*>(g.rope_cos + (size_t)pos * 32);
-                const float4* st = reinterpret_cast<const float4*>(g.rope_sin + (size_t)pos * 32);
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {          // 4 complex pairs per float4 of the table
-                  const float4 c = __ldg(ct + i), s = __ldg(st + i);
-                  const float cc[4] = {c.x, c.y, c.z, c.w}, ss[4] = {s.x, s.y, s.z, s.w};
-#pragma unroll
-                  for (int p = 0; p < 4; ++p) {
-                    const float x = va[8 * i + 2 * p], y = va[8 * i + 2 * p + 1];
-                    va[8 * i + 2 * p] = x * cc[p] - y * ss[p];
-                    va[8 * i + 2 * p + 1] = x * ss[p] + y * cc[p];
-                  }
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const float4 c = __ldg(ct + 4 + i), s = __ldg(st + 4 + i);
-                  const float cc[4] = {c.x, c.y, c.z, c.w}, ss[4] = {s.x, s.y, s.z, s.w};
-#pragma unroll
-                  for (int p = 0; p < 4; ++p) {
-                    const float x = vb[8 * i + 2 * p], y = vb[8 * i + 2 * p + 1];
-                    vb[8 * i + 2 * p] = x * cc[p] - y * ss[p];
-                    vb[8 * i + 2 * p + 1] = x * ss[p] + y * cc[p];
-                  }
-                }
-              }
-              // sum of squares and inv * scale on packed pairs (FFMA2 / FMUL2: half the issue slots of the scalar forms)
-              float2 sq0 = make_float2(0.f, 0.f), sq1 = make_float2(0.f, 0.f);
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float2 a0 = make_float2(va[j], va[j + 1]), a1 = make_float2(va[j + 2], va[j + 3]);
-                sq0 = ffma2(a0, a0, sq0); sq1 = ffma2(a1, a1, sq1);
-              }
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float2 b0 = make_float2(vb[j], vb[j + 1]), b1 = make_float2(vb[j + 2], vb[j + 3]);
-                sq0 = ffma2(b0, b0, sq0); sq1 = ffma2(b1, b1, sq1);
-              }
-              const float inv = 1.0f / fmaxf(sqrtf((sq0.x + sq0.y) + (sq1.x + sq1.y)), 1e-12f);
-              const float2 inv2 = make_float2(inv, inv);
-              const float4* scv = reinterpret_cast<const float4*>((nh < g.qk_cols / 2) ? g.q_scale : g.k_scale);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 sa = __ldg(scv + i), sb = __ldg(scv + 8 + i);
-                float2 t;
-                t = fmul2(fmul2(make_float2(va[4 * i], va[4 * i + 1]), inv2), make_float2(sa.x, sa.y)); va[4 * i] = t.x; va[4 * i + 1] = t.y;
-                t = fmul2(fmul2(make_float2(va[4 * i + 2], va[4 * i + 3]), inv2), make_float2(sa.z, sa.w)); va[4 * i + 2] = t.x; va[4 * i + 3] = t.y;
-                t = fmul2(fmul2(make_float2(vb[4 * i], vb[4 * i + 1]), inv2), make_float2(sb.x, sb.y)); vb[4 * i] = t.x; vb[4 * i + 1] = t.y;
-                t = fmul2(fmul2(make_float2(vb[4 * i + 2], vb[4 * i + 3]), inv2), make_float2(sb.z, sb.w)); vb[4 * i + 2] = t.x; vb[4 * i + 3] = t.y;
-              }
-            }
-            if constexpr (EPI == OMT_EPI_QKV) {
-              store_box(nh, va);
-              if (nh + 32 < g.N) store_box(nh + 32, vb);
-            } else {
-              // operand planes for the attention core: q / k with the layer's static power-of-two scale, v scaled per
-              // (row, head) -- this lane holds the whole head of its row -- with the inverse scale kept in vinv
-              float sc = nh < g.qk_cols / 2 ? g.q_ps : g.k_ps;
-              if (nh >= g.qk_cols) {
-                float mx = 0.f;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) mx = fmaxf(mx, fmaxf(fabsf(va[j]), fabsf(vb[j])));
-                float inv;
-                row_scale(mx, sc, inv);
-                if (row_ok) g.vinv[(size_t)((nh - g.qk_cols) >> 6) * g.M + m] = inv;
-              }
-              uint32_t wh[32], wl[32];
-              const float2 sc2 = make_float2(sc, sc);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                split2u_pk(fmul2(make_float2(va[2 * i], va[2 * i + 1]), sc2), wh[i], wl[i]);
-                split2u_pk(fmul2(make_float2(vb[2 * i], vb[2 * i + 1]), sc2), wh[16 + i], wl[16 + i]);
-              }
-              store_plane(&tmPh, nh, wh);
-              store_plane(&tmPl, nh, wl);
-            }
-          }
-        }
-      } else if constexpr (EPI == OMT_EPI_GEGLU) {
-        // ---- packed columns (2j, 2j+1) = (value_j, gate_j): U[:, j] = gelu_erf(gate) * value, written as the fp16 hi / lo
-        //      planes the second FeedForward GEMM reads (16 outputs = one 32-byte segment per row and plane)
-#pragma unroll
-        for (int c = 0; c < CH; ++c) {
-          const int n = n0 + c * 32;
-          if (n < g.N) {
-            uint32_t hi[8], lo[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float o0 = gelu_erf(v[c][4 * i + 1]) * v[c][4 * i];
-              const float o1 = gelu_erf(v[c][4 * i + 3]) * v[c][4 * i + 2];
-              if (g.u_scale > 0.f) split2u(o0 * g.u_scale, o1 * g.u_scale, hi[i], lo[i]);
-              else split2(o0, o1, hi[i], lo[i]);
-            }
-            if (row_ok) {
-              const size_t off = (size_t)prow * g.ldu + (n >> 1);
-              uint4* ph = reinterpret_cast<uint4*>(g.u_hi + off);
-              uint4* pl = reinterpret_cast<uint4*>(g.u_lo + off);
-              ph[0] = make_uint4(hi[0], hi[1], hi[2], hi[3]); ph[1] = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-              pl[0] = make_uint4(lo[0], lo[1], lo[2], lo[3]); pl[1] = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-            }
-          }
-        }
-      } else {
-        // ---- plain: (+bias)(+residual), fp32 box by TMA store
-        if (BN != 128) load_res(0);
-#pragma unroll
-        for (int c = 0; c < CH; ++c) {
-          const int n = n0 + c * 32;
-          if constexpr (PER_CHUNK) {
-            drain(c);
-            if (c == CH - 1) release();
-          }
-          if (n < g.N) {
-            if (g.bias != nullptr) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 bb = __ldg(reinterpret_cast<const float4*>(g.bias + n) + i);
-                v[c][4 * i] += bb.x; v[c][4 * i + 1] += bb.y; v[c][4 * i + 2] += bb.z; v[c][4 * i + 3] += bb.w;
-              }
-            }
-            if (g.residual != nullptr) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 r = res[i];
-                v[c][4 * i] += r.x; v[c][4 * i + 1] += r.y; v[c][4 * i + 2] += r.z; v[c][4 * i + 3] += r.w;
-              }
-              if (c + 1 < CH) load_res(c + 1);
-            }
-            store_box(n, v[c]);
-          }
-        }
-      }
-    }
-    if (lane == 0) bulk_wait<0>();      // every box has been written out before the CTA (and its shared memory) retires
-    __syncwarp();
-  }
-  // ---- teardown: nobody may leave while the peer can still signal our barriers / read our smem
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-  }
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static int encode_map(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const cuuint64_t* dims,
-                      const cuuint64_t* strides, const cuuint32_t* box) {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  if (fn == nullptr) { set_error("cuTensorMapEncodeTiled entry point not found"); return OMT_E_CUDA; }
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(m, dt, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return OMT_E_CUDA; }
-  return OMT_OK;
-}
-
-// [K, seg, n_seg] map over a row-mapped matrix of 16-bit (esize 2) or fp32 (esize 4) elements
-static int row_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const void* ptr, int ld, int rows, int cols,
-                   int seg, int seg_stride, int seg_off, int box_cols, int box_rows) {
-  const int s = seg > 0 ? seg : rows;
-  const int nseg = seg > 0 ? rows / seg : 1;
-  const long long sstride = seg > 0 ? seg_stride : rows;
-  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)s, (cuuint64_t)nseg};
-  cuuint64_t strides[2] = {(cuuint64_t)ld * esize, (cuuint64_t)sstride * ld * esize};
-  cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows, 1};
-  const uint8_t* base = static_cast<const uint8_t*>(ptr) + (size_t)(seg > 0 ? seg_off : 0) * ld * esize;
-  return encode_map(m, dt, base, 3, dims, strides, box);
-}
-
-template <int BN, int NACC, int EPI>
-static int launch(const CUtensorMap* maps, const HArgs& g, cudaStream_t st) {
-  auto kern = gemm_f16_kernel<BN, NACC, EPI>;
-  static bool attr[64];
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr[dev]) {
-    OMT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN, NACC>::SMEM));
-    attr[dev] = true;
-  }
-  const int num_tiles = g.num_m_blk * g.num_n_blk;
-  int clusters = omt::sm_count() / 2;
-  if (clusters > num_tiles) clusters = num_tiles;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = Cfg<BN, NACC>::SMEM;
-  cfg.stream = st;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = g_pdl ? 2 : 1;
-  OMT_CUDA(cudaLaunchKernelEx(&cfg, kern, maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], maps[6], maps[7], maps[8], g));
-  return OMT_OK;
-}
-
-}  // namespace f16g
-
-int g_f16_bn = 0;   // omt_set_option("f16_bn", 0|128|256): tile N of the two-accumulator form (0 = by shape)
-
-// A planes: [M, lda] fp16; W planes: [n_pad, K] fp16 (rows padded to 256); C fp32 (plain / QKV) or U planes (GEGLU)
+// A planes: [M, lda] fp16; W planes: [n_pad, K] fp16 (rows padded to 256); C fp32 (plain / QKV) or U planes (GEGLU / QKV planes)
 int launch_gemm_f16(const omt_linear_h_args& a, cudaStream_t st) {
-  using namespace f16g;
-  const bool rs = a.a_rs != nullptr || a.a_rs_uniform > 0.f;   // row-scaled planes: one accumulator, 256-wide double-buffered tiles
-  // two accumulators: 256-wide tiles hold ONE TMEM buffer (the drain is exposed: 1/3 of a K = 512 main loop), 128-wide
-  // tiles two (but read A from L2 once per 128 columns) -- measured on B200: 128 wins only for the K = N = 512 shapes
-  int BN = rs ? 256 : (g_f16_bn != 0 ? g_f16_bn : ((a.K <= 512 && a.N <= 512) ? 128 : 256));
-  OMT_REQUIRE(a.K % BK == 0 && a.lda % 8 == 0, "omt_linear_h: K=%d must be a multiple of 64 and lda %% 8 == 0", a.K);
+  using namespace wgg;
+  const bool rs = a.a_rs != nullptr || a.a_rs_uniform > 0.f;   // row-scaled planes: one accumulator
+  OMT_REQUIRE(a.K % 64 == 0 && a.lda % 8 == 0, "omt_linear_h: K=%d must be a multiple of 64 and lda %% 8 == 0", a.K);
   if (a.a_seg > 0)
     OMT_REQUIRE(a.a_seg % 64 == 0 && a.M % a.a_seg == 0, "omt_linear_h: A row-map segment %d must be a multiple of 64 dividing M=%d", a.a_seg, a.M);
   if (a.c_seg > 0)
@@ -567,49 +33,31 @@ int launch_gemm_f16(const omt_linear_h_args& a, cudaStream_t st) {
   OMT_REQUIRE(a.N % 32 == 0, "omt_linear_h: N=%d must be a multiple of 32", a.N);
   if (a.a2_hi != nullptr) OMT_REQUIRE(a.n_split > 0 && a.n_split % 256 == 0, "omt_linear_h: n_split=%d must be a multiple of 256", a.n_split);
   const int n_pad = (a.N + 255) / 256 * 256;
-  const CUtensorMapDataType dt_hi = CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dt_lo = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  CUtensorMap maps[9];
-  int rc;
-  if ((rc = row_map(&maps[0], dt_hi, 2, a.a_hi, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off, BK, 64))) return rc;
-  if ((rc = row_map(&maps[1], dt_lo, 2, a.a_lo, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off, BK, 64))) return rc;
+  const CUtensorMapDataType f16 = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const bool dual = a.a2_hi != nullptr;
-  if ((rc = row_map(&maps[2], dt_hi, 2, dual ? a.a2_hi : a.a_hi, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off, BK, 64))) return rc;
-  if ((rc = row_map(&maps[3], dt_lo, 2, dual ? a.a2_lo : a.a_lo, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off, BK, 64))) return rc;
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)a.K, (cuuint64_t)n_pad};
-    cuuint64_t strides[1] = {(cuuint64_t)a.K * 2};
-    cuuint32_t box[2] = {BK, (cuuint32_t)(BN / 2)};
-    if ((rc = encode_map(&maps[4], dt_hi, a.w_hi, 2, dims, strides, box))) return rc;
-    if ((rc = encode_map(&maps[5], dt_lo, a.w_lo, 2, dims, strides, box))) return rc;
-  }
-  maps[7] = maps[0]; maps[8] = maps[0];
-  if (a.epilogue == OMT_EPI_GEGLU) {
-    maps[6] = maps[0];      // unused by the GEGLU epilogue (direct stores of the U planes)
-  } else if (a.epilogue == OMT_EPI_QKV_PLANES) {
-    maps[6] = maps[0];
-    cuuint64_t dims[2] = {(cuuint64_t)a.N, (cuuint64_t)a.M};
-    cuuint64_t strides[1] = {(cuuint64_t)a.ldu * 2};
-    cuuint32_t box[2] = {64, 32};
-    if ((rc = encode_map(&maps[7], dt_hi, a.u_hi, 2, dims, strides, box))) return rc;
-    if ((rc = encode_map(&maps[8], dt_lo, a.u_lo, 2, dims, strides, box))) return rc;
-  } else {
-    if ((rc = row_map(&maps[6], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, a.c, a.ldc, a.M, a.N, a.c_seg, a.c_seg_stride, a.c_seg_off, 32, 32))) return rc;
-  }
-  HArgs g{};
+  CUtensorMap maps[6];
+  int rc;
+  if ((rc = row_map(&maps[0], f16, 2, a.a_hi, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off))) return rc;
+  if ((rc = row_map(&maps[1], f16, 2, a.a_lo, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off))) return rc;
+  if ((rc = row_map(&maps[2], f16, 2, dual ? a.a2_hi : a.a_hi, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off))) return rc;
+  if ((rc = row_map(&maps[3], f16, 2, dual ? a.a2_lo : a.a_lo, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off))) return rc;
+  if ((rc = w_map(&maps[4], f16, 2, a.w_hi, n_pad, a.K))) return rc;
+  if ((rc = w_map(&maps[5], f16, 2, a.w_lo, n_pad, a.K))) return rc;
+  Args g{};
   g.M = a.M; g.N = a.N; g.K = a.K;
-  g.num_m_blk = (a.M + 2 * BM - 1) / (2 * BM);
-  g.num_n_blk = (a.N + BN - 1) / BN;
+  g.num_m_blk = (a.M + BM - 1) / BM;
   g.n_split = dual ? a.n_split : 0x7fffffff;
   g.a_seg = a.a_seg; g.a_seg_stride = a.a_seg_stride; g.a_seg_off = a.a_seg_off;
   g.a_rs = a.a_rs; g.a2_rs = dual ? a.a2_rs : a.a_rs; g.w_scale = a.w_scale;
   g.a_rs_uniform = a.a_rs_uniform; g.u_scale = a.u_scale;
+  g.c = a.c; g.ldc = a.ldc;
   g.c_seg = a.c_seg; g.c_seg_stride = a.c_seg_stride; g.c_seg_off = a.c_seg_off;
   g.bias = a.bias; g.residual = a.residual; g.ldr = a.ldr;
   g.u_hi = a.u_hi; g.u_lo = a.u_lo; g.ldu = a.ldu;
   g.rope_cos = a.rope_cos; g.rope_sin = a.rope_sin; g.q_scale = a.q_scale; g.k_scale = a.k_scale;
   g.qk_cols = a.qk_cols; g.tokens = a.tokens > 0 ? a.tokens : 1;
   g.q_ps = a.q_plane_scale; g.k_ps = a.k_plane_scale; g.vinv = a.vinv;
-#define OMT_F16_LAUNCH(EPI_) (rs ? launch<256, 1, EPI_>(maps, g, st) : (BN == 256 ? launch<256, 2, EPI_>(maps, g, st) : launch<128, 2, EPI_>(maps, g, st)))
+#define OMT_F16_LAUNCH(EPI_) (rs ? launch<false, 1, EPI_>(maps, g, st) : launch<false, 2, EPI_>(maps, g, st))
   if (a.epilogue == OMT_EPI_QKV) return OMT_F16_LAUNCH(OMT_EPI_QKV);
   if (a.epilogue == OMT_EPI_QKV_PLANES) return OMT_F16_LAUNCH(OMT_EPI_QKV_PLANES);
   if (a.epilogue == OMT_EPI_GEGLU) return OMT_F16_LAUNCH(OMT_EPI_GEGLU);

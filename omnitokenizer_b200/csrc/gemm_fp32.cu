@@ -161,7 +161,7 @@ extern "C" int omt_linear(const float* A, int lda, int a_seg, int a_seg_stride, 
                      M, N, K, bias, residual, ldr, epilogue, math, stream);
 }
 
-namespace omt { int tc_fuses_qkprep(int math); }   // gemm_tc.cu: does the selected tcgen05 kernel apply OMT_EPI_QKV itself?
+namespace omt { int tc_fuses_qkprep(int math); }   // gemm_tc2.cu: does the selected tensor-core kernel apply OMT_EPI_QKV itself?
 
 extern "C" int omt_linear2(const float* A1, const float* A2, int n_split, int lda, const float* W, const float* W_lo,
                            float* C, int ldc, int M, int N, int K, int math, const float* q_scale,
@@ -178,6 +178,6 @@ extern "C" int omt_linear2(const float* A1, const float* A2, int n_split, int ld
   int rc = linear_impl(&qk, A1, A2, n_split, lda, 0, 0, 0, W, W_lo, C, ldc, 0, 0, 0, M, N, K, nullptr, nullptr, 0,
                        fused ? OMT_EPI_QKV : OMT_EPI_NONE, math, stream);
   if (rc != OMT_OK || fused) return rc;
-  // kernels without the fused epilogue (fp32 / v1 tcgen05): same arithmetic as a separate pass over q and k
+  // kernels without the fused epilogue (fp32): same arithmetic as a separate pass over q and k
   return omt_qk_prep(C, ldc, C + qk_cols / 2, ldc, q_scale, k_scale, rope_cos, rope_sin, M, tokens, qk_cols / 2 / 64, stream);
 }

@@ -1,469 +1,50 @@
-// GEMM v2: persistent, 2-CTA (cta_group::2) tcgen05 GEMM with 3xTF32 error compensation.
+// GEMM v2: 3xTF32 error-compensated GEMM on sm_90a wgmma (the kernel lives in gemm_wgmma.cuh, shared with gemm_f16.cu).
 //
-//   C[M,N] = A[M,K] . W[N,K]^T (+bias)(+residual) | GEGLU,   fp32 in / out, fp32-grade accuracy.
+//   C[M,N] = A[M,K] . W[N,K]^T (+bias)(+residual) | GEGLU | rope+l2norm+scale,   fp32 in / out, fp32-grade accuracy.
 //
-// Why 2 CTAs: tf32 operands are 4 bytes, so a 128x128 (or 128x256) single-CTA tile needs more
-// operand bytes in flight per MMA-cycle than shared memory can hold against the TMA latency
-// (measured: 3 stages, tensor pipe 41 % busy).  A CTA pair computes a 256(M) x 256(N) tile with
-// UMMA M=256: each CTA stages only ITS 128 rows of A and ITS 128 rows (half of N) of W_hi/W_lo
-// -> 48 KiB of TMA traffic per 1536 MMA-cycles per SM instead of 80 KiB, and W's L2->SM traffic halves.
-//
-// Per CTA (320 threads):
-//   warp 0     TMA producer: A rows -> local a_full[s];  W_hi/W_lo half -> the LEADER's w_full[s]
-//              (cp.async.bulk.tensor .cta_group::2, peer bit masked)
-//   warp 1     TMEM alloc (both CTAs, cta_group::2); in the leader: single-thread tcgen05.mma issue,
-//              tcgen05.commit multicast -> empty[s] / tmem_full[acc] of BOTH CTAs
-//   warps 2-5  transform: split the A stage into tf32 hi / lo in shared memory, fence.proxy.async,
-//              arrive (remote for the peer) on the leader's ready[s]
-//   warps 6-13 epilogue: tcgen05.ld the 128 x 256 accumulator half, bias / residual / GEGLU, coalesced
-//              stores; arrive on the leader's tmem_empty[acc].  Accumulators are double-buffered in
-//              TMEM (2 x 256 columns) so the epilogue of tile i overlaps the main loop of tile i+1.
-// Tiles are walked m-fastest so the 74 concurrently running clusters share one W tile in L2.
-#include "omt_common.cuh"
-#include "tc_ptx.cuh"
-#include <cuda.h>
+// A arrives as fp32 by TMA and each consumer warpgroup splits its 64 rows into tf32 hi / lo in shared memory; W arrives
+// pre-split (hi = tf32(W), lo = W - hi).  Three tf32 MMAs per k-step (A_lo.W_hi + A_hi.W_lo + A_hi.W_hi) accumulate into
+// one fp32 accumulator in registers.
+#include "gemm_wgmma.cuh"
 
 namespace omt {
-namespace tc2 {
-using namespace omt::ptx;
-
-constexpr int BM = 128;                     // rows per CTA (tile M = 256 per pair)
-constexpr int BN = 256;                     // tile N per pair; each CTA stages BN/2 rows of W
-constexpr int BK = 32;
-constexpr int A_BYTES = BM * BK * 4;        // 16 KiB
-constexpr int W_BYTES = (BN / 2) * BK * 4;  // 16 KiB per CTA
-constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;   // A, A_lo, W_hi, W_lo
-constexpr int STAGES = 3;
-constexpr int EPI_WARPS = 8;                // two warps per TMEM lane quarter, each takes half of the tile's columns
-constexpr int STG_BYTES = EPI_WARPS * 32 * 33 * 4;  // epilogue transpose staging, one slab per warp
-constexpr int SMEM = STAGES * STAGE_BYTES + STG_BYTES + 1024;
-constexpr int THREADS = 192 + EPI_WARPS * 32;   // TMA, MMA, 4 transform warps, 8 epilogue warps
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-__device__ __forceinline__ void mma_tf32_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-
-// Tile raster: clusters walk the tiles in groups of G = num_clusters m-blocks; inside a group all clusters
-// take the same n-block at the same time, so a group's slice of A (G x 256 rows, ~40 MB for K=512) and W stay
-// L2-resident across the n sweep instead of re-streaming A from HBM once per n-block (measured 7.5x re-read).
-__device__ __forceinline__ void decode_tile(int linear, int num_m_blk, int num_n_blk, int G, int& m_blk, int& n_blk) {
-  const int per_group = G * num_n_blk;
-  const int g = linear / per_group;
-  const int m_lo = g * G;
-  const int gm = min(G, num_m_blk - m_lo);          // m-blocks in this (possibly last, smaller) group
-  const int r = linear - g * per_group;
-  n_blk = r / gm;
-  m_blk = m_lo + r % gm;
-}
-
-template <bool QKV>     // QKV: the epilogue applies rope + l2norm + scale to the q / k heads (separate instantiation so the
-                        // common path's code and register allocation are untouched)
-__global__ void __launch_bounds__(THREADS, 1)
-gemm_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-                const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmWlo, const GemmArgs g,
-                const int epilogue, const int num_m_blk, const int num_n_blk, const int n_split) {
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment (SW128 operand tiles) by POINTER OFFSET: an integer round trip would lose the shared address
-  // space and turn every staging / transform access into a generic LD/ST
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t a_full[STAGES];      // local: this CTA's A stage landed
-  __shared__ __align__(8) uint64_t w_full[STAGES];      // used in the leader: both W halves landed
-  __shared__ __align__(8) uint64_t ready[STAGES];       // used in the leader: both CTAs' transforms done
-  __shared__ __align__(8) uint64_t empty[STAGES];       // local: MMAs reading this stage retired (multicast commit)
-  __shared__ __align__(8) uint64_t tmem_full[2];        // local: accumulator complete (multicast commit)
-  __shared__ __align__(8) uint64_t tmem_empty[2];       // used in the leader: both epilogues drained the accumulator
-  __shared__ uint32_t tmem_base_s;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_rank();
-  const bool leader = rank == 0;
-  const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-  const int num_kb = g.K / BK;
-  const int num_tiles = num_m_blk * num_n_blk;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA2)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmW)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmWlo)) : "memory");
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&a_full[s], 1);
-      mbar_init(&w_full[s], 1);
-      mbar_init(&ready[s], 8);        // 4 transform warps x 2 CTAs
-      mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 2 * EPI_WARPS);   // epilogue warps of both CTAs
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();                     // peer barriers are initialised before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
-  pdl_sync();      // prologue above overlapped the previous kernel's tail; no global memory touched before this point
-
-  auto stage_ptr = [&](int s) { return smem + (size_t)s * STAGE_BYTES; };
-
-  if (warp == 0) {
-    // ================= TMA producer =================
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-        int m_blk, n_blk;
-        decode_tile(tile, num_m_blk, num_n_blk, num_clusters, m_blk, n_blk);
-        const int m0 = m_blk * (2 * BM) + (int)rank * BM;
-        const int n0 = n_blk * BN + (int)rank * (BN / 2);
-        const CUtensorMap* mapA = (n0 < n_split) ? &tmA : &tmA2;     // dual-A: columns >= n_split read the second matrix
-        int c1[2], c2[2];
-        for (int hf = 0; hf < 2; ++hf) {
-          const int r = m0 + hf * 64;
-          if (g.a_seg > 0) { c1[hf] = r % g.a_seg; c2[hf] = r / g.a_seg; }
-          else { c1[hf] = r; c2[hf] = 0; }
-        }
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&empty[s], ph ^ 1);
-          uint8_t* sp = stage_ptr(s);
-          mbar_expect_tx(&a_full[s], A_BYTES);
-          tma_load_3d(mapA, &a_full[s], sp, kb * BK, c1[0], c2[0]);
-          tma_load_3d(mapA, &a_full[s], sp + A_BYTES / 2, kb * BK, c1[1], c2[1]);
-          if (leader) mbar_expect_tx(&w_full[s], 4 * W_BYTES);          // hi + lo from both CTAs
-          tma_load_2d_pair(&tmW, &w_full[s], sp + 2 * A_BYTES, kb * BK, n0);
-          tma_load_2d_pair(&tmWlo, &w_full[s], sp + 2 * A_BYTES + W_BYTES, kb * BK, n0);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ================= MMA issuer (leader CTA; the warp stays converged, one elected lane issues) =================
-    if (leader) {
-      uint32_t it = 0, tcount = 0;
-      for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tcount) {
-        const uint32_t acc = tcount & 1, acc_ph = (tcount >> 1) & 1;
-        mbar_wait(&tmem_empty[acc], acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&w_full[s], ph);
-          mbar_wait(&ready[s], ph);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t sa = smem_u32(stage_ptr(s));
-            const uint64_t d_ahi = desc_kmajor(sa), d_alo = desc_kmajor(sa + A_BYTES);
-            const uint64_t d_whi = desc_kmajor(sa + 2 * A_BYTES), d_wlo = desc_kmajor(sa + 2 * A_BYTES + W_BYTES);
-#pragma unroll
-            for (int k = 0; k < BK / 8; ++k) {
-              const uint64_t adv = (uint64_t)(k * 32 >> 4);
-              mma_tf32_pair(d_tmem, d_alo + adv, d_whi + adv, IDESC, (kb | k) != 0);
-              mma_tf32_pair(d_tmem, d_ahi + adv, d_wlo + adv, IDESC, 1);
-              mma_tf32_pair(d_tmem, d_ahi + adv, d_whi + adv, IDESC, 1);
-            }
-            tc_commit_pair(&empty[s]);
-            if (kb == num_kb - 1) tc_commit_pair(&tmem_full[acc]);
-          }
-          __syncwarp();
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp < 6) {
-    // ================= transform: A -> tf32 hi (in place) + lo =================
-    const int t = threadIdx.x - 64;   // 0..127
-    uint32_t it = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters) {
-      for (int kb = 0; kb < num_kb; ++kb, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        mbar_wait(&a_full[s], ph);
-        float4* a = reinterpret_cast<float4*>(stage_ptr(s));
-        float4* alo = reinterpret_cast<float4*>(stage_ptr(s) + A_BYTES);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int idx = t + i * 128;
-          const float4 v = a[idx];
-          float4 hi, lo;
-          hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
-          lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
-          a[idx] = hi;
-          alo[idx] = lo;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive_remote(mapa(smem_u32(&ready[s]), 0));
-      }
-    }
-  } else {
-    // ================= epilogue =================
-    const int q = warp & 3;                            // TMEM lane quarter this warp may read
-    const int hf = (warp - 6) >> 2;                    // which half of the tile's columns
-    float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES) + (warp - 6) * (32 * 33);
-    const int rl0 = lane >> 3, col = (lane & 7) * 4;
-    uint32_t tcount = 0;
-    for (int tile = cluster_id; tile < num_tiles; tile += num_clusters, ++tcount) {
-      const uint32_t acc = tcount & 1, acc_ph = (tcount >> 1) & 1;
-      int m_blk, n_blk;
-      decode_tile(tile, num_m_blk, num_n_blk, num_clusters, m_blk, n_blk);
-      const int m0 = m_blk * (2 * BM) + (int)rank * BM;
-      const int n0 = n_blk * BN;
-      // residual rows are prefetched one 32-column chunk ahead so their latency hides behind the TMEM read
-      float4 res[2][8];
-      auto load_res = [&](int c, float4* dst) {
-#pragma unroll
-        for (int i8 = 0; i8 < 8; ++i8) {
-          const int m = m0 + q * 32 + i8 * 4 + rl0, n = n0 + c * 32 + col;
-          dst[i8] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (g.residual != nullptr && m < g.M && n < g.N)
-            dst[i8] = *reinterpret_cast<const float4*>(g.residual + map_row(m, g.c_seg, g.c_seg_stride, g.c_seg_off) * g.ldr + n);
-        }
-      };
-      // transpose a 32-row x 32-column chunk through the warp's staging slab and store it with 16-byte accesses
-      auto store_chunk = [&](const int c, const uint32_t (&r)[32], const float4 (&rs)[8], const bool use_res) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) stg[lane * 33 + j] = __uint_as_float(r[j]);
-        __syncwarp();
-#pragma unroll
-        for (int i8 = 0; i8 < 8; ++i8) {
-          const int rl = i8 * 4 + rl0;
-          const int m = m0 + q * 32 + rl, n = n0 + c * 32 + col;
-          if (m < g.M && n < g.N) {
-            const float* sp = stg + rl * 33 + col;
-            float4 v = make_float4(sp[0], sp[1], sp[2], sp[3]);
-            if (g.bias != nullptr) {
-              const float4 bb = *reinterpret_cast<const float4*>(g.bias + n);
-              v.x += bb.x; v.y += bb.y; v.z += bb.z; v.w += bb.w;
-            }
-            const long long prow = map_row(m, g.c_seg, g.c_seg_stride, g.c_seg_off);
-            if (epilogue == OMT_EPI_GEGLU) {
-              float2 o;
-              o.x = gelu_erf(v.y) * v.x;
-              o.y = gelu_erf(v.w) * v.z;
-              *reinterpret_cast<float2*>(g.C + prow * g.ldc + (n >> 1)) = o;
-            } else {
-              if (use_res) { v.x += rs[i8].x; v.y += rs[i8].y; v.z += rs[i8].z; v.w += rs[i8].w; }
-              *reinterpret_cast<float4*>(g.C + prow * g.ldc + n) = v;
-            }
-          }
-        }
-        __syncwarp();
-      };
-      if constexpr (QKV) {
-        // ---- q / k heads: rope + l2norm + per-dim scale on the accumulator before it is stored
-        //      (attention.py:417-421, 435-437).  A head = two 32-column chunks; both are transposed through
-        //      the staging slab first so that a row's 64 values sit in 8 lanes x 2 float4 -- table reads and
-        //      stores are then coalesced and the l2 norm is a 3-step shuffle inside each 8-lane group.
-        mbar_wait(&tmem_full[acc], acc_ph);
-        tc_fence_after();
-#pragma unroll
-        for (int pr = 0; pr < 2; ++pr) {
-          const int c = hf * 4 + pr * 2;
-          const int nh = n0 + c * 32;                         // first column of this head
-          if (nh >= g.N) break;
-          float4 va[8], vb[8];
-          {
-            uint32_t r[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN + (uint32_t)(c * 32);
-            tmem_ld32(taddr, r);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) stg[lane * 33 + j] = __uint_as_float(r[j]);
-            __syncwarp();
-#pragma unroll
-            for (int i8 = 0; i8 < 8; ++i8) {
-              const float* sp = stg + (i8 * 4 + rl0) * 33 + col;
-              va[i8] = make_float4(sp[0], sp[1], sp[2], sp[3]);
-            }
-            __syncwarp();
-            tmem_ld32(taddr + 32, r);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) stg[lane * 33 + j] = __uint_as_float(r[j]);
-            __syncwarp();
-#pragma unroll
-            for (int i8 = 0; i8 < 8; ++i8) {
-              const float* sp = stg + (i8 * 4 + rl0) * 33 + col;
-              vb[i8] = make_float4(sp[0], sp[1], sp[2], sp[3]);
-            }
-            __syncwarp();
-          }
-          const bool prep = nh < g.qk_cols;
-          float4 sa = make_float4(1.f, 1.f, 1.f, 1.f), sb = sa;
-          if (prep) {
-            const float* scv = (nh < g.qk_cols / 2) ? g.q_scale : g.k_scale;
-            sa = *reinterpret_cast<const float4*>(scv + col);
-            sb = *reinterpret_cast<const float4*>(scv + 32 + col);
-          }
-#pragma unroll
-          for (int i8 = 0; i8 < 8; ++i8) {
-            const int m = m0 + q * 32 + i8 * 4 + rl0;
-            float4 xa = va[i8], xb = vb[i8];
-            if (prep) {
-              if (g.rope_cos != nullptr) {
-                const int pos = (m < g.M ? m : 0) % g.tokens;
-                const float* ct = g.rope_cos + (size_t)pos * 32 + (col >> 1);
-                const float* st_ = g.rope_sin + (size_t)pos * 32 + (col >> 1);
-                const float2 ca = *reinterpret_cast<const float2*>(ct), sna = *reinterpret_cast<const float2*>(st_);
-                const float2 cb = *reinterpret_cast<const float2*>(ct + 16), snb = *reinterpret_cast<const float2*>(st_ + 16);
-                float4 t;
-                t.x = xa.x * ca.x - xa.y * sna.x; t.y = xa.x * sna.x + xa.y * ca.x;
-                t.z = xa.z * ca.y - xa.w * sna.y; t.w = xa.z * sna.y + xa.w * ca.y;
-                xa = t;
-                t.x = xb.x * cb.x - xb.y * snb.x; t.y = xb.x * snb.x + xb.y * cb.x;
-                t.z = xb.z * cb.y - xb.w * snb.y; t.w = xb.z * snb.y + xb.w * cb.y;
-                xb = t;
-              }
-              float ss = (xa.x * xa.x + xa.y * xa.y) + (xa.z * xa.z + xa.w * xa.w) +
-                         (xb.x * xb.x + xb.y * xb.y) + (xb.z * xb.z + xb.w * xb.w);
-              ss += __shfl_xor_sync(0xffffffffu, ss, 1);
-              ss += __shfl_xor_sync(0xffffffffu, ss, 2);
-              ss += __shfl_xor_sync(0xffffffffu, ss, 4);
-              const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);     // one division per row instead of 64 (<= 1 ulp vs x / den)
-              xa.x = xa.x * inv * sa.x; xa.y = xa.y * inv * sa.y; xa.z = xa.z * inv * sa.z; xa.w = xa.w * inv * sa.w;
-              xb.x = xb.x * inv * sb.x; xb.y = xb.y * inv * sb.y; xb.z = xb.z * inv * sb.z; xb.w = xb.w * inv * sb.w;
-            }
-            if (m < g.M) {
-              float* crow = g.C + map_row(m, g.c_seg, g.c_seg_stride, g.c_seg_off) * g.ldc + nh + col;
-              *reinterpret_cast<float4*>(crow) = xa;
-              if (nh + 32 + col < g.N) *reinterpret_cast<float4*>(crow + 32) = xb;
-            }
-          }
-        }
-      } else {
-        load_res(hf * 4, res[0]);
-        mbar_wait(&tmem_full[acc], acc_ph);
-        tc_fence_after();
-#pragma unroll
-        for (int ci = 0; ci < 4; ++ci) {
-          const int c = hf * 4 + ci;
-          if (n0 + c * 32 < g.N) {
-            if (ci + 1 < 4) load_res(c + 1, res[(ci + 1) & 1]);
-            uint32_t r[32];
-            tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN + (uint32_t)(c * 32), r);
-            store_chunk(c, r, res[ci & 1], g.residual != nullptr);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(mapa(smem_u32(&tmem_empty[acc]), 0));
-    }
-  }
-  // ---- teardown: nobody may leave while the peer can still signal our barriers / read our smem
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-  }
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static int encode_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
-                      const cuuint32_t* box) {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  if (fn == nullptr) { set_error("cuTensorMapEncodeTiled entry point not found"); return OMT_E_CUDA; }
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return OMT_E_CUDA; }
-  return OMT_OK;
-}
-
-}  // namespace tc2
 
 int launch_gemm_tc2(const GemmArgs& g, const float* W_lo, int epilogue, cudaStream_t st, const float* A2, int n_split) {
-  using namespace tc2;
-  OMT_REQUIRE(g.K % BK == 0 && g.lda % 4 == 0, "omt_linear(tcgen05 v2): K=%d must be a multiple of 32", g.K);
+  using namespace wgg;
+  OMT_REQUIRE(g.K % 32 == 0 && g.lda % 4 == 0, "omt_linear(wgmma 3xTF32): K=%d must be a multiple of 32", g.K);
   if (g.a_seg > 0) {
-    OMT_REQUIRE(g.a_seg % 64 == 0 && g.M % g.a_seg == 0, "omt_linear(tcgen05 v2): A row-map segment %d must be a multiple of 64 dividing M=%d", g.a_seg, g.M);
+    OMT_REQUIRE(g.a_seg % 64 == 0 && g.M % g.a_seg == 0, "omt_linear(wgmma 3xTF32): A row-map segment %d must be a multiple of 64 dividing M=%d", g.a_seg, g.M);
   }
+  if (A2 != nullptr) OMT_REQUIRE(n_split > 0 && n_split % 256 == 0, "omt_linear2: n_split=%d must be a multiple of 256", n_split);
   const int n_pad = (g.N + 127) / 128 * 128;
-  CUtensorMap tmA, tmA2, tmW, tmWlo;
-  if (A2 != nullptr) OMT_REQUIRE(n_split > 0 && n_split % BN == 0, "omt_linear2: n_split=%d must be a multiple of 256", n_split);
-  {
-    const int seg = g.a_seg > 0 ? g.a_seg : g.M;
-    const int nseg = g.a_seg > 0 ? g.M / g.a_seg : 1;
-    const long long sstride = g.a_seg > 0 ? g.a_seg_stride : g.M;
-    cuuint64_t dims[3] = {(cuuint64_t)g.K, (cuuint64_t)seg, (cuuint64_t)nseg};
-    cuuint64_t strides[2] = {(cuuint64_t)g.lda * 4, (cuuint64_t)sstride * g.lda * 4};
-    cuuint32_t box[3] = {BK, 64, 1};
-    const float* base = g.A + (size_t)(g.a_seg > 0 ? g.a_seg_off : 0) * g.lda;
-    int rc = encode_map(&tmA, base, 3, dims, strides, box);
-    if (rc) return rc;
-    const float* base2 = (A2 != nullptr ? A2 : g.A) + (size_t)(g.a_seg > 0 ? g.a_seg_off : 0) * g.lda;
-    rc = encode_map(&tmA2, base2, 3, dims, strides, box);
-    if (rc) return rc;
-  }
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)g.K, (cuuint64_t)n_pad};
-    cuuint64_t strides[1] = {(cuuint64_t)g.K * 4};
-    cuuint32_t box[2] = {BK, BN / 2};
-    int rc = encode_map(&tmW, g.W, 2, dims, strides, box);
-    if (rc) return rc;
-    rc = encode_map(&tmWlo, W_lo, 2, dims, strides, box);
-    if (rc) return rc;
-  }
-  static bool attr[64];        // the attribute is per device
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr[dev]) {
-    OMT_CUDA(cudaFuncSetAttribute(gemm_tc2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    OMT_CUDA(cudaFuncSetAttribute(gemm_tc2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attr[dev] = true;
-  }
-  const int num_m_blk = (g.M + 2 * BM - 1) / (2 * BM);
-  const int num_n_blk = (g.N + BN - 1) / BN;
-  const int num_tiles = num_m_blk * num_n_blk;
-  int clusters = omt::sm_count() / 2;
-  if (clusters > num_tiles) clusters = num_tiles;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = SMEM;
-  cfg.stream = st;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = g_pdl ? 2 : 1;
-  const int ns = A2 != nullptr ? n_split : 0x7fffffff;
-  if (epilogue == OMT_EPI_QKV)
-    OMT_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc2_kernel<true>, tmA, tmA2, tmW, tmWlo, g, epilogue, num_m_blk, num_n_blk, ns));
-  else
-    OMT_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc2_kernel<false>, tmA, tmA2, tmW, tmWlo, g, epilogue, num_m_blk, num_n_blk, ns));
-  return OMT_OK;
+  const CUtensorMapDataType f32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUtensorMap maps[6];
+  int rc;
+  if ((rc = row_map(&maps[0], f32, 4, g.A, g.lda, g.M, g.K, g.a_seg, g.a_seg_stride, g.a_seg_off))) return rc;
+  if ((rc = row_map(&maps[2], f32, 4, A2 != nullptr ? A2 : g.A, g.lda, g.M, g.K, g.a_seg, g.a_seg_stride, g.a_seg_off))) return rc;
+  maps[1] = maps[0]; maps[3] = maps[2];       // no lo planes: A is split in shared memory
+  if ((rc = w_map(&maps[4], f32, 4, g.W, n_pad, g.K))) return rc;
+  if ((rc = w_map(&maps[5], f32, 4, W_lo, n_pad, g.K))) return rc;
+  Args a{};
+  a.M = g.M; a.N = g.N; a.K = g.K;
+  a.num_m_blk = (g.M + BM - 1) / BM;
+  a.n_split = A2 != nullptr ? n_split : 0x7fffffff;
+  a.a_seg = g.a_seg; a.a_seg_stride = g.a_seg_stride; a.a_seg_off = g.a_seg_off;
+  a.c = g.C; a.ldc = g.ldc;
+  a.c_seg = g.c_seg; a.c_seg_stride = g.c_seg_stride; a.c_seg_off = g.c_seg_off;
+  a.bias = g.bias; a.residual = g.residual; a.ldr = g.ldr;
+  a.rope_cos = g.rope_cos; a.rope_sin = g.rope_sin; a.q_scale = g.q_scale; a.k_scale = g.k_scale;
+  a.qk_cols = g.qk_cols; a.tokens = g.tokens > 0 ? g.tokens : 1;
+  if (epilogue == OMT_EPI_QKV) return launch<true, 1, OMT_EPI_QKV>(maps, a, st);
+  if (epilogue == OMT_EPI_GEGLU) return launch<true, 1, OMT_EPI_GEGLU>(maps, a, st);
+  return launch<true, 1, OMT_EPI_NONE>(maps, a, st);
 }
 
-// the tcgen05 3xTF32 kernel applies OMT_EPI_QKV (rope + l2norm + scale) in its own epilogue
+// the wgmma 3xTF32 kernel applies OMT_EPI_QKV (rope + l2norm + scale) in its own epilogue
 int tc_fuses_qkprep(int math) { return math == OMT_MATH_3XTF32; }
 
 int launch_gemm_tc(const GemmArgs& g, const float* W_lo, int epilogue, int math, cudaStream_t st, const float* A2, int n_split) {
-  OMT_REQUIRE(math == OMT_MATH_3XTF32 && W_lo != nullptr, "omt_linear: the tcgen05 fp32-operand path is 3xTF32 (needs W_lo)");
+  OMT_REQUIRE(math == OMT_MATH_3XTF32 && W_lo != nullptr, "omt_linear: the tensor-core fp32-operand path is 3xTF32 (needs W_lo)");
   return launch_gemm_tc2(g, W_lo, epilogue, st, A2, n_split);
 }
 

@@ -1,0 +1,368 @@
+// The tensor-core GEMM of both error-compensated paths, on sm_90a wgmma:
+//
+//   C[M,N] = A[M,K] . W[N,K]^T (+bias)(+residual) | GEGLU | rope+l2norm+scale,   fp32-grade accuracy.
+//
+//   TF32 = true  (3xTF32, gemm_tc2.cu): A arrives as fp32 and is split into tf32 hi / lo in shared memory by the warpgroup
+//                that consumes it; W arrives pre-split (hi = tf32(W), lo = W - hi).  A.W ~= A_lo.W_hi + A_hi.W_lo + A_hi.W_hi.
+//   TF32 = false (f16x3, gemm_f16.cu): A and W arrive as fp16 hi / lo planes written by their producers (omt_common.cuh).
+//                NACC = 2: lo planes carry 2^11, the cross products go to a second accumulator folded in as main + cross * 2^-11;
+//                NACC = 1: row-scaled planes, all three products share one accumulator, the epilogue multiplies by the exact
+//                inverse scales (a_rs[row] * w_scale).
+//
+// One CTA = two consumer warpgroups computing a 128 x 128 tile (64 rows each, accumulators in registers).  Every 128-byte
+// k-block of the operands lands by TMA (SWIZZLE_128B, the canonical K-major wgmma layout) in one of STAGES stages; thread 0
+// keeps STAGES k-blocks in flight.  The epilogue works on the accumulator fragments in place: a row's 64-column head is
+// spread over the 4 lanes of a quad, so the l2 norm and the v-plane maximum are two-step shuffles.
+#pragma once
+#include "omt_common.cuh"
+#include "tc_ptx.cuh"
+#include <cuda.h>
+
+namespace omt {
+namespace wgg {
+using namespace omt::ptx;
+
+constexpr int BM = 128, BN = 128;
+constexpr int THREADS = 256;
+constexpr int STAGE_BYTES = 4 * 16384;        // A (hi), A_lo, W_hi, W_lo: 128 rows x 128 bytes each
+constexpr int STAGES = 3;
+constexpr int SMEM = STAGES * STAGE_BYTES + 1024;
+
+struct Args {
+  int M, N, K;
+  int num_m_blk, n_split;
+  int a_seg, a_seg_stride, a_seg_off;         // A row map (the TMA strides live in the tensor maps; the epilogue needs it for a_rs)
+  const float* a_rs; const float* a2_rs;      // NACC == 1: inverse row scales of the A planes (second: dual-A columns >= n_split)
+  float a_rs_uniform;                         // NACC == 1 with a_rs == NULL: one inverse scale for every row
+  float w_scale;                              // NACC == 1: inverse scale of the W planes
+  float u_scale;                              // f16 GEGLU: > 0 -> U planes in the static-scaled form (unscaled lo), else 2^11-scaled lo
+  float* c; int ldc;                          // fp32 output (plain / QKV; 3xTF32 GEGLU: C has N/2 columns)
+  int c_seg, c_seg_stride, c_seg_off;         // C / residual row map
+  const float* bias;
+  const float* residual; int ldr;
+  uint16_t* u_hi; uint16_t* u_lo; int ldu;    // f16 GEGLU: planes of U[M, N/2]; QKV_PLANES: planes of q | k | v [M, N]
+  const float* rope_cos; const float* rope_sin; const float* q_scale; const float* k_scale;
+  int qk_cols; int tokens;
+  float q_ps, k_ps;                           // QKV_PLANES: static plane scales of the q and k heads (powers of two)
+  float* vinv;                                // QKV_PLANES: [v heads][M] inverse per-(row, head) scale of the v planes
+};
+
+template <bool TF32, int NACC, int EPI>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAl,
+                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmA2l,
+                  const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const Args g) {
+  constexpr int BK = TF32 ? 32 : 64;          // elements per 128-byte row
+  constexpr int A_BYTES = BM * 128, W_BYTES = BN * 128;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  __shared__ __align__(8) uint64_t full[STAGES];
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;                   // consumer warpgroup: rows [64 wg, +64) of the tile
+  const int m_blk = blockIdx.x, n_blk = blockIdx.y;
+  const int m0 = m_blk * BM, n0 = n_blk * BN;
+  const int num_kb = g.K / BK;
+  const bool second = n0 >= g.n_split;        // dual-A: columns >= n_split read the second matrix
+
+  if (tid == 0) {
+    prefetch_map(&tmA); prefetch_map(&tmA2); prefetch_map(&tmWh); prefetch_map(&tmWl);
+    if (!TF32) { prefetch_map(&tmAl); prefetch_map(&tmA2l); }
+    for (int s = 0; s < STAGES; ++s) mbar_init(&full[s], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_sync();
+
+  int c1[2], c2[2];                           // TMA coordinates of the two 64-row boxes of A (row map)
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) {
+    const int r = m0 + hf * 64;
+    if (g.a_seg > 0) { c1[hf] = r % g.a_seg; c2[hf] = r / g.a_seg; }
+    else { c1[hf] = r; c2[hf] = 0; }
+  }
+  const CUtensorMap* mah = second ? &tmA2 : &tmA;
+  const CUtensorMap* mal = second ? &tmA2l : &tmAl;
+  auto issue = [&](int kb) {
+    const int s = kb % STAGES;
+    uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
+    mbar_expect_tx(&full[s], TF32 ? A_BYTES + 2 * W_BYTES : 2 * A_BYTES + 2 * W_BYTES);
+    tma_load_3d(mah, &full[s], sp, kb * BK, c1[0], c2[0]);
+    tma_load_3d(mah, &full[s], sp + A_BYTES / 2, kb * BK, c1[1], c2[1]);
+    if (!TF32) {
+      tma_load_3d(mal, &full[s], sp + A_BYTES, kb * BK, c1[0], c2[0]);
+      tma_load_3d(mal, &full[s], sp + A_BYTES + A_BYTES / 2, kb * BK, c1[1], c2[1]);
+    }
+    tma_load_2d(&tmWh, &full[s], sp + 2 * A_BYTES, kb * BK, n0);
+    tma_load_2d(&tmWl, &full[s], sp + 2 * A_BYTES + W_BYTES, kb * BK, n0);
+  };
+  if (tid == 0)
+    for (int kb = 0; kb < STAGES && kb < num_kb; ++kb) issue(kb);
+
+  float acc[BN / 2], crs[NACC == 2 ? BN / 2 : 1];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < (NACC == 2 ? BN / 2 : 1); ++i) crs[i] = 0.f;
+
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % STAGES;
+    uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
+    mbar_wait(&full[s], (kb / STAGES) & 1);
+    if (TF32) {
+      // this warpgroup's 64 rows of A (one 8 KiB box): tf32 hi in place, lo into the A_lo slot
+      float4* a = reinterpret_cast<float4*>(sp + wg * (A_BYTES / 2));
+      float4* alo = reinterpret_cast<float4*>(sp + A_BYTES + wg * (A_BYTES / 2));
+      const int t = tid & 127;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int idx = t + i * 128;
+        const float4 v = a[idx];
+        float4 hi, lo;
+        hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
+        lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
+        a[idx] = hi;
+        alo[idx] = lo;
+      }
+      fence_async_smem();
+      wg_bar(1 + wg);
+    }
+    const uint32_t sa = smem_u32(sp);
+    const uint64_t d_ahi = desc_sw128(sa + wg * (A_BYTES / 2)), d_alo = desc_sw128(sa + A_BYTES + wg * (A_BYTES / 2));
+    const uint64_t d_whi = desc_sw128(sa + 2 * A_BYTES), d_wlo = desc_sw128(sa + 2 * A_BYTES + W_BYTES);
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {               // 32 bytes of the 128-byte row per MMA
+      const uint64_t adv = (uint64_t)(k * 2);
+      if constexpr (TF32) {
+        wgmma_tf32_n128(acc, d_alo + adv, d_whi + adv, 1);
+        wgmma_tf32_n128(acc, d_ahi + adv, d_wlo + adv, 1);
+        wgmma_tf32_n128(acc, d_ahi + adv, d_whi + adv, 1);
+      } else if constexpr (NACC == 2) {
+        wgmma_f16_n128(crs, d_alo + adv, d_whi + adv, 1);
+        wgmma_f16_n128(crs, d_ahi + adv, d_wlo + adv, 1);
+        wgmma_f16_n128(acc, d_ahi + adv, d_whi + adv, 1);
+      } else {
+        wgmma_f16_n128(acc, d_alo + adv, d_whi + adv, 1);
+        wgmma_f16_n128(acc, d_ahi + adv, d_wlo + adv, 1);
+        wgmma_f16_n128(acc, d_ahi + adv, d_whi + adv, 1);
+      }
+    }
+    wg_commit();
+    wg_wait<0>();
+    __syncthreads();                            // both warpgroups are done with stage s
+    if (tid == 0 && kb + STAGES < num_kb) issue(kb + STAGES);
+  }
+
+  // ================= epilogue on the fragments =================
+  const int qd = lane & 3;                      // column pair 8 j + 2 qd inside every 8-column block
+  int mrow[2];
+  mrow[0] = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  mrow[1] = mrow[0] + 8;
+  float v[2][BN / 4];                           // [row (+0 / +8)][2 j + e]: columns 8 j + 2 qd + e of the tile
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float os = 1.f;
+    if (!TF32 && NACC == 1) {
+      const float* rs = second ? g.a2_rs : g.a_rs;
+      const int m = mrow[h];
+      os = g.w_scale * (rs == nullptr ? g.a_rs_uniform : (m < g.M ? __ldg(rs + map_row(m, g.a_seg, g.a_seg_stride, g.a_seg_off)) : 1.0f));
+    }
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int i = 4 * j + 2 * h + e;
+        float x = acc[i];
+        if constexpr (!TF32 && NACC == 2) x = fmaf(crs[i], 1.0f / F16X3_LO_SCALE, x);
+        if (!TF32 && NACC == 1) x = x * os;
+        v[h][2 * j + e] = x;
+      }
+  }
+
+  if constexpr (EPI == OMT_EPI_QKV || EPI == OMT_EPI_QKV_PLANES) {
+#pragma unroll
+    for (int hd = 0; hd < BN / 64; ++hd) {
+      const int nh = n0 + hd * 64;              // first column of this head
+      if (nh >= g.N) break;                     // warp-uniform
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = mrow[h];
+        float* x = &v[h][hd * 16];              // this lane's 16 values of the head: dims 8 j + 2 qd + e, j < 8
+        if (nh < g.qk_cols) {
+          // rope + l2norm + per-dim scale (attention.py:417-421, 435-437)
+          if (g.rope_cos != nullptr) {
+            const int pos = (m < g.M ? m : 0) % g.tokens;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int p = 4 * j + qd;         // complex pair (dims 2p, 2p + 1)
+              const float cc = __ldg(g.rope_cos + (size_t)pos * 32 + p), ss = __ldg(g.rope_sin + (size_t)pos * 32 + p);
+              const float a = x[2 * j], b = x[2 * j + 1];
+              x[2 * j] = a * cc - b * ss;
+              x[2 * j + 1] = a * ss + b * cc;
+            }
+          }
+          float sq = 0.f;
+#pragma unroll
+          for (int i = 0; i < 16; ++i) sq = fmaf(x[i], x[i], sq);
+          sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+          sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+          const float inv = 1.0f / fmaxf(sqrtf(sq), 1e-12f);
+          const float* scv = (nh < g.qk_cols / 2) ? g.q_scale : g.k_scale;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float2 s2 = __ldg(reinterpret_cast<const float2*>(scv + 8 * j + 2 * qd));
+            x[2 * j] = x[2 * j] * inv * s2.x;
+            x[2 * j + 1] = x[2 * j + 1] * inv * s2.y;
+          }
+        }
+        if constexpr (EPI == OMT_EPI_QKV) {
+          if (m < g.M) {
+            float* crow = g.c + map_row(m, g.c_seg, g.c_seg_stride, g.c_seg_off) * g.ldc + nh + 2 * qd;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(crow + 8 * j) = make_float2(x[2 * j], x[2 * j + 1]);
+          }
+        } else {
+          // operand planes for the attention core: q / k with the layer's static power-of-two scale, v scaled per
+          // (row, head) with the inverse scale kept in vinv
+          float sc = nh < g.qk_cols / 2 ? g.q_ps : g.k_ps;
+          if (nh >= g.qk_cols) {
+            float mx = 0.f;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) mx = fmaxf(mx, fabsf(x[i]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            float inv;
+            row_scale(mx, sc, inv);
+            if (m < g.M && qd == 0) g.vinv[(size_t)((nh - g.qk_cols) >> 6) * g.M + m] = inv;
+          }
+          if (m < g.M) {
+            const size_t off = (size_t)m * g.ldu + nh + 2 * qd;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              uint32_t hw, lw;
+              split2u(x[2 * j] * sc, x[2 * j + 1] * sc, hw, lw);
+              *reinterpret_cast<uint32_t*>(g.u_hi + off + 8 * j) = hw;
+              *reinterpret_cast<uint32_t*>(g.u_lo + off + 8 * j) = lw;
+            }
+          }
+        }
+      }
+    }
+  } else if constexpr (EPI == OMT_EPI_GEGLU) {
+    // packed columns (2i, 2i+1) = (value_i, gate_i): U[:, i] = gelu_erf(gate) * value; lanes qd and qd ^ 1 hold neighbouring
+    // outputs, so the even lane stores both
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = mrow[h];
+      const long long prow = map_row(m < g.M ? m : 0, g.c_seg, g.c_seg_stride, g.c_seg_off);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * qd;
+        float val = v[h][2 * j], gate = v[h][2 * j + 1];
+        if (g.bias != nullptr && n < g.N) { val += __ldg(g.bias + n); gate += __ldg(g.bias + n + 1); }
+        const float o = gelu_erf(gate) * val;
+        const float o1 = __shfl_xor_sync(0xffffffffu, o, 1);
+        if ((qd & 1) == 0 && m < g.M && n < g.N) {
+          if (TF32) {
+            *reinterpret_cast<float2*>(g.c + prow * g.ldc + (n >> 1)) = make_float2(o, o1);
+          } else {
+            uint32_t hw, lw;
+            if (g.u_scale > 0.f) split2u(o * g.u_scale, o1 * g.u_scale, hw, lw);
+            else split2(o, o1, hw, lw);
+            const size_t off = (size_t)prow * g.ldu + (n >> 1);
+            *reinterpret_cast<uint32_t*>(g.u_hi + off) = hw;
+            *reinterpret_cast<uint32_t*>(g.u_lo + off) = lw;
+          }
+        }
+      }
+    }
+  } else {
+    // plain: (+bias)(+residual); residual may alias C (each element is read and written by the same thread)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = mrow[h];
+      if (m < g.M) {
+        const long long prow = map_row(m, g.c_seg, g.c_seg_stride, g.c_seg_off);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int n = n0 + 8 * j + 2 * qd;
+          if (n < g.N) {
+            float2 o = make_float2(v[h][2 * j], v[h][2 * j + 1]);
+            if (g.bias != nullptr) {
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(g.bias + n));
+              o.x += bb.x; o.y += bb.y;
+            }
+            if (g.residual != nullptr) {
+              const float2 r = *reinterpret_cast<const float2*>(g.residual + prow * g.ldr + n);
+              o.x += r.x; o.y += r.y;
+            }
+            *reinterpret_cast<float2*>(g.c + prow * g.ldc + n) = o;
+          }
+        }
+      }
+    }
+  }
+}
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static inline int encode_map(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const cuuint64_t* dims,
+                             const cuuint64_t* strides, const cuuint32_t* box) {
+  static EncodeTiledFn fn = nullptr;
+  if (fn == nullptr) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
+        qres == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+  }
+  if (fn == nullptr) { set_error("cuTensorMapEncodeTiled entry point not found"); return OMT_E_CUDA; }
+  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  CUresult r = fn(m, dt, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return OMT_E_CUDA; }
+  return OMT_OK;
+}
+
+// [K, seg, n_seg] map over a row-mapped matrix of 16-bit (esize 2) or fp32 (esize 4) elements, 128-byte x 64-row boxes
+static inline int row_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const void* ptr, int ld, int rows, int cols,
+                          int seg, int seg_stride, int seg_off) {
+  const int s = seg > 0 ? seg : rows;
+  const int nseg = seg > 0 ? rows / seg : 1;
+  const long long sstride = seg > 0 ? seg_stride : rows;
+  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)s, (cuuint64_t)nseg};
+  cuuint64_t strides[2] = {(cuuint64_t)ld * esize, (cuuint64_t)sstride * ld * esize};
+  cuuint32_t box[3] = {(cuuint32_t)(128 / esize), 64, 1};
+  const uint8_t* base = static_cast<const uint8_t*>(ptr) + (size_t)(seg > 0 ? seg_off : 0) * ld * esize;
+  return encode_map(m, dt, base, 3, dims, strides, box);
+}
+
+// W [n_pad, K] (rows padded to a multiple of 128), 128-byte x 128-row boxes
+static inline int w_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const void* ptr, int n_pad, int K) {
+  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)n_pad};
+  cuuint64_t strides[1] = {(cuuint64_t)K * esize};
+  cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)BN};
+  return encode_map(m, dt, ptr, 2, dims, strides, box);
+}
+
+template <bool TF32, int NACC, int EPI>
+static int launch(const CUtensorMap* maps, const Args& g, cudaStream_t st) {
+  auto kern = gemm_wgmma_kernel<TF32, NACC, EPI>;
+  static bool attr[64];        // the attribute is per device
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev >= 0 && dev < 64 && !attr[dev]) {
+    OMT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    attr[dev] = true;
+  }
+  const dim3 grid(g.num_m_blk, (g.N + BN - 1) / BN);     // m fastest: concurrently running CTAs share the W tile in L2
+  OMT_CUDA(launch_k(kern, grid, dim3(THREADS), SMEM, st, maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], g));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+}  // namespace wgg
+}  // namespace omt

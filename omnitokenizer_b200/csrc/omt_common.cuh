@@ -1,4 +1,4 @@
-// Shared helpers for the omnitok_b200 kernels (sm_100a only).
+// Shared helpers for the omnitok_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -9,7 +9,7 @@
 namespace omt {
 
 void set_error(const char* fmt, ...);
-int check_device();   // OMT_OK when the current device is sm_100; caches per device
+int check_device();   // OMT_OK when the current device is sm_90; caches per device
 int sm_count();
 
 #define OMT_REQUIRE(cond, ...)                  \
@@ -42,7 +42,7 @@ int sm_count();
 // Every kernel calls pdl_sync() before its first global-memory access: griddepcontrol.wait blocks until the
 // previous kernel in the stream has completed and flushed (a no-op when the launch carried no PDL attribute);
 // launch_dependents then lets the NEXT kernel's CTAs be scheduled as soon as all of ours are resident, so its
-// prologue (barrier init, TMEM alloc, descriptor prefetch, launch latency) overlaps our last wave.
+// prologue (barrier init, descriptor prefetch, launch latency) overlaps our last wave.
 __device__ __forceinline__ void pdl_sync() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -74,10 +74,9 @@ __device__ __forceinline__ float warp_max(float v) {
 // ---- fp16 hi / lo operand split of the f16x3 tensor-core path -----------------------------------------------------------
 // x ~= hi + lo * 2^-11 with hi = fp16(x) (round to nearest, saturating at +-65504) and lo = fp16((x - hi) * 2^11):
 // 11 + 11 significant bits, representation error <= 2^-23 |x| (tighter than the tf32 hi/lo split), and both halves are
-// 16-bit operands of kind::f16 MMAs (2x the tf32 rate, half the operand bytes).  The 2^11 keeps lo in fp16's normal
+// 16-bit operands of f16 wgmma (2x the tf32 rate, half the operand bytes).  The 2^11 keeps lo in fp16's normal
 // range for every |x| < 65504; the cross products  hi.lo + lo.hi  therefore carry a factor 2^11 and accumulate in their
-// own TMEM accumulator, folded in as  main + cross * 2^-11  by the epilogue.  (A bf16 lo plane would need no scaling and
-// a single accumulator, but a B200 raises "illegal instruction" on a kind::f16 MMA whose A and B formats differ.)
+// own fp32 accumulator, folded in as  main + cross * 2^-11  by the epilogue.
 constexpr float F16X3_LO_SCALE = 2048.0f;
 __device__ __forceinline__ uint32_t pack_f16x2_sat(float a, float b) {   // {low half = a, high half = b}
   uint32_t r;
@@ -115,7 +114,7 @@ __device__ __forceinline__ void store_split2(uint16_t* hi, uint16_t* lo, size_t 
 // multiplied by a power of two that puts its largest magnitude in [2^14, 2^15), hi = fp16(x'), lo = fp16(x' - hi)
 // UNSCALED.  fp16 keeps 11 significant bits down to 2^-14, so every element within 2^16 of the row maximum is carried to
 // 2^-23 relative and smaller ones to 2^-40 of the row maximum.  With the weights pre-scaled the same way per matrix, the
-// three products hi.hi + hi.lo + lo.hi share ONE fp32 accumulator (half the TMEM, half the drain) and the epilogue
+// three products hi.hi + hi.lo + lo.hi share ONE fp32 accumulator (half the accumulator registers) and the epilogue
 // multiplies by the exact inverse scales.  row_scale(): scale and inverse for a row whose largest |value| is mx.
 __device__ __forceinline__ void row_scale(float mx, float& scale, float& inv) {
   uint32_t eb = (__float_as_uint(mx) >> 23) & 0xffu;          // mx in [2^(eb-127), 2^(eb-126))
@@ -135,25 +134,10 @@ __device__ __forceinline__ void store_split4u(uint16_t* hi, uint16_t* lo, size_t
   *reinterpret_cast<uint2*>(hi + off) = h;
   *reinterpret_cast<uint2*>(lo + off) = l;
 }
-// packed fp32 pairs (sm_100 FFMA2 / FMUL2 / FADD2): one issue slot for two lanes of work, each half rounds like the scalar op
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(*reinterpret_cast<uint64_t*>(&d))
-      : "l"(*reinterpret_cast<const uint64_t*>(&a)), "l"(*reinterpret_cast<const uint64_t*>(&b)), "l"(*reinterpret_cast<const uint64_t*>(&c)));
-  return d;
-}
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-  float2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(*reinterpret_cast<uint64_t*>(&d))
-      : "l"(*reinterpret_cast<const uint64_t*>(&a)), "l"(*reinterpret_cast<const uint64_t*>(&b)));
-  return d;
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  float2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(*reinterpret_cast<uint64_t*>(&d))
-      : "l"(*reinterpret_cast<const uint64_t*>(&a)), "l"(*reinterpret_cast<const uint64_t*>(&b)));
-  return d;
-}
+// fp32 pairs: two scalar ops per call (sm_90 has no packed f32x2 arithmetic); each half rounds like the scalar op
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float ex2_fast(float x) {      // MUFU.EX2 alone; results below 2^-126 flush to zero
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

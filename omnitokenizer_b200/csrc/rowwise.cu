@@ -16,7 +16,7 @@ void set_error(const char* fmt, ...) {
 }
 
 int g_peg_kernel = 4;   // omt_set_option("peg_kernel", 3|4): 4 = peg_tile4_kernel (cp.async gather + FFMA2, default), 3 = peg_tile_kernel
-int g_pdl = 0;   // measured on B200: PDL made the step 2-4 % slower (dependent CTAs hold SM resources during the tail), so it is opt-in
+int g_pdl = 0;   // programmatic dependent launch is opt-in (dependent CTAs hold SM resources during the tail)
 static int g_dev_ok[64];   // 0 unknown, 1 ok, -1 bad
 static int g_sms[64];
 
@@ -28,10 +28,10 @@ int check_device() {
     cudaDeviceProp p;
     OMT_CUDA(cudaGetDeviceProperties(&p, dev));
     g_sms[dev] = p.multiProcessorCount;
-    g_dev_ok[dev] = (p.major == 10) ? 1 : -1;
+    g_dev_ok[dev] = (p.major == 9 && p.minor == 0) ? 1 : -1;
   }
   if (g_dev_ok[dev] < 0) {
-    set_error("omnitok_b200 kernels are built for sm_100a only (no fallback path)");
+    set_error("omnitok_b200 kernels are built for sm_90a (H100) only (no fallback path)");
     return OMT_E_ARCH;
   }
   return OMT_OK;
@@ -475,7 +475,7 @@ __global__ void __launch_bounds__(256) peg_tile_kernel(const float* __restrict__
 //     pass; one warp walks one halo row at a time so the only divisions are per row (warp-uniform) and the
 //     temporal  f -> (f % T, f / T)  split is a multiply-shift on the in-row offset;
 //   * the 3x3x3 register window rotates by renaming (w loop unrolled by 3) instead of 36 MOVs per output;
-//   * packed fma.rn.f32x2 (FFMA2): one instruction per channel PAIR and tap.
+//   * channel pairs (float2) per thread: one 8-byte shared-memory load per pair and tap.
 // Requires T <= 64, w <= 254 (multiply-shift range) and 16-byte aligned x; the host falls back to v3 otherwise.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float2 lds_f2(uint32_t addr) {

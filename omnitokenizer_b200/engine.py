@@ -1,4 +1,4 @@
-"""Kernel orchestration for OmniTokenizer_VQGAN.encode / decode / forward on one B200.
+"""Kernel orchestration for OmniTokenizer_VQGAN.encode / decode / forward on one H100.
 
 The engine owns (a) the packed device copies of the checkpoint in kernel layouts and (b) the
 per-shape workspace; every arithmetic step is a call into libomnitok_b200.so (see
@@ -282,14 +282,14 @@ class Engine:
 
     def _linear(self, A, lda, lin: PackedLinear, C, ldc, M, *, a_map=(0, 0, 0), c_map=(0, 0, 0), residual=None,
                 ldr=0, epi=_cabi.EPI_NONE, bias=True):
-        """nn.Linear on the fp32-operand paths (CUDA-core fp32 / tcgen05 3xTF32)."""
+        """nn.Linear on the fp32-operand paths (CUDA-core fp32 / wgmma 3xTF32)."""
         _cabi.call("omt_linear", A, lda, a_map[0], a_map[1], a_map[2], lin.w, lin.w_lo, C, ldc, c_map[0], c_map[1],
                    c_map[2], M, lin.n, lin.k, lin.bias if bias else None, residual, ldr, epi, lin.math)
 
     def _linear_h(self, A: Planes, lin: PackedLinear, M, *, C=None, ldc=0, U: Optional[Planes] = None, A2: Optional[Planes] = None,
                   n_split=0, a_map=(0, 0, 0), c_map=(0, 0, 0), residual=None, ldr=0, epi=_cabi.EPI_NONE, qk=None,
                   planes=None, a_uniform=0.0, u_scale=0.0):
-        """nn.Linear on operand planes (tcgen05 f16x3).  U: GEGLU output planes; qk: (q_scale, k_scale, cos, sin, qk_cols, tokens)."""
+        """nn.Linear on operand planes (wgmma f16x3).  U: GEGLU output planes; qk: (q_scale, k_scale, cos, sin, qk_cols, tokens)."""
         if ((A.rs is not None) or a_uniform > 0.0) != lin.row_scaled:
             raise RuntimeError("operand planes and weight planes are in different f16x3 forms (row-scaled vs 2^11-scaled lo)")
         kw = dict(a_hi=A.hi, a_lo=A.lo, lda=A.ld, a_seg=a_map[0], a_seg_stride=a_map[1], a_seg_off=a_map[2],

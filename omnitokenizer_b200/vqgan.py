@@ -202,7 +202,7 @@ _BACKFILL = dict(twod_window_size=4, defer_temporal_pool=False, defer_spatial_po
 
 
 class OmniTokenizer_VQGAN(nn.Module):
-    """B200-native stand-in for OmniTokenizer.OmniTokenizer_VQGAN (omnitokenizer.py:63)."""
+    """H100-native stand-in for OmniTokenizer.OmniTokenizer_VQGAN (omnitokenizer.py:63)."""
 
     def __init__(self, args):
         super().__init__()

@@ -10,7 +10,6 @@ import omnitokenizer_b200 as ob
 from omnitokenizer_b200 import _cabi
 from omnitokenizer_b200 import layout as L
 from oracle import omni_oracle as oo
-from oracle import ref_loader as rl
 from oracle import weights as W
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -35,24 +34,18 @@ def test_state_dict_layout_matches_reference_checkpoint():
     assert res.unexpected_keys == ["image_discriminator.model0.0.weight"]
 
 
-@pytest.mark.reference
-@pytest.mark.skipif(not rl.available(), reason="/root/reference not present")
 def test_state_dict_and_flags_vs_live_reference():
-    ref, args = rl.make_model(perturb=False)
+    """State-dict layout, parser defaults and latent shape of the reference, as recorded by oracle/make_golden_live.py."""
+    g = torch.load(os.path.join(ROOT, "tests", "golden", "live_reference.pt"), weights_only=False)
     m = ob.OmniTokenizer_VQGAN(ob.canonical_args())
-    rsd = {k: v for k, v in ref.state_dict().items()
-           if not k.startswith(("image_discriminator", "video_discriminator", "perceptual_model"))}
     msd = m.state_dict()
-    assert set(rsd) == set(msd)
-    for k in rsd:
-        assert rsd[k].shape == msd[k].shape and rsd[k].dtype == msd[k].dtype, k
+    assert set(g["state_dict_layout"]) == set(msd)
+    for k, (shape, dtype) in g["state_dict_layout"].items():
+        assert shape == tuple(msd[k].shape) and dtype == str(msd[k].dtype), k
     # every flag of the reference's two parsers exists with the same default
-    ot, base = rl.load()
-    rp = ot.VQGAN.add_model_specific_args(base.VQGAN.add_model_specific_args(argparse.ArgumentParser()))
     mp = ob.OmniTokenizer_VQGAN.add_model_specific_args(ob.OmniTokenizer_VQGAN.add_base_model_args(argparse.ArgumentParser()))
-    rd, md = vars(rp.parse_args([])), vars(mp.parse_args([]))
-    assert rd == md
-    assert m.latent_shape == ref.latent_shape
+    assert g["parser_defaults"] == vars(mp.parse_args([]))
+    assert tuple(m.latent_shape) == g["latent_shape"]
 
 
 def test_module_surface():

@@ -335,7 +335,7 @@ def _static_planes(x, ps):
 @pytest.mark.parametrize("ramp", [False, True])
 @pytest.mark.parametrize("N", [128, 256, 1024])
 def test_attn_spatial_h(cuda, N, ramp, ctas):
-    """tcgen05 kind::f16 attention core on operand planes (Q / P in tensor memory, V as MN-major B) vs fp64 softmax;
+    """wgmma f16 attention core on operand planes (V as MN-major B) vs fp64 softmax;
     q, k unit-norm x scale as the QKV epilogue leaves them, v rows of very different magnitude.  ramp: key norms grow
     along the sequence so that the row maxima keep rising from tile to tile -- the in-place rescale of the O accumulator
     (lazy running maximum) fires several times per row."""
