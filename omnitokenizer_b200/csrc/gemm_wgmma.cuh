@@ -9,10 +9,16 @@
 //                NACC = 1: row-scaled planes, all three products share one accumulator, the epilogue multiplies by the exact
 //                inverse scales (a_rs[row] * w_scale).
 //
-// One CTA = two consumer warpgroups computing a 128 x 128 tile (64 rows each, accumulators in registers).  Every 128-byte
-// k-block of the operands lands by TMA (SWIZZLE_128B, the canonical K-major wgmma layout) in one of STAGES stages; thread 0
-// keeps STAGES k-blocks in flight.  The epilogue works on the accumulator fragments in place: a row's 64-column head is
-// spread over the 4 lanes of a quad, so the l2 norm and the v-plane maximum are two-step shuffles.
+// Warp-specialised and persistent:
+//   * one producer warpgroup (one thread) issues every TMA load; two consumer warpgroups compute a 128 x 128 tile, 64 rows
+//     each, accumulators in registers.  setmaxnreg moves registers from the producer to the consumers.
+//   * every 128-byte k-block of the operands lands by TMA (SWIZZLE_128B, the canonical K-major wgmma layout) in one of
+//     STAGES stages of a full / empty mbarrier ring.  A consumer keeps one wgmma group in flight and releases a stage once
+//     the wgmmas that read it have retired, so the producer refills it while the next k-block computes.
+//   * the grid is as many CTAs as are resident; each walks the tiles (n fastest) with a static stride, and the producer
+//     runs ahead into the next tile while the consumers run the epilogue.
+// The epilogue works on the accumulator fragments in place: a row's 64-column head is spread over the 4 lanes of a quad,
+// so the l2 norm and the v-plane maximum are two-step shuffles.
 #pragma once
 #include "omt_common.cuh"
 #include "tc_ptx.cuh"
@@ -23,10 +29,12 @@ namespace wgg {
 using namespace omt::ptx;
 
 constexpr int BM = 128, BN = 128;
-constexpr int THREADS = 256;
+constexpr int THREADS = 384;                  // warpgroup 0: producer; 1, 2: consumers of rows [64 (wg - 1), +64)
 constexpr int STAGE_BYTES = 4 * 16384;        // A (hi), A_lo, W_hi, W_lo: 128 rows x 128 bytes each
 constexpr int STAGES = 3;
 constexpr int SMEM = STAGES * STAGE_BYTES + 1024;
+// __launch_bounds__(384, 1) caps the kernel at 168 registers a thread: 40 * 128 + 232 * 256 == 168 * 384
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
 struct Args {
   int M, N, K;
@@ -47,114 +55,10 @@ struct Args {
   float* vinv;                                // QKV_PLANES: [v heads][M] inverse per-(row, head) scale of the v planes
 };
 
+// Epilogue of one tile on consumer warpgroup wg's fragments (rows [m0 + 64 wg, +64), columns [n0, +128)).
 template <bool TF32, int NACC, int EPI>
-__global__ void __launch_bounds__(THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAl,
-                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmA2l,
-                  const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const Args g) {
-  constexpr int BK = TF32 ? 32 : 64;          // elements per 128-byte row
-  constexpr int A_BYTES = BM * 128, W_BYTES = BN * 128;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t full[STAGES];
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int wg = warp >> 2;                   // consumer warpgroup: rows [64 wg, +64) of the tile
-  const int m_blk = blockIdx.x, n_blk = blockIdx.y;
-  const int m0 = m_blk * BM, n0 = n_blk * BN;
-  const int num_kb = g.K / BK;
-  const bool second = n0 >= g.n_split;        // dual-A: columns >= n_split read the second matrix
-
-  if (tid == 0) {
-    prefetch_map(&tmA); prefetch_map(&tmA2); prefetch_map(&tmWh); prefetch_map(&tmWl);
-    if (!TF32) { prefetch_map(&tmAl); prefetch_map(&tmA2l); }
-    for (int s = 0; s < STAGES; ++s) mbar_init(&full[s], 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  pdl_sync();
-
-  int c1[2], c2[2];                           // TMA coordinates of the two 64-row boxes of A (row map)
-#pragma unroll
-  for (int hf = 0; hf < 2; ++hf) {
-    const int r = m0 + hf * 64;
-    if (g.a_seg > 0) { c1[hf] = r % g.a_seg; c2[hf] = r / g.a_seg; }
-    else { c1[hf] = r; c2[hf] = 0; }
-  }
-  const CUtensorMap* mah = second ? &tmA2 : &tmA;
-  const CUtensorMap* mal = second ? &tmA2l : &tmAl;
-  auto issue = [&](int kb) {
-    const int s = kb % STAGES;
-    uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
-    mbar_expect_tx(&full[s], TF32 ? A_BYTES + 2 * W_BYTES : 2 * A_BYTES + 2 * W_BYTES);
-    tma_load_3d(mah, &full[s], sp, kb * BK, c1[0], c2[0]);
-    tma_load_3d(mah, &full[s], sp + A_BYTES / 2, kb * BK, c1[1], c2[1]);
-    if (!TF32) {
-      tma_load_3d(mal, &full[s], sp + A_BYTES, kb * BK, c1[0], c2[0]);
-      tma_load_3d(mal, &full[s], sp + A_BYTES + A_BYTES / 2, kb * BK, c1[1], c2[1]);
-    }
-    tma_load_2d(&tmWh, &full[s], sp + 2 * A_BYTES, kb * BK, n0);
-    tma_load_2d(&tmWl, &full[s], sp + 2 * A_BYTES + W_BYTES, kb * BK, n0);
-  };
-  if (tid == 0)
-    for (int kb = 0; kb < STAGES && kb < num_kb; ++kb) issue(kb);
-
-  float acc[BN / 2], crs[NACC == 2 ? BN / 2 : 1];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-#pragma unroll
-  for (int i = 0; i < (NACC == 2 ? BN / 2 : 1); ++i) crs[i] = 0.f;
-
-  for (int kb = 0; kb < num_kb; ++kb) {
-    const int s = kb % STAGES;
-    uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
-    mbar_wait(&full[s], (kb / STAGES) & 1);
-    if (TF32) {
-      // this warpgroup's 64 rows of A (one 8 KiB box): tf32 hi in place, lo into the A_lo slot
-      float4* a = reinterpret_cast<float4*>(sp + wg * (A_BYTES / 2));
-      float4* alo = reinterpret_cast<float4*>(sp + A_BYTES + wg * (A_BYTES / 2));
-      const int t = tid & 127;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int idx = t + i * 128;
-        const float4 v = a[idx];
-        float4 hi, lo;
-        hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
-        lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
-        a[idx] = hi;
-        alo[idx] = lo;
-      }
-      fence_async_smem();
-      wg_bar(1 + wg);
-    }
-    const uint32_t sa = smem_u32(sp);
-    const uint64_t d_ahi = desc_sw128(sa + wg * (A_BYTES / 2)), d_alo = desc_sw128(sa + A_BYTES + wg * (A_BYTES / 2));
-    const uint64_t d_whi = desc_sw128(sa + 2 * A_BYTES), d_wlo = desc_sw128(sa + 2 * A_BYTES + W_BYTES);
-    wg_fence();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {               // 32 bytes of the 128-byte row per MMA
-      const uint64_t adv = (uint64_t)(k * 2);
-      if constexpr (TF32) {
-        wgmma_tf32_n128(acc, d_alo + adv, d_whi + adv, 1);
-        wgmma_tf32_n128(acc, d_ahi + adv, d_wlo + adv, 1);
-        wgmma_tf32_n128(acc, d_ahi + adv, d_whi + adv, 1);
-      } else if constexpr (NACC == 2) {
-        wgmma_f16_n128(crs, d_alo + adv, d_whi + adv, 1);
-        wgmma_f16_n128(crs, d_ahi + adv, d_wlo + adv, 1);
-        wgmma_f16_n128(acc, d_ahi + adv, d_whi + adv, 1);
-      } else {
-        wgmma_f16_n128(acc, d_alo + adv, d_whi + adv, 1);
-        wgmma_f16_n128(acc, d_ahi + adv, d_wlo + adv, 1);
-        wgmma_f16_n128(acc, d_ahi + adv, d_whi + adv, 1);
-      }
-    }
-    wg_commit();
-    wg_wait<0>();
-    __syncthreads();                            // both warpgroups are done with stage s
-    if (tid == 0 && kb + STAGES < num_kb) issue(kb + STAGES);
-  }
-
-  // ================= epilogue on the fragments =================
+__device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 2], const float (&crs)[NACC == 2 ? BN / 2 : 1],
+                                         int m0, int n0, bool second, int wg, int warp, int lane) {
   const int qd = lane & 3;                      // column pair 8 j + 2 qd inside every 8-column block
   int mrow[2];
   mrow[0] = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -305,6 +209,146 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   }
 }
 
+template <bool TF32, int NACC, int EPI>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAl,
+                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmA2l,
+                  const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const Args g) {
+  constexpr int BK = TF32 ? 32 : 64;          // elements per 128-byte row
+  constexpr int A_BYTES = BM * 128, W_BYTES = BN * 128;
+  constexpr uint32_t TX_BYTES = TF32 ? A_BYTES + 2 * W_BYTES : 2 * A_BYTES + 2 * W_BYTES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  __shared__ __align__(8) uint64_t full[STAGES], empty[STAGES];
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int num_kb = g.K / BK;
+  const int num_n_blk = (g.N + BN - 1) / BN;
+  const int num_tiles = g.num_m_blk * num_n_blk;
+
+  if (tid == 0) {
+    prefetch_map(&tmA); prefetch_map(&tmA2); prefetch_map(&tmWh); prefetch_map(&tmWl);
+    if (!TF32) { prefetch_map(&tmAl); prefetch_map(&tmA2l); }
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full[s], 1);                   // the producer's expect_tx
+      mbar_init(&empty[s], 2);                  // both consumer warpgroups
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_sync();
+
+  // Producer and consumers walk the same (tile, k-block) sequence; the running k-block count `it` alone gives the stage
+  // (it % STAGES) and the phase parity ((it / STAGES) & 1) of its full barrier.  The producer waits on the phase before
+  // it: a fresh empty barrier counts as released.
+  // n fastest: W (at most a few MB of planes) stays in L2 while the CTAs running at the same time share the rows of A,
+  // so A is read from HBM about once.  (m fastest re-reads all of A per n block once A outgrows L2.)
+  auto tile_origin = [&](int t, int& m0, int& n0) { m0 = (t / num_n_blk) * BM; n0 = (t % num_n_blk) * BN; };
+
+  if (warp < 4) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (tid == 0) {
+      uint32_t it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int m0, n0;
+        tile_origin(tile, m0, n0);
+        const bool second = n0 >= g.n_split;    // dual-A: columns >= n_split read the second matrix
+        int c1[2], c2[2];                       // TMA coordinates of the two 64-row boxes of A (row map)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          const int r = m0 + hf * 64;
+          if (g.a_seg > 0) { c1[hf] = r % g.a_seg; c2[hf] = r / g.a_seg; }
+          else { c1[hf] = r; c2[hf] = 0; }
+        }
+        const CUtensorMap* mah = second ? &tmA2 : &tmA;
+        const CUtensorMap* mal = second ? &tmA2l : &tmAl;
+        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+          const int s = it % STAGES;
+          uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
+          mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+          mbar_expect_tx(&full[s], TX_BYTES);
+          tma_load_3d(mah, &full[s], sp, kb * BK, c1[0], c2[0]);
+          tma_load_3d(mah, &full[s], sp + A_BYTES / 2, kb * BK, c1[1], c2[1]);
+          if (!TF32) {
+            tma_load_3d(mal, &full[s], sp + A_BYTES, kb * BK, c1[0], c2[0]);
+            tma_load_3d(mal, &full[s], sp + A_BYTES + A_BYTES / 2, kb * BK, c1[1], c2[1]);
+          }
+          tma_load_2d(&tmWh, &full[s], sp + 2 * A_BYTES, kb * BK, n0);
+          tma_load_2d(&tmWl, &full[s], sp + 2 * A_BYTES + W_BYTES, kb * BK, n0);
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int wg = (warp >> 2) - 1;             // consumer warpgroup: rows [64 wg, +64) of the tile
+    auto release = [&](uint32_t i) {            // the wgmmas of k-block i have retired: free its stage
+      if ((tid & 127) == 0) mbar_arrive(&empty[i % STAGES]);
+    };
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int m0, n0;
+      tile_origin(tile, m0, n0);
+      const bool second = n0 >= g.n_split;
+      float acc[BN / 2], crs[NACC == 2 ? BN / 2 : 1];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+      for (int i = 0; i < (NACC == 2 ? BN / 2 : 1); ++i) crs[i] = 0.f;
+
+      for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        const int s = it % STAGES;
+        uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
+        mbar_wait(&full[s], (it / STAGES) & 1);
+        if (TF32) {
+          // this warpgroup's 64 rows of A (one 8 KiB box): tf32 hi in place, lo into the A_lo slot
+          float4* a = reinterpret_cast<float4*>(sp + wg * (A_BYTES / 2));
+          float4* alo = reinterpret_cast<float4*>(sp + A_BYTES + wg * (A_BYTES / 2));
+          const int t = tid & 127;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int idx = t + i * 128;
+            const float4 v = a[idx];
+            float4 hi, lo;
+            hi.x = tf32_rn(v.x); hi.y = tf32_rn(v.y); hi.z = tf32_rn(v.z); hi.w = tf32_rn(v.w);
+            lo.x = v.x - hi.x; lo.y = v.y - hi.y; lo.z = v.z - hi.z; lo.w = v.w - hi.w;
+            a[idx] = hi;
+            alo[idx] = lo;
+          }
+          fence_async_smem();
+          wg_bar(1 + wg);
+        }
+        const uint32_t sa = smem_u32(sp);
+        const uint64_t d_ahi = desc_sw128(sa + wg * (A_BYTES / 2)), d_alo = desc_sw128(sa + A_BYTES + wg * (A_BYTES / 2));
+        const uint64_t d_whi = desc_sw128(sa + 2 * A_BYTES), d_wlo = desc_sw128(sa + 2 * A_BYTES + W_BYTES);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {             // 32 bytes of the 128-byte row per MMA
+          const uint64_t adv = (uint64_t)(k * 2);
+          if constexpr (TF32) {
+            wgmma_tf32_n128(acc, d_alo + adv, d_whi + adv, 1);
+            wgmma_tf32_n128(acc, d_ahi + adv, d_wlo + adv, 1);
+            wgmma_tf32_n128(acc, d_ahi + adv, d_whi + adv, 1);
+          } else if constexpr (NACC == 2) {
+            wgmma_f16_n128(crs, d_alo + adv, d_whi + adv, 1);
+            wgmma_f16_n128(crs, d_ahi + adv, d_wlo + adv, 1);
+            wgmma_f16_n128(acc, d_ahi + adv, d_whi + adv, 1);
+          } else {
+            wgmma_f16_n128(acc, d_alo + adv, d_whi + adv, 1);
+            wgmma_f16_n128(acc, d_ahi + adv, d_wlo + adv, 1);
+            wgmma_f16_n128(acc, d_ahi + adv, d_whi + adv, 1);
+          }
+        }
+        wg_commit();
+        wg_wait<1>();
+        if (kb > 0) release(it - 1);
+      }
+      wg_wait<0>();
+      release(it - 1);
+      epilogue<TF32, NACC, EPI>(g, acc, crs, m0, n0, second, wg, warp, lane);
+    }
+  }
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -351,14 +395,20 @@ static inline int w_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const
 template <bool TF32, int NACC, int EPI>
 static int launch(const CUtensorMap* maps, const Args& g, cudaStream_t st) {
   auto kern = gemm_wgmma_kernel<TF32, NACC, EPI>;
-  static bool attr[64];        // the attribute is per device
+  static int resident[64];     // CTAs of this kernel resident at once, per device (0: not queried yet)
   int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr[dev]) {
+  OMT_CUDA(cudaGetDevice(&dev));
+  OMT_REQUIRE(dev >= 0 && dev < 64, "wgmma GEMM: device ordinal %d out of range", dev);
+  if (resident[dev] == 0) {
     OMT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attr[dev] = true;
+    int per_sm = 0, sms = 0;
+    OMT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, THREADS, SMEM));
+    OMT_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    OMT_REQUIRE(per_sm > 0, "wgmma GEMM: no CTA fits on an SM of device %d", dev);
+    resident[dev] = per_sm * sms;
   }
-  const dim3 grid(g.num_m_blk, (g.N + BN - 1) / BN);     // m fastest: concurrently running CTAs share the W tile in L2
+  const int tiles = g.num_m_blk * ((g.N + BN - 1) / BN);
+  const dim3 grid(tiles < resident[dev] ? tiles : resident[dev]);
   OMT_CUDA(launch_k(kern, grid, dim3(THREADS), SMEM, st, maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], g));
   OMT_LAUNCH_CHECK();
   return OMT_OK;

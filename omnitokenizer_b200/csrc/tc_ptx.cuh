@@ -1,5 +1,6 @@
 // sm_90a PTX wrappers shared by the wgmma kernels (gemm_tc2.cu, gemm_f16.cu, attention_tc3.cu, attention_f16.cu):
-// mbarriers, TMA tile loads, wgmma (warpgroup MMA from shared-memory descriptors, fp32 accumulators in registers).
+// mbarriers, TMA tile loads, wgmma (warpgroup MMA from shared-memory descriptors, fp32 accumulators in registers),
+// thread-block cluster helpers (vq.cu) and warpgroup register reallocation.
 #pragma once
 #include <cuda.h>
 #include <cstdint>
@@ -36,6 +37,22 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+
+// ---- thread-block clusters -----------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+// shared::cta address of this CTA -> the shared::cluster address of the same offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
+// every thread of every CTA of the cluster (warps converged)
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+
+// ---- warpgroup register reallocation (the kernel needs a register limit: __launch_bounds__ / maxnreg) ---------------
+template <uint32_t R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ---- TMA tile loads (complete_tx on an mbarrier of this CTA) ----------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {

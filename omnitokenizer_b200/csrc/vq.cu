@@ -2,6 +2,7 @@
 // reference's  (sum z^2 - 2 z.E) + sum E^2  association and first-min tie rule -- fused into one cluster
 // kernel (vq_fused_kernel) -- and the decode-side gather + post_vq projection.
 #include "omt_common.cuh"
+#include "tc_ptx.cuh"
 
 namespace omt {
 
@@ -75,15 +76,6 @@ constexpr int VQF_SLICES = 8;                 // cluster size = codebook slices
 constexpr int VQF_THREADS = 128;
 constexpr int VQF_GROUP = 8;                  // codes per minimum group
 
-__device__ __forceinline__ uint32_t vq_cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t vq_mapa(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void vq_cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void vq_cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
-
 // distance of one row (2 z in z2[], sum z^2 in zz) to one code: the exact instruction sequence both passes share
 __device__ __forceinline__ float vq_dist(const float (&z2)[8], float zz, const float4 ea, const float4 eb, float ek) {
   float dot = __fmul_rn(z2[0], ea.x);
@@ -107,11 +99,11 @@ vq_fused_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ 
   float4* wsm = reinterpret_cast<float4*>(vq_smem);                          // PROJECT, phase A only: [8][C/4] weights
   float4* zsm = reinterpret_cast<float4*>(vq_smem + (size_t)per * 36);       // [ROWS][2] float4: the block's z rows
   float2* part = reinterpret_cast<float2*>(zsm);                             // phase C: [8 slices][OWN] (distance, index bits)
-  const uint32_t rank = vq_cluster_rank();
+  const uint32_t rank = ptx::cluster_ctarank();
   const int row0 = (blockIdx.x / VQF_SLICES) * ROWS;
   const int k0 = (int)rank * per;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  vq_cluster_arrive();          // no CTA touches a peer's shared memory before every CTA of the cluster is running
+  ptx::cluster_arrive();          // no CTA touches a peer's shared memory before every CTA of the cluster is running
 
   // ---- A. this CTA's OWN rows of z -> the z table of every CTA of the cluster
   const uint32_t zsm_s = static_cast<uint32_t>(__cvta_generic_to_shared(zsm));
@@ -119,7 +111,7 @@ vq_fused_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ 
     const int C4 = C >> 2;
     for (int i = tid; i < 8 * C4; i += VQF_THREADS) wsm[i] = reinterpret_cast<const float4*>(Wt)[i];
     __syncthreads();
-    vq_cluster_wait();
+    ptx::cluster_wait();
     for (int rr = warp; rr < OWN; rr += VQF_THREADS / 32) {
       const int lrow = (int)rank * OWN + rr, row = row0 + lrow;
       float acc[8];
@@ -153,7 +145,7 @@ vq_fused_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ 
         for (int j = 0; j < 8; ++j) acc[j] = 0.f;
       }
       if (lane < VQF_SLICES) {            // lane r writes the row into CTA r's table
-        const uint32_t dst = vq_mapa(zsm_s + (uint32_t)lrow * 32u, (uint32_t)lane);
+        const uint32_t dst = ptx::mapa(zsm_s + (uint32_t)lrow * 32u, (uint32_t)lane);
         asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "f"(acc[0]), "f"(acc[1]), "f"(acc[2]), "f"(acc[3]) : "memory");
         asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst + 16u), "f"(acc[4]), "f"(acc[5]), "f"(acc[6]), "f"(acc[7]) : "memory");
       }
@@ -164,18 +156,18 @@ vq_fused_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ 
       }
     }
   } else {
-    vq_cluster_wait();
+    ptx::cluster_wait();
     for (int i = tid; i < OWN * 2; i += VQF_THREADS) {              // this CTA's rows, 2 float4 each
       const int lrow = (int)rank * OWN + (i >> 1), row = row0 + lrow;
       const float4 v = row < M ? reinterpret_cast<const float4*>(z_in + (size_t)row * 8)[i & 1] : make_float4(0.f, 0.f, 0.f, 0.f);
       for (uint32_t r = 0; r < VQF_SLICES; ++r) {
-        const uint32_t dst = vq_mapa(zsm_s + (uint32_t)lrow * 32u + (uint32_t)(i & 1) * 16u, r);
+        const uint32_t dst = ptx::mapa(zsm_s + (uint32_t)lrow * 32u + (uint32_t)(i & 1) * 16u, r);
         asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
       }
     }
   }
-  vq_cluster_arrive();          // every CTA holds all z rows after this barrier; this CTA is also done with wsm
-  vq_cluster_wait();
+  ptx::cluster_arrive();          // every CTA holds all z rows after this barrier; this CTA is also done with wsm
+  ptx::cluster_wait();
   for (int i = tid; i < 2 * per; i += VQF_THREADS) esm[i] = reinterpret_cast<const float4*>(E + (size_t)k0 * 8)[i];
   for (int i = tid; i < per; i += VQF_THREADS) e2s[i] = e2[k0 + i];
 
@@ -193,7 +185,7 @@ vq_fused_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ 
     z2[r][0] = 2.f * za.x; z2[r][1] = 2.f * za.y; z2[r][2] = 2.f * za.z; z2[r][3] = 2.f * za.w;
     z2[r][4] = 2.f * zb.x; z2[r][5] = 2.f * zb.y; z2[r][6] = 2.f * zb.z; z2[r][7] = 2.f * zb.w;
   }
-  vq_cluster_arrive();          // this CTA's z table is dead: the peers may overwrite it with partial minima (phase C)
+  ptx::cluster_arrive();          // this CTA's z table is dead: the peers may overwrite it with partial minima (phase C)
   __syncthreads();              // the table slice is staged
   float best[R];
   int bg[R];
@@ -228,17 +220,17 @@ vq_fused_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ 
     }
   }
   // ---- C. partial minima -> the owner CTA of each row (every CTA has left its z table: second cluster barrier)
-  vq_cluster_wait();
+  ptx::cluster_wait();
   const uint32_t part_s = static_cast<uint32_t>(__cvta_generic_to_shared(part));
 #pragma unroll
   for (int r = 0; r < R; ++r) {
     const int lrow = tid + r * VQF_THREADS;
     const uint32_t owner = (uint32_t)(lrow / OWN);
-    const uint32_t dst = vq_mapa(part_s + (uint32_t)((rank * OWN + (lrow % OWN)) * 8), owner);
+    const uint32_t dst = ptx::mapa(part_s + (uint32_t)((rank * OWN + (lrow % OWN)) * 8), owner);
     asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(dst), "f"(best[r]), "f"(__int_as_float(k0 + bi[r])) : "memory");
   }
-  vq_cluster_arrive();
-  vq_cluster_wait();
+  ptx::cluster_arrive();
+  ptx::cluster_wait();
   if (tid < OWN) {
     const int row = row0 + (int)rank * OWN + tid;
     if (row < M) {
