@@ -10,13 +10,22 @@
 //                inverse scales (a_rs[row] * w_scale).
 //
 // Warp-specialised and persistent:
-//   * one producer warpgroup (one thread) issues every TMA load; two consumer warpgroups compute a 128 x 128 tile, 64 rows
-//     each, accumulators in registers.  setmaxnreg moves registers from the producer to the consumers.
+//   * one producer warpgroup (one thread) issues every TMA load; two consumer warpgroups hold the accumulators in
+//     registers.  setmaxnreg moves registers from the producer to the consumers.
 //   * every 128-byte k-block of the operands lands by TMA (SWIZZLE_128B, the canonical K-major wgmma layout) in one of
 //     STAGES stages of a full / empty mbarrier ring.  A consumer keeps one wgmma group in flight and releases a stage once
 //     the wgmmas that read it have retired, so the producer refills it while the next k-block computes.
 //   * the grid is as many CTAs as are resident; each walks the tiles (n fastest) with a static stride, and the producer
 //     runs ahead into the next tile while the consumers run the epilogue.
+// Two consumer schedules, fixed by the template arguments:
+//   * ping-pong (TF32 == false, NACC == 1): each consumer warpgroup owns whole 128 x 128 tiles (128 accumulators a
+//     thread), warpgroup 1 the even tiles of the CTA's walk and warpgroup 2 the odd ones.  An ordering barrier lets a
+//     warpgroup issue a tile's wgmmas only once the other one has issued its last k-block, so one warpgroup's epilogue
+//     runs while the other keeps the tensor pipe busy.
+//   * cooperative (NACC == 2, whose two accumulators would need 256 registers for 128 rows, and TF32, whose warpgroups
+//     split their own 64 rows of A in shared memory): both warpgroups compute every tile, 64 rows each, and run the
+//     epilogue together.
+// Both issue the same products in the same k order for every output element, so they give the same bits.
 // The epilogue works on the accumulator fragments in place: a row's 64-column head is spread over the 4 lanes of a quad,
 // so the l2 norm and the v-plane maximum are two-step shuffles.
 #pragma once
@@ -29,7 +38,8 @@ namespace wgg {
 using namespace omt::ptx;
 
 constexpr int BM = 128, BN = 128;
-constexpr int THREADS = 384;                  // warpgroup 0: producer; 1, 2: consumers of rows [64 (wg - 1), +64)
+constexpr int THREADS = 384;                  // warpgroup 0: producer; 1, 2: consumers
+constexpr int ORDER_BAR = 3;                  // ping-pong: named barriers 3, 4 ("consumer 0 / 1 may issue"); 1, 2 are wg_bar
 constexpr int STAGE_BYTES = 4 * 16384;        // A (hi), A_lo, W_hi, W_lo: 128 rows x 128 bytes each
 constexpr int STAGES = 3;
 constexpr int SMEM = STAGES * STAGE_BYTES + 1024;
@@ -55,13 +65,13 @@ struct Args {
   float* vinv;                                // QKV_PLANES: [v heads][M] inverse per-(row, head) scale of the v planes
 };
 
-// Epilogue of one tile on consumer warpgroup wg's fragments (rows [m0 + 64 wg, +64), columns [n0, +128)).
+// Epilogue of one 64-row half of a tile on a consumer warpgroup's fragments (rows [m0 + 64 half, +64), columns [n0, +128)).
 template <bool TF32, int NACC, int EPI>
 __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 2], const float (&crs)[NACC == 2 ? BN / 2 : 1],
-                                         int m0, int n0, bool second, int wg, int warp, int lane) {
+                                         int m0, int n0, bool second, int half, int warp, int lane) {
   const int qd = lane & 3;                      // column pair 8 j + 2 qd inside every 8-column block
   int mrow[2];
-  mrow[0] = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  mrow[0] = m0 + half * 64 + (warp & 3) * 16 + (lane >> 2);
   mrow[1] = mrow[0] + 8;
   float v[2][BN / 4];                           // [row (+0 / +8)][2 j + e]: columns 8 j + 2 qd + e of the tile
 #pragma unroll
@@ -215,6 +225,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmA2l,
                   const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const Args g) {
   constexpr int BK = TF32 ? 32 : 64;          // elements per 128-byte row
+  constexpr bool PINGPONG = !TF32 && NACC == 1;
+  constexpr int HALVES = PINGPONG ? 2 : 1;    // 64-row halves of a tile one consumer warpgroup computes
   constexpr int A_BYTES = BM * 128, W_BYTES = BN * 128;
   constexpr uint32_t TX_BYTES = TF32 ? A_BYTES + 2 * W_BYTES : 2 * A_BYTES + 2 * W_BYTES;
   extern __shared__ uint8_t smem_raw[];
@@ -231,7 +243,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (!TF32) { prefetch_map(&tmAl); prefetch_map(&tmA2l); }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);                   // the producer's expect_tx
-      mbar_init(&empty[s], 2);                  // both consumer warpgroups
+      mbar_init(&empty[s], PINGPONG ? 1 : 2);   // the warpgroup that owns the tile / both consumer warpgroups
     }
     fence_barrier_init();
   }
@@ -280,20 +292,28 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
   } else {
     setmaxnreg_inc<CONSUMER_REGS>();
-    const int wg = (warp >> 2) - 1;             // consumer warpgroup: rows [64 wg, +64) of the tile
+    // consumer warpgroup: ping-pong, the tiles j = wg, wg + 2, ... of the CTA's walk; cooperative, rows [64 wg, +64) of
+    // every tile
+    const int wg = (warp >> 2) - 1;
     auto release = [&](uint32_t i) {            // the wgmmas of k-block i have retired: free its stage
       if ((tid & 127) == 0) mbar_arrive(&empty[i % STAGES]);
     };
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    // Ping-pong order: before each tile but the CTA's first, a warpgroup waits on its barrier ORDER_BAR + wg; the owner
+    // of the previous tile arrives on it once it has issued that tile's last k-block, and only if a next tile exists, so
+    // every arrival meets exactly one wait.  The chain also keeps the consumers' full-barrier waits in k-block order.
+    uint32_t it = PINGPONG ? wg * num_kb : 0;
+    for (int tile = blockIdx.x + (PINGPONG ? wg : 0) * gridDim.x; tile < num_tiles; tile += (PINGPONG ? 2 : 1) * gridDim.x) {
       int m0, n0;
       tile_origin(tile, m0, n0);
       const bool second = n0 >= g.n_split;
-      float acc[BN / 2], crs[NACC == 2 ? BN / 2 : 1];
+      float acc[HALVES][BN / 2], crs[NACC == 2 ? BN / 2 : 1];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int h = 0; h < HALVES; ++h)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
 #pragma unroll
       for (int i = 0; i < (NACC == 2 ? BN / 2 : 1); ++i) crs[i] = 0.f;
+      if (PINGPONG && tile != (int)blockIdx.x) named_bar_sync(ORDER_BAR + wg, 256);
 
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
         const int s = it % STAGES;
@@ -318,33 +338,42 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           wg_bar(1 + wg);
         }
         const uint32_t sa = smem_u32(sp);
-        const uint64_t d_ahi = desc_sw128(sa + wg * (A_BYTES / 2)), d_alo = desc_sw128(sa + A_BYTES + wg * (A_BYTES / 2));
         const uint64_t d_whi = desc_sw128(sa + 2 * A_BYTES), d_wlo = desc_sw128(sa + 2 * A_BYTES + W_BYTES);
         wg_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {             // 32 bytes of the 128-byte row per MMA
           const uint64_t adv = (uint64_t)(k * 2);
-          if constexpr (TF32) {
-            wgmma_tf32_n128(acc, d_alo + adv, d_whi + adv, 1);
-            wgmma_tf32_n128(acc, d_ahi + adv, d_wlo + adv, 1);
-            wgmma_tf32_n128(acc, d_ahi + adv, d_whi + adv, 1);
-          } else if constexpr (NACC == 2) {
-            wgmma_f16_n128(crs, d_alo + adv, d_whi + adv, 1);
-            wgmma_f16_n128(crs, d_ahi + adv, d_wlo + adv, 1);
-            wgmma_f16_n128(acc, d_ahi + adv, d_whi + adv, 1);
-          } else {
-            wgmma_f16_n128(acc, d_alo + adv, d_whi + adv, 1);
-            wgmma_f16_n128(acc, d_ahi + adv, d_wlo + adv, 1);
-            wgmma_f16_n128(acc, d_ahi + adv, d_whi + adv, 1);
+#pragma unroll
+          for (int h = 0; h < HALVES; ++h) {      // rows [64 r, +64) of the tile
+            const int r = PINGPONG ? h : wg;
+            const uint64_t d_ahi = desc_sw128(sa + r * (A_BYTES / 2)), d_alo = desc_sw128(sa + A_BYTES + r * (A_BYTES / 2));
+            if constexpr (TF32) {
+              wgmma_tf32_n128(acc[h], d_alo + adv, d_whi + adv, 1);
+              wgmma_tf32_n128(acc[h], d_ahi + adv, d_wlo + adv, 1);
+              wgmma_tf32_n128(acc[h], d_ahi + adv, d_whi + adv, 1);
+            } else if constexpr (NACC == 2) {
+              wgmma_f16_n128(crs, d_alo + adv, d_whi + adv, 1);
+              wgmma_f16_n128(crs, d_ahi + adv, d_wlo + adv, 1);
+              wgmma_f16_n128(acc[h], d_ahi + adv, d_whi + adv, 1);
+            } else {
+              wgmma_f16_n128(acc[h], d_alo + adv, d_whi + adv, 1);
+              wgmma_f16_n128(acc[h], d_ahi + adv, d_wlo + adv, 1);
+              wgmma_f16_n128(acc[h], d_ahi + adv, d_whi + adv, 1);
+            }
           }
         }
         wg_commit();
         wg_wait<1>();
         if (kb > 0) release(it - 1);
       }
+      // every wgmma of the tile is issued: the other warpgroup may start the next tile while this one drains
+      if (PINGPONG && tile + (int)gridDim.x < num_tiles) named_bar_arrive(ORDER_BAR + (wg ^ 1), 256);
       wg_wait<0>();
       release(it - 1);
-      epilogue<TF32, NACC, EPI>(g, acc, crs, m0, n0, second, wg, warp, lane);
+      if (PINGPONG) it += num_kb;               // the k-blocks of the other warpgroup's tile
+#pragma unroll
+      for (int h = 0; h < HALVES; ++h)
+        epilogue<TF32, NACC, EPI>(g, acc[h], crs, m0, n0, second, PINGPONG ? h : wg, warp, lane);
     }
   }
 }

@@ -72,6 +72,9 @@ __device__ __forceinline__ void prefetch_map(const CUtensorMap* map) {
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // named barrier of one warpgroup (ids 1..)
 __device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// named barrier over `n` threads (a multiple of 32): wait for it, or only count this warp's arrival
+__device__ __forceinline__ void named_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // Round-to-nearest (ties away) on the 13 dropped mantissa bits == cvt.rna.tf32.f32 for finite x, but 2 integer ops
 // instead of the ~7-instruction sequence ptxas emits for the cvt.

@@ -1,16 +1,34 @@
-"""CUDA-event timing of the model's GEMM shapes (L2 flushed between launches) for the tensor-core math modes:
-   python scripts/bench_gemm_shapes.py [M ...]      -> one line per (math, shape): us, algorithmic TFLOP/s, fraction of tf32 peak"""
-import json, os, sys
+"""CUDA-event timing of the model's GEMM shapes (L2 flushed between launches, median of 7 launches):
+   python scripts/bench_gemm_shapes.py [M ...]      -> one line per (form, shape): us, algorithmic TFLOP/s, fraction of tf32 peak
+   python scripts/bench_gemm_shapes.py --ksweep     -> FF1 + GEGLU and QKV -> planes (row-scaled) at M = 40 960 over
+                                                       K = 512, 1024, 2048, fitted to t(K) = a + b K
+
+Forms: "rs" = the row-scaled single-accumulator f16x3 GEMM (LayerNorm / patch-gather fed), "2^11" = the two-accumulator
+f16x3 GEMM (2^11-scaled lo planes), "3xtf32" = the fp32-operand GEMM.  These are the three gemm_wgmma_kernel forms the
+engine launches.  In the K sweep the intercept a is the per-launch cost that does not grow with K: with a persistent grid
+it is mostly the per-tile work that the mainloop does not hide (the epilogue) plus the pipeline fill."""
+import argparse
+import json
+import os
+import sys
+
+import numpy as np
 import torch
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from omnitokenizer_b200 import _cabi, layout as L
+from omnitokenizer_b200 import _cabi, layout as L  # noqa: E402
+
+ap = argparse.ArgumentParser()
+ap.add_argument("M", type=int, nargs="*", default=[40960, 5120])
+ap.add_argument("--ksweep", action="store_true")
+args = ap.parse_args()
 
 dev = torch.device("cuda:0")
-Ms = [int(a) for a in sys.argv[1:]] or [40960, 5120]
 # tf32 dense = half the dense bf16 rate; without a measured peak, the H100 SXM data sheet's 989 TFLOP/s bf16 (as bench.py)
 pk = (json.load(open("MEASURED_PEAKS.json"))["bf16_tflops"] if os.path.exists("MEASURED_PEAKS.json") else 989.0) / 2
 flush = torch.zeros(64 * 1024 * 1024, device=dev)
 _cabi.load()
+C, INNER, HEADS = 512, 1365, 8
 
 
 def timeit(fn, reps=7):
@@ -24,51 +42,71 @@ def timeit(fn, reps=7):
     return sorted(a.elapsed_time(b) for a, b in evs)[reps // 2] * 1e3
 
 
-SHAPES = [("qkv", 1536, 512, "qkv"), ("out+res", 512, 512, "res"), ("ff1+geglu", 2730, 512, "geglu"), ("ff2+res", 512, 1365, "res")]
-for scheme in [int(v) for v in os.environ.get("F16_BN", "256,128,1").split(",")]:       # 1 = row-scaled single-accumulator form
-  _cabi.set_option("f16_bn", scheme if scheme > 1 else 0)
-  for M in Ms:
-    for name, N, K, kind in SHAPES:
-        g = torch.Generator(device=dev).manual_seed(1)
-        for math in (("3xtf32", "f16x3") if scheme == 256 else ("f16x3",)):
-            mult = 64 if math == "f16x3" else 32
-            if kind == "geglu":
-                inner = 1365; ku = L.round_up(inner, mult); Np = 2 * ku; Kp = K
-                W = L.pack_geglu(torch.rand(2 * inner, K, device=dev, generator=g) * 0.1 - 0.05, inner, ku)
-            else:
-                Kp = L.round_up(K, mult); Np = N
-                W = L.pad_cols(torch.rand(N, K, device=dev, generator=g) * 0.1 - 0.05, Kp)
-            A = torch.rand(M, Kp, device=dev, generator=g) - 0.5
-            R = torch.rand(M, 512, device=dev, generator=g)
-            flops = 2.0 * M * N * K
-            if math == "3xtf32":
-                Wp = L.pad_rows(W, 128); hi = L.tf32_round(Wp); lo = (Wp - hi).contiguous()
-                if kind == "geglu":
-                    U = torch.empty(M, Np // 2, device=dev)
-                    fn = lambda: _cabi.call("omt_linear", A, Kp, 0, 0, 0, hi, lo, U, Np // 2, 0, 0, 0, M, Np, Kp, None, None, 0, _cabi.EPI_GEGLU, _cabi.MATH_3XTF32)
-                elif kind == "qkv":
-                    C = torch.empty(M, Np, device=dev)
-                    fn = lambda: _cabi.call("omt_linear", A, Kp, 0, 0, 0, hi, lo, C, Np, 0, 0, 0, M, Np, Kp, None, None, 0, _cabi.EPI_NONE, _cabi.MATH_3XTF32)
-                else:
-                    fn = lambda: _cabi.call("omt_linear", A, Kp, 0, 0, 0, hi, lo, R, 512, 0, 0, 0, M, Np, Kp, None, R, 512, _cabi.EPI_NONE, _cabi.MATH_3XTF32)
-            else:
-                rsk = {}
-                if scheme == 1:
-                    ah, al, ars = L.split_rows_rs(A); wh, wl, wsc = L.split_f16_rs(L.pad_rows(W, 256)); rsk = dict(a_rs=ars, w_scale=wsc)
-                else:
-                    ah, al = L.split_f16(A); wh, wl = L.split_f16(L.pad_rows(W, 256))
-                if kind == "geglu":
-                    U = torch.empty(2, M, Np // 2, dtype=torch.int16, device=dev)
-                    fn = lambda: _cabi.linear_h(a_hi=ah, a_lo=al, lda=Kp, w_hi=wh, w_lo=wl, u_hi=U[0], u_lo=U[1], ldu=Np // 2, M=M, N=Np, K=Kp, epilogue=_cabi.EPI_GEGLU, **rsk)
-                elif kind == "qkv":
-                    C = torch.empty(M, Np, device=dev)
-                    fn = lambda: _cabi.linear_h(a_hi=ah, a_lo=al, lda=Kp, w_hi=wh, w_lo=wl, c=C, ldc=Np, M=M, N=Np, K=Kp, epilogue=_cabi.EPI_NONE, **rsk)
-                else:
-                    fn = lambda: _cabi.linear_h(a_hi=ah, a_lo=al, lda=Kp, w_hi=wh, w_lo=wl, c=R, ldc=512, M=M, N=Np, K=Kp, residual=R, ldr=512, epilogue=_cabi.EPI_NONE, **rsk)
-            try:
-                us = timeit(fn)
-                tf = flops / us / 1e6
-                print(f"bn{scheme} M={M:6d} {name:10s} {math:7s} {us:8.1f} us  {tf:7.1f} TFLOP/s  {tf / pk:.3f} of tf32 peak", flush=True)
-            except Exception as e:
-                print(f"bn{scheme} M={M} {name} {math} FAILED: {e}", flush=True)
-                raise
+def make(kind, form, M, K, g):
+    """(launch, N, K) of one GEMM of the model: kind in qkv (plain C), qkv-planes, out+res, ff1+geglu, ff2+res."""
+    mult = 32 if form == "3xtf32" else 64
+    if kind == "ff1+geglu":
+        ku = L.round_up(INNER, mult); Np = 2 * ku; Kp = K
+        W = L.pack_geglu(torch.rand(2 * INNER, K, device=dev, generator=g) * 0.1 - 0.05, INNER, ku)
+    else:
+        Np = {"qkv": 3 * C, "qkv-planes": 3 * C, "out+res": C, "ff2+res": C}[kind]; Kp = L.round_up(K, mult)
+        W = L.pad_cols(torch.rand(Np, K, device=dev, generator=g) * 0.1 - 0.05, Kp)
+    A = torch.rand(M, Kp, device=dev, generator=g) - 0.5
+    R = torch.rand(M, C, device=dev, generator=g)
+    if form == "3xtf32":
+        Wp = L.pad_rows(W, 128); hi = L.tf32_round(Wp); lo = (Wp - hi).contiguous()
+        if kind == "ff1+geglu":
+            U = torch.empty(M, Np // 2, device=dev)
+            return lambda: _cabi.call("omt_linear", A, Kp, 0, 0, 0, hi, lo, U, Np // 2, 0, 0, 0, M, Np, Kp, None, None, 0, _cabi.EPI_GEGLU, _cabi.MATH_3XTF32), Np
+        if kind in ("qkv", "qkv-planes"):
+            Cq = torch.empty(M, Np, device=dev)
+            return lambda: _cabi.call("omt_linear", A, Kp, 0, 0, 0, hi, lo, Cq, Np, 0, 0, 0, M, Np, Kp, None, None, 0, _cabi.EPI_NONE, _cabi.MATH_3XTF32), Np
+        return lambda: _cabi.call("omt_linear", A, Kp, 0, 0, 0, hi, lo, R, C, 0, 0, 0, M, Np, Kp, None, R, C, _cabi.EPI_NONE, _cabi.MATH_3XTF32), Np
+    if form == "rs":
+        ah, al, ars = L.split_rows_rs(A); wh, wl, wsc = L.split_f16_rs(L.pad_rows(W, 256)); kw = dict(a_rs=ars, w_scale=wsc)
+    else:
+        ah, al = L.split_f16(A); wh, wl = L.split_f16(L.pad_rows(W, 256)); kw = {}
+    kw.update(a_hi=ah, a_lo=al, lda=Kp, w_hi=wh, w_lo=wl, M=M, N=Np, K=Kp)
+    if kind == "ff1+geglu":
+        U = torch.empty(2, M, Np // 2, dtype=torch.int16, device=dev)
+        return lambda: _cabi.linear_h(u_hi=U[0], u_lo=U[1], ldu=Np // 2, epilogue=_cabi.EPI_GEGLU, **kw), Np
+    if kind == "qkv-planes":
+        # the spatial-attention layer's launch: q from the normalised rows, k / v from the raw rows (dual A), rope +
+        # l2norm + scale on q / k, q | k | v written as operand planes, N = 1024 tokens per frame
+        a2h, a2l, a2rs = (L.split_rows_rs(A.flip(1)) if form == "rs" else L.split_f16(A.flip(1)) + (None,))
+        cos, sin = (t.to(dev).contiguous() for t in L.rope_tables(1024, C // HEADS))
+        qs = torch.rand(C // HEADS, device=dev, generator=g) + 0.5; ks = torch.rand(C // HEADS, device=dev, generator=g) + 0.5
+        U = torch.empty(2, M, Np, dtype=torch.int16, device=dev); vinv = torch.empty(HEADS, M, device=dev)
+        return lambda: _cabi.linear_h(a2_hi=a2h, a2_lo=a2l, a2_rs=a2rs, n_split=C, u_hi=U[0], u_lo=U[1], ldu=Np,
+                                      epilogue=_cabi.EPI_QKV_PLANES, q_scale=qs, k_scale=ks, rope_cos=cos, rope_sin=sin,
+                                      qk_cols=2 * C, tokens=1024, q_plane_scale=2.0 ** 13, k_plane_scale=2.0 ** 13, vinv=vinv,
+                                      **kw), Np
+    if kind == "qkv":
+        Cq = torch.empty(M, Np, device=dev)
+        return lambda: _cabi.linear_h(c=Cq, ldc=Np, epilogue=_cabi.EPI_NONE, **kw), Np
+    return lambda: _cabi.linear_h(c=R, ldc=C, residual=R, ldr=C, epilogue=_cabi.EPI_NONE, **kw), Np
+
+
+def run(kind, form, M, N, K):
+    fn, Np = make(kind, form, M, K, torch.Generator(device=dev).manual_seed(1))
+    us = timeit(fn)
+    tf = 2.0 * M * N * K / us / 1e6
+    print(f"{form:6s} M={M:6d} {kind:10s} N={Np:5d} K={K:5d} {us:8.1f} us  {tf:7.1f} TFLOP/s  {tf / pk:.3f} of tf32 peak", flush=True)
+    return us
+
+
+print(f"device: {torch.cuda.get_device_name(dev)}", flush=True)
+if args.ksweep:
+    Ks = [512, 1024, 2048]
+    for kind, N in (("ff1+geglu", 2 * INNER), ("qkv-planes", 3 * C)):
+        t = [run(kind, "rs", 40960, N, K) for K in Ks]
+        b, a = np.polyfit(Ks, t, 1)
+        print(f"fit {kind}: t(K) = {a:.1f} us + {b * 1e3:.2f} us per 1000 K;  a / t(512) = {a / t[0]:.1%}", flush=True)
+else:
+    SHAPES = [("qkv", 3 * C, C), ("qkv-planes", 3 * C, C), ("out+res", C, C), ("ff1+geglu", 2 * INNER, C), ("ff2+res", C, INNER)]
+    for M in args.M:
+        for kind, N, K in SHAPES:
+            for form in ("rs", "2^11", "3xtf32"):
+                if kind == "qkv-planes" and form == "3xtf32":
+                    continue
+                run(kind, form, M, N, K)
