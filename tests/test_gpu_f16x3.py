@@ -2,8 +2,6 @@
 every producer that writes planes (LayerNorm, patch gather, the three attention cores, the GEGLU epilogue), against
 fp64 torch on the same inputs.  Tolerance: fp32 round-off class (2e-5 on |A.W| ~ 1), the same bar as 3xTF32."""
 
-import os
-
 import pytest
 import torch
 
@@ -11,13 +9,9 @@ from oracle import omni_oracle as oo
 
 pytestmark = pytest.mark.gpu
 
-BNS = [int(v) for v in os.environ.get("OMT_TEST_F16_BN", "256,128").split(",") if v]     # tile widths of the kernel
-
-
-def _cabi(bn=256):
+def _cabi():
     from omnitokenizer_b200 import _cabi
     _cabi.load()
-    _cabi.set_option("f16_bn", bn)
     return _cabi
 
 
@@ -25,7 +19,7 @@ def _rand(shape, seed, scale=1.0):
     return (torch.rand(shape, generator=torch.Generator().manual_seed(seed)) - 0.5) * 2 * scale
 
 
-def _planes(t, dev, bn=None, pad_rows=0):
+def _planes(t, dev, pad_rows=0):
     from omnitokenizer_b200 import layout as L
     if pad_rows:
         t = L.pad_rows(t, pad_rows)
@@ -33,26 +27,28 @@ def _planes(t, dev, bn=None, pad_rows=0):
     return hi.to(dev), lo.to(dev)
 
 
-def _join(hi, lo, bn=None):
+def _join(hi, lo):
     """fp32 value the planes stand for."""
     from omnitokenizer_b200 import layout as L
     return L.join_f16(hi.cpu(), lo.cpu())
 
 
-@pytest.mark.parametrize("bn", BNS)
-@pytest.mark.parametrize("M,N,K", [(64, 512, 512), (320, 192, 512), (1024, 1024, 768), (4160, 2816, 512), (192, 512, 192)])
-def test_linear_h_plain_bias_residual(cuda, M, N, K, bn):
-    cabi = _cabi(bn)
+# the last five: partial last m / n blocks, and 133 to 268 tiles so the persistent CTAs walk two or three tiles each
+@pytest.mark.parametrize("M,N,K", [(64, 512, 512), (320, 192, 512), (1024, 1024, 768), (4160, 2816, 512), (192, 512, 192),
+                                   (127, 96, 64), (200, 544, 192), (2305, 896, 1408), (8449, 512, 128),
+                                   (16896, 192, 256)])
+def test_linear_h_plain_bias_residual(cuda, M, N, K):
+    cabi = _cabi()
     A, Wt, b, R = _rand((M, K), 1), _rand((N, K), 2, 0.05), _rand((N,), 3), _rand((M, N), 4)
     ref = (A.double() @ Wt.double().t() + b.double() + R.double()).float()
-    ah, al = _planes(A, cuda, bn)
-    wh, wl = _planes(Wt, cuda, bn, 256)
+    ah, al = _planes(A, cuda)
+    wh, wl = _planes(Wt, cuda, 256)
     out = torch.full((M, N), float("nan"), device=cuda)
     cabi.linear_h(a_hi=ah, a_lo=al, lda=K, w_hi=wh, w_lo=wl, c=out, ldc=N, M=M, N=N, K=K, bias=b.to(cuda),
                   residual=R.to(cuda), ldr=N, epilogue=cabi.EPI_NONE)
     torch.cuda.synchronize()
     err = (out.cpu() - ref).abs().max().item()
-    assert err < 2e-5, f"f16x3 bn {bn} M{M} N{N} K{K}: max err {err:.3e}"
+    assert err < 2e-5, f"f16x3 M{M} N{N} K{K}: max err {err:.3e}"
     # in-place residual (C aliases the residual, as every out-projection / FF2 call does)
     X = R.to(cuda).clone()
     cabi.linear_h(a_hi=ah, a_lo=al, lda=K, w_hi=wh, w_lo=wl, c=X, ldc=N, M=M, N=N, K=K, bias=b.to(cuda), residual=X,
@@ -60,36 +56,42 @@ def test_linear_h_plain_bias_residual(cuda, M, N, K, bn):
     assert torch.equal(X, out)
 
 
-@pytest.mark.parametrize("bn", BNS)
-def test_linear_h_geglu_and_rowmaps(cuda, bn):
-    cabi = _cabi(bn)
+@pytest.mark.parametrize("part", ["geglu_ff2", "rowmaps"])
+def test_linear_h_geglu_and_rowmaps(cuda, part):
+    cabi = _cabi()
     from omnitokenizer_b200 import layout as L
+    if part == "rowmaps":
+        _rowmaps(cabi, cuda)
+        return
     M, K, inner = 320, 512, 1365
     ku = L.round_up(inner, 64)
     A, W1 = _rand((M, K), 5), _rand((2 * inner, K), 6, 0.05)
     y = A.double() @ W1.double().t()
     ref = (oo.gelu_erf(y[:, inner:]) * y[:, :inner]).float()
-    ah, al = _planes(A, cuda, bn)
-    wh, wl = _planes(L.pack_geglu(W1, inner, ku), cuda, bn, 256)
+    ah, al = _planes(A, cuda)
+    wh, wl = _planes(L.pack_geglu(W1, inner, ku), cuda, 256)
     U = torch.full((2, M, ku), -1, dtype=torch.int16, device=cuda)
     cabi.linear_h(a_hi=ah, a_lo=al, lda=K, w_hi=wh, w_lo=wl, u_hi=U[0], u_lo=U[1], ldu=ku, M=M, N=2 * ku, K=K,
                   epilogue=cabi.EPI_GEGLU)
     torch.cuda.synchronize()
-    got = _join(U[0], U[1], bn)
+    got = _join(U[0], U[1])
     assert (got[:, :inner] - ref).abs().max().item() < 2e-5
     assert torch.count_nonzero(U[:, :, inner:]).item() == 0          # zero padding columns are exact zeros in both planes
     # second FF GEMM straight from the planes (K = ku, zero-padded)
     W2 = _rand((512, inner), 16, 0.05)
-    w2h, w2l = _planes(L.pad_cols(W2, ku), cuda, bn, 256)
+    w2h, w2l = _planes(L.pad_cols(W2, ku), cuda, 256)
     X = torch.empty(M, 512, device=cuda)
     cabi.linear_h(a_hi=U[0], a_lo=U[1], lda=ku, w_hi=w2h, w_lo=w2l, c=X, ldc=512, M=M, N=512, K=ku, epilogue=cabi.EPI_NONE)
     assert (X.cpu() - (ref.double() @ W2.double().t()).float()).abs().max().item() < 2e-5
-    # row maps: logical rows gather from / scatter into the canonical buffer (first-frame / rest-frames)
+
+
+def _rowmaps(cabi, cuda):
+    """Row maps: logical rows gather from / scatter into the canonical buffer (first-frame / rest-frames)."""
     B, T, N, Kp = 2, 3, 64, 192
     Xc = _rand((B * T * N, 512), 7)
-    xh, xl = _planes(Xc, cuda, bn)
+    xh, xl = _planes(Xc, cuda)
     Wt = _rand((Kp, 512), 8, 0.05)
-    wqh, wql = _planes(Wt, cuda, bn, 256)
+    wqh, wql = _planes(Wt, cuda, 256)
     rows = B * (T - 1) * N
     P = torch.full((rows, Kp), float("nan"), device=cuda)
     cabi.linear_h(a_hi=xh, a_lo=xl, lda=512, a_seg=(T - 1) * N, a_seg_stride=T * N, a_seg_off=N, w_hi=wqh, w_lo=wql,
@@ -98,8 +100,8 @@ def test_linear_h_geglu_and_rowmaps(cuda, bn):
     assert (P.cpu() - (sel.double() @ Wt.double().t()).float()).abs().max().item() < 2e-5
     Xo = torch.zeros(B * T * N, 512, device=cuda)
     Wb = _rand((512, Kp), 9, 0.05)
-    wbh, wbl = _planes(Wb, cuda, bn, 256)
-    ph, pl = _planes(P.cpu(), cuda, bn)
+    wbh, wbl = _planes(Wb, cuda, 256)
+    ph, pl = _planes(P.cpu(), cuda)
     cabi.linear_h(a_hi=ph, a_lo=pl, lda=Kp, w_hi=wbh, w_lo=wbl, c=Xo, ldc=512, c_seg=(T - 1) * N, c_seg_stride=T * N,
                   c_seg_off=N, M=rows, N=512, K=Kp, epilogue=cabi.EPI_NONE)
     want = torch.zeros(B, T, N, 512)
@@ -107,21 +109,22 @@ def test_linear_h_geglu_and_rowmaps(cuda, bn):
     assert (Xo.cpu().view(B, T, N, 512) - want).abs().max().item() < 2e-5
 
 
-@pytest.mark.parametrize("bn", BNS)
-def test_linear_h_dual_a_qkv(cuda, bn):
+@pytest.mark.parametrize("epilogue", ["qkv_rope", "qkv", "plain"])
+def test_linear_h_dual_a_qkv(cuda, epilogue):
     """q from LN(x), k/v from raw x in one launch (attention.py:407-412), rope + l2norm + scale in the epilogue."""
-    cabi = _cabi(bn)
+    cabi = _cabi()
     from omnitokenizer_b200 import layout as L
     M, K, N = 640, 512, 128
     A1, A2, Wt = _rand((M, K), 70), _rand((M, K), 71), _rand((1536, K), 72, 0.05)
     ref = torch.cat([A1.double() @ Wt[:512].double().t(), A2.double() @ Wt[512:].double().t()], dim=1).float()
-    a1h, a1l = _planes(A1, cuda, bn)
-    a2h, a2l = _planes(A2, cuda, bn)
-    wh, wl = _planes(Wt, cuda, bn, 256)
+    a1h, a1l = _planes(A1, cuda)
+    a2h, a2l = _planes(A2, cuda)
+    wh, wl = _planes(Wt, cuda, 256)
     qs, ks = _rand((64,), 73, 0.5) + 1.0, _rand((64,), 74, 0.5) + 1.0
     cos, sin = L.rope_tables(N, 64)
     out = torch.empty(M, 1536, device=cuda)
-    for tables in ((cos, sin), (None, None)):
+    if epilogue != "plain":
+        tables = (cos, sin) if epilogue == "qkv_rope" else (None, None)
         out.fill_(float("nan"))
         cabi.linear_h(a_hi=a1h, a_lo=a1l, a2_hi=a2h, a2_lo=a2l, n_split=512, lda=K, w_hi=wh, w_lo=wl, c=out, ldc=1536,
                       M=M, N=1536, K=K, epilogue=cabi.EPI_QKV, q_scale=qs.to(cuda), k_scale=ks.to(cuda),
@@ -135,30 +138,37 @@ def test_linear_h_dual_a_qkv(cuda, bn):
             want = (oo.l2norm(t) * sc).reshape(M, 512)
             assert (got[:, sl] - want).abs().max().item() < 2e-5
         assert (got[:, 1024:] - ref[:, 1024:]).abs().max().item() < 2e-5
-    # plain dual-A form too (window qkv uses the plain epilogue)
+        return
+    # plain dual-A form (window qkv uses the plain epilogue)
     out.fill_(float("nan"))
     cabi.linear_h(a_hi=a1h, a_lo=a1l, a2_hi=a2h, a2_lo=a2l, n_split=512, lda=K, w_hi=wh, w_lo=wl, c=out, ldc=1536,
                   M=M, N=1536, K=K, epilogue=cabi.EPI_NONE)
     assert (out.cpu() - ref).abs().max().item() < 2e-5
 
 
-@pytest.mark.parametrize("bn", BNS)
+@pytest.mark.parametrize("form", ["two_acc", "row_scaled"])
 @pytest.mark.parametrize("M,N,K", [(20480, 1024, 1408), (5120, 512, 512), (40960, 512, 512)])
-def test_linear_h_multiwave_deterministic(cuda, M, N, K, bn):
-    """Several waves of tiles per cluster (accumulator double-buffering, slab reuse, TMA-store ordering): the same bits
-    run after run, and the first / last rows are right."""
-    cabi = _cabi(bn)
+def test_linear_h_multiwave_deterministic(cuda, M, N, K, form):
+    """Many tiles per persistent CTA (up to 10 on 132 SMs), in the two-accumulator (cooperative) and the row-scaled
+    (ping-pong) forms: the same bits run after run, and the first / last rows are right."""
+    cabi = _cabi()
     from omnitokenizer_b200 import layout as L
     A = (torch.rand((M, K), device=cuda, generator=torch.Generator(device=cuda).manual_seed(31)) - 0.5)
     W = (torch.rand((N, K), device=cuda, generator=torch.Generator(device=cuda).manual_seed(32)) - 0.5) * 0.05
     R = (torch.rand((M, N), device=cuda, generator=torch.Generator(device=cuda).manual_seed(33)) - 0.5)
-    ah, al = L.split_f16(A)
-    wh, wl = L.split_f16(L.pad_rows(W, 256))
+    if form == "row_scaled":
+        ah, al, ars = L.split_rows_rs(A)
+        wh, wl, wsc = L.split_f16_rs(L.pad_rows(W, 256))
+        scales = dict(a_rs=ars, w_scale=wsc)
+    else:
+        ah, al = L.split_f16(A)
+        wh, wl = L.split_f16(L.pad_rows(W, 256))
+        scales = {}
     outs = []
     for _ in range(4):
         out = torch.full((M, N), float("nan"), device=cuda)
         cabi.linear_h(a_hi=ah, a_lo=al, lda=K, w_hi=wh, w_lo=wl, c=out, ldc=N, M=M, N=N, K=K, residual=R, ldr=N,
-                      epilogue=cabi.EPI_NONE)
+                      epilogue=cabi.EPI_NONE, **scales)
         outs.append(out)
     torch.cuda.synchronize()
     for o in outs[1:]:
@@ -170,10 +180,9 @@ def test_linear_h_multiwave_deterministic(cuda, M, N, K, bn):
 
 
 def test_plane_producers(cuda):
-    bn = 256
     """LayerNorm (+ raw-row planes), patch gather and the attention cores write planes that stand for the same fp32 values
     their fp32 forms produce (within the split's 2^-22 relative representation error)."""
-    cabi = _cabi(bn)
+    cabi = _cabi()
     from omnitokenizer_b200 import layout as L
     M = 320
     x = _rand((M, 512), 10, 3.0)
@@ -188,11 +197,11 @@ def test_plane_producers(cuda):
     d = (y - y2).abs()
     assert torch.equal(y, y2), f"fp32 output differs between the two entry points: max {d.max().item():.3e}, {int((d > 0).sum())} elements"
     tol = lambda t: 2.0 ** -21 * t.abs().max().item()
-    assert (_join(yp[0], yp[1], bn) - y.cpu()).abs().max().item() <= tol(y.cpu())
-    assert (_join(xp[0], xp[1], bn) - x).abs().max().item() <= tol(x)
+    assert (_join(yp[0], yp[1]) - y.cpu()).abs().max().item() <= tol(y.cpu())
+    assert (_join(xp[0], xp[1]) - x).abs().max().item() <= tol(x)
     cabi.call("omt_layernorm_h", x.to(cuda), 512, None, 0, yp[0], yp[1], None, None, None, None, 512, g.to(cuda), b.to(cuda),
               M, 512, 1e-5, 0, 0, 0)                             # planes only
-    assert (_join(yp[0], yp[1], bn) - y.cpu()).abs().max().item() <= tol(y.cpu())
+    assert (_join(yp[0], yp[1]) - y.cpu()).abs().max().item() <= tol(y.cpu())
     # row-scaled form: hi + lo (unscaled) times the inverse row scale; the scale puts the row maximum in [2^14, 2^15)
     yrs, xrs = torch.zeros(M, device=cuda), torch.zeros(M, device=cuda)
     cabi.call("omt_layernorm_h", x.to(cuda), 512, None, 0, yp[0], yp[1], yrs, xp[0], xp[1], xrs, 512, g.to(cuda), b.to(cuda),
@@ -215,7 +224,7 @@ def test_plane_producers(cuda):
         Ap = torch.zeros(2, rows, K, dtype=torch.int16, device=cuda)
         cabi.call("omt_patchify_ln", v.to(cuda), None, Ap[0], Ap[1], None, lw.to(cuda), lb.to(cuda), 2, 3, 5, 64, 64, 8, 4,
                   is_first, 1e-5)
-        assert (_join(Ap[0], Ap[1], bn) - A.cpu()).abs().max().item() <= tol(A.cpu())
+        assert (_join(Ap[0], Ap[1]) - A.cpu()).abs().max().item() <= tol(A.cpu())
         ars = torch.zeros(rows, device=cuda)
         cabi.call("omt_patchify_ln", v.to(cuda), None, Ap[0], Ap[1], ars, lw.to(cuda), lb.to(cuda), 2, 3, 5, 64, 64, 8, 4,
                   is_first, 1e-5)
@@ -232,23 +241,23 @@ def test_plane_producers(cuda):
         cabi.set_option("attn_kernel", kern)
         cabi.call("omt_attn_spatial", p, 1536, p + 2048, 1536, p + 4096, 1536, o, None, None, 512, nseq, N, 8, 8.0)
         cabi.call("omt_attn_spatial", p, 1536, p + 2048, 1536, p + 4096, 1536, None, op[0], op[1], 512, nseq, N, 8, 8.0)
-        assert (_join(op[0], op[1], bn) - o.cpu()).abs().max().item() <= tol(o.cpu())
+        assert (_join(op[0], op[1]) - o.cpu()).abs().max().item() <= tol(o.cpu())
     cabi.set_option("attn_kernel", 3)
     bias = _rand((8, 64, 64), 33).to(cuda)
     cabi.call("omt_attn_window", p, 1536, p + 2048, 1536, p + 4096, 1536, o, None, None, 512, bias, nseq, 16, 16, 8, 8, 0.125)
     cabi.call("omt_attn_window", p, 1536, p + 2048, 1536, p + 4096, 1536, None, op[0], op[1], 512, bias, nseq, 16, 16, 8, 8,
               0.125)
-    assert (_join(op[0], op[1], bn) - o.cpu()).abs().max().item() <= tol(o.cpu())
+    assert (_join(op[0], op[1]) - o.cpu()).abs().max().item() <= tol(o.cpu())
     cabi.call("omt_attn_temporal", p, 1536, p + 2048, 1536, p + 4096, 1536, o, None, None, 512, 2, 4, 64, 8, 8.0, 1)
     cabi.call("omt_attn_temporal", p, 1536, p + 2048, 1536, p + 4096, 1536, None, op[0], op[1], 512, 2, 4, 64, 8, 8.0, 1)
-    assert (_join(op[0], op[1], bn) - o.cpu()).abs().max().item() <= tol(o.cpu())
+    assert (_join(op[0], op[1]) - o.cpu()).abs().max().item() <= tol(o.cpu())
 
 
 @pytest.mark.parametrize("M,N,K", [(64, 512, 512), (320, 192, 512), (1024, 1024, 768), (4160, 2816, 512), (192, 512, 192)])
 def test_linear_h_row_scaled(cuda, M, N, K):
     """Single-accumulator form: row-scaled A planes (per-row power-of-two scale, unscaled lo) x per-matrix-scaled W planes,
     rows of very different magnitude in one call (1e-3 .. 1e3)."""
-    cabi = _cabi(0)
+    cabi = _cabi()
     from omnitokenizer_b200 import layout as L
     A, Wt, b, R = _rand((M, K), 1), _rand((N, K), 2, 0.05), _rand((N,), 3), _rand((M, N), 4)
     A = A * torch.logspace(-3, 3, M)[:, None]
@@ -266,7 +275,7 @@ def test_linear_h_row_scaled(cuda, M, N, K):
 
 def test_linear_h_row_scaled_epilogues(cuda):
     """Row-scaled form through the GEGLU and the dual-A QKV epilogues and the A row map (to_pixels reads X through one)."""
-    cabi = _cabi(0)
+    cabi = _cabi()
     from omnitokenizer_b200 import layout as L
     M, K, inner = 320, 512, 1365
     ku = L.round_up(inner, 64)
@@ -339,7 +348,7 @@ def test_attn_spatial_h(cuda, N, ramp, ctas):
     q, k unit-norm x scale as the QKV epilogue leaves them, v rows of very different magnitude.  ramp: key norms grow
     along the sequence so that the row maxima keep rising from tile to tile -- the in-place rescale of the O accumulator
     (lazy running maximum) fires several times per row."""
-    cabi = _cabi(0)
+    cabi = _cabi()
     cabi.set_option("attn_f16_ctas", ctas)           # both shapes of the kernel (conftest restores the default)
     from omnitokenizer_b200 import layout as L
     nseq, H = 3, 8
@@ -372,7 +381,7 @@ def test_attn_spatial_h(cuda, N, ramp, ctas):
 def test_linear_h_qkv_planes(cuda):
     """The QKV GEMM epilogue that feeds the f16 attention core: q / k planes with static power-of-two scales, v planes
     scaled per (row, head) with vinv -- reconstructed values vs the fp32-output epilogue of the same GEMM."""
-    cabi = _cabi(0)
+    cabi = _cabi()
     from omnitokenizer_b200 import layout as L
     M, K, N = 640, 512, 128
     A1, A2, Wt = _rand((M, K), 70, 0.3), _rand((M, K), 71, 5.0), _rand((1536, K), 72, 0.05)

@@ -31,8 +31,7 @@ def _pad128(w):
 def test_linear_plain_bias_residual(cuda, M, N, K, math):
     cabi = _cabi()
     from omnitokenizer_b200 import layout as L
-    if math != "fp32" and (K % 32 or M % 64):
-        pytest.skip("the tensor-core path needs K % 32 == 0 and 64-row granularity")
+    # any M: the tensor-core path reads rows past M as zeros (TMA bounds) and stores only rows below M
     A, Wt, b, R = _rand((M, K), 1), _rand((N, K), 2, 0.05), _rand((N,), 3), _rand((M, N), 4)
     ref = (A.double() @ Wt.double().t() + b.double() + R.double()).float()
     Ad, bd, Rd = A.to(cuda), b.to(cuda), R.to(cuda)
