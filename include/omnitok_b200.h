@@ -97,6 +97,22 @@ int omt_patchify_ln(const float* video, float* A, uint16_t* A_hi, uint16_t* A_lo
                     int B, int Cin, int T, int H, int W, int p, int pt, int first, float eps,
                     omt_stream_t stream);
 
+/* omt_patchify_ln on uint8 frames: the data pipelines' byte -> fp32 normalisation fused into the gather.
+ * frames (B, T, H, W, Cin) uint8 contiguous, channels last (decord / PIL / decode_u8 layout), 4-byte aligned; Cin <= 4.
+ * lut: fp32 [n_tab][Cin][256], the value byte u of channel c stands for, built on the host with the pipeline's own CPU
+ * expression (e.g. (u / 255 - mean_c) / std_c), so the kernel never divides and its values are the pipeline's bits.
+ * sel: NULL (n_tab = 1, every sample uses table 0) or int32 [B] table index per sample, 0 or 1 (n_tab = 2; see
+ * omt_u8_norm_select).  Outputs, forms and the ln_w == NULL im2col form as omt_patchify_ln; the result equals
+ * omt_patchify_ln on the fp32 video the table maps the frames to, bit for bit. */
+int omt_patchify_ln_u8(const uint8_t* frames, const float* lut, const int32_t* sel, float* A, uint16_t* A_hi, uint16_t* A_lo,
+                       float* A_rs, const float* ln_w, const float* ln_b, int B, int Cin, int T, int H, int W, int p, int pt,
+                       int first, float eps, omt_stream_t stream);
+
+/* VideoNorm's test (OmniTokenizer/video_utils.py:33-58: `if max(clip) > 1: div_(255)`) on the device, per sample:
+ * sel[b] = (max byte of the per_sample bytes of sample b > 1) ? 0 : 1.  Writes every sel[b] (no prior reset needed,
+ * no host sync): two launches, safe inside a captured CUDA graph. */
+int omt_u8_norm_select(const uint8_t* frames, int B, long long per_sample, int32_t* sel, omt_stream_t stream);
+
 /* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W). */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,
                    int first, omt_stream_t stream);

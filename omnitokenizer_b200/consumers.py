@@ -14,10 +14,18 @@ from typing import Optional, Tuple
 
 import torch
 
+from .layout import U8Norm, u8_normalize
+
 LATENT_SCALE = 0.18215            # Diffusion/DiT/train.py:242, Diffusion/Latte/train.py:216
 
 EVAL_U8 = (1.0, 0.5, 0.0, 1.0, 255.0)        # (clamp(x + 0.5, 0, 1) * 255).byte()     vqgan_eval.py:139,147-148; Latte sample_ddp.py:206
 DIT_U8 = (255.0, 128.0, 0.0, 255.0, 1.0)     # clamp(255 * x + 128.0, 0, 255).to(uint8)  DiT sample_ddp.py:163
+
+# The data pipelines' uint8 -> fp32 normalisations (input side of encode_u8 / forward_u8): (u / 255 - mean) / std in fp32.
+VIDEO_NORM = U8Norm("video_norm", (0.5, 0.5, 0.5), (1.0, 1.0, 1.0), max_test=True)   # VideoNorm, video_utils.py:33-58 (data.py:165,229-232)
+IMAGE_NORM = U8Norm("image_norm", (0.5, 0.5, 0.5), (1.0, 1.0, 1.0))   # ToTensor + Normalize((.5,.5,.5), (1,1,1)), data.py:88-97
+DIT_NORM = U8Norm("dit_norm", (0.5, 0.5, 0.5), (0.5, 0.5, 0.5))       # ToTensor + Normalize(.5, .5), DiT train.py:185-198
+LATTE_NORM = U8Norm("latte_norm", (0.5, 0.5, 0.5), (0.5, 0.5, 0.5))   # ToTensorVideo + Normalize(.5, .5), Latte datasets/*
 
 
 def _to_u8(video: torch.Tensor, affine) -> torch.Tensor:
@@ -61,6 +69,10 @@ def encode_to_z(vqgan, x: torch.Tensor, is_image: bool, sample_every_n_latent_fr
     """Net2NetTransformer.encode_to_z (lm_transformer.py:258-268): the GPT's view of a clip.
     Returns (embeddings channels-last (B, T'', h, w, C), targets int64 (B, T''*h*w)) where T'' keeps every n-th latent frame."""
     emb, targets = vqgan.encode(x, is_image, include_embeddings=True)
+    return _z_wire_format(emb, targets, sample_every_n_latent_frames)
+
+
+def _z_wire_format(emb, targets, sample_every_n_latent_frames):
     if sample_every_n_latent_frames > 0:
         emb = emb[:, :, ::sample_every_n_latent_frames]
         targets = targets[:, ::sample_every_n_latent_frames]
@@ -120,3 +132,63 @@ def latte_decode_latents(vae, samples_bfchw: torch.Tensor, as_uint8: bool = True
     if not as_uint8:
         return video.permute(0, 2, 1, 3, 4).contiguous()
     return _to_u8(video, EVAL_U8)
+
+
+# ----------------------------------------------------------------------------------------------- uint8 input side
+# The same callers fed the uint8 frames their loaders decode (decord / PIL), before the loader's own normalisation.  With
+# this package's module the normalisation runs in the patch-gather kernel (encode_u8 / forward_u8: the host->device copy
+# shrinks 4x and the host does no float work); any other object gets the pipeline's fp32 input, computed on the host.
+def _check_u8(frames: torch.Tensor, ndims: Tuple[int, ...], what: str):
+    if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+        raise TypeError(f"{what}: expected uint8 frames, got {getattr(frames, 'dtype', type(frames))}")
+    if frames.ndim not in ndims:
+        raise ValueError(f"{what}: expected channels-last frames of {' or '.join(map(str, ndims))} dimensions, "
+                         f"got shape {tuple(frames.shape)}")
+
+
+def _encode_u8(vqgan, frames: torch.Tensor, is_image: bool, norm: U8Norm, include_embeddings: bool = False):
+    _check_u8(frames, (4,) if is_image else (5,), "encode_u8")
+    if hasattr(vqgan, "encode_u8"):
+        return vqgan.encode_u8(frames, is_image, include_embeddings=include_embeddings, norm=norm)
+    x = u8_normalize(frames.unsqueeze(1) if is_image else frames, norm)
+    return vqgan.encode(x.squeeze(2) if is_image else x, is_image, include_embeddings=include_embeddings)
+
+
+@torch.no_grad()
+def eval_step_u8(vqgan, frames: torch.Tensor, total_usage: Optional[torch.Tensor] = None, norm: U8Norm = VIDEO_NORM):
+    """eval_step from the decoder's uint8 frames (B, T, H, W, C) (or images (B, H, W, C)): vqgan_eval.py's loop over a
+    DecordVideoDataset whose VideoNorm (data.py:229-232) is applied in the kernel.  Returns (frames uint8 'b t h w c',
+    vq_output), equal to eval_step's frames and vq_output on the normalised input."""
+    _check_u8(frames, (4, 5), "eval_step_u8")
+    is_image = frames.ndim == 4
+    if hasattr(vqgan, "forward_u8"):
+        out, vq_output = vqgan.forward_u8(frames, norm, EVAL_U8)
+    else:
+        x = u8_normalize(frames.unsqueeze(1) if is_image else frames, norm)
+        _, _, _, x_recons, vq_output = vqgan(x.squeeze(2) if is_image else x, log_image=True)
+        out = _to_u8(x_recons.unsqueeze(2) if is_image else x_recons, EVAL_U8)
+    if total_usage is not None and vq_output is not None:
+        total_usage += vq_output["batch_usage"]
+    return out, vq_output
+
+
+@torch.no_grad()
+def encode_to_z_u8(vqgan, frames: torch.Tensor, is_image: bool, sample_every_n_latent_frames: int = 0,
+                   norm: U8Norm = VIDEO_NORM) -> Tuple[torch.Tensor, torch.Tensor]:
+    """encode_to_z (lm_transformer.py:258-268) from the uint8 frames of the LM's VideoNorm data loader."""
+    emb, targets = _encode_u8(vqgan, frames, is_image, norm, include_embeddings=True)
+    return _z_wire_format(emb, targets, sample_every_n_latent_frames)
+
+
+@torch.no_grad()
+def dit_encode_latents_u8(vae, images: torch.Tensor, norm: U8Norm = DIT_NORM) -> torch.Tensor:
+    """dit_encode_latents from (B, H, W, 3) uint8 images (DiT train.py:185-198 ToTensor + Normalize, then :242)."""
+    return _encode_u8(vae, images, True, norm).mul_(LATENT_SCALE)
+
+
+@torch.no_grad()
+def latte_encode_latents_u8(vae, clips: torch.Tensor, norm: U8Norm = LATTE_NORM) -> torch.Tensor:
+    """latte_encode_latents from (B, F, H, W, 3) uint8 clips (Latte ToTensorVideo + Normalize, then train.py:215-217):
+    scaled latents 'b f c h w'."""
+    z = _encode_u8(vae, clips, False, norm).mul_(LATENT_SCALE)
+    return z.permute(0, 2, 1, 3, 4).contiguous()              # 'b c f h w -> b f c h w'

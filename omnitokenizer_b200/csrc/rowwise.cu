@@ -156,46 +156,35 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
 // ------------------------------------------------------------------------------------------
 // Patch gather + LayerNorm.  One warp per patch row; K = Cin*p*p (first frame) or Cin*pt*p*p.
 // Feature f = ((c*PT + dt)*p + p1)*p + p2 ; p2 is contiguous in the video (p % 4 == 0).
+// The gather (fp32 video or uint8 frames) fills the lane's v[i] = features f = (i*32 + lane)*4 .. +3 (zeros past K);
+// patch_ln_emit() is the LayerNorm and output stage both gathers share, so equal v[] give equal bits.
 // ------------------------------------------------------------------------------------------
-template <int NV>
-__global__ void __launch_bounds__(256) patchify_ln_kernel(const float* __restrict__ video,
-                                                          float* __restrict__ A, uint16_t* __restrict__ A_hi,
-                                                          uint16_t* __restrict__ A_lo, float* __restrict__ A_rs,
-                                                          const float* __restrict__ lw,
-                                                          const float* __restrict__ lb, int rows,
-                                                          int Cin, int T, int H, int W, int p, int pt,
-                                                          int first, float eps) {
-  pdl_sync();
-  const int lane = threadIdx.x & 31;
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= rows) return;
+struct PatchRow {             // patch row -> (sample, first frame of the row, token row / column)
+  int bi, t0, hi, wi;
+};
+
+__device__ __forceinline__ PatchRow patch_row(int row, int T, int H, int W, int p, int pt, int first) {
   const int hh = H / p, ww = W / p;
-  const int PT = first ? 1 : pt;
-  const int K = Cin * PT * p * p;
   int r = row;
-  const int wi = r % ww; r /= ww;
-  const int hi = r % hh; r /= hh;
+  PatchRow pr;
+  pr.wi = r % ww; r /= ww;
+  pr.hi = r % hh; r /= hh;
   int ti = 0;
   if (!first) { const int tn = (T - 1) / pt; ti = r % tn; r /= tn; }
-  const int bi = r;
-  const int t0 = first ? 0 : 1 + ti * pt;
-  float4 v[NV];
+  pr.bi = r;
+  pr.t0 = first ? 0 : 1 + ti * pt;
+  return pr;
+}
+
+template <int NV>
+__device__ __forceinline__ void patch_ln_emit(float4 (&v)[NV], int row, int K, int lane, float* __restrict__ A,
+                                              uint16_t* __restrict__ A_hi, uint16_t* __restrict__ A_lo,
+                                              float* __restrict__ A_rs, const float* __restrict__ lw,
+                                              const float* __restrict__ lb, float eps) {
   float s = 0.f;
 #pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int f = (i * 32 + lane) * 4;
-    if (f < K) {
-      const int p2 = f % p;
-      const int p1 = (f / p) % p;
-      const int dt = (f / (p * p)) % PT;
-      const int c = f / (p * p * PT);
-      const size_t off = ((((size_t)bi * Cin + c) * T + (t0 + dt)) * H + (hi * p + p1)) * W + wi * p + p2;
-      v[i] = *reinterpret_cast<const float4*>(video + off);
-      s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-    } else {
-      v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-  }
+  for (int i = 0; i < NV; ++i)
+    if ((i * 32 + lane) * 4 < K) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
   const size_t rbase = (size_t)row * K;
   // write a finished row: fp32, 2^11-scaled planes, or row-scaled planes (+ the inverse row scale)
   auto emit = [&](float4 (&o)[NV]) {
@@ -245,6 +234,125 @@ __global__ void __launch_bounds__(256) patchify_ln_kernel(const float* __restric
     }
   }
   emit(v);
+}
+
+template <int NV>
+__global__ void __launch_bounds__(256) patchify_ln_kernel(const float* __restrict__ video,
+                                                          float* __restrict__ A, uint16_t* __restrict__ A_hi,
+                                                          uint16_t* __restrict__ A_lo, float* __restrict__ A_rs,
+                                                          const float* __restrict__ lw,
+                                                          const float* __restrict__ lb, int rows,
+                                                          int Cin, int T, int H, int W, int p, int pt,
+                                                          int first, float eps) {
+  pdl_sync();
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const int PT = first ? 1 : pt;
+  const int K = Cin * PT * p * p;
+  const PatchRow pr = patch_row(row, T, H, W, p, pt, first);
+  float4 v[NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int f = (i * 32 + lane) * 4;
+    if (f < K) {
+      const int p2 = f % p;
+      const int p1 = (f / p) % p;
+      const int dt = (f / (p * p)) % PT;
+      const int c = f / (p * p * PT);
+      const size_t off = ((((size_t)pr.bi * Cin + c) * T + (pr.t0 + dt)) * H + (pr.hi * p + p1)) * W + pr.wi * p + p2;
+      v[i] = *reinterpret_cast<const float4*>(video + off);
+    } else {
+      v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
+  patch_ln_emit<NV>(v, row, K, lane, A, A_hi, A_lo, A_rs, lw, lb, eps);
+}
+
+// uint8 twin: frames (B, T, H, W, Cin) channels-last bytes, each byte of channel c mapped through lut[tab][c][256], the
+// host-built table of the data pipeline's normalisation (tab = sel[b], or 0 without sel).  A patch line of one row is p*Cin
+// contiguous, 4-byte aligned bytes: each warp stages its row's PT*p lines in shared memory with 32-bit loads, then builds
+// the same v[] as patchify_ln_kernel.  Warps walk rows with a grid stride so the table is loaded once per CTA.
+constexpr int PU8_WARPS = 8;
+constexpr int PU8_MAX_K = 1024;   // = the bytes of one row (K features, one byte each)
+
+template <int NV>
+__global__ void __launch_bounds__(256) patchify_ln_u8_kernel(const uint8_t* __restrict__ frames,
+                                                             const float* __restrict__ lut, const int32_t* __restrict__ sel,
+                                                             float* __restrict__ A, uint16_t* __restrict__ A_hi,
+                                                             uint16_t* __restrict__ A_lo, float* __restrict__ A_rs,
+                                                             const float* __restrict__ lw, const float* __restrict__ lb,
+                                                             int rows, int Cin, int T, int H, int W, int p, int pt,
+                                                             int first, float eps) {
+  __shared__ float tab[2 * 4 * 256];
+  __shared__ uint32_t stage[PU8_WARPS][PU8_MAX_K / 4];
+  pdl_sync();
+  const int ntab = sel != nullptr ? 2 : 1;
+  for (int i = threadIdx.x; i < ntab * Cin * 256; i += blockDim.x) tab[i] = lut[i];
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int PT = first ? 1 : pt;
+  const int K = Cin * PT * p * p;
+  const int line_words = p * Cin / 4;
+  uint32_t* st = stage[warp];
+  const uint8_t* sb = reinterpret_cast<const uint8_t*>(st);
+  for (int row = blockIdx.x * PU8_WARPS + warp; row < rows; row += gridDim.x * PU8_WARPS) {
+    const PatchRow pr = patch_row(row, T, H, W, p, pt, first);
+    for (int j = lane; j < K / 4; j += 32) {          // word j of line l = dt * p + p1
+      const int l = j / line_words;
+      const int dt = l / p, p1 = l - dt * p;
+      const size_t pix = (((size_t)pr.bi * T + (pr.t0 + dt)) * H + (pr.hi * p + p1)) * W + pr.wi * p;
+      st[j] = __ldg(reinterpret_cast<const uint32_t*>(frames + pix * Cin) + (j - l * line_words));
+    }
+    __syncwarp();
+    const float* tb = tab;
+    if (sel != nullptr) tb += (sel[pr.bi] != 0 ? Cin * 256 : 0);
+    float4 v[NV];
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+      const int f = (i * 32 + lane) * 4;
+      if (f < K) {
+        const int p2 = f % p;
+        const int p1 = (f / p) % p;
+        const int dt = (f / (p * p)) % PT;
+        const int c = f / (p * p * PT);
+        const uint8_t* px = sb + ((dt * p + p1) * p + p2) * Cin + c;
+        const float* tc = tb + c * 256;
+        v[i] = make_float4(tc[px[0]], tc[px[Cin]], tc[px[2 * Cin]], tc[px[3 * Cin]]);
+      } else {
+        v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    }
+    __syncwarp();                                      // the stage is rewritten by the next row
+    patch_ln_emit<NV>(v, row, K, lane, A, A_hi, A_lo, A_rs, lw, lb, eps);
+  }
+}
+
+// sel[b] = 1 until a byte > 1 is found in sample b (VideoNorm's `if max(clip) > 1: div_(255)`), then 0.
+__global__ void __launch_bounds__(256) u8_sel_init_kernel(int32_t* __restrict__ sel, int B) {
+  pdl_sync();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B) sel[b] = 1;
+}
+
+__global__ void __launch_bounds__(256) u8_sel_scan_kernel(const uint8_t* __restrict__ frames, long long per_sample,
+                                                          int32_t* __restrict__ sel) {
+  pdl_sync();
+  const uint8_t* x = frames + (size_t)blockIdx.y * per_sample;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  uint32_t acc = 0;
+  if (per_sample % 16 == 0 && (reinterpret_cast<uintptr_t>(frames) & 15) == 0) {
+    const uint4* x4 = reinterpret_cast<const uint4*>(x);
+    for (long long i = t0; i < per_sample / 16; i += stride) {
+      const uint4 w = __ldg(x4 + i);
+      acc |= w.x | w.y | w.z | w.w;
+    }
+  } else {
+    for (long long i = t0; i < per_sample; i += stride) acc |= x[i];
+  }
+  // a byte is > 1 exactly when one of its bits 1..7 is set
+  if (__syncthreads_or((acc & 0xFEFEFEFEu) != 0) && threadIdx.x == 0) sel[blockIdx.y] = 0;
 }
 
 __global__ void __launch_bounds__(256) unpatchify_kernel(const float* __restrict__ P,
@@ -744,6 +852,56 @@ extern "C" int omt_patchify_ln(const float* video, float* A, uint16_t* A_hi, uin
     OMT_CUDA(launch_k(patchify_ln_kernel<6>, grid, block, 0, st, video, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
   else
     OMT_CUDA(launch_k(patchify_ln_kernel<8>, grid, block, 0, st, video, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_patchify_ln_u8(const uint8_t* frames, const float* lut, const int32_t* sel, float* A, uint16_t* A_hi,
+                                  uint16_t* A_lo, float* A_rs, const float* ln_w, const float* ln_b, int B, int Cin, int T,
+                                  int H, int W, int p, int pt, int first, float eps, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(frames && lut && (A || A_hi) && ((ln_w == nullptr) == (ln_b == nullptr)) && ((A_hi == nullptr) == (A_lo == nullptr)),
+              "omt_patchify_ln_u8: null pointer");
+  OMT_REQUIRE(((uintptr_t)A_hi | (uintptr_t)A_lo) % 8 == 0, "omt_patchify_ln_u8: planes must be 8-byte aligned");
+  OMT_REQUIRE((uintptr_t)frames % 4 == 0, "omt_patchify_ln_u8: frames must be 4-byte aligned");
+  OMT_REQUIRE(A_rs == nullptr || A_hi != nullptr, "omt_patchify_ln_u8: row scales without planes");
+  OMT_REQUIRE(Cin >= 1 && Cin <= 4, "omt_patchify_ln_u8: Cin=%d must be 1..4", Cin);
+  OMT_REQUIRE(p % 4 == 0 && p > 0 && H % p == 0 && W % p == 0, "omt_patchify_ln_u8: patch %d must be a multiple of 4 dividing %dx%d", p, H, W);
+  OMT_REQUIRE(first || (T > 1 && pt > 0 && (T - 1) % pt == 0), "omt_patchify_ln_u8: (T-1) %% pt != 0");
+  const int PT = first ? 1 : pt;
+  const int K = Cin * PT * p * p;
+  OMT_REQUIRE(K <= PU8_MAX_K, "omt_patchify_ln_u8: patch vector %d > %d", K, PU8_MAX_K);
+  const long long rows = (long long)B * (first ? 1 : (T - 1) / pt) * (H / p) * (W / p);
+  if (rows == 0) return OMT_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  long long blocks = (rows + PU8_WARPS - 1) / PU8_WARPS;
+  if (blocks > (long long)sm_count() * 8) blocks = (long long)sm_count() * 8;   // 8 CTAs of 256 threads fill an SM
+  dim3 grid((unsigned)blocks), block(32 * PU8_WARPS);
+  const int nv = (K / 4 + 31) / 32;
+  if (nv <= 2)
+    OMT_CUDA(launch_k(patchify_ln_u8_kernel<2>, grid, block, 0, st, frames, lut, sel, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
+  else if (nv <= 6)
+    OMT_CUDA(launch_k(patchify_ln_u8_kernel<6>, grid, block, 0, st, frames, lut, sel, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
+  else
+    OMT_CUDA(launch_k(patchify_ln_u8_kernel<8>, grid, block, 0, st, frames, lut, sel, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_u8_norm_select(const uint8_t* frames, int B, long long per_sample, int32_t* sel, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(frames && sel, "omt_u8_norm_select: null pointer");
+  OMT_REQUIRE(B >= 0 && B <= 65535 && per_sample >= 0, "omt_u8_norm_select: B=%d, per_sample=%lld", B, per_sample);
+  if (B == 0) return OMT_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  OMT_CUDA(launch_k(u8_sel_init_kernel, dim3((B + 255) / 256), dim3(256), 0, st, sel, B));
+  OMT_LAUNCH_CHECK();
+  if (per_sample == 0) return OMT_OK;
+  long long bx = (per_sample / 16 + 255) / 256;                  // one 16-byte load per thread and block
+  const long long cap = ((long long)sm_count() * 8 + B - 1) / B;    // about 8 CTAs per SM over the whole batch
+  if (bx > cap) bx = cap;
+  if (bx < 1) bx = 1;
+  OMT_CUDA(launch_k(u8_sel_scan_kernel, dim3((unsigned)bx, (unsigned)B), dim3(256), 0, st, frames, per_sample, sel));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

@@ -91,6 +91,7 @@ class Workspace:
         self.counts = torch.zeros(8192, device=device, dtype=torch.int32)
         # static I/O buffers + captured CUDA graphs of this shape
         self.x_in = None
+        self.u8_in, self.u8_sel = None, None      # encode_u8: uint8 frames, per-sample table index
         self.video_u8 = None
         self.idx_in = torch.empty(M, device=device, dtype=torch.int64)
         self.zc_in = torch.empty(M, cd, **f)
@@ -441,8 +442,9 @@ class Engine:
             _cabi.launch_count += g[1]        # kernels inside the replayed graph (bench.py accounting)
 
     # ------------------------------------------------------------------ encoder side
-    def _encode_body(self, ws: Workspace, x, dims, mode: str):
-        """patch embed -> spatial -> temporal -> pre_vq [-> VQ search].  omnitokenizer.py:881-947, 247-258."""
+    def _encode_body(self, ws: Workspace, gather, dims, mode: str):
+        """patch embed -> spatial -> temporal -> pre_vq [-> VQ search].  omnitokenizer.py:881-947, 247-258.
+        gather(first, A, A_hi, A_lo, A_rs, ln_w, ln_b) launches the patch gather + LayerNorm of the input video."""
         B, T, H, W, Tp, h, w = dims
         N, C = h * w, self.C
         ws.reset()
@@ -452,12 +454,10 @@ class Engine:
             if self.planes:
                 Pp = Planes.__new__(Planes)          # dense [rows, K] view at the start of the patch planes
                 Pp.hi, Pp.lo, Pp.ld, Pp.rs = ws.Pp.hi, ws.Pp.lo, K, ws.Pp.rs
-                _cabi.call("omt_patchify_ln", x, None, Pp.hi, Pp.lo, Pp.rs, pe["ln1_g"], pe["ln1_b"], B, self.cin, T, H, W,
-                           self.p, self.pt, first, 1e-5)
+                gather(first, None, Pp.hi, Pp.lo, Pp.rs, pe["ln1_g"], pe["ln1_b"])
                 self._linear_h(Pp, pe["lin"], rows, C=ws.X, ldc=C, c_map=cmap)
             else:
-                _cabi.call("omt_patchify_ln", x, ws.P, None, None, None, pe["ln1_g"], pe["ln1_b"], B, self.cin, T, H, W, self.p,
-                           self.pt, first, 1e-5)
+                gather(first, ws.P, None, None, None, pe["ln1_g"], pe["ln1_b"])
                 self._linear(ws.P, K, pe["lin"], ws.X, C, rows, c_map=cmap)
             if not self.cnn:
                 self._ln(ws.X, ws.X, pe["ln2_g"], pe["ln2_b"], rows, seg=cmap)
@@ -487,7 +487,40 @@ class Engine:
             ws.x_in = torch.empty_like(x, memory_format=torch.contiguous_format)
             ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("enc")}
         ws.x_in.copy_(x)
-        self._run(ws, ("enc:" + mode, tuple(x.shape)), lambda: self._encode_body(ws, ws.x_in, dims, mode))
+
+        def gather(first, *out):
+            _cabi.call("omt_patchify_ln", ws.x_in, *out, B, self.cin, T, H, W, self.p, self.pt, first, 1e-5)
+
+        self._run(ws, ("enc:" + mode, tuple(x.shape)), lambda: self._encode_body(ws, gather, dims, mode))
+        return ws, (B, Tp, h, w)
+
+    def encode_u8(self, frames: torch.Tensor, mode: str, norm: L.U8Norm):
+        """encode() from uint8 frames (B,T,H,W,C) on the device: the patch gather maps every byte through the host-built
+        table of `norm` (layout.u8_norm_table), so the result equals encode() of the pipeline's fp32 video bit for bit.
+        With norm.max_test the table is picked per sample on the device (omt_u8_norm_select), inside the graph."""
+        if frames.dtype != torch.uint8 or frames.ndim != 5:
+            raise TypeError(f"encode_u8 takes (B, T, H, W, C) uint8 frames, got {tuple(frames.shape)} {frames.dtype}")
+        Bf, Tf, Hf, Wf, Cf = frames.shape
+        dims = self._shape((Bf, Cf, Tf, Hf, Wf))
+        B, T, H, W, Tp, h, w = dims
+        ws = self._workspace(B * Tp * h * w)
+        if ws.u8_in is None or ws.u8_in.shape != frames.shape:
+            ws.u8_in = torch.empty(frames.shape, device=self.device, dtype=torch.uint8)
+            ws.u8_sel = torch.empty(B, device=self.device, dtype=torch.int32)
+            ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("enc_u8")}
+        ws.u8_in.copy_(frames)
+        lut = self._table(("u8norm", norm), lambda: L.u8_norm_table(norm, self.cin))
+        sel = ws.u8_sel if norm.max_test else None
+
+        def gather(first, *out):
+            _cabi.call("omt_patchify_ln_u8", ws.u8_in, lut, sel, *out, B, self.cin, T, H, W, self.p, self.pt, first, 1e-5)
+
+        def body():
+            if sel is not None:
+                _cabi.call("omt_u8_norm_select", ws.u8_in, B, T * H * W * self.cin, sel)
+            self._encode_body(ws, gather, dims, mode)
+
+        self._run(ws, ("enc_u8:" + mode, tuple(frames.shape), norm), body)
         return ws, (B, Tp, h, w)
 
     def z_view(self, ws: Workspace) -> torch.Tensor:

@@ -6,9 +6,48 @@ the per-token arithmetic all happens in the CUDA kernels.
 from __future__ import annotations
 
 import math
-from typing import Tuple
+from typing import NamedTuple, Tuple
 
 import torch
+
+
+class U8Norm(NamedTuple):
+    """A data pipeline's uint8 -> fp32 normalisation, (u / 255 - mean_c) / std_c per channel in fp32.
+    max_test: VideoNorm's `if max(clip) > 1: div_(255)` (OmniTokenizer/video_utils.py:53-54) -- a clip whose largest
+    byte is <= 1 is only shifted and scaled, (u - mean_c) / std_c."""
+    name: str
+    mean: Tuple[float, ...]
+    std: Tuple[float, ...]
+    max_test: bool = False
+
+
+def u8_norm_table(norm: U8Norm, channels: int) -> torch.Tensor:
+    """fp32 [n_tab, channels, 256]: the value every byte of every channel stands for, computed on the host CPU with the
+    pipelines' own torch expression and op order (ToTensor / to_tensor / VideoNorm: / 255; Normalize / VideoNorm:
+    .sub_(mean).div_(std) with fp32 mean / std tensors).  Table 0 is the normal mapping; with max_test, table 1 is
+    the undivided one.  Kernels only look values up, so they reproduce the pipeline's bits (CUDA would divide by
+    multiplying with the reciprocal, which differs in about half of the byte values)."""
+    if len(norm.mean) != channels or len(norm.std) != channels:
+        raise ValueError(f"normalisation {norm.name!r} has {len(norm.mean)} channels, the model takes {channels}")
+    mean = torch.tensor(norm.mean, dtype=torch.float32).view(channels, 1)
+    std = torch.tensor(norm.std, dtype=torch.float32).view(channels, 1)
+    u = torch.arange(256, dtype=torch.uint8).float().expand(channels, 256).contiguous()
+    tabs = [(u / 255.0).sub_(mean).div_(std)]
+    if norm.max_test:
+        tabs.append(u.clone().sub_(mean).div_(std))
+    return torch.stack(tabs).contiguous()
+
+
+def u8_normalize(frames: torch.Tensor, norm: U8Norm) -> torch.Tensor:
+    """(B, T, H, W, C) uint8 -> the (B, C, T, H, W) fp32 video the pipeline hands the model, by table lookup (exact on
+    any device).  With max_test the table is chosen per sample from its largest byte, as VideoNorm sees one clip."""
+    B, C = frames.shape[0], frames.shape[-1]
+    tab = u8_norm_table(norm, C).to(frames.device)
+    sel = torch.zeros(B, dtype=torch.long, device=frames.device)
+    if norm.max_test and frames.numel() > 0:
+        sel = (frames.reshape(B, -1).amax(dim=1) <= 1).long()
+    x = frames.permute(0, 4, 1, 2, 3).long()
+    return tab[sel.view(B, 1, 1, 1, 1), torch.arange(C, device=frames.device).view(1, C, 1, 1, 1), x]
 
 
 def peg_neighbour_table(T: int, h: int, w: int, temporal: bool, causal: bool) -> torch.Tensor:

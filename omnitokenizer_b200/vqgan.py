@@ -23,6 +23,7 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
+from .consumers import EVAL_U8, VIDEO_NORM
 from .engine import Engine
 
 
@@ -331,23 +332,54 @@ class OmniTokenizer_VQGAN(nn.Module):
             return self._empty_encode(x, is_image, include_embeddings)
         with torch.cuda.device(self.device):
             xv = x.unsqueeze(2) if is_image else x
-            ws, (B, Tp, h, w) = eng.encode(xv.float(), "raw" if self.use_vae else "vq")
-            if not self.use_vae:
-                enc = ws.idx.view(B, Tp, h, w).clone()
-                self._track_usage(ws.counts, ws.M)             # Codebook.forward runs inside encode() too
-                if include_embeddings:
-                    z = eng.z_view(ws)
-                    e = eng.E[ws.idx]
-                    st = (e - z) + z
-                    return st.view(B, Tp, h, w, -1).permute(0, 4, 1, 2, 3).contiguous(), enc
-                return enc
-            hpar = eng.z_view(ws)                                                 # (M, 2*cd) moments
-            c = hpar.shape[1] // 2
-            hpar = hpar.view(B, Tp, h, w, 2 * c).permute(0, 4, 1, 2, 3)
-            mean, logvar = hpar[:, :c], torch.clamp(hpar[:, c:], -30.0, 20.0)     # vae.py:7-8
-            noise = torch.randn(mean.shape).to(device=self.device)                # CPU generator, vae.py:16
-            z = mean + torch.exp(0.5 * logvar) * noise
-            return z.squeeze(2) if is_image else z.contiguous()
+            ws, dims = eng.encode(xv.float(), "raw" if self.use_vae else "vq")
+            return self._encode_result(eng, ws, dims, is_image, include_embeddings)
+
+    def _u8_frames(self, frames, is_image):
+        """Checks uint8 frames (B, T, H, W, C) / images (B, H, W, C) and returns them as (B, T, H, W, C)."""
+        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+            raise TypeError(f"expected uint8 frames, got {getattr(frames, 'dtype', type(frames))}")
+        if frames.ndim != (4 if is_image else 5):
+            raise ValueError(f"expected {'(B, H, W, C)' if is_image else '(B, T, H, W, C)'} frames, got {tuple(frames.shape)}")
+        if frames.shape[-1] != self.args.image_channels:
+            raise ValueError(f"expected {self.args.image_channels} channels (last dimension), got {frames.shape[-1]}")
+        return frames.unsqueeze(1) if is_image else frames
+
+    @torch.no_grad()
+    def encode_u8(self, frames, is_image, include_embeddings=False, norm=VIDEO_NORM):
+        """encode() straight from the uint8 frames the data loaders produce: (B, T, H, W, C), or (B, H, W, C) images,
+        channels last (decord / PIL / decode_u8 layout).  The patch-gather kernel applies the loader's normalisation
+        `norm` (a layout.U8Norm; default VIDEO_NORM, VideoNorm of the reference's video datasets) by table
+        lookup, so the result -- codes, embeddings, VAE latents, usage statistics, CPU RNG draws -- is exactly
+        encode(norm(frames) as (B, C, T, H, W) fp32, is_image, include_embeddings).  The copy to the device is 4x smaller."""
+        f = self._u8_frames(frames, is_image)
+        eng = self.engine()
+        if f.shape[0] == 0:
+            shape = (0, f.shape[4], f.shape[2], f.shape[3]) if is_image else (0, f.shape[4], f.shape[1], f.shape[2], f.shape[3])
+            return self._empty_encode(torch.empty(shape, device="meta"), is_image, include_embeddings)
+        with torch.cuda.device(self.device):
+            ws, dims = eng.encode_u8(f, "raw" if self.use_vae else "vq", norm)
+            return self._encode_result(eng, ws, dims, is_image, include_embeddings)
+
+    def _encode_result(self, eng, ws, dims, is_image, include_embeddings):
+        """What encode() returns from the engine's workspace (omnitokenizer.py:247-266), with Codebook.forward's usage side effects."""
+        B, Tp, h, w = dims
+        if not self.use_vae:
+            enc = ws.idx.view(B, Tp, h, w).clone()
+            self._track_usage(ws.counts, ws.M)             # Codebook.forward runs inside encode() too
+            if include_embeddings:
+                z = eng.z_view(ws)
+                e = eng.E[ws.idx]
+                st = (e - z) + z
+                return st.view(B, Tp, h, w, -1).permute(0, 4, 1, 2, 3).contiguous(), enc
+            return enc
+        hpar = eng.z_view(ws)                                                 # (M, 2*cd) moments
+        c = hpar.shape[1] // 2
+        hpar = hpar.view(B, Tp, h, w, 2 * c).permute(0, 4, 1, 2, 3)
+        mean, logvar = hpar[:, :c], torch.clamp(hpar[:, c:], -30.0, 20.0)     # vae.py:7-8
+        noise = torch.randn(mean.shape).to(device=self.device)                # CPU generator, vae.py:16
+        z = mean + torch.exp(0.5 * logvar) * noise
+        return z.squeeze(2) if is_image else z.contiguous()
 
     def _check_cnn_grid(self, h, w):
         # the cnn decoder's Rearrange pins h to image_size // patch_size (omnitokenizer.py:1021): other grids raise there
@@ -442,33 +474,8 @@ class OmniTokenizer_VQGAN(nn.Module):
         with torch.cuda.device(self.device):
             xv = (x.unsqueeze(2) if is_image else x).float()
             ws, dims = eng.encode(xv, "raw" if self.use_vae else "vq")
-            B, Tp, h, w = dims
-            M = ws.M
-            vq_output = None
-            if not self.use_vae:
-                z = eng.z_view(ws).clone()
-                idx, counts = ws.idx.clone(), ws.counts.clone()
-                x_recon = eng.decode(dims, idx=idx, straight_through=True)           # decoder sees (e - z) + z
-                zq = eng.zq_view(ws).clone()
-                cb = self.codebook
-                n_codes = cb.n_codes
-                usage = self._track_usage(counts, M)                                  # codebook.py:54-72, 133-138
-                e = eng.E[idx]
-                commitment = 0.25 * torch.mean((z - e) ** 2)                           # codebook.py:93
-                perplexity = torch.exp(-torch.sum(usage * torch.log(usage + 1e-10)))   # codebook.py:122-123
-                avg_usage = (cb.codebook_usage.data > (1 / n_codes)).sum() / n_codes
-                vq_output = dict(embeddings=zq.view(B, Tp, h, w, -1).permute(0, 4, 1, 2, 3).contiguous(),
-                                 encodings=idx.view(B, Tp, h, w), commitment_loss=commitment, perplexity=perplexity,
-                                 avg_usage=avg_usage, batch_usage=usage)
-            else:
-                hpar = eng.z_view(ws)
-                c = hpar.shape[1] // 2
-                hp5 = hpar.view(B, Tp, h, w, 2 * c).permute(0, 4, 1, 2, 3)
-                mean, logvar = hp5[:, :c], torch.clamp(hp5[:, c:], -30.0, 20.0)
-                noise = torch.randn(mean.shape).to(device=self.device)               # drawn BEFORE randint (:368 vs :401)
-                z = mean + torch.exp(0.5 * logvar) * noise
-                zc = z.permute(0, 2, 3, 4, 1).reshape(M, c).contiguous()
-                x_recon = eng.decode(dims, zc=zc)
+            B = dims[0]
+            x_recon, vq_output = self._forward_decode(eng, ws, dims)
             if is_image:
                 x_recon = x_recon.squeeze(2)
                 frames, frames_recon = x, x_recon
@@ -478,6 +485,58 @@ class OmniTokenizer_VQGAN(nn.Module):
                 ar = torch.arange(B, device=self.device)
                 frames, frames_recon = x[ar, :, frame_idx], x_recon[ar, :, frame_idx]
             return frames, frames_recon, x, x_recon, vq_output
+
+    def _forward_decode(self, eng, ws, dims, u8=None):
+        """forward()'s quantise -> decode -> statistics on the encoder output in the workspace.  Returns (x_recon 5-D, or
+        uint8 'b t h w c' with u8 = the output affine; vq_output or None for the VAE)."""
+        B, Tp, h, w = dims
+        M = ws.M
+        vq_output = None
+        if not self.use_vae:
+            z = eng.z_view(ws).clone()
+            idx, counts = ws.idx.clone(), ws.counts.clone()
+            x_recon = eng.decode(dims, idx=idx, straight_through=True, u8=u8)     # decoder sees (e - z) + z
+            zq = eng.zq_view(ws).clone()
+            cb = self.codebook
+            n_codes = cb.n_codes
+            usage = self._track_usage(counts, M)                                  # codebook.py:54-72, 133-138
+            e = eng.E[idx]
+            commitment = 0.25 * torch.mean((z - e) ** 2)                           # codebook.py:93
+            perplexity = torch.exp(-torch.sum(usage * torch.log(usage + 1e-10)))   # codebook.py:122-123
+            avg_usage = (cb.codebook_usage.data > (1 / n_codes)).sum() / n_codes
+            vq_output = dict(embeddings=zq.view(B, Tp, h, w, -1).permute(0, 4, 1, 2, 3).contiguous(),
+                             encodings=idx.view(B, Tp, h, w), commitment_loss=commitment, perplexity=perplexity,
+                             avg_usage=avg_usage, batch_usage=usage)
+        else:
+            hpar = eng.z_view(ws)
+            c = hpar.shape[1] // 2
+            hp5 = hpar.view(B, Tp, h, w, 2 * c).permute(0, 4, 1, 2, 3)
+            mean, logvar = hp5[:, :c], torch.clamp(hp5[:, c:], -30.0, 20.0)
+            noise = torch.randn(mean.shape).to(device=self.device)               # drawn BEFORE randint (:368 vs :401)
+            z = mean + torch.exp(0.5 * logvar) * noise
+            zc = z.permute(0, 2, 3, 4, 1).reshape(M, c).contiguous()
+            x_recon = eng.decode(dims, zc=zc, u8=u8)
+        return x_recon, vq_output
+
+    @torch.no_grad()
+    def forward_u8(self, frames, norm=VIDEO_NORM, out_affine=EVAL_U8):
+        """forward(x, log_image=True) from uint8 frames, with uint8 out: frames (B, T, H, W, C) or images (B, H, W, C),
+        normalised in the patch gather by `norm` (default VIDEO_NORM).  Returns (x_recon, vq_output): x_recon is
+        the reconstruction as uint8 'b t h w c' (T = 1 for images) = _to_u8(forward's x_recon, out_affine) byte for byte
+        (default: vqgan_eval.py:139,147-148), vq_output is forward's (None for the VAE).  The CPU RNG is consumed as
+        forward consumes it (VAE noise, then the random frame's randint), so a seeded eval loop stays in step."""
+        if self.resolution_scale is not None:
+            raise NotImplementedError("resolution_scale resizes the fp32 frames between the / 255 and the shift "
+                                      "(omnitokenizer.py:334-355); no byte table expresses that -- use forward()")
+        is_image = frames.ndim == 4
+        f = self._u8_frames(frames, is_image)
+        eng = self.engine()
+        with torch.cuda.device(self.device):
+            ws, dims = eng.encode_u8(f, "raw" if self.use_vae else "vq", norm)
+            x_recon, vq_output = self._forward_decode(eng, ws, dims, u8=tuple(float(v) for v in out_affine))
+            if not is_image:
+                torch.randint(0, f.shape[1], [f.shape[0]])                      # forward's random-frame draw (omnitokenizer.py:401)
+            return x_recon, vq_output
 
     # ---------------------------------------------------------------- CLI surface
     @staticmethod
