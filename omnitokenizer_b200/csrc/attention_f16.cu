@@ -1,4 +1,4 @@
-// Attention v4: spatial (full, non-causal) attention core on sm_90a wgmma (f16) with row-scaled fp16 operand planes.
+// Attention v5: spatial (full, non-causal) attention core on sm_90a wgmma (f16) with row-scaled fp16 operand planes.
 //   O = softmax(scale * Q K^T) V  per (sequence, head), head dim 64, N % 128 == 0
 //   (F.scaled_dot_product_attention at modules/attention.py:451).
 //
@@ -7,13 +7,23 @@
 //          power of two per layer puts them in fp16 range: planes hi = fp16(x * 2^e), lo = fp16(x * 2^e - hi)
 //   v    : unbounded, scaled per (row, head); the inverse scales live in vinv[head][row]
 // so S = Q K^T and O_j = P_j V_j each take THREE f16 wgmmas per 16-deep k-step into ONE fp32 accumulator
-// (hi.hi + hi.lo + lo.hi).
-//   * Q, K and V tiles come straight from TMA; V is consumed as an MN-MAJOR B operand (the token-major [64 keys][64 dims]
+// (lo.hi, hi.lo, hi.hi in that order).
+//   * K and V tiles come straight from TMA; V is consumed as an MN-MAJOR B operand (the token-major [64 keys][64 dims]
 //     tile the TMA lands is the canonical SWIZZLE_128B MN-major layout), so nothing is transposed anywhere.
-//   * the per-key inverse V scale is folded into P: P'' = p * vinv_j * 2^ep with ONE power of two per CTA taken from the
-//     largest vinv of the sequence, so p'' stays in fp16 range; 2^-ep comes off with the final 1 / row-sum.
-// One CTA = two warpgroups, 64 query rows each (S and O in registers, online softmax); P'' goes through a per-warpgroup
-// shared-memory tile as the A operand of the P.V wgmmas.  K / V tiles are double-buffered; thread 0 issues the TMA loads.
+//   * the per-key inverse V scale is folded into P: P'' = p * vinv_j * 2^ep with ONE power of two per (sequence, head)
+//     taken from the largest vinv of the sequence, so p'' stays in fp16 range; 2^-ep comes off with the final 1 / row-sum.
+//
+// Warp-specialised and persistent.  One CTA per SM walks the work items (128-query tile, head, sequence) with a static
+// stride.  Warpgroup 0 is the producer: its first warp finds each item's largest vinv and issues every load (Q by TMA
+// into one buffer, K / V by TMA and the tile's 64 vinv by a bulk copy into a STAGES-deep full / empty mbarrier ring),
+// running ahead into the next item while the consumers finish the current one.  Warpgroups 1 and 2 each own 64 query
+// rows of the item and run decoupled, with no CTA barrier in the key loop:
+//   * Q hi / lo are copied from shared memory into registers once per item (the A fragments of every Q.K^T wgmma); the
+//     Q buffer is handed back as soon as both warpgroups have them.
+//   * S_{j+1} = Q K_{j+1}^T is issued before the softmax of S_j (two S register arrays), so the tensor pipe works while
+//     the softmax runs.  P'' hi / lo are packed from the S accumulator straight into the A fragments of the P.V wgmmas.
+//   * a K / V stage is released once the P.V wgmmas that read it have retired.
+// Every output row sees the same products in the same order as a serial loop over the key tiles would give it.
 #include "omt_common.cuh"
 #include "tc_ptx.cuh"
 #include <cuda.h>
@@ -25,18 +35,22 @@ using namespace omt::ptx;
 
 constexpr int QT = 128, KT = 64, D = 64;
 constexpr int TILE = KT * D * 2;                    // 8 KiB: one 64 x 64 fp16 plane tile
+constexpr int STAGES = 4;
 constexpr int OFF_Q = 0;                            // Q_hi [2 warpgroups] | Q_lo [2]
-constexpr int OFF_KV = 4 * TILE;                    // [2 stages] x (K_hi | K_lo | V_hi | V_lo)
-constexpr int OFF_P = OFF_KV + 8 * TILE;            // [2 warpgroups] x (P_hi | P_lo)
-constexpr int OFF_CTRL = OFF_P + 4 * TILE;
-constexpr int SMEM = OFF_CTRL + 1024 + 1024;        // barriers / reduction + alignment slack
-constexpr int THREADS = 256;
+constexpr int OFF_KV = 4 * TILE;                    // [STAGES] x (K_hi | K_lo | V_hi | V_lo)
+constexpr int OFF_VI = OFF_KV + STAGES * 4 * TILE;  // [STAGES] x the 64 vinv of the tile's keys
+constexpr int OFF_CTRL = OFF_VI + STAGES * KT * 4;  // mbarriers, the item's largest vinv
+constexpr int SMEM = OFF_CTRL + 128 + 1024;         // + alignment slack
+constexpr int THREADS = 384;                        // warpgroup 0: producer; 1, 2: consumers
+constexpr uint32_t KV_BYTES = 4 * TILE + KT * 4;
+// __launch_bounds__(384, 1) caps the kernel at 168 registers a thread: 40 * 128 + 232 * 256 == 168 * 384
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
 struct Args {
   const float* vinv;                                       // [heads][rows] inverse scales of the v rows
   long long rows;                                          // n_seq * N
   float* o; uint16_t* o_hi; uint16_t* o_lo; int ldo;
-  int N;
+  int N, heads, items;                                     // items = n_seq * heads * N / QT
   float scale_log2;                                        // scale * log2(e) / (q plane scale * k plane scale)
 };
 
@@ -47,158 +61,239 @@ attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant_
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_CTRL);
-  uint64_t& q_full = bars[0];
-  uint64_t* full = bars + 1;                                          // [2] K / V planes of a key tile landed
-  float* red = reinterpret_cast<float*>(smem + OFF_CTRL + 64);        // [8] per-warp maxima of vinv
+  uint64_t& q_full = bars[0];                                         // Q planes (and vmax) of an item landed
+  uint64_t& q_empty = bars[1];                                        // every consumer thread has its Q fragments
+  uint64_t* full = bars + 2;                                          // [STAGES] K / V planes and vinv of a key tile landed
+  uint64_t* empty = full + STAGES;                                    // [STAGES] both consumer warpgroups are done with it
+  float* vmax = reinterpret_cast<float*>(bars + 2 + 2 * STAGES);      // largest vinv of the item's (sequence, head)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int wg = warp >> 2, qd = lane & 3;
-  const int qt = blockIdx.x, head = blockIdx.y, seq = blockIdx.z;
-  const int ntiles = a.N / KT;
-  const int row_q0 = seq * a.N + qt * QT;
-  const int row_k0 = seq * a.N;
-  const int col0 = head * D;
+  const int ntiles = a.N / KT, nqt = a.N / QT;
 
   if (tid == 0) {
     prefetch_map(&tmQh); prefetch_map(&tmQl); prefetch_map(&tmKh); prefetch_map(&tmKl); prefetch_map(&tmVh); prefetch_map(&tmVl);
-    mbar_init(&q_full, 1); mbar_init(&full[0], 1); mbar_init(&full[1], 1);
+    mbar_init(&q_full, 1);
+    mbar_init(&q_empty, 256);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     fence_barrier_init();
   }
   __syncthreads();
   pdl_sync();
 
-  auto issue_kv = [&](int j) {
-    const int s = j & 1;
-    uint8_t* sp = smem + OFF_KV + s * 4 * TILE;
-    const int kr = row_k0 + j * KT;
-    mbar_expect_tx(&full[s], 4 * TILE);
-    tma_load_2d(&tmKh, &full[s], sp, col0, kr);
-    tma_load_2d(&tmKl, &full[s], sp + TILE, col0, kr);
-    tma_load_2d(&tmVh, &full[s], sp + 2 * TILE, col0, kr);
-    tma_load_2d(&tmVl, &full[s], sp + 3 * TILE, col0, kr);
+  // work item -> query tile (fastest), head, sequence: the CTAs running at once share a (sequence, head)'s K / V in L2
+  auto decode = [&](int item, int& row_q0, int& row_k0, int& col0, int& head) {
+    const int qt = item % nqt, hs = item / nqt, seq = hs / a.heads;
+    head = hs % a.heads;
+    row_k0 = seq * a.N;
+    row_q0 = row_k0 + qt * QT;
+    col0 = head * D;
   };
-  if (tid == 0) {
-    mbar_expect_tx(&q_full, 4 * TILE);
-    for (int w = 0; w < 2; ++w) {
-      tma_load_2d(&tmQh, &q_full, smem + OFF_Q + w * TILE, col0, row_q0 + w * 64);
-      tma_load_2d(&tmQl, &q_full, smem + OFF_Q + (2 + w) * TILE, col0, row_q0 + w * 64);
-    }
-    issue_kv(0);
-    if (ntiles > 1) issue_kv(1);
-  }
 
-  // ---- one power of two for P'' = p * vinv_j: the largest inverse V scale of this sequence and head
-  const float* vinv_h = a.vinv + (size_t)head * a.rows + row_k0;
-  float vmx = 0.f;
-  for (int i = tid; i < a.N; i += THREADS) vmx = fmaxf(vmx, __ldg(vinv_h + i));
-  vmx = warp_max(vmx);
-  if (lane == 0) red[warp] = vmx;
-  __syncthreads();
-#pragma unroll
-  for (int i = 0; i < 8; ++i) vmx = fmaxf(vmx, red[i]);
-  float p_scale, p_inv;
-  row_scale(vmx, p_scale, p_inv);                  // p * vinv_j * p_scale <= 2^15 for every key (p <= 1)
-
-  const uint32_t sb = smem_u32(smem);
-  const uint64_t dq_hi = desc_sw128(sb + OFF_Q + wg * TILE), dq_lo = desc_sw128(sb + OFF_Q + (2 + wg) * TILE);
-  const uint32_t p_hi = sb + OFF_P + wg * 2 * TILE, p_lo = p_hi + TILE;
-  const uint64_t dp_hi = desc_sw128(p_hi), dp_lo = desc_sw128(p_lo);
-  const int rl0 = (warp & 3) * 16 + (lane >> 2);   // this thread's rows (rl0, rl0 + 8) inside the warpgroup's 64
-  float o_acc[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-  mbar_wait(&q_full, 0);
-
-  for (int j = 0; j < ntiles; ++j) {
-    const int s = j & 1;
-    const uint32_t kv = sb + OFF_KV + s * 4 * TILE;
-    mbar_wait(&full[s], (j >> 1) & 1);
-    float sv[32];
-    {
-      const uint64_t dk_hi = desc_sw128(kv), dk_lo = desc_sw128(kv + TILE);
-      wg_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {             // 16 of the 64 head dims per MMA
-        const uint64_t adv = (uint64_t)(kk * 2);
-        wgmma_f16_n64(sv, dq_lo + adv, dk_hi + adv, kk != 0);
-        wgmma_f16_n64(sv, dq_hi + adv, dk_lo + adv, 1);
-        wgmma_f16_n64(sv, dq_hi + adv, dk_hi + adv, 1);
+  // Producer and consumers walk the same items and key tiles; the running tile count `it` alone gives the stage
+  // (it % STAGES) and the phase parity ((it / STAGES) & 1) of its full barrier, the item count `c` the parity of the Q
+  // barriers.  The producer waits on the phase before it: a fresh empty barrier counts as released.
+  if (warp < 4) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 0) {
+      uint32_t it = 0, c = 0;
+      for (int item = blockIdx.x; item < a.items; item += gridDim.x, ++c) {
+        int row_q0, row_k0, col0, head;
+        decode(item, row_q0, row_k0, col0, head);
+        const float* vinv_h = a.vinv + (size_t)head * a.rows + row_k0;
+        float vmx = 0.f;
+        for (int i = 4 * lane; i < a.N; i += 128) {
+          const float4 v = __ldg(reinterpret_cast<const float4*>(vinv_h + i));
+          vmx = fmaxf(vmx, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+        }
+        vmx = warp_max(vmx);
+        mbar_wait(&q_empty, (c & 1) ^ 1);
+        if (lane == 0) {
+          *vmax = vmx;                                                // published by the arrive below
+          mbar_expect_tx(&q_full, 4 * TILE);
+          for (int w = 0; w < 2; ++w) {
+            tma_load_2d(&tmQh, &q_full, smem + OFF_Q + w * TILE, col0, row_q0 + w * 64);
+            tma_load_2d(&tmQl, &q_full, smem + OFF_Q + (2 + w) * TILE, col0, row_q0 + w * 64);
+          }
+        }
+        for (int j = 0; j < ntiles; ++j, ++it) {
+          const int s = it % STAGES;
+          mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+          if (lane == 0) {
+            uint8_t* sp = smem + OFF_KV + s * 4 * TILE;
+            const int kr = row_k0 + j * KT;
+            mbar_expect_tx(&full[s], KV_BYTES);
+            tma_load_2d(&tmKh, &full[s], sp, col0, kr);
+            tma_load_2d(&tmKl, &full[s], sp + TILE, col0, kr);
+            tma_load_2d(&tmVh, &full[s], sp + 2 * TILE, col0, kr);
+            tma_load_2d(&tmVl, &full[s], sp + 3 * TILE, col0, kr);
+            bulk_load(smem + OFF_VI + s * KT * 4, vinv_h + j * KT, KT * 4, &full[s]);
+          }
+        }
       }
+    }
+  } else {
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int wg = (warp >> 2) - 1, qd = lane & 3;
+    const int rl0 = (warp & 3) * 16 + (lane >> 2);   // this thread's rows (rl0, rl0 + 8) inside the warpgroup's 64
+    const uint32_t sb = smem_u32(smem);
+    auto release = [&](uint32_t t) {                 // the wgmmas that read running tile t have retired: free its stage
+      if ((tid & 127) == 0) mbar_arrive(&empty[t % STAGES]);
+    };
+    // S of one key tile.  The first wgmma of a tile overwrites it, but it is defined once here: ptxas serialises the
+    // wgmmas of a kernel whose accumulator registers can be undefined when a wgmma reads them.
+    float sv[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) sv[i] = 0.f;
+    uint32_t it = 0, c = 0;
+    for (int item = blockIdx.x; item < a.items; item += gridDim.x, ++c) {
+      int row_q0, row_k0, col0, head;
+      decode(item, row_q0, row_k0, col0, head);
+      mbar_wait(&q_full, c & 1);
+      float p_scale, p_inv;
+      row_scale(*vmax, p_scale, p_inv);              // p * vinv_j * p_scale <= 2^15 for every key (p <= 1)
+      // Q A fragments, qh[4 kk + 2 e + h]: rows rl0 + 8 h, columns 16 kk + 8 e + 2 qd (+1), i.e. 16-byte chunk 2 kk + e
+      // of the 128-byte row, stored at chunk (2 kk + e) ^ (row & 7) by the 128-byte swizzle
+      uint32_t qh[16], ql[16];
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = rl0 + 8 * h;
+            const uint8_t* p = smem + OFF_Q + wg * TILE + r * 128 + (((2 * kk + e) ^ (r & 7)) << 4) + qd * 4;
+            qh[4 * kk + 2 * e + h] = *reinterpret_cast<const uint32_t*>(p);
+            ql[4 * kk + 2 * e + h] = *reinterpret_cast<const uint32_t*>(p + 2 * TILE);
+          }
+      mbar_arrive(&q_empty);
+
+      float o_acc[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
+      float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+      uint32_t p_a[2][16], p_b[2][16];               // P'' hi / lo A fragments of two tiles, laid out like qh / ql
+      float alpha[2];
+
+      auto wait_full = [&](uint32_t t) { mbar_wait(&full[t % STAGES], (t / STAGES) & 1); };
+      auto issue_s = [&](uint32_t t) {               // S = Q . K^T of running tile t
+        const uint32_t kv = sb + OFF_KV + (t % STAGES) * 4 * TILE;
+        const uint64_t dk_hi = desc_sw128(kv), dk_lo = desc_sw128(kv + TILE);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {             // 16 of the 64 head dims per MMA
+          const uint64_t adv = (uint64_t)(kk * 2);
+          wgmma_f16_n64_ra<0>(sv, ql + 4 * kk, dk_hi + adv, kk != 0);
+          wgmma_f16_n64_ra<0>(sv, qh + 4 * kk, dk_lo + adv, 1);
+          wgmma_f16_n64_ra<0>(sv, qh + 4 * kk, dk_hi + adv, 1);
+        }
+      };
+      auto issue_pv = [&](const uint32_t (&p)[2][16], uint32_t t) {    // O += P''_t . V_t
+        const uint32_t vh = sb + OFF_KV + (t % STAGES) * 4 * TILE + 2 * TILE, vl = vh + TILE;
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {             // 16 keys per MMA: 16 rows of the MN-major V tile = 2 KiB
+          const uint64_t dvh = desc_sw128(vh + kk * 2048), dvl = desc_sw128(vl + kk * 2048);
+          wgmma_f16_n64_ra<1>(o_acc, p[1] + 4 * kk, dvh, 1);
+          wgmma_f16_n64_ra<1>(o_acc, p[0] + 4 * kk, dvl, 1);
+          wgmma_f16_n64_ra<1>(o_acc, p[0] + 4 * kk, dvh, 1);
+        }
+      };
+      // online softmax of S (running tile t) into alpha, m_run, l_run and the P'' fragments p: a row's 64 keys sit in the
+      // 4 lanes of a quad (16 each).  O *= alpha is left to the caller, once the P.V wgmmas of the tile before retired.
+      auto softmax = [&](uint32_t (&p)[2][16], uint32_t t) {
+        float nm[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float mx = -INFINITY;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sv[4 * jj + 2 * h], sv[4 * jj + 2 * h + 1]));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          const float m_new = fmaxf(m_run[h], mx);
+          alpha[h] = ex2_fast((m_run[h] - m_new) * a.scale_log2);
+          m_run[h] = m_new;
+          nm[h] = -m_new;
+        }
+        const float* vi = reinterpret_cast<const float*>(smem + OFF_VI + (t % STAGES) * KT * 4);
+        float ps[2] = {0.f, 0.f};
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const float2 w = *reinterpret_cast<const float2*>(vi + 8 * jj + 2 * qd);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float e0 = ex2_fast((sv[4 * jj + 2 * h] + nm[h]) * a.scale_log2);      // the row maximum maps to exactly 1
+            const float e1 = ex2_fast((sv[4 * jj + 2 * h + 1] + nm[h]) * a.scale_log2);
+            ps[h] += e0 + e1;
+            // keys 8 jj + 2 qd (+1) of row rl0 + 8 h: word 2 (jj & 1) + h of k-step jj / 2
+            const int wd = 4 * (jj >> 1) + 2 * (jj & 1) + h;
+            split2u(e0 * (w.x * p_scale), e1 * (w.y * p_scale), p[0][wd], p[1][wd]);
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) l_run[h] = fmaf(l_run[h], alpha[h], ps[h]);     // partial row sum over this lane's keys
+      };
+      auto rescale = [&]() {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) { o_acc[4 * jj + 2 * h] *= alpha[h]; o_acc[4 * jj + 2 * h + 1] *= alpha[h]; }
+      };
+      // tile j, its P'' in p: issue S_{j+1} (if `next`) and P''_j . V_j, run the softmax of S_{j+1} into pn while
+      // P''_j . V_j is in flight, then retire both and free tile j's stage.  Nothing is in flight between two steps.
+      auto step = [&](const uint32_t (&p)[2][16], uint32_t (&pn)[2][16], int j, bool next) {
+        const uint32_t t = it + j;
+        if (next) wait_full(t + 1);
+        reg_fence(sv);
+        reg_fence(o_acc);
+        wg_fence();
+        if (next) {
+          issue_s(t + 1);
+          wg_commit();
+        }
+        issue_pv(p, t);
+        wg_commit();
+        if (next) {
+          wg_wait<1>();
+          reg_fence(sv);
+          softmax(pn, t + 1);
+        }
+        wg_wait<0>();
+        reg_fence(o_acc);
+        release(t);
+        if (next) rescale();
+      };
+
+      wait_full(it);
+      reg_fence(sv);
+      wg_fence();
+      issue_s(it);
       wg_commit();
       wg_wait<0>();
-    }
-    // online softmax over this tile: a row's 64 keys sit in the 4 lanes of a quad (16 each)
-    float alpha[2], nm[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sv[4 * jj + 2 * h], sv[4 * jj + 2 * h + 1]));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      const float m_new = fmaxf(m_run[h], mx);
-      alpha[h] = ex2_fast((m_run[h] - m_new) * a.scale_log2);
-      m_run[h] = m_new;
-      nm[h] = -m_new;
-    }
-    const float* vi = vinv_h + j * KT;
-    float ps[2] = {0.f, 0.f};
-#pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-      const int key = 8 * jj + 2 * qd;
-      const float2 w = __ldg(reinterpret_cast<const float2*>(vi + key));
+      reg_fence(sv);
+      softmax(p_a, it);
+      rescale();
+      int j = 0;
+      for (; j + 2 < ntiles; j += 2) {               // ntiles is even (N % 128 == 0)
+        step(p_a, p_b, j, true);
+        step(p_b, p_a, j + 1, true);
+      }
+      step(p_a, p_b, j, true);
+      step(p_b, p_a, j + 1, false);
+      it += ntiles;
+
+      // total row sum over the quad; 2^-ep undoes the P'' scale
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const float e0 = ex2_fast((sv[4 * jj + 2 * h] + nm[h]) * a.scale_log2);      // the row maximum maps to exactly 1
-        const float e1 = ex2_fast((sv[4 * jj + 2 * h + 1] + nm[h]) * a.scale_log2);
-        ps[h] += e0 + e1;
-        uint32_t hw, lw;
-        split2u(e0 * (w.x * p_scale), e1 * (w.y * p_scale), hw, lw);
-        const int r = rl0 + 8 * h;
-        const uint32_t off = (uint32_t)r * 128u + (uint32_t)((jj ^ (r & 7)) << 4) + (uint32_t)(qd * 4);
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(p_hi + off), "r"(hw) : "memory");
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(p_lo + off), "r"(lw) : "memory");
+        float l = l_run[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = p_inv / l;
+        const size_t ooff = (size_t)(row_q0 + wg * 64 + rl0 + 8 * h) * a.ldo + col0 + 2 * qd;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const float2 ov = make_float2(o_acc[4 * jj + 2 * h] * inv, o_acc[4 * jj + 2 * h + 1] * inv);
+          if (a.o_hi != nullptr) store_split2(a.o_hi, a.o_lo, ooff + 8 * jj, ov);
+          else *reinterpret_cast<float2*>(a.o + ooff + 8 * jj) = ov;
+        }
       }
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      l_run[h] = fmaf(l_run[h], alpha[h], ps[h]);  // partial row sum over this lane's keys
-#pragma unroll
-      for (int jj = 0; jj < 8; ++jj) { o_acc[4 * jj + 2 * h] *= alpha[h]; o_acc[4 * jj + 2 * h + 1] *= alpha[h]; }
-    }
-    fence_async_smem();
-    wg_bar(1 + wg);
-    {
-      const uint32_t vh = kv + 2 * TILE, vl = kv + 3 * TILE;
-      wg_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {             // 16 keys per MMA: 16 rows of the MN-major V tile = 2 KiB
-        const uint64_t adv = (uint64_t)(kk * 2);
-        const uint64_t dvh = desc_sw128(vh + kk * 2048), dvl = desc_sw128(vl + kk * 2048);
-        wgmma_f16_n64_tb(o_acc, dp_lo + adv, dvh, 1);
-        wgmma_f16_n64_tb(o_acc, dp_hi + adv, dvl, 1);
-        wgmma_f16_n64_tb(o_acc, dp_hi + adv, dvh, 1);
-      }
-      wg_commit();
-      wg_wait<0>();
-    }
-    __syncthreads();                               // both warpgroups are done with K / V stage s and their P tiles
-    if (tid == 0 && j + 2 < ntiles) issue_kv(j + 2);
-  }
-  // total row sum over the quad; 2^-ep undoes the P'' scale
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    float l = l_run[h];
-    l += __shfl_xor_sync(0xffffffffu, l, 1);
-    l += __shfl_xor_sync(0xffffffffu, l, 2);
-    const float inv = p_inv / l;
-    const size_t ooff = (size_t)(row_q0 + wg * 64 + rl0 + 8 * h) * a.ldo + col0 + 2 * qd;
-#pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
-      const float2 ov = make_float2(o_acc[4 * jj + 2 * h] * inv, o_acc[4 * jj + 2 * h + 1] * inv);
-      if (a.o_hi != nullptr) store_split2(a.o_hi, a.o_lo, ooff + 8 * jj, ov);
-      else *reinterpret_cast<float2*>(a.o + ooff + 8 * jj) = ov;
     }
   }
 }
@@ -248,6 +343,8 @@ extern "C" int omt_attn_spatial_h(const uint16_t* q_hi, const uint16_t* q_lo, in
   OMT_REQUIRE(heads > 0 && heads <= 65535 && n_seq <= 65535 && qk_plane_scale > 0.f, "omt_attn_spatial_h: bad arguments");
   if (n_seq == 0) return OMT_OK;
   const long long rows = (long long)n_seq * N;
+  const long long items = rows / QT * heads;
+  OMT_REQUIRE(rows < (1LL << 31) && items < (1LL << 31), "omt_attn_spatial_h: n_seq * N = %lld rows is too many", rows);
   CUtensorMap tmQh, tmQl, tmKh, tmKl, tmVh, tmVl;
   int rc;
   if ((rc = encode2d(&tmQh, q_hi, heads * D, rows, ldq))) return rc;
@@ -256,15 +353,20 @@ extern "C" int omt_attn_spatial_h(const uint16_t* q_hi, const uint16_t* q_lo, in
   if ((rc = encode2d(&tmKl, k_lo, heads * D, rows, ldk))) return rc;
   if ((rc = encode2d(&tmVh, v_hi, heads * D, rows, ldv))) return rc;
   if ((rc = encode2d(&tmVl, v_lo, heads * D, rows, ldv))) return rc;
-  static bool attr[64];
+  static int resident[64];     // CTAs of the kernel resident at once, per device (0: not queried yet)
   int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr[dev]) {
+  OMT_CUDA(cudaGetDevice(&dev));
+  OMT_REQUIRE(dev >= 0 && dev < 64, "omt_attn_spatial_h: device ordinal %d out of range", dev);
+  if (resident[dev] == 0) {
     OMT_CUDA(cudaFuncSetAttribute(attn_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attr[dev] = true;
+    int per_sm = 0, sms = 0;
+    OMT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attn_f16_kernel, THREADS, SMEM));
+    OMT_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    OMT_REQUIRE(per_sm > 0, "omt_attn_spatial_h: no CTA fits on an SM of device %d", dev);
+    resident[dev] = per_sm * sms;
   }
-  Args a{vinv, rows, o, o_hi, o_lo, ldo, N, scale * 1.4426950408889634f / qk_plane_scale};
-  dim3 grid(N / QT, heads, n_seq);
+  Args a{vinv, rows, o, o_hi, o_lo, ldo, N, heads, (int)items, scale * 1.4426950408889634f / qk_plane_scale};
+  const dim3 grid(items < resident[dev] ? (int)items : resident[dev]);
   OMT_CUDA(launch_k(attn_f16_kernel, grid, dim3(THREADS), SMEM, (cudaStream_t)stream, tmQh, tmQl, tmKh, tmKl, tmVh, tmVl, a));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
