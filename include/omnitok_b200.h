@@ -181,8 +181,11 @@ int omt_pre_vq(const float* x, int ldx, const float* Wt, const float* b, float* 
 
 /* Codebook.forward nearest-neighbour search (modules/codebook.py:82-86), cd == 8:
  * d[n,k] = (sum z^2 - 2 z.E_k) + sum E_k^2 in that association, idx = first argmin.
- * e2: [n_codes] precomputed sum E^2; n_codes % 32 == 0.  Also accumulates counts[n_codes] (int32, caller zeroes) --
- * the fixed-size replacement of torch.unique (:65).  One launch, no workspace. */
+ * e2: [n_codes] precomputed sum E^2; n_codes % 64 == 0 and n_codes <= 41856 (an eighth of the table, 36 B per code,
+ * and the z rows of a 512-row block share 200 KB of shared memory; launches of few rows take 256-row blocks and accept
+ * up to 43648).  Pad a smaller table with zero rows whose e2 is +inf: they never win.  Also accumulates
+ * counts[n_codes] (int32, caller zeroes) -- the fixed-size replacement of torch.unique (:65).  counts may be NULL.
+ * One launch, no workspace. */
 int omt_vq_search(const float* z, const float* E, const float* e2, int M, int n_codes,
                   int64_t* idx, int32_t* counts, omt_stream_t stream);
 

@@ -76,6 +76,13 @@ constexpr int VQF_SLICES = 8;                 // cluster size = codebook slices
 constexpr int VQF_THREADS = 128;
 constexpr int VQF_GROUP = 8;                  // codes per minimum group
 
+// bytes of the first shared-memory region: the table slice (36 B / code), or the projection weights of phase A if those
+// are larger (small codebooks); the z table starts right after it
+__host__ __device__ __forceinline__ size_t vq_region0_bytes(int per, bool project, int C) {
+  const size_t table = (size_t)per * 36, weights = project ? (size_t)32 * C : 0;
+  return table > weights ? table : weights;
+}
+
 // distance of one row (2 z in z2[], sum z^2 in zz) to one code: the exact instruction sequence both passes share
 __device__ __forceinline__ float vq_dist(const float (&z2)[8], float zz, const float4 ea, const float4 eb, float ek) {
   float dot = __fmul_rn(z2[0], ea.x);
@@ -97,7 +104,7 @@ vq_fused_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ 
   float4* esm = reinterpret_cast<float4*>(vq_smem);                          // [per][2] float4: this slice of the table
   float* e2s = reinterpret_cast<float*>(esm + 2 * per);                      // [per]
   float4* wsm = reinterpret_cast<float4*>(vq_smem);                          // PROJECT, phase A only: [8][C/4] weights
-  float4* zsm = reinterpret_cast<float4*>(vq_smem + (size_t)per * 36);       // [ROWS][2] float4: the block's z rows
+  float4* zsm = reinterpret_cast<float4*>(vq_smem + vq_region0_bytes(per, PROJECT, C));   // [ROWS][2] float4: the block's z rows
   float2* part = reinterpret_cast<float2*>(zsm);                             // phase C: [8 slices][OWN] (distance, index bits)
   const uint32_t rank = ptx::cluster_ctarank();
   const int row0 = (blockIdx.x / VQF_SLICES) * ROWS;
@@ -342,9 +349,9 @@ template <bool PROJECT, int R>
 static int vq_launch_r(const float* x, int ldx, const float* Wt, const float* b, int C, int l2, const float* z_in, float* z_out,
                        const float* E, const float* e2, int M, int n_codes, int64_t* idx, int32_t* counts, cudaStream_t st) {
   const int per = n_codes / VQF_SLICES;
-  const size_t smem = (size_t)per * 36 + (size_t)R * VQF_THREADS * 32;
-  OMT_REQUIRE(smem <= 200 * 1024, "omt_vq: n_codes=%d too large for the shared-memory table slice", n_codes);
-  OMT_REQUIRE(!PROJECT || (size_t)8 * C * 4 <= (size_t)per * 36, "omt_vq_fused: C=%d too large for n_codes=%d", C, n_codes);
+  const size_t smem = vq_region0_bytes(per, PROJECT, C) + (size_t)R * VQF_THREADS * 32;
+  OMT_REQUIRE(smem <= 200 * 1024, "omt_vq: n_codes=%d too large for the shared-memory table slice (C=%d, %d rows per thread)",
+              n_codes, C, R);
   static size_t set[64];
   int dev = 0;
   cudaGetDevice(&dev);
@@ -363,7 +370,7 @@ static int vq_launch_r(const float* x, int ldx, const float* Wt, const float* b,
 static int vq_launch(bool project, const float* x, int ldx, const float* Wt, const float* b, int C, int l2, const float* z_in,
                      float* z_out, const float* E, const float* e2, int M, int n_codes, int64_t* idx, int32_t* counts,
                      cudaStream_t st) {
-  OMT_REQUIRE(n_codes % (VQF_SLICES * VQF_GROUP) == 0 && n_codes >= VQF_SLICES * VQF_GROUP, "omt_vq: n_codes %% 64 != 0");
+  OMT_REQUIRE(n_codes % (VQF_SLICES * VQF_GROUP) == 0 && n_codes >= VQF_SLICES * VQF_GROUP, "omt_vq: n_codes=%d is not a positive multiple of 64", n_codes);
   // 4 rows per thread amortise the table reads best; small inputs take 2 so that more SMs get a cluster
   const bool small = (M + 4 * VQF_THREADS - 1) / (4 * VQF_THREADS) * VQF_SLICES < omt::sm_count();
   if (project)

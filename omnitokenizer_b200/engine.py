@@ -23,6 +23,10 @@ from . import layout as L
 
 MATH_MODES = {"fp32": _cabi.MATH_FP32, "3xtf32": _cabi.MATH_3XTF32, "f16x3": _cabi.MATH_F16X3}
 DEFAULT_MATH = "f16x3"
+# largest codebook of the VQ search kernel (csrc/vq.cu): an eighth of the table (36 B per code) and the z rows of a 512-row
+# block (16 KB) share 200 KB of shared memory.  Launches of few rows take 256-row blocks and would fit 43 648 codes, but a
+# codebook must not work for small batches and fail for large ones.
+VQ_MAX_CODES = 41856
 
 
 def default_math() -> str:
@@ -247,11 +251,20 @@ class Engine:
                        "rest": lin("decoder.to_pixels.0", row_scaled=True)}
         self.pre_w, self.pre_b = f32(sd["pre_vq_conv.1.weight"]), f32(sd["pre_vq_conv.1.bias"])
         self.post_w, self.post_b = f32(sd["post_vq_conv.1.weight"]), f32(sd["post_vq_conv.1.bias"])
-        E = sd["codebook.embeddings"].detach().float()
-        self.E = E.to(dev).contiguous()
-        # sum E^2 with the reference's own expression (modules/codebook.py:84), evaluated on the host
-        self.e2 = (E.cpu().t() ** 2).sum(dim=0).to(dev).contiguous()
+        E = sd["codebook.embeddings"].detach().float().cpu()
         self.n_codes = E.shape[0]
+        # the search kernel takes whole groups of 8 codes in each of its 8 slices: zero rows pad the table to a multiple
+        # of 64, and their sum E^2 of +inf makes every distance to them +inf, so they never win and the first-minimum
+        # rule over the real codes is unchanged
+        self.n_codes_padded = L.round_up(self.n_codes, 64)
+        if not self.use_vae and self.n_codes_padded > VQ_MAX_CODES:
+            raise NotImplementedError(f"--n_codes {self.n_codes}: the VQ search kernel holds an eighth of the codebook in "
+                                      f"shared memory and takes at most {VQ_MAX_CODES} codes")
+        # sum E^2 with the reference's own expression (modules/codebook.py:84), evaluated on the host
+        e2 = (E.t() ** 2).sum(dim=0)
+        pad = self.n_codes_padded - self.n_codes
+        self.E = torch.cat([E, E.new_zeros(pad, E.shape[1])]).to(dev).contiguous()
+        self.e2 = torch.cat([e2, e2.new_full((pad,), math.inf)]).to(dev).contiguous()
 
     # ------------------------------------------------------------------ helpers
     @staticmethod
@@ -472,7 +485,7 @@ class Engine:
         if mode == "vq":      # pre_vq + l2norm + modules/codebook.py:82-86 in one cluster kernel
             ws.counts.zero_()
             _cabi.call("omt_vq_fused", ws.X, C, self.pre_w, self.pre_b, C, int(self.l2), z, self.E, self.e2, ws.M,
-                       self.n_codes, ws.idx, ws.counts)
+                       self.n_codes_padded, ws.idx, ws.counts)
         else:
             _cabi.call("omt_pre_vq", ws.X, C, self.pre_w, self.pre_b, z, ws.M, C, cd, 0)
 
