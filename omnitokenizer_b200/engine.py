@@ -27,6 +27,9 @@ DEFAULT_MATH = "f16x3"
 # block (16 KB) share 200 KB of shared memory.  Launches of few rows take 256-row blocks and would fit 43 648 codes, but a
 # codebook must not work for small batches and fail for large ones.
 VQ_MAX_CODES = 41856
+# longest latent sequence of the temporal attention core (csrc/attention_fp32.cu attn_temporal_kernel keeps the K / V of
+# one pixel's T' frames in registers, one template instance per T'): 17 latent frames, 65 frames at temporal patch 4
+TEMPORAL_MAX_FRAMES = 17
 
 
 def default_math() -> str:
@@ -426,7 +429,16 @@ class Engine:
                              f"{self.ws}, grid {H // self.p}x{W // self.p}): omt_attn_window is specialised for 8x8 windows")
         if ((H // self.p) * (W // self.p)) % 64 != 0:
             raise ValueError(f"tokens per frame ({(H // self.p) * (W // self.p)}) must be a multiple of 64 (attention tiles)")
-        return B, T, H, W, 1 + (T - 1) // self.pt, H // self.p, W // self.p
+        Tp = 1 + (T - 1) // self.pt
+        self._check_latent_frames(Tp)
+        return B, T, H, W, Tp, H // self.p, W // self.p
+
+    def _check_latent_frames(self, Tp):
+        """Reject what the temporal attention core cannot run before the first launch, not in the middle of a pass."""
+        if Tp > TEMPORAL_MAX_FRAMES and self.enc_temporal["layers"]:
+            raise NotImplementedError(f"{Tp} latent frames: the temporal attention kernel takes at most "
+                                      f"{TEMPORAL_MAX_FRAMES} latent frames ({1 + (TEMPORAL_MAX_FRAMES - 1) * self.pt} "
+                                      f"frames)")
 
     @staticmethod
     def graphs_enabled() -> bool:
@@ -589,6 +601,7 @@ class Engine:
         Returns a fresh (B,C,T,H,W) tensor (the reference's decoder ends in .clone(), omnitokenizer.py:1116);
         with u8 = (mul, add, lo, hi, post) a fresh uint8 (B,T,H,W,C) tensor (fused consumer conversion)."""
         B, Tp, h, w = dims
+        self._check_latent_frames(Tp)
         ws = self._workspace(B * Tp * h * w)
         vshape = (B, self.cin, 1 + (Tp - 1) * self.pt, h * self.p, w * self.p)
         if ws.video is None or tuple(ws.video.shape) != vshape:
