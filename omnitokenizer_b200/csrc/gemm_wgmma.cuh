@@ -27,7 +27,8 @@
 //     epilogue together.
 // Both issue the same products in the same k order for every output element, so they give the same bits.
 // The epilogue works on the accumulator fragments in place: a row's 64-column head is spread over the 4 lanes of a quad,
-// so the l2 norm and the v-plane maximum are two-step shuffles.
+// so the l2 norm and the v-plane maximum are two-step shuffles.  The f16 GEGLU epilogue, whose fragments hold only 8 bytes
+// of a U-plane row per quad, stages each 64-row half of its U planes in shared memory and stores whole 128-byte rows.
 #pragma once
 #include "omt_common.cuh"
 #include "tc_ptx.cuh"
@@ -42,7 +43,12 @@ constexpr int THREADS = 384;                  // warpgroup 0: producer; 1, 2: co
 constexpr int ORDER_BAR = 3;                  // ping-pong: named barriers 3, 4 ("consumer 0 / 1 may issue"); 1, 2 are wg_bar
 constexpr int STAGE_BYTES = 4 * 16384;        // A (hi), A_lo, W_hi, W_lo: 128 rows x 128 bytes each
 constexpr int STAGES = 3;
-constexpr int SMEM = STAGES * STAGE_BYTES + 1024;
+// f16 GEGLU epilogue: per consumer warpgroup, the U planes of one 64-row half of a tile (64 rows x 64 columns x 2 planes)
+// staged in shared memory so that they leave as whole 128-byte rows.  Only those instantiations reserve it: the others
+// keep the larger L1 for their epilogue's loads.
+constexpr int EPI_STAGE_BYTES = 2 * 64 * 128;
+template <bool TF32, int EPI>
+constexpr int smem_bytes() { return STAGES * STAGE_BYTES + (!TF32 && EPI == OMT_EPI_GEGLU ? 2 * EPI_STAGE_BYTES : 0) + 1024; }
 // __launch_bounds__(384, 1) caps the kernel at 168 registers a thread: 40 * 128 + 232 * 256 == 168 * 384
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
@@ -66,9 +72,10 @@ struct Args {
 };
 
 // Epilogue of one 64-row half of a tile on a consumer warpgroup's fragments (rows [m0 + 64 half, +64), columns [n0, +128)).
+// `stage` is the warpgroup's EPI_STAGE_BYTES of shared memory, `bar` its named barrier.
 template <bool TF32, int NACC, int EPI>
 __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 2], const float (&crs)[NACC == 2 ? BN / 2 : 1],
-                                         int m0, int n0, bool second, int half, int warp, int lane) {
+                                         int m0, int n0, bool second, int half, int warp, int lane, uint8_t* stage, int bar) {
   const int qd = lane & 3;                      // column pair 8 j + 2 qd inside every 8-column block
   int mrow[2];
   mrow[0] = m0 + half * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -165,7 +172,10 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
     }
   } else if constexpr (EPI == OMT_EPI_GEGLU) {
     // packed columns (2i, 2i+1) = (value_i, gate_i): U[:, i] = gelu_erf(gate) * value; lanes qd and qd ^ 1 hold neighbouring
-    // outputs, so the even lane stores both
+    // outputs, so the even lane takes both.  f16: the 64 x 64 U values of the half go to the planes in `stage` (row r at
+    // r * 128 bytes, its 16-byte chunk c at chunk c ^ (r & 7): the 8 rows of a store land in 8 different bank groups),
+    // then every thread of the warpgroup copies whole 16-byte chunks out, 8 threads per 128-byte row.
+    if (!TF32) wg_bar(bar);                     // the previous half's copy-out has read the stage
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int m = mrow[h];
@@ -177,17 +187,33 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
         if (g.bias != nullptr && n < g.N) { val += __ldg(g.bias + n); gate += __ldg(g.bias + n + 1); }
         const float o = gelu_erf(gate) * val;
         const float o1 = __shfl_xor_sync(0xffffffffu, o, 1);
-        if ((qd & 1) == 0 && m < g.M && n < g.N) {
-          if (TF32) {
-            *reinterpret_cast<float2*>(g.c + prow * g.ldc + (n >> 1)) = make_float2(o, o1);
-          } else {
-            uint32_t hw, lw;
-            if (g.u_scale > 0.f) split2u(o * g.u_scale, o1 * g.u_scale, hw, lw);
-            else split2(o, o1, hw, lw);
-            const size_t off = (size_t)prow * g.ldu + (n >> 1);
-            *reinterpret_cast<uint32_t*>(g.u_hi + off) = hw;
-            *reinterpret_cast<uint32_t*>(g.u_lo + off) = lw;
-          }
+        if (TF32 && (qd & 1) == 0 && m < g.M && n < g.N) {
+          *reinterpret_cast<float2*>(g.c + prow * g.ldc + (n >> 1)) = make_float2(o, o1);
+        } else if (!TF32 && (qd & 1) == 0) {
+          uint32_t hw, lw;
+          if (g.u_scale > 0.f) split2u(o * g.u_scale, o1 * g.u_scale, hw, lw);
+          else split2(o, o1, hw, lw);
+          const int r = (warp & 3) * 16 + (lane >> 2) + 8 * h;
+          const int b = 8 * j + 2 * qd;             // byte of U column (8 j + 2 qd) / 2 in the row
+          const int off = r * 128 + ((((b >> 4) ^ (r & 7)) << 4) | (b & 15));
+          *reinterpret_cast<uint32_t*>(stage + off) = hw;
+          *reinterpret_cast<uint32_t*>(stage + 64 * 128 + off) = lw;
+        }
+      }
+    }
+    if (!TF32) {
+      wg_bar(bar);
+      const int t = (warp & 3) * 32 + lane;
+      const int uc = n0 >> 1;                   // first U column of the tile
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int r = (t >> 3) + 16 * i, c = t & 7;
+        const int m = m0 + half * 64 + r;
+        if (m < g.M && 2 * (uc + 8 * c) < g.N) {   // N % 32 == 0: a 16-byte chunk is wholly inside or outside
+          const size_t off = (size_t)map_row(m, g.c_seg, g.c_seg_stride, g.c_seg_off) * g.ldu + uc + 8 * c;
+          const int so = r * 128 + ((c ^ (r & 7)) << 4);
+          *reinterpret_cast<uint4*>(g.u_hi + off) = *reinterpret_cast<const uint4*>(stage + so);
+          *reinterpret_cast<uint4*>(g.u_lo + off) = *reinterpret_cast<const uint4*>(stage + 64 * 128 + so);
         }
       }
     }
@@ -373,7 +399,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (PINGPONG) it += num_kb;               // the k-blocks of the other warpgroup's tile
 #pragma unroll
       for (int h = 0; h < HALVES; ++h)
-        epilogue<TF32, NACC, EPI>(g, acc[h], crs, m0, n0, second, PINGPONG ? h : wg, warp, lane);
+        epilogue<TF32, NACC, EPI>(g, acc[h], crs, m0, n0, second, PINGPONG ? h : wg, warp, lane,
+                                  smem + STAGES * STAGE_BYTES + wg * EPI_STAGE_BYTES, 1 + wg);
     }
   }
 }
@@ -424,6 +451,7 @@ static inline int w_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const
 template <bool TF32, int NACC, int EPI>
 static int launch(const CUtensorMap* maps, const Args& g, cudaStream_t st) {
   auto kern = gemm_wgmma_kernel<TF32, NACC, EPI>;
+  constexpr int SMEM = smem_bytes<TF32, EPI>();
   static int resident[64];     // CTAs of this kernel resident at once, per device (0: not queried yet)
   int dev = 0;
   OMT_CUDA(cudaGetDevice(&dev));
