@@ -138,6 +138,18 @@ int omt_peg(const float* x, float* y, const float* w27, const float* bias, const
 int omt_peg_volume(const float* x, float* y, const float* w27, const float* bias, int B, int T, int h, int w,
                    int C, int temporal, int causal, omt_stream_t stream);
 
+/* Packed batch ("varlen"): samples of different lengths in one canonical buffer, every sample on the same h x w grid.
+ * Sample b owns latent frames [t_off[b], t_off[b+1]) = canonical rows [t_off[b]*N, t_off[b+1]*N), N = h*w, and has
+ * T'_b = t_off[b+1] - t_off[b] frames.  t_off: int32 [B+1] in DEVICE memory (read by the kernel); t_off_host: the same
+ * B+1 values in HOST memory, checked before the launch (t_off[0] == 0, every T'_b in 1..17, t_off[B]*N == M rows) and
+ * used to size the grid.  Each sample's output equals the uniform entry point's on that sample alone, bit for bit.
+ *
+ * omt_peg_volume over a packed batch, in ONE launch: zero padding at each sample's own edges (no tile reads a
+ * neighbour's rows); in the temporal volume the '(b h w) t d' reshape is taken per sample with its own T'_b. */
+int omt_peg_volume_varlen(const float* x, float* y, const float* w27, const float* bias, const int32_t* t_off_host,
+                          const int32_t* t_off, int B, int M, int h, int w, int C, int temporal, int causal,
+                          omt_stream_t stream);
+
 /* In-place rope + l2norm + per-dim scale on q and k (attention.py:417-421, :435-437).
  * q[M, heads*64] (ld ldq), k likewise; cos/sin [N, 32] or NULL (no rope; temporal blocks);
  * the rope position of row r is r % N. */
@@ -173,6 +185,14 @@ int omt_attn_window(const float* q, int ldq, const float* k, int ldk, const floa
 int omt_attn_temporal(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
                       float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo, int B, int T, int N, int heads, float scale, int causal,
                       omt_stream_t stream);
+
+/* omt_attn_temporal over a packed batch (t_off_host / t_off / M as for omt_peg_volume_varlen), in ONE launch: pixel n of
+ * sample b attends over the rows (t_off[b] + t)*N + n, t < T'_b.  The kernel is instantiated for the longest sample
+ * and skips every step past T'_b, so each output goes through the same operations as the <T'_b> instance. */
+int omt_attn_temporal_varlen(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                             float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo, const int32_t* t_off_host,
+                             const int32_t* t_off, int B, int M, int N, int heads, float scale, int causal,
+                             omt_stream_t stream);
 
 /* pre_vq_conv (omnitokenizer.py:144-154) [+ F.normalize(dim=channels) :251-252]:
  * z[M, cd] = x[M, C] . Wt^T + b, cd in {8, 16}; l2 != 0 divides each row by max(||z||, 1e-12). */

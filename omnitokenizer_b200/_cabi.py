@@ -58,6 +58,7 @@ SIGNATURES = {
     "omt_unpatchify_u8": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float] * 5 + [c_void_p]),
     "omt_peg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "omt_peg_volume": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 7 + [c_void_p]),
+    "omt_peg_volume_varlen": (c_int, [c_void_p] * 6 + [c_int] * 7 + [c_void_p]),
     "omt_qk_prep": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                             c_int, c_void_p]),
     "omt_attn_spatial": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
@@ -68,6 +69,8 @@ SIGNATURES = {
                                 c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "omt_attn_temporal": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                   c_int, c_int, c_int, c_int, c_float, c_int, c_void_p]),
+    "omt_attn_temporal_varlen": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                         c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p]),
     "omt_pre_vq": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "omt_vq_search": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "omt_vq_fused": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,

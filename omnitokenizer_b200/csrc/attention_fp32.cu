@@ -177,14 +177,17 @@ __global__ void __launch_bounds__(256, 2) attn_flash_kernel(const AttnArgs a) {
 }
 
 // Temporal attention: one warp per (b, n, head); lane l owns dims (2l, 2l+1); K/V of the
-// whole (short) sequence stay in registers.
-template <int T>
+// whole (short) sequence stay in registers.  VARLEN (packed batch, t_off = the layout table): sample b has its own
+// Tb = t_off[b+1] - t_off[b] <= T frames from row t_off[b] * N on; every step past Tb is skipped, so an output of a
+// Tb-frame sample goes through the same operations, in the same order, as in the <Tb> instance.
+template <int T, bool VARLEN>
 __global__ void __launch_bounds__(256) attn_temporal_kernel(const float* __restrict__ q, int ldq,
                                                             const float* __restrict__ k, int ldk,
                                                             const float* __restrict__ v, int ldv,
                                                             float* __restrict__ o, uint16_t* __restrict__ o_hi,
                                                             uint16_t* __restrict__ o_lo, int ldo, int B,
-                                                            int N, int heads, float scale, int causal) {
+                                                            int N, int heads, float scale, int causal,
+                                                            const int32_t* __restrict__ t_off) {
   pdl_sync();
   const int lane = threadIdx.x & 31;
   const long long wid = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -195,35 +198,46 @@ __global__ void __launch_bounds__(256) attn_temporal_kernel(const float* __restr
   const int n = (int)(bn % N);
   const int b = (int)(bn / N);
   const size_t col = (size_t)head * 64 + 2 * lane;
+  const size_t f0 = VARLEN ? (size_t)t_off[b] : (size_t)b * T;       // first latent frame of the sample
+  const int Tb = VARLEN ? t_off[b + 1] - t_off[b] : T;
   float2 kr[T], vr[T], qr[T];           // all 3 T loads of the sequence are in flight before the first use
 #pragma unroll
   for (int t = 0; t < T; ++t) {
-    const size_t row = ((size_t)b * T + t) * N + n;
+    if (VARLEN && t >= Tb) break;
+    const size_t row = (f0 + t) * N + n;
     kr[t] = *reinterpret_cast<const float2*>(k + row * ldk + col);
     vr[t] = *reinterpret_cast<const float2*>(v + row * ldv + col);
     qr[t] = *reinterpret_cast<const float2*>(q + row * ldq + col);
   }
 #pragma unroll
   for (int i = 0; i < T; ++i) {
-    const size_t row = ((size_t)b * T + i) * N + n;
+    if (VARLEN && i >= Tb) break;
+    const size_t row = (f0 + i) * N + n;
     const float2 qv = qr[i];
     float s[T];
 #pragma unroll
-    for (int j = 0; j < T; ++j) s[j] = qv.x * kr[j].x + qv.y * kr[j].y;
+    for (int j = 0; j < T; ++j) {
+      if (VARLEN && j >= Tb) break;
+      s[j] = qv.x * kr[j].x + qv.y * kr[j].y;
+    }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1)
 #pragma unroll
-      for (int j = 0; j < T; ++j) s[j] += __shfl_xor_sync(0xffffffffu, s[j], off);
+      for (int j = 0; j < T; ++j) {
+        if (VARLEN && j >= Tb) break;      // Tb is warp-uniform: the whole warp takes the same shuffles
+        s[j] += __shfl_xor_sync(0xffffffffu, s[j], off);
+      }
     float mx = -INFINITY;
 #pragma unroll
     for (int j = 0; j < T; ++j) {
+      if (VARLEN && j >= Tb) break;
       s[j] *= scale;
       if (!causal || j <= i) mx = fmaxf(mx, s[j]);
     }
     float den = 0.f, ox = 0.f, oy = 0.f;
 #pragma unroll
     for (int j = 0; j < T; ++j) {
-      if (!causal || j <= i) {
+      if ((!causal || j <= i) && (!VARLEN || j < Tb)) {
         const float p = expf(s[j] - mx);
         den += p;
         ox = fmaf(p, vr[j].x, ox);
@@ -239,10 +253,13 @@ __global__ void __launch_bounds__(256) attn_temporal_kernel(const float* __restr
 template <int T>
 static int launch_temporal(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
                            float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo, int B, int N, int heads, float scale, int causal,
-                           cudaStream_t st) {
+                           const int32_t* t_off, cudaStream_t st) {
   const long long warps = (long long)B * N * heads;
   const unsigned blocks = (unsigned)((warps + 7) / 8);
-  OMT_CUDA(launch_k(attn_temporal_kernel<T>, dim3(blocks), dim3(256), 0, st, q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo, B, N, heads, scale, causal));
+  if (t_off != nullptr)
+    OMT_CUDA(launch_k(attn_temporal_kernel<T, true>, dim3(blocks), dim3(256), 0, st, q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo, B, N, heads, scale, causal, t_off));
+  else
+    OMT_CUDA(launch_k(attn_temporal_kernel<T, false>, dim3(blocks), dim3(256), 0, st, q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo, B, N, heads, scale, causal, t_off));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }
@@ -317,16 +334,13 @@ extern "C" int omt_attn_window(const float* q, int ldq, const float* k, int ldk,
   return OMT_OK;
 }
 
-extern "C" int omt_attn_temporal(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
-                                 float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo, int B, int T, int N, int heads,
-                                 float scale, int causal, omt_stream_t stream) {
-  OMT_ENTER();
-  int rc = check_attn_ptrs("omt_attn_temporal", q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo);
-  if (rc) return rc;
-  OMT_REQUIRE(T >= 1 && T <= 17, "omt_attn_temporal: T'=%d unsupported (1..17)", T);
+// T = every sample's T' (t_off == NULL) or the longest sample of a packed batch
+static int attn_temporal_launch(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* o,
+                                uint16_t* o_hi, uint16_t* o_lo, int ldo, const int32_t* t_off, int B, int T, int N, int heads,
+                                float scale, int causal, omt_stream_t stream) {
   if ((long long)B * N == 0) return OMT_OK;
   cudaStream_t st = (cudaStream_t)stream;
-#define OMT_T_CASE(t) case t: return launch_temporal<t>(q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo, B, N, heads, scale, causal, st);
+#define OMT_T_CASE(t) case t: return launch_temporal<t>(q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo, B, N, heads, scale, causal, t_off, st);
   switch (T) {
     OMT_T_CASE(1) OMT_T_CASE(2) OMT_T_CASE(3) OMT_T_CASE(4) OMT_T_CASE(5) OMT_T_CASE(6) OMT_T_CASE(7)
     OMT_T_CASE(8) OMT_T_CASE(9) OMT_T_CASE(10) OMT_T_CASE(11) OMT_T_CASE(12) OMT_T_CASE(13) OMT_T_CASE(14)
@@ -334,4 +348,28 @@ extern "C" int omt_attn_temporal(const float* q, int ldq, const float* k, int ld
   }
 #undef OMT_T_CASE
   return OMT_E_ARG;
+}
+
+extern "C" int omt_attn_temporal(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                                 float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo, int B, int T, int N, int heads,
+                                 float scale, int causal, omt_stream_t stream) {
+  OMT_ENTER();
+  int rc = check_attn_ptrs("omt_attn_temporal", q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo);
+  if (rc) return rc;
+  OMT_REQUIRE(T >= 1 && T <= 17, "omt_attn_temporal: T'=%d unsupported (1..17)", T);
+  return attn_temporal_launch(q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo, nullptr, B, T, N, heads, scale, causal, stream);
+}
+
+extern "C" int omt_attn_temporal_varlen(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
+                                        float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo, const int32_t* t_off_host,
+                                        const int32_t* t_off, int B, int M, int N, int heads, float scale, int causal,
+                                        omt_stream_t stream) {
+  OMT_ENTER();
+  int rc = check_attn_ptrs("omt_attn_temporal_varlen", q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo);
+  if (rc) return rc;
+  int t_max = 0;
+  rc = check_t_off("omt_attn_temporal_varlen", t_off_host, t_off, B, M, N, &t_max);
+  if (rc) return rc;
+  return attn_temporal_launch(q, ldq, k, ldk, v, ldv, o, o_hi, o_lo, ldo, t_off, B, t_max < 1 ? 1 : t_max, N, heads, scale,
+                              causal, stream);
 }

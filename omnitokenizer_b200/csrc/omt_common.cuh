@@ -165,6 +165,26 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
 }
 
+// ---- packed batches (include/omnitok_b200.h, "varlen" entry points) ----------------------------------------------------
+// Sample b owns latent frames [t_off[b], t_off[b+1]) and canonical rows [t_off[b] * N, t_off[b+1] * N).  The host copy of
+// the table is checked before any launch: t_off[0] == 0, every sample 1..17 frames long, t_off[B] * N == M rows.
+// *t_max receives the longest sample.
+inline int check_t_off(const char* who, const int32_t* t_off_host, const int32_t* t_off, int B, long long M, long long N,
+                       int* t_max) {
+  OMT_REQUIRE(t_off_host && t_off, "%s: null layout table", who);
+  OMT_REQUIRE(B >= 0 && B <= 65535, "%s: B=%d samples unsupported (0..65535)", who, B);
+  OMT_REQUIRE(t_off_host[0] == 0, "%s: t_off[0]=%d must be 0", who, t_off_host[0]);
+  int mx = 0;
+  for (int b = 0; b < B; ++b) {
+    const int tb = t_off_host[b + 1] - t_off_host[b];
+    OMT_REQUIRE(tb >= 1 && tb <= 17, "%s: sample %d has T'=%d latent frames (t_off must increase by 1..17)", who, b, tb);
+    mx = tb > mx ? tb : mx;
+  }
+  OMT_REQUIRE((long long)t_off_host[B] * N == M, "%s: t_off[B]=%d frames of %lld rows != %lld rows", who, t_off_host[B], N, M);
+  *t_max = mx;
+  return OMT_OK;
+}
+
 // logical GEMM row -> physical row (see include/omnitok_b200.h)
 __host__ __device__ __forceinline__ long long map_row(int r, int seg, int seg_stride, int seg_off) {
   if (seg <= 0) return r;

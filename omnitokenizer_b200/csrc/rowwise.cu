@@ -488,14 +488,21 @@ constexpr int PEG_CC = 16;       // channels per CTA
 __global__ void __launch_bounds__(256) peg_tile_kernel(const float* __restrict__ x, float* __restrict__ y,
                                                        const float* __restrict__ w27,
                                                        const float* __restrict__ bias, int T, int h, int w,
-                                                       int C, int temporal, int causal, int TT, int HB, int RS) {
+                                                       int C, int temporal, int causal, int TT, int HB, int RS,
+                                                       const int32_t* __restrict__ t_off) {
   pdl_sync();
   extern __shared__ __align__(16) float tile[];      // [(TT+2)][(HB+2)] rows of RS floats ((w+2)*16 + pad)
   const int N = h * w;
   const int n_hblk = (h + HB - 1) / HB;
   const int t0 = (blockIdx.x / n_hblk) * TT, h0 = (blockIdx.x % n_hblk) * HB;
   const int c0 = blockIdx.y * PEG_CC;
-  const long long bbase = (long long)blockIdx.z * T * N;
+  long long bbase = (long long)blockIdx.z * T * N;
+  if (t_off != nullptr) {                            // packed batch: this sample's own T' and rows (T = the longest)
+    const int f0 = t_off[blockIdx.z];
+    T = t_off[blockIdx.z + 1] - f0;
+    bbase = (long long)f0 * N;
+    if (t0 >= T) return;
+  }
   const int pad_lo = causal ? 2 : 1;
   const int rows = (TT + 2) * (HB + 2);
   const int nth = blockDim.x;
@@ -611,7 +618,8 @@ __device__ __forceinline__ float2 peg_step(float2 (&win)[9][3], const float2 (&w
 __global__ void __launch_bounds__(160, 3) peg_tile4_kernel(const float* __restrict__ x, float* __restrict__ y,
                                                            const float* __restrict__ w27,
                                                            const float* __restrict__ bias, int T, int h, int w,
-                                                           int C, int temporal, int causal, int TT, int HB, int RS, int zrow) {
+                                                           int C, int temporal, int causal, int TT, int HB, int RS, int zrow,
+                                                           const int32_t* __restrict__ t_off) {
   pdl_sync();
   // [valid planes of the tile][(HB+2)] rows of RS floats ((w+2)*16 + pad), then ONE all-zero row at index zrow: planes
   // outside the volume (the causal pad in front, the halo behind the last plane) are not stored -- every window row that
@@ -621,7 +629,13 @@ __global__ void __launch_bounds__(160, 3) peg_tile4_kernel(const float* __restri
   const int n_hblk = (h + HB - 1) / HB;
   const int t0 = (blockIdx.x / n_hblk) * TT, h0 = (blockIdx.x % n_hblk) * HB;
   const int c0 = blockIdx.y * PEG_CC;
-  const long long bbase = (long long)blockIdx.z * T * N;
+  long long bbase = (long long)blockIdx.z * T * N;
+  if (t_off != nullptr) {                            // packed batch: this sample's own T' and rows (T = the longest)
+    const int f0 = t_off[blockIdx.z];
+    T = t_off[blockIdx.z + 1] - f0;
+    bbase = (long long)f0 * N;
+    if (t0 >= T) return;
+  }
   const int pad_lo = causal ? 2 : 1;
   const int rows = (TT + 2) * (HB + 2);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -964,13 +978,15 @@ extern "C" int omt_peg(const float* x, float* y, const float* w27, const float* 
   return OMT_OK;
 }
 
-extern "C" int omt_peg_volume(const float* x, float* y, const float* w27, const float* bias, int B, int T, int h,
-                              int w, int C, int temporal, int causal, omt_stream_t stream) {
-  OMT_ENTER();
-  OMT_REQUIRE(x && y && w27 && bias, "omt_peg_volume: null pointer");
-  OMT_REQUIRE(x != y, "omt_peg_volume: in-place is not supported (stencil)");
-  OMT_REQUIRE(C % PEG_CC == 0 && C / PEG_CC <= 65535 && B <= 65535, "omt_peg_volume: C=%d must be a multiple of 16", C);
-  OMT_REQUIRE(T >= 1 && h >= 1 && w >= 1, "omt_peg_volume: bad volume");
+// Both PEG entry points: T = every sample's T' (t_off == NULL) or the longest one of a packed batch (t_off = the device table).
+// The tile geometry depends on T only, and a CTA whose planes lie past its sample's end exits at once.
+static int peg_volume_launch(const char* who, const float* x, float* y, const float* w27, const float* bias,
+                             const int32_t* t_off, int B, int T, int h, int w, int C, int temporal, int causal,
+                             omt_stream_t stream) {
+  OMT_REQUIRE(x && y && w27 && bias, "%s: null pointer", who);
+  OMT_REQUIRE(x != y, "%s: in-place is not supported (stencil)", who);
+  OMT_REQUIRE(C % PEG_CC == 0 && C / PEG_CC <= 65535 && B <= 65535, "%s: C=%d must be a multiple of 16", who, C);
+  OMT_REQUIRE(T >= 1 && h >= 1 && w >= 1, "%s: bad volume", who);
   if (B == 0) return OMT_OK;
   // tile geometry: planes per CTA (TT) and rows per CTA (HB) so that threads <= 256 and smem <= ~100 KB
   int RS = (w + 2) * PEG_CC;
@@ -980,7 +996,7 @@ extern "C" int omt_peg_volume(const float* x, float* y, const float* w27, const 
   while (HB > 1 && (smem_of(TT, HB) > 112 * 1024 || TT * HB * 8 > 256)) --HB;
   while (TT > 1 && (smem_of(TT, HB) > 112 * 1024 || TT * HB * 8 > 256)) --TT;
   const size_t smem = smem_of(TT, HB);
-  OMT_REQUIRE(smem <= 200 * 1024, "omt_peg_volume: row of %d tokens does not fit the shared-memory tile", w);
+  OMT_REQUIRE(smem <= 200 * 1024, "%s: row of %d tokens does not fit the shared-memory tile", who, w);
   static size_t smem_set[64];        // per device
   int dev = 0;
   cudaGetDevice(&dev);
@@ -1007,12 +1023,29 @@ extern "C" int omt_peg_volume(const float* x, float* y, const float* w27, const 
       OMT_CUDA(cudaFuncSetAttribute(peg_tile4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4));
       smem4_set[dev] = smem4;
     }
-    OMT_CUDA(launch_k(peg_tile4_kernel, grid, dim3(threads), smem4, (cudaStream_t)stream, x, y, w27, bias, T, h, w, C, temporal, causal, TT, HB, RS, zrow));
+    OMT_CUDA(launch_k(peg_tile4_kernel, grid, dim3(threads), smem4, (cudaStream_t)stream, x, y, w27, bias, T, h, w, C, temporal, causal, TT, HB, RS, zrow, t_off));
   } else {
-    OMT_CUDA(launch_k(peg_tile_kernel, grid, dim3(threads), smem, (cudaStream_t)stream, x, y, w27, bias, T, h, w, C, temporal, causal, TT, HB, RS));
+    OMT_CUDA(launch_k(peg_tile_kernel, grid, dim3(threads), smem, (cudaStream_t)stream, x, y, w27, bias, T, h, w, C, temporal, causal, TT, HB, RS, t_off));
   }
   OMT_LAUNCH_CHECK();
   return OMT_OK;
+}
+
+extern "C" int omt_peg_volume(const float* x, float* y, const float* w27, const float* bias, int B, int T, int h,
+                              int w, int C, int temporal, int causal, omt_stream_t stream) {
+  OMT_ENTER();
+  return peg_volume_launch("omt_peg_volume", x, y, w27, bias, nullptr, B, T, h, w, C, temporal, causal, stream);
+}
+
+extern "C" int omt_peg_volume_varlen(const float* x, float* y, const float* w27, const float* bias, const int32_t* t_off_host,
+                                     const int32_t* t_off, int B, int M, int h, int w, int C, int temporal, int causal,
+                                     omt_stream_t stream) {
+  OMT_ENTER();
+  int t_max = 0;
+  const int rc = check_t_off("omt_peg_volume_varlen", t_off_host, t_off, B, M, (long long)h * w, &t_max);
+  if (rc) return rc;
+  return peg_volume_launch("omt_peg_volume_varlen", x, y, w27, bias, t_off, B, t_max < 1 ? 1 : t_max, h, w, C, temporal,
+                           causal, stream);
 }
 
 extern "C" int omt_qk_prep(float* q, int ldq, float* k, int ldk, const float* q_scale, const float* k_scale,

@@ -14,7 +14,7 @@ from __future__ import annotations
 
 import math
 import os
-from typing import Dict, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 
@@ -104,10 +104,67 @@ class Workspace:
         self.zc_in = torch.empty(M, cd, **f)
         self.zq = torch.empty(M, cd, **f)
         self.video = None
+        # packed batches: encode_batch's (layout key, per-group static input videos); decode_batch's static outputs per
+        # dtype {uint8?: (layout key, per-group videos)}; the layout tables of those layouts (Engine._layout_tables)
+        self.batch_in, self.batch_out, self.layout_tables = None, {}, {}
         self.graphs = {}
 
     def reset(self):
         self.X, self.Y = self.buf0, self.buf1
+
+
+class Group(NamedTuple):
+    """Equal-length samples of a packed batch: n samples of tp latent frames from latent frame f0 on (sorted order s0..)."""
+    tp: int
+    s0: int
+    n: int
+    f0: int
+
+
+class BatchLayout:
+    """Where the samples of one pass lie in the canonical buffer X[frames][N][C].  Samples are sorted stably by their
+    number of latent frames T', so equal lengths are contiguous (one group each); sample i of the caller's order sits at
+    slot[i] = (group, index in the group) and owns latent frames [f_in[i], f_in[i] + tps[i]).  Row-wise kernels never
+    see the layout; PEG and temporal attention take the per-sample offsets t_off (device table, a single launch for every
+    length); the patch gather / un-patchify and the patch GEMMs run once per group.  A uniform batch is the one-group
+    case and runs the uniform kernels (no table)."""
+
+    def __init__(self, tps: Sequence[int], h: int, w: int):
+        self.tps = tuple(int(t) for t in tps)
+        self.B, self.h, self.w, self.N = len(self.tps), h, w, h * w
+        self.order = sorted(range(self.B), key=self.tps.__getitem__)       # stable: equal lengths keep the caller's order
+        self.pos = [0] * self.B                                              # caller's sample i -> its sorted position
+        for s_, i in enumerate(self.order):
+            self.pos[i] = s_
+        sorted_tp = [self.tps[i] for i in self.order]
+        self.t_off = [0]
+        for t in sorted_tp:
+            self.t_off.append(self.t_off[-1] + t)
+        self.groups: List[Group] = []
+        s0 = 0
+        while s0 < self.B:
+            n = 1
+            while s0 + n < self.B and sorted_tp[s0 + n] == sorted_tp[s0]:
+                n += 1
+            self.groups.append(Group(sorted_tp[s0], s0, n, self.t_off[s0]))
+            s0 += n
+        self.frames = self.t_off[-1]
+        self.M = self.frames * self.N
+        self.uniform = len(self.groups) <= 1
+        # caller's sample i -> (group, index inside the group) and its first latent frame
+        self.slot = [None] * self.B
+        self.f_in = [0] * self.B
+        for gi, g in enumerate(self.groups):
+            for k in range(g.n):
+                i = self.order[g.s0 + k]
+                self.slot[i] = (gi, k)
+                self.f_in[i] = g.f0 + k * g.tp
+        # graphs and static I/O buffers are keyed on this: two layouts with the same M differ here
+        self.key = (tuple(sorted_tp), h, w)
+
+    def rows(self, i: int) -> slice:
+        """Canonical rows of sample i (caller's order)."""
+        return slice(self.f_in[i] * self.N, (self.f_in[i] + self.tps[i]) * self.N)
 
 
 class Engine:
@@ -339,18 +396,54 @@ class Engine:
                    None if xp is None else xp.lo, None if xp is None else xp.rs, yp.ld, g, b, M, C, 1e-5, 0, 0, 0)
 
     # ------------------------------------------------------------------ transformer
-    def _transformer(self, tr, ws: Workspace, B, T, h, w, temporal: bool, out_planes: Optional[Planes] = None):
+    def _layout_tables(self, ws: Workspace, lay: BatchLayout):
+        """(t_off host copy, t_off device copy, int64 [M] sorted position of the sample each row belongs to) of a packed
+        layout.  They live in the workspace for as long as a static buffer set of that layout does (_keep_layouts), and
+        with it every graph that reads them; the copy to the device is asynchronous (pinned host memory)."""
+        t = ws.layout_tables.get(lay.key)
+        if t is None:
+            host = torch.tensor(lay.t_off, dtype=torch.int32).pin_memory()
+            dev = host.to(self.device, non_blocking=True)
+            frame = torch.arange(lay.M, device=self.device, dtype=torch.int32) // lay.N
+            t = ws.layout_tables[lay.key] = (host, dev, torch.searchsorted(dev, frame, right=True) - 1)
+        return t
+
+    @staticmethod
+    def _keep_layouts(ws: Workspace):
+        """Drop the layout tables of layouts no static buffer set of the workspace holds any more (their graphs are gone)."""
+        live = {v[0] for v in ws.batch_out.values()} | ({ws.batch_in[0]} if ws.batch_in is not None else set())
+        ws.layout_tables = {k: v for k, v in ws.layout_tables.items() if k in live}
+
+    def row_sample(self, ws: Workspace, lay: BatchLayout) -> torch.Tensor:
+        """int64 [M] on the device: sorted position (lay.pos) of the sample each canonical row of the layout belongs to."""
+        return self._layout_tables(ws, lay)[2]
+
+    def _check_packed(self, tps: Sequence[int]):
+        """A batch of different lengths runs PEG and temporal attention through the layout-table entry points, which take
+        1..17 latent frames per sample -- also in a model without temporal blocks, where encode() takes longer clips."""
+        if len(set(tps)) > 1 and max(tps) > TEMPORAL_MAX_FRAMES:
+            raise NotImplementedError(f"{max(tps)} latent frames: an element of a batch of different lengths takes at most "
+                                      f"{TEMPORAL_MAX_FRAMES} latent frames ({1 + (TEMPORAL_MAX_FRAMES - 1) * self.pt} frames)")
+
+    def _transformer(self, tr, ws: Workspace, lay: BatchLayout, temporal: bool, out_planes: Optional[Planes] = None):
         """modules/attention.py:655-689.  out_planes: norm_out goes to operand planes (decoder -> to_pixels GEMMs)."""
-        C, N, M = self.C, h * w, ws.M
+        C, N, M = self.C, lay.N, ws.M
+        h, w, F = lay.h, lay.w, lay.frames
+        B, T = lay.B, lay.groups[0].tp
         H = self.planes
         q_ptr = ws.QKV.data_ptr()
         k_ptr, v_ptr = q_ptr + C * 4, q_ptr + 2 * C * 4
         ld3 = 3 * C
         o, o_hi, o_lo = (None, ws.Op.hi, ws.Op.lo) if H else (ws.O, None, None)
+        t_off = None if lay.uniform else self._layout_tables(ws, lay)[:2]
         for lyr in tr["layers"]:
             if lyr["kind"] == "t":
-                _cabi.call("omt_peg_volume", ws.X, ws.Y, lyr["peg_w"], lyr["peg_b"], B, T, h, w, C, int(temporal),
-                           int(self.causal_peg))
+                if lay.uniform:
+                    _cabi.call("omt_peg_volume", ws.X, ws.Y, lyr["peg_w"], lyr["peg_b"], B, T, h, w, C, int(temporal),
+                               int(self.causal_peg))
+                else:
+                    _cabi.call("omt_peg_volume_varlen", ws.X, ws.Y, lyr["peg_w"], lyr["peg_b"], *t_off, B, M, h, w, C,
+                               int(temporal), int(self.causal_peg))
                 ws.X, ws.Y = ws.Y, ws.X
                 # q from the normalised input, k / v from the RAW input (attention.py:407-412), one launch;
                 # rope (spatial blocks) + l2norm + q/k scale ride in the same launch (fused GEMM epilogue)
@@ -381,12 +474,15 @@ class Engine:
                 if f16_core:
                     ph, pl = ws.QKVp.hi.data_ptr(), ws.QKVp.lo.data_ptr()
                     _cabi.call("omt_attn_spatial_h", ph, pl, ld3, ph + 2 * C, pl + 2 * C, ld3, ph + 4 * C, pl + 4 * C, ld3,
-                               ws.vinv, lyr["q_ps"] * lyr["k_ps"], None, o_hi, o_lo, C, B * T, N, self.heads, 8.0)
-                elif temporal:
+                               ws.vinv, lyr["q_ps"] * lyr["k_ps"], None, o_hi, o_lo, C, F, N, self.heads, 8.0)
+                elif temporal and lay.uniform:
                     _cabi.call("omt_attn_temporal", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, B, T, N,
                                self.heads, 8.0, int(self.causal_attn))
+                elif temporal:
+                    _cabi.call("omt_attn_temporal_varlen", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, *t_off, B,
+                               M, N, self.heads, 8.0, int(self.causal_attn))
                 else:
-                    _cabi.call("omt_attn_spatial", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, B * T, N,
+                    _cabi.call("omt_attn_spatial", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, F, N,
                                self.heads, 8.0)
                 proj = lyr["to_out"]
             else:
@@ -396,7 +492,7 @@ class Engine:
                 else:
                     self._ln(ws.X, ws.XN, lyr["norm_g"], lyr["norm_b"], M)
                     self._linear(ws.XN, C, lyr["qkv"], q_ptr, ld3, M)
-                _cabi.call("omt_attn_window", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, lyr["bias"], B * T, h,
+                _cabi.call("omt_attn_window", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, lyr["bias"], F, h,
                            w, self.ws, self.heads, float(self.dh) ** -0.5)
                 proj = lyr["proj"]
             if H:
@@ -467,31 +563,31 @@ class Engine:
             _cabi.launch_count += g[1]        # kernels inside the replayed graph (bench.py accounting)
 
     # ------------------------------------------------------------------ encoder side
-    def _encode_body(self, ws: Workspace, gather, dims, mode: str):
+    def _encode_body(self, ws: Workspace, gather, lay: BatchLayout, mode: str):
         """patch embed -> spatial -> temporal -> pre_vq [-> VQ search].  omnitokenizer.py:881-947, 247-258.
-        gather(first, A, A_hi, A_lo, A_rs, ln_w, ln_b) launches the patch gather + LayerNorm of the input video."""
-        B, T, H, W, Tp, h, w = dims
-        N, C = h * w, self.C
+        gather(group, first, A, A_hi, A_lo, A_rs, ln_w, ln_b) launches the patch gather + LayerNorm of one group's videos."""
+        N, C = lay.N, self.C
         ws.reset()
         k1 = self.cin * self.p * self.p
 
-        def embed(pe, first, rows, K, cmap):
+        def embed(pe, gi, first, rows, K, cmap):
             if self.planes:
                 Pp = Planes.__new__(Planes)          # dense [rows, K] view at the start of the patch planes
                 Pp.hi, Pp.lo, Pp.ld, Pp.rs = ws.Pp.hi, ws.Pp.lo, K, ws.Pp.rs
-                gather(first, None, Pp.hi, Pp.lo, Pp.rs, pe["ln1_g"], pe["ln1_b"])
+                gather(gi, first, None, Pp.hi, Pp.lo, Pp.rs, pe["ln1_g"], pe["ln1_b"])
                 self._linear_h(Pp, pe["lin"], rows, C=ws.X, ldc=C, c_map=cmap)
             else:
-                gather(first, ws.P, None, None, None, pe["ln1_g"], pe["ln1_b"])
+                gather(gi, first, ws.P, None, None, None, pe["ln1_g"], pe["ln1_b"])
                 self._linear(ws.P, K, pe["lin"], ws.X, C, rows, c_map=cmap)
             if not self.cnn:
                 self._ln(ws.X, ws.X, pe["ln2_g"], pe["ln2_b"], rows, seg=cmap)
 
-        embed(self.pe["first"], 1, B * N, k1, (N, Tp * N, 0))
-        if Tp > 1:
-            embed(self.pe["rest"], 0, B * (Tp - 1) * N, k1 * self.pt, ((Tp - 1) * N, Tp * N, N))
-        self._transformer(self.enc_spatial, ws, B, Tp, h, w, temporal=False)
-        self._transformer(self.enc_temporal, ws, B, Tp, h, w, temporal=True)
+        for gi, g in enumerate(lay.groups):      # each group's frames start at canonical row g.f0 * N
+            embed(self.pe["first"], gi, 1, g.n * N, k1, (N, g.tp * N, g.f0 * N))
+            if g.tp > 1:
+                embed(self.pe["rest"], gi, 0, g.n * (g.tp - 1) * N, k1 * self.pt, ((g.tp - 1) * N, g.tp * N, g.f0 * N + N))
+        self._transformer(self.enc_spatial, ws, lay, temporal=False)
+        self._transformer(self.enc_temporal, ws, lay, temporal=True)
         cd = self.pre_w.shape[0]
         z = ws.z.view(-1)[: ws.M * cd].view(ws.M, cd)
         if mode == "vq":      # pre_vq + l2norm + modules/codebook.py:82-86 in one cluster kernel
@@ -513,11 +609,41 @@ class Engine:
             ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("enc")}
         ws.x_in.copy_(x)
 
-        def gather(first, *out):
+        def gather(gi, first, *out):
             _cabi.call("omt_patchify_ln", ws.x_in, *out, B, self.cin, T, H, W, self.p, self.pt, first, 1e-5)
 
-        self._run(ws, ("enc:" + mode, tuple(x.shape)), lambda: self._encode_body(ws, gather, dims, mode))
+        lay = BatchLayout((Tp,) * B, h, w)
+        self._run(ws, ("enc:" + mode, tuple(x.shape)), lambda: self._encode_body(ws, gather, lay, mode))
         return ws, (B, Tp, h, w)
+
+    def encode_batch(self, xs: Sequence[torch.Tensor], mode: str):
+        """encode() of a list of single videos xs[i] (C, T_i, H, W) fp32 on the device, all with the same C, H, W, in ONE pass:
+        the samples are packed by length (BatchLayout).  Returns (ws, lay): sample i's results are the rows lay.rows(i)
+        of ws.z / ws.idx, equal bit for bit to what encode(xs[i][None]) leaves there.  ws.counts is not filled."""
+        dims = [self._shape((1,) + tuple(x.shape)) for x in xs]
+        H, W = dims[0][2], dims[0][3]
+        for d in dims:
+            if (d[2], d[3]) != (H, W):
+                raise ValueError(f"every element of a batch must have the same frame size: {H}x{W} and {d[2]}x{d[3]}")
+        self._check_packed([d[4] for d in dims])
+        lay = BatchLayout([d[4] for d in dims], dims[0][5], dims[0][6])
+        ws = self._workspace(lay.M)
+        if ws.batch_in is None or ws.batch_in[0] != lay.key:
+            ws.batch_in = (lay.key, [torch.empty((g.n, self.cin, 1 + (g.tp - 1) * self.pt, H, W), device=self.device)
+                                     for g in lay.groups])
+            ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("encb")}
+            self._keep_layouts(ws)
+        bufs = ws.batch_in[1]
+        for g, buf in zip(lay.groups, bufs):
+            torch.stack([xs[i].to(device=self.device, dtype=torch.float32) for i in lay.order[g.s0:g.s0 + g.n]], out=buf)
+
+        def gather(gi, first, *out):
+            g = lay.groups[gi]
+            _cabi.call("omt_patchify_ln", bufs[gi], *out, g.n, self.cin, bufs[gi].shape[2], H, W, self.p, self.pt, first,
+                       1e-5)
+
+        self._run(ws, ("encb:" + mode, lay.key), lambda: self._encode_body(ws, gather, lay, mode))
+        return ws, lay
 
     def encode_u8(self, frames: torch.Tensor, mode: str, norm: L.U8Norm):
         """encode() from uint8 frames (B,T,H,W,C) on the device: the patch gather maps every byte through the host-built
@@ -537,13 +663,15 @@ class Engine:
         lut = self._table(("u8norm", norm), lambda: L.u8_norm_table(norm, self.cin))
         sel = ws.u8_sel if norm.max_test else None
 
-        def gather(first, *out):
+        def gather(gi, first, *out):
             _cabi.call("omt_patchify_ln_u8", ws.u8_in, lut, sel, *out, B, self.cin, T, H, W, self.p, self.pt, first, 1e-5)
+
+        lay = BatchLayout((Tp,) * B, h, w)
 
         def body():
             if sel is not None:
                 _cabi.call("omt_u8_norm_select", ws.u8_in, B, T * H * W * self.cin, sel)
-            self._encode_body(ws, gather, dims, mode)
+            self._encode_body(ws, gather, lay, mode)
 
         self._run(ws, ("enc_u8:" + mode, tuple(frames.shape), norm), body)
         return ws, (B, Tp, h, w)
@@ -560,11 +688,11 @@ class Engine:
         return self._dense(ws.zq, ws.M, self.post_w.shape[1])
 
     # ------------------------------------------------------------------ decoder side
-    def _decode_body(self, ws: Workspace, dims, mode: str, u8=None):
+    def _decode_body(self, ws: Workspace, lay: BatchLayout, mode: str, outs, u8=None):
         """[gather +] post_vq -> temporal -> spatial -> to_pixels.  omnitokenizer.py:268-317, 1059-1118.
-        u8 = (mul, add, lo, hi, post): the pixels leave as uint8 (B,T,H,W,C) = trunc(clamp(x*mul+add, lo, hi)*post)."""
-        B, Tp, h, w = dims
-        N, M, C = h * w, ws.M, self.C
+        outs[g]: the output videos of group g, (n,C,T,H,W) fp32, or with u8 = (mul, add, lo, hi, post) uint8 (n,T,H,W,C)
+        = trunc(clamp(x*mul+add, lo, hi)*post)."""
+        N, M, C = lay.N, ws.M, self.C
         ws.reset()
         cdp = self.post_w.shape[1]
         if mode == "idx":
@@ -575,25 +703,30 @@ class Engine:
         else:
             _cabi.call("omt_post_vq", None, None, self._dense(ws.zc_in, M, cdp), None, None, self.post_w, self.post_b,
                        ws.X, M, C, cdp)
-        self._transformer(self.dec_temporal, ws, B, Tp, h, w, temporal=True)
-        self._transformer(self.dec_spatial, ws, B, Tp, h, w, temporal=False, out_planes=ws.XNp if self.planes else None)
-        T = 1 + (Tp - 1) * self.pt
-        H, W = h * self.p, w * self.p
+        self._transformer(self.dec_temporal, ws, lay, temporal=True)
+        self._transformer(self.dec_spatial, ws, lay, temporal=False, out_planes=ws.XNp if self.planes else None)
+        H, W = lay.h * self.p, lay.w * self.p
         k1 = self.cin * self.p * self.p
 
-        def pixels(px, first, rows, K, amap):
+        def pixels(px, g, out, first, rows, K, amap):
             if self.planes:
                 self._linear_h(ws.XNp, px, rows, C=ws.P, ldc=K, a_map=amap)
             else:
                 self._linear(ws.X, C, px, ws.P, K, rows, a_map=amap)
+            T = 1 + (g.tp - 1) * self.pt
             if u8 is None:
-                _cabi.call("omt_unpatchify", ws.P, ws.video, B, self.cin, T, H, W, self.p, self.pt, first)
+                _cabi.call("omt_unpatchify", ws.P, out, g.n, self.cin, T, H, W, self.p, self.pt, first)
             else:
-                _cabi.call("omt_unpatchify_u8", ws.P, ws.video_u8, B, self.cin, T, H, W, self.p, self.pt, first, *u8)
+                _cabi.call("omt_unpatchify_u8", ws.P, out, g.n, self.cin, T, H, W, self.p, self.pt, first, *u8)
 
-        pixels(self.px["first"], 1, B * N, k1, (N, Tp * N, 0))
-        if Tp > 1:
-            pixels(self.px["rest"], 0, B * (Tp - 1) * N, k1 * self.pt, ((Tp - 1) * N, Tp * N, N))
+        for g, out in zip(lay.groups, outs):     # each group's frames start at canonical row g.f0 * N
+            pixels(self.px["first"], g, out, 1, g.n * N, k1, (N, g.tp * N, g.f0 * N))
+            if g.tp > 1:
+                pixels(self.px["rest"], g, out, 0, g.n * (g.tp - 1) * N, k1 * self.pt, ((g.tp - 1) * N, g.tp * N, g.f0 * N + N))
+
+    def _video_shape(self, n, tp, h, w, u8: bool):
+        T, H, W = 1 + (tp - 1) * self.pt, h * self.p, w * self.p
+        return (n, T, H, W, self.cin) if u8 else (n, self.cin, T, H, W)
 
     def decode(self, dims, *, idx=None, zc=None, straight_through=False, u8=None) -> torch.Tensor:
         """dims (B,T',h,w).  idx: int64 [M] codes | zc: fp32 [M, cd] latents (VAE).  With straight_through
@@ -603,11 +736,11 @@ class Engine:
         B, Tp, h, w = dims
         self._check_latent_frames(Tp)
         ws = self._workspace(B * Tp * h * w)
-        vshape = (B, self.cin, 1 + (Tp - 1) * self.pt, h * self.p, w * self.p)
+        vshape = self._video_shape(B, Tp, h, w, False)
         if ws.video is None or tuple(ws.video.shape) != vshape:
             ws.video = torch.empty(vshape, device=self.device, dtype=torch.float32)
-            ws.video_u8 = torch.empty((B, vshape[2], vshape[3], vshape[4], self.cin), device=self.device, dtype=torch.uint8)
-            ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("dec")}
+            ws.video_u8 = torch.empty(self._video_shape(B, Tp, h, w, True), device=self.device, dtype=torch.uint8)
+            ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("dec:")}
         if idx is not None:
             ws.idx_in.copy_(idx.reshape(-1))
             mode = "idx_st" if straight_through else "idx"
@@ -615,5 +748,35 @@ class Engine:
             self._dense(ws.zc_in, ws.M, zc.shape[1]).copy_(zc)
             mode = "zc"
         u8 = None if u8 is None else tuple(float(v) for v in u8)
-        self._run(ws, ("dec:" + mode, dims, u8), lambda: self._decode_body(ws, dims, mode, u8))
+        lay = BatchLayout((Tp,) * B, h, w)
+        outs = [ws.video if u8 is None else ws.video_u8]
+        self._run(ws, ("dec:" + mode, dims, u8), lambda: self._decode_body(ws, lay, mode, outs, u8))
         return ws.video.clone() if u8 is None else ws.video_u8.clone()
+
+    def decode_batch(self, tps: Sequence[int], h: int, w: int, *, idx=None, zc=None, u8=None) -> List[torch.Tensor]:
+        """decode() of a list of single samples in ONE pass.  tps[i]: latent frames of sample i; idx: list of int64 codes
+        (tps[i]*h*w each) | zc: list of fp32 [tps[i]*h*w, cd] latents.  Returns, in the caller's order, what
+        decode((1, tps[i], h, w), ...) returns for each sample, bit for bit."""
+        for tp in tps:
+            self._check_latent_frames(tp)
+        self._check_packed(tps)
+        lay = BatchLayout(tps, h, w)
+        ws = self._workspace(lay.M)
+        u8 = None if u8 is None else tuple(float(v) for v in u8)
+        is_u8 = u8 is not None
+        if is_u8 not in ws.batch_out or ws.batch_out[is_u8][0] != lay.key:      # one static output set per dtype
+            dt = torch.uint8 if is_u8 else torch.float32
+            ws.batch_out[is_u8] = (lay.key, [torch.empty(self._video_shape(g.n, g.tp, h, w, is_u8), device=self.device, dtype=dt)
+                                             for g in lay.groups])
+            ws.graphs = {k: v for k, v in ws.graphs.items() if not (k[0].startswith("decb") and (k[2] is not None) == is_u8)}
+            self._keep_layouts(ws)
+        outs = ws.batch_out[is_u8][1]
+        if idx is not None:
+            ws.idx_in.copy_(torch.cat([idx[i].reshape(-1) for i in lay.order]))
+            mode = "idx"
+        else:
+            cdp = zc[0].shape[-1]
+            self._dense(ws.zc_in, ws.M, cdp).copy_(torch.cat([zc[i].reshape(-1, cdp) for i in lay.order]))
+            mode = "zc"
+        self._run(ws, ("decb:" + mode, lay.key, u8), lambda: self._decode_body(ws, lay, mode, outs, u8))
+        return [outs[gi][k].clone() for gi, k in lay.slot]

@@ -333,7 +333,7 @@ class OmniTokenizer_VQGAN(nn.Module):
         with torch.cuda.device(self.device):
             xv = x.unsqueeze(2) if is_image else x
             ws, dims = eng.encode(xv.float(), "raw" if self.use_vae else "vq")
-            return self._encode_result(eng, ws, dims, is_image, include_embeddings)
+            return self._encode_result(eng, ws.idx, eng.z_view(ws), ws.counts, dims, is_image, include_embeddings)
 
     def _u8_frames(self, frames, is_image):
         """Checks uint8 frames (B, T, H, W, C) / images (B, H, W, C) and returns them as (B, T, H, W, C)."""
@@ -359,27 +359,69 @@ class OmniTokenizer_VQGAN(nn.Module):
             return self._empty_encode(torch.empty(shape, device="meta"), is_image, include_embeddings)
         with torch.cuda.device(self.device):
             ws, dims = eng.encode_u8(f, "raw" if self.use_vae else "vq", norm)
-            return self._encode_result(eng, ws, dims, is_image, include_embeddings)
+            return self._encode_result(eng, ws.idx, eng.z_view(ws), ws.counts, dims, is_image, include_embeddings)
 
-    def _encode_result(self, eng, ws, dims, is_image, include_embeddings):
-        """What encode() returns from the engine's workspace (omnitokenizer.py:247-266), with Codebook.forward's usage side effects."""
+    def _encode_result(self, eng, idx, z, counts, dims, is_image, include_embeddings):
+        """What encode() returns (omnitokenizer.py:247-266), with Codebook.forward's usage side effects, from the encoder's
+        rows of the dims (B,T',h,w) batch: idx [M] codes, z [M, cd] (VQ) or [M, 2 cd] moments (VAE), counts the code histogram."""
         B, Tp, h, w = dims
         if not self.use_vae:
-            enc = ws.idx.view(B, Tp, h, w).clone()
-            self._track_usage(ws.counts, ws.M)             # Codebook.forward runs inside encode() too
+            enc = idx.view(B, Tp, h, w).clone()
+            self._track_usage(counts, idx.numel())           # Codebook.forward runs inside encode() too
             if include_embeddings:
-                z = eng.z_view(ws)
-                e = eng.E[ws.idx]
+                e = eng.E[idx]
                 st = (e - z) + z
                 return st.view(B, Tp, h, w, -1).permute(0, 4, 1, 2, 3).contiguous(), enc
             return enc
-        hpar = eng.z_view(ws)                                                 # (M, 2*cd) moments
+        hpar = z                                                              # (M, 2*cd) moments
         c = hpar.shape[1] // 2
         hpar = hpar.view(B, Tp, h, w, 2 * c).permute(0, 4, 1, 2, 3)
         mean, logvar = hpar[:, :c], torch.clamp(hpar[:, c:], -30.0, 20.0)     # vae.py:7-8
         noise = torch.randn(mean.shape).to(device=self.device)                # CPU generator, vae.py:16
         z = mean + torch.exp(0.5 * logvar) * noise
         return z.squeeze(2) if is_image else z.contiguous()
+
+    @torch.no_grad()
+    def encode_batch(self, xs, include_embeddings=False):
+        """encode() of a mixed list in ONE pass: xs[i] is an image (C, H, W) or a video (C, T, H, W), every element with the
+        same H x W and channel count (clip lengths may differ).  Returns a list in input order; element i is what
+        encode(xs[i][None], is_image)[0] returns -- codes (T', h, w), the (embeddings, codes) pair with include_embeddings,
+        or VAE latents (c, h, w) / (c, T', h, w) -- except that image codes (and embeddings) come without the frame axis,
+        (h, w) and (cd, h, w), the form decode_batch takes for an image.  Bit for bit, with the side effects of the
+        sequential calls: codebook_usage / call_cnt move once per element in input order, VAE noise is drawn from the CPU
+        generator per element in input order.  Every element is checked (with encode's messages) before any launch."""
+        xs = list(xs)
+        if not xs:
+            return []
+        eng = self.engine()
+        cin = self.args.image_channels
+        for x in xs:
+            if x.ndim not in (3, 4):
+                raise ValueError(f"encode_batch takes images (C, H, W) and videos (C, T, H, W), got {tuple(x.shape)}")
+            if x.shape[0] != cin:
+                raise ValueError(f"expected {cin} channels, got {x.shape[0]}")
+            if tuple(x.shape[-2:]) != tuple(xs[0].shape[-2:]):
+                raise ValueError(f"every element of a batch must have the same frame size: "
+                                 f"{tuple(xs[0].shape[-2:])} and {tuple(x.shape[-2:])}")
+        with torch.cuda.device(self.device):
+            ws, lay = eng.encode_batch([x.unsqueeze(1) if x.ndim == 3 else x for x in xs], "raw" if self.use_vae else "vq")
+            z, hist = eng.z_view(ws), None
+            if not self.use_vae:          # per-element code histograms (sorted order) from the packed codes: one scatter, no host sync
+                n = self.codebook.n_codes
+                hist = torch.zeros(lay.B * n, dtype=torch.int64, device=self.device)
+                hist = hist.scatter_add_(0, eng.row_sample(ws, lay) * n + ws.idx, torch.ones_like(ws.idx)).view(lay.B, n)
+            out = []
+            for i, x in enumerate(xs):
+                r, is_image = lay.rows(i), x.ndim == 3
+                res = self._encode_result(eng, ws.idx[r], z[r], None if hist is None else hist[lay.pos[i]],
+                                          (1, lay.tps[i], lay.h, lay.w), is_image, include_embeddings)
+                if self.use_vae:
+                    out.append(res[0])
+                elif include_embeddings:
+                    out.append((res[0][0, :, 0], res[1][0, 0]) if is_image else (res[0][0], res[1][0]))
+                else:
+                    out.append(res[0, 0] if is_image else res[0])
+            return out
 
     def _check_cnn_grid(self, h, w):
         # the cnn decoder's Rearrange pins h to image_size // patch_size (omnitokenizer.py:1021): other grids raise there
@@ -453,6 +495,59 @@ class OmniTokenizer_VQGAN(nn.Module):
         Default affine: vqgan_eval.py:139,147-148 `(clamp(x_recons + 0.5, 0, 1) * 255).byte()` in 'b t h w c' order;
         (255, 128, 0, 255, 1): DiT sample_ddp.py:163.  The device->host copy is 4x smaller than the fp32 video."""
         return self._decode(encodings, is_image, u8=affine)
+
+    def _decode_batch(self, encodings, u8=None):
+        """decode_batch / decode_u8_batch: element i in decode's form without the batch dimension -- VQ codes (h, w) of an
+        image or (T', h, w) of a video, VAE latents (c, h, w) of an image or (T', h, w, c) of a video."""
+        encs = list(encodings)
+        if not encs:
+            return []
+        eng = self.engine()
+        tps, is_image, grid = [], [], None
+        img_ndim, forms = (3, "(c, h, w) / (T', h, w, c) latents") if self.use_vae else (2, "(h, w) / (T', h, w) codes")
+        for e in encs:
+            img = e.ndim == img_ndim
+            if e.ndim != img_ndim + 1 and not img:
+                raise ValueError(f"decode_batch takes {forms}, got {tuple(e.shape)}")
+            if img:
+                tp, g = 1, tuple(e.shape[-2:])
+            else:
+                tp, g = e.shape[0], tuple(e.shape[1:3])
+            if grid is not None and g != grid:
+                raise ValueError(f"every element of a batch must have the same token grid: {grid} and {g}")
+            grid = g
+            self._check_cnn_grid(*g)
+            eng._check_latent_frames(int(tp))
+            tps.append(int(tp))
+            is_image.append(img)
+        eng._check_packed(tps)
+        h, w = grid
+        with torch.cuda.device(self.device):
+            if not self.use_vae:
+                idx = [e.reshape(-1).to(device=self.device, dtype=torch.int64) for e in encs]
+                allidx = torch.cat(idx)
+                torch._assert_async(((allidx >= 0) & (allidx < self.codebook.n_codes)).all(),
+                                    "decode: code index out of range [0, n_codes)")
+                outs = eng.decode_batch(tps, h, w, idx=idx, u8=u8)
+            else:
+                # rows (t, h, w) x latent channels, as decode reads the 4-D 'b c h w' / 5-D 'b t h w c' forms
+                zc = [(e.permute(1, 2, 0) if img else e).to(device=self.device, dtype=torch.float32) for e, img in zip(encs, is_image)]
+                zc = [z.reshape(-1, z.shape[-1]) for z in zc]
+                outs = eng.decode_batch(tps, h, w, zc=zc, u8=u8)
+        return [o.squeeze(1) if img and u8 is None else o for o, img in zip(outs, is_image)]
+
+    @torch.no_grad()
+    def decode_batch(self, encodings):
+        """decode() of a mixed list in ONE pass; element i is what decode(encodings[i][None], is_image)[0] returns, bit for
+        bit: (C, H, W) for an image, (C, T, H, W) for a video.  Forms of the elements: see _decode_batch (the forms
+        encode_batch returns, with VAE video latents as decode takes them, 't h w c')."""
+        return self._decode_batch(encodings)
+
+    @torch.no_grad()
+    def decode_u8_batch(self, encodings, affine=(1.0, 0.5, 0.0, 1.0, 255.0)):
+        """decode_u8() of a mixed list in ONE pass: element i is decode_u8(encodings[i][None], is_image, affine)[0],
+        uint8 (T, H, W, C) with T = 1 for images."""
+        return self._decode_batch(encodings, u8=tuple(float(v) for v in affine))
 
     @torch.no_grad()
     def forward(self, x, optimizer_idx=None, log_image=False):
