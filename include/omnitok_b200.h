@@ -51,6 +51,8 @@ int omt_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* GEMM math selectors */
 #define OMT_MATH_FP32 0      /* CUDA-core FFMA, exact fp32 (parity anchor) */
 #define OMT_MATH_3XTF32 1    /* wgmma tf32, error-compensated hi/lo split, fp32 accumulate in registers */
+#define OMT_MATH_F16X1 2     /* throughput mode: ONE wgmma f16 per product on the hi planes (omt_linear_h1, omt_attn_spatial_h1);
+                                NOT reference-exact (about 11 significant bits per operand, like single-pass TF32) */
 #define OMT_MATH_F16X3 3     /* wgmma f16 on pre-split fp16 hi / lo operand planes (omt_linear_h) */
 
 /* C[M, N] = A[M, K] . W[N, K]^T (+ bias[N]) (+ residual[M, N]); nn.Linear everywhere on the path:
@@ -173,6 +175,13 @@ int omt_attn_spatial_h(const uint16_t* q_hi, const uint16_t* q_lo, int ldq, cons
                        float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo, int n_seq, int N, int heads, float scale,
                        omt_stream_t stream);
 
+/* f16x1 (throughput) form of omt_attn_spatial_h on the hi planes alone: S = Q_hi . K_hi^T and O += P''_hi . V_hi take ONE
+ * f16 wgmma per k-step (P'' = p * vinv * 2^e rounded to fp16, as in the three-product core).  o fp32, or o_hi != NULL:
+ * the hi plane of O (fp16(o)) for the f16x1 out-projection; o may then be NULL.  NOT reference-exact. */
+int omt_attn_spatial_h1(const uint16_t* q_hi, int ldq, const uint16_t* k_hi, int ldk, const uint16_t* v_hi, int ldv,
+                        const float* vinv, float qk_plane_scale, float* o, uint16_t* o_hi, int ldo, int n_seq, int N,
+                        int heads, float scale, omt_stream_t stream);
+
 /* 8x8 (ws x ws, ws*ws == 64) window attention with relative position bias (attention.py:254-286):
  * o = softmax(scale * q k^T + bias[head]) v within each window of the (h, w) token grid.
  * bias: [heads, 64, 64] already gathered from the 225-entry table. */
@@ -261,6 +270,14 @@ typedef struct omt_linear_h_args {
 
 /* Same contract as omt_linear / omt_linear2 (nn.Linear + the fused epilogues) on operand planes. */
 int omt_linear_h(const omt_linear_h_args* args, omt_stream_t stream);
+
+/* f16x1 (throughput) form of omt_linear_h: the same argument block, forms and epilogues, ONE f16 product A_hi . W_hi per
+ * k-step with fp32 accumulation.  a_lo, a2_lo, w_lo and u_lo must be NULL (a non-NULL one is rejected), so no caller can
+ * take the result for the three-product one.  Row-scaled / uniform-scaled A: the epilogue multiplies by a_rs[row] * w_scale
+ * (a_rs_uniform * w_scale); the 2^11 form (a_rs == NULL, a_rs_uniform == 0): hi planes of unscaled values, no factor.
+ * OMT_EPI_QKV_PLANES and OMT_EPI_GEGLU write the hi planes only (u_hi; vinv as before).  Results are NOT reference-exact:
+ * expect relative errors near 2^-11 per product term. */
+int omt_linear_h1(const omt_linear_h_args* args, omt_stream_t stream);
 
 /* LayerNorm as omt_layernorm with plane outputs for the GEMM that consumes it:
  * y (fp32, may be NULL), (y_hi, y_lo) planes of the normalised row, and optionally (x_hi, x_lo) planes of the RAW

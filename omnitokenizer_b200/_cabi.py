@@ -15,7 +15,7 @@ _LIB_NAME = "libomnitok_b200.so"
 _lib = None
 
 EPI_NONE, EPI_GEGLU, EPI_QKV, EPI_QKV_PLANES = 0, 1, 2, 3
-MATH_FP32, MATH_3XTF32, MATH_F16X3 = 0, 1, 3
+MATH_FP32, MATH_3XTF32, MATH_F16X1, MATH_F16X3 = 0, 1, 2, 3
 ABI_VERSION = 2
 
 
@@ -47,6 +47,7 @@ SIGNATURES = {
     "omt_linear2": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                             c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "omt_linear_h": (c_int, [POINTER(LinearHArgs), c_void_p]),
+    "omt_linear_h1": (c_int, [POINTER(LinearHArgs), c_void_p]),
     "omt_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_int,
                               c_int, c_void_p]),
     "omt_layernorm_h": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -65,6 +66,8 @@ SIGNATURES = {
                                  c_int, c_int, c_int, c_float, c_void_p]),
     "omt_attn_spatial_h": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
                                    c_float, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
+    "omt_attn_spatial_h1": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_float, c_void_p, c_void_p,
+                                    c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "omt_attn_window": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                 c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "omt_attn_temporal": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
@@ -133,17 +136,18 @@ def call(name: str, *args):
         raise RuntimeError(f"{name} failed ({rc}): {lib.omt_last_error().decode()}")
 
 
-def linear_h(**kw):
-    """omt_linear_h with keyword fields of omt_linear_h_args (tensors -> device pointers; missing fields = 0 / NULL)."""
+def linear_h(name="omt_linear_h", **kw):
+    """omt_linear_h (or, with name="omt_linear_h1", its single-product form) with keyword fields of omt_linear_h_args
+    (tensors -> device pointers; missing fields = 0 / NULL)."""
     global launch_count
     lib = load()
     a = LinearHArgs()
     for k, v in kw.items():
         setattr(a, k, _ptr(v) if (v is None or isinstance(v, torch.Tensor)) else v)
     launch_count += 1
-    rc = lib.omt_linear_h(ctypes.byref(a), _stream())
+    rc = getattr(lib, name)(ctypes.byref(a), _stream())
     if rc != 0:
-        raise RuntimeError(f"omt_linear_h failed ({rc}): {lib.omt_last_error().decode()}")
+        raise RuntimeError(f"{name} failed ({rc}): {lib.omt_last_error().decode()}")
 
 
 # process-wide kernel selectors and their library defaults (omt_set_option); tests restore these after flipping them

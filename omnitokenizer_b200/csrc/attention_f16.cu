@@ -24,6 +24,11 @@
 //     the softmax runs.  P'' hi / lo are packed from the S accumulator straight into the A fragments of the P.V wgmmas.
 //   * a K / V stage is released once the P.V wgmmas that read it have retired.
 // Every output row sees the same products in the same order as a serial loop over the key tiles would give it.
+//
+// H1 = true (omt_attn_spatial_h1, "f16x1", the throughput mode): the same kernel on the hi planes alone.  S = Q_hi.K_hi^T
+// and O += P''_hi.V_hi take ONE wgmma per k-step, the ring carries K_hi / V_hi and vinv only (twice the stages in less
+// shared memory), and O leaves as fp32 or as a hi plane.  The per-(row, head) V scale and the P'' packing are unchanged:
+// they keep P.V in fp16 range whatever the number of products.
 #include "omt_common.cuh"
 #include "tc_ptx.cuh"
 #include <cuda.h>
@@ -35,14 +40,21 @@ using namespace omt::ptx;
 
 constexpr int QT = 128, KT = 64, D = 64;
 constexpr int TILE = KT * D * 2;                    // 8 KiB: one 64 x 64 fp16 plane tile
-constexpr int STAGES = 4;
-constexpr int OFF_Q = 0;                            // Q_hi [2 warpgroups] | Q_lo [2]
-constexpr int OFF_KV = 4 * TILE;                    // [STAGES] x (K_hi | K_lo | V_hi | V_lo)
-constexpr int OFF_VI = OFF_KV + STAGES * 4 * TILE;  // [STAGES] x the 64 vinv of the tile's keys
-constexpr int OFF_CTRL = OFF_VI + STAGES * KT * 4;  // mbarriers, the item's largest vinv
-constexpr int SMEM = OFF_CTRL + 128 + 1024;         // + alignment slack
 constexpr int THREADS = 384;                        // warpgroup 0: producer; 1, 2: consumers
-constexpr uint32_t KV_BYTES = 4 * TILE + KT * 4;
+// Shared memory of the two forms; PL = planes per operand (hi / lo, or hi alone)
+template <bool H1> struct Smem {
+  static constexpr int PL = H1 ? 1 : 2;
+  static constexpr int STAGES = H1 ? 8 : 4;
+  static constexpr int STAGE = 2 * PL * TILE;                   // K planes | V planes of one key tile
+  static constexpr int OFF_Q = 0;                               // Q_hi [2 warpgroups] | Q_lo [2]
+  static constexpr int OFF_KV = 2 * PL * TILE;                  // [STAGES] x (K_hi | K_lo | V_hi | V_lo)
+  static constexpr int OFF_VI = OFF_KV + STAGES * STAGE;        // [STAGES] x the 64 vinv of the tile's keys
+  static constexpr int OFF_CTRL = OFF_VI + STAGES * KT * 4;     // mbarriers, the item's largest vinv
+  static constexpr int SMEM = OFF_CTRL + (H1 ? 256 : 128) + 1024;   // + alignment slack
+  static constexpr uint32_t Q_BYTES = 2 * PL * TILE;
+  static constexpr uint32_t KV_BYTES = STAGE + KT * 4;
+  static_assert((2 + 2 * STAGES) * 8 + 4 <= (H1 ? 256 : 128), "control block");
+};
 // __launch_bounds__(384, 1) caps the kernel at 168 registers a thread: 40 * 128 + 232 * 256 == 168 * 384
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
@@ -54,13 +66,16 @@ struct Args {
   float scale_log2;                                        // scale * log2(e) / (q plane scale * k plane scale)
 };
 
+template <bool H1>
 __global__ void __launch_bounds__(THREADS, 1)
 attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
                 const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,
                 const __grid_constant__ CUtensorMap tmVh, const __grid_constant__ CUtensorMap tmVl, const Args a) {
+  using L = Smem<H1>;
+  constexpr int PL = L::PL, STAGES = L::STAGES, OFF_Q = L::OFF_Q, OFF_KV = L::OFF_KV, OFF_VI = L::OFF_VI;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_CTRL);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_CTRL);
   uint64_t& q_full = bars[0];                                         // Q planes (and vmax) of an item landed
   uint64_t& q_empty = bars[1];                                        // every consumer thread has its Q fragments
   uint64_t* full = bars + 2;                                          // [STAGES] K / V planes and vinv of a key tile landed
@@ -71,7 +86,8 @@ attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant_
   const int ntiles = a.N / KT, nqt = a.N / QT;
 
   if (tid == 0) {
-    prefetch_map(&tmQh); prefetch_map(&tmQl); prefetch_map(&tmKh); prefetch_map(&tmKl); prefetch_map(&tmVh); prefetch_map(&tmVl);
+    if (H1) { prefetch_map(&tmQh); prefetch_map(&tmKh); prefetch_map(&tmVh); }
+    else { prefetch_map(&tmQh); prefetch_map(&tmQl); prefetch_map(&tmKh); prefetch_map(&tmKl); prefetch_map(&tmVh); prefetch_map(&tmVl); }
     mbar_init(&q_full, 1);
     mbar_init(&q_empty, 256);
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
@@ -109,23 +125,23 @@ attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant_
         mbar_wait(&q_empty, (c & 1) ^ 1);
         if (lane == 0) {
           *vmax = vmx;                                                // published by the arrive below
-          mbar_expect_tx(&q_full, 4 * TILE);
+          mbar_expect_tx(&q_full, L::Q_BYTES);
           for (int w = 0; w < 2; ++w) {
             tma_load_2d(&tmQh, &q_full, smem + OFF_Q + w * TILE, col0, row_q0 + w * 64);
-            tma_load_2d(&tmQl, &q_full, smem + OFF_Q + (2 + w) * TILE, col0, row_q0 + w * 64);
+            if (!H1) tma_load_2d(&tmQl, &q_full, smem + OFF_Q + (2 + w) * TILE, col0, row_q0 + w * 64);
           }
         }
         for (int j = 0; j < ntiles; ++j, ++it) {
           const int s = it % STAGES;
           mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
           if (lane == 0) {
-            uint8_t* sp = smem + OFF_KV + s * 4 * TILE;
+            uint8_t* sp = smem + OFF_KV + s * L::STAGE;
             const int kr = row_k0 + j * KT;
-            mbar_expect_tx(&full[s], KV_BYTES);
+            mbar_expect_tx(&full[s], L::KV_BYTES);
             tma_load_2d(&tmKh, &full[s], sp, col0, kr);
-            tma_load_2d(&tmKl, &full[s], sp + TILE, col0, kr);
-            tma_load_2d(&tmVh, &full[s], sp + 2 * TILE, col0, kr);
-            tma_load_2d(&tmVl, &full[s], sp + 3 * TILE, col0, kr);
+            if (!H1) tma_load_2d(&tmKl, &full[s], sp + TILE, col0, kr);
+            tma_load_2d(&tmVh, &full[s], sp + PL * TILE, col0, kr);
+            if (!H1) tma_load_2d(&tmVl, &full[s], sp + 3 * TILE, col0, kr);
             bulk_load(smem + OFF_VI + s * KT * 4, vinv_h + j * KT, KT * 4, &full[s]);
           }
         }
@@ -163,7 +179,7 @@ attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant_
             const int r = rl0 + 8 * h;
             const uint8_t* p = smem + OFF_Q + wg * TILE + r * 128 + (((2 * kk + e) ^ (r & 7)) << 4) + qd * 4;
             qh[4 * kk + 2 * e + h] = *reinterpret_cast<const uint32_t*>(p);
-            ql[4 * kk + 2 * e + h] = *reinterpret_cast<const uint32_t*>(p + 2 * TILE);
+            if (!H1) ql[4 * kk + 2 * e + h] = *reinterpret_cast<const uint32_t*>(p + 2 * TILE);
           }
       mbar_arrive(&q_empty);
 
@@ -171,34 +187,42 @@ attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant_
 #pragma unroll
       for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
       float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-      uint32_t p_a[2][16], p_b[2][16];               // P'' hi / lo A fragments of two tiles, laid out like qh / ql
+      uint32_t p_a[PL][16], p_b[PL][16];             // P'' hi (/ lo) A fragments of two tiles, laid out like qh / ql
       float alpha[2];
 
       auto wait_full = [&](uint32_t t) { mbar_wait(&full[t % STAGES], (t / STAGES) & 1); };
       auto issue_s = [&](uint32_t t) {               // S = Q . K^T of running tile t
-        const uint32_t kv = sb + OFF_KV + (t % STAGES) * 4 * TILE;
+        const uint32_t kv = sb + OFF_KV + (t % STAGES) * L::STAGE;
         const uint64_t dk_hi = desc_sw128(kv), dk_lo = desc_sw128(kv + TILE);
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {             // 16 of the 64 head dims per MMA
           const uint64_t adv = (uint64_t)(kk * 2);
-          wgmma_f16_n64_ra<0>(sv, ql + 4 * kk, dk_hi + adv, kk != 0);
-          wgmma_f16_n64_ra<0>(sv, qh + 4 * kk, dk_lo + adv, 1);
-          wgmma_f16_n64_ra<0>(sv, qh + 4 * kk, dk_hi + adv, 1);
+          if constexpr (H1) {
+            wgmma_f16_n64_ra<0>(sv, qh + 4 * kk, dk_hi + adv, kk != 0);
+          } else {
+            wgmma_f16_n64_ra<0>(sv, ql + 4 * kk, dk_hi + adv, kk != 0);
+            wgmma_f16_n64_ra<0>(sv, qh + 4 * kk, dk_lo + adv, 1);
+            wgmma_f16_n64_ra<0>(sv, qh + 4 * kk, dk_hi + adv, 1);
+          }
         }
       };
-      auto issue_pv = [&](const uint32_t (&p)[2][16], uint32_t t) {    // O += P''_t . V_t
-        const uint32_t vh = sb + OFF_KV + (t % STAGES) * 4 * TILE + 2 * TILE, vl = vh + TILE;
+      auto issue_pv = [&](const uint32_t (&p)[PL][16], uint32_t t) {    // O += P''_t . V_t
+        const uint32_t vh = sb + OFF_KV + (t % STAGES) * L::STAGE + PL * TILE, vl = vh + TILE;
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {             // 16 keys per MMA: 16 rows of the MN-major V tile = 2 KiB
           const uint64_t dvh = desc_sw128(vh + kk * 2048), dvl = desc_sw128(vl + kk * 2048);
-          wgmma_f16_n64_ra<1>(o_acc, p[1] + 4 * kk, dvh, 1);
-          wgmma_f16_n64_ra<1>(o_acc, p[0] + 4 * kk, dvl, 1);
-          wgmma_f16_n64_ra<1>(o_acc, p[0] + 4 * kk, dvh, 1);
+          if constexpr (H1) {
+            wgmma_f16_n64_ra<1>(o_acc, p[0] + 4 * kk, dvh, 1);
+          } else {
+            wgmma_f16_n64_ra<1>(o_acc, p[PL - 1] + 4 * kk, dvh, 1);
+            wgmma_f16_n64_ra<1>(o_acc, p[0] + 4 * kk, dvl, 1);
+            wgmma_f16_n64_ra<1>(o_acc, p[0] + 4 * kk, dvh, 1);
+          }
         }
       };
       // online softmax of S (running tile t) into alpha, m_run, l_run and the P'' fragments p: a row's 64 keys sit in the
       // 4 lanes of a quad (16 each).  O *= alpha is left to the caller, once the P.V wgmmas of the tile before retired.
-      auto softmax = [&](uint32_t (&p)[2][16], uint32_t t) {
+      auto softmax = [&](uint32_t (&p)[PL][16], uint32_t t) {
         float nm[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -224,7 +248,8 @@ attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant_
             ps[h] += e0 + e1;
             // keys 8 jj + 2 qd (+1) of row rl0 + 8 h: word 2 (jj & 1) + h of k-step jj / 2
             const int wd = 4 * (jj >> 1) + 2 * (jj & 1) + h;
-            split2u(e0 * (w.x * p_scale), e1 * (w.y * p_scale), p[0][wd], p[1][wd]);
+            if constexpr (H1) p[0][wd] = pack_f16x2_sat(e0 * (w.x * p_scale), e1 * (w.y * p_scale));
+            else split2u(e0 * (w.x * p_scale), e1 * (w.y * p_scale), p[0][wd], p[PL - 1][wd]);
           }
         }
 #pragma unroll
@@ -238,7 +263,7 @@ attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant_
       };
       // tile j, its P'' in p: issue S_{j+1} (if `next`) and P''_j . V_j, run the softmax of S_{j+1} into pn while
       // P''_j . V_j is in flight, then retire both and free tile j's stage.  Nothing is in flight between two steps.
-      auto step = [&](const uint32_t (&p)[2][16], uint32_t (&pn)[2][16], int j, bool next) {
+      auto step = [&](const uint32_t (&p)[PL][16], uint32_t (&pn)[PL][16], int j, bool next) {
         const uint32_t t = it + j;
         if (next) wait_full(t + 1);
         reg_fence(sv);
@@ -290,7 +315,8 @@ attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant_
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const float2 ov = make_float2(o_acc[4 * jj + 2 * h] * inv, o_acc[4 * jj + 2 * h + 1] * inv);
-          if (a.o_hi != nullptr) store_split2(a.o_hi, a.o_lo, ooff + 8 * jj, ov);
+          if (H1 && a.o_hi != nullptr) *reinterpret_cast<uint32_t*>(a.o_hi + ooff + 8 * jj) = pack_f16x2_sat(ov.x, ov.y);
+          else if (a.o_hi != nullptr) store_split2(a.o_hi, a.o_lo, ooff + 8 * jj, ov);
           else *reinterpret_cast<float2*>(a.o + ooff + 8 * jj) = ov;
         }
       }
@@ -323,6 +349,53 @@ static int encode2d(CUtensorMap* m, const uint16_t* base, int cols, long long ro
   return OMT_OK;
 }
 
+// Launch of either form: h1 takes the hi planes alone (the lo pointers are NULL and their maps never loaded).
+template <bool H1>
+static int launch(const char* who, const uint16_t* q_hi, const uint16_t* q_lo, int ldq, const uint16_t* k_hi,
+                  const uint16_t* k_lo, int ldk, const uint16_t* v_hi, const uint16_t* v_lo, int ldv, const float* vinv,
+                  float qk_plane_scale, float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo, int n_seq, int N, int heads,
+                  float scale, cudaStream_t stream) {
+  using L = Smem<H1>;
+  OMT_REQUIRE(N > 0 && N % QT == 0, "%s: N=%d must be a multiple of 128", who, N);
+  OMT_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 4 == 0, "%s: bad leading dims", who);
+  OMT_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)k_hi | (uintptr_t)k_lo | (uintptr_t)v_hi | (uintptr_t)v_lo | (uintptr_t)vinv |
+               (uintptr_t)o | (uintptr_t)o_hi | (uintptr_t)o_lo) % 16 == 0, "%s: pointers must be 16-byte aligned", who);
+  OMT_REQUIRE(heads > 0 && heads <= 65535 && n_seq <= 65535 && qk_plane_scale > 0.f, "%s: bad arguments", who);
+  if (n_seq == 0) return OMT_OK;
+  const long long rows = (long long)n_seq * N;
+  const long long items = rows / QT * heads;
+  OMT_REQUIRE(rows < (1LL << 31) && items < (1LL << 31), "%s: n_seq * N = %lld rows is too many", who, rows);
+  CUtensorMap tmQh, tmQl, tmKh, tmKl, tmVh, tmVl;
+  int rc;
+  if ((rc = encode2d(&tmQh, q_hi, heads * D, rows, ldq))) return rc;
+  if ((rc = encode2d(&tmKh, k_hi, heads * D, rows, ldk))) return rc;
+  if ((rc = encode2d(&tmVh, v_hi, heads * D, rows, ldv))) return rc;
+  if (H1) {
+    tmQl = tmQh; tmKl = tmKh; tmVl = tmVh;
+  } else {
+    if ((rc = encode2d(&tmQl, q_lo, heads * D, rows, ldq))) return rc;
+    if ((rc = encode2d(&tmKl, k_lo, heads * D, rows, ldk))) return rc;
+    if ((rc = encode2d(&tmVl, v_lo, heads * D, rows, ldv))) return rc;
+  }
+  static int resident[64];     // CTAs of the kernel resident at once, per device (0: not queried yet)
+  int dev = 0;
+  OMT_CUDA(cudaGetDevice(&dev));
+  OMT_REQUIRE(dev >= 0 && dev < 64, "%s: device ordinal %d out of range", who, dev);
+  if (resident[dev] == 0) {
+    OMT_CUDA(cudaFuncSetAttribute(attn_f16_kernel<H1>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM));
+    int per_sm = 0, sms = 0;
+    OMT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attn_f16_kernel<H1>, THREADS, L::SMEM));
+    OMT_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    OMT_REQUIRE(per_sm > 0, "%s: no CTA fits on an SM of device %d", who, dev);
+    resident[dev] = per_sm * sms;
+  }
+  Args a{vinv, rows, o, o_hi, o_lo, ldo, N, heads, (int)items, scale * 1.4426950408889634f / qk_plane_scale};
+  const dim3 grid(items < resident[dev] ? (int)items : resident[dev]);
+  OMT_CUDA(launch_k(attn_f16_kernel<H1>, grid, dim3(THREADS), L::SMEM, stream, tmQh, tmQl, tmKh, tmKl, tmVh, tmVl, a));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
 }  // namespace af16
 }  // namespace omt
 
@@ -332,42 +405,19 @@ extern "C" int omt_attn_spatial_h(const uint16_t* q_hi, const uint16_t* q_lo, in
                                   const uint16_t* k_lo, int ldk, const uint16_t* v_hi, const uint16_t* v_lo, int ldv,
                                   const float* vinv, float qk_plane_scale, float* o, uint16_t* o_hi, uint16_t* o_lo, int ldo,
                                   int n_seq, int N, int heads, float scale, omt_stream_t stream) {
-  using namespace af16;
   OMT_ENTER();
   OMT_REQUIRE(q_hi && q_lo && k_hi && k_lo && v_hi && v_lo && vinv && (o || o_hi) && ((o_hi == nullptr) == (o_lo == nullptr)),
               "omt_attn_spatial_h: null pointer");
-  OMT_REQUIRE(N > 0 && N % QT == 0, "omt_attn_spatial_h: N=%d must be a multiple of 128", N);
-  OMT_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 4 == 0, "omt_attn_spatial_h: bad leading dims");
-  OMT_REQUIRE(((uintptr_t)q_hi | (uintptr_t)q_lo | (uintptr_t)k_hi | (uintptr_t)k_lo | (uintptr_t)v_hi | (uintptr_t)v_lo | (uintptr_t)vinv |
-               (uintptr_t)o | (uintptr_t)o_hi | (uintptr_t)o_lo) % 16 == 0, "omt_attn_spatial_h: pointers must be 16-byte aligned");
-  OMT_REQUIRE(heads > 0 && heads <= 65535 && n_seq <= 65535 && qk_plane_scale > 0.f, "omt_attn_spatial_h: bad arguments");
-  if (n_seq == 0) return OMT_OK;
-  const long long rows = (long long)n_seq * N;
-  const long long items = rows / QT * heads;
-  OMT_REQUIRE(rows < (1LL << 31) && items < (1LL << 31), "omt_attn_spatial_h: n_seq * N = %lld rows is too many", rows);
-  CUtensorMap tmQh, tmQl, tmKh, tmKl, tmVh, tmVl;
-  int rc;
-  if ((rc = encode2d(&tmQh, q_hi, heads * D, rows, ldq))) return rc;
-  if ((rc = encode2d(&tmQl, q_lo, heads * D, rows, ldq))) return rc;
-  if ((rc = encode2d(&tmKh, k_hi, heads * D, rows, ldk))) return rc;
-  if ((rc = encode2d(&tmKl, k_lo, heads * D, rows, ldk))) return rc;
-  if ((rc = encode2d(&tmVh, v_hi, heads * D, rows, ldv))) return rc;
-  if ((rc = encode2d(&tmVl, v_lo, heads * D, rows, ldv))) return rc;
-  static int resident[64];     // CTAs of the kernel resident at once, per device (0: not queried yet)
-  int dev = 0;
-  OMT_CUDA(cudaGetDevice(&dev));
-  OMT_REQUIRE(dev >= 0 && dev < 64, "omt_attn_spatial_h: device ordinal %d out of range", dev);
-  if (resident[dev] == 0) {
-    OMT_CUDA(cudaFuncSetAttribute(attn_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    int per_sm = 0, sms = 0;
-    OMT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attn_f16_kernel, THREADS, SMEM));
-    OMT_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    OMT_REQUIRE(per_sm > 0, "omt_attn_spatial_h: no CTA fits on an SM of device %d", dev);
-    resident[dev] = per_sm * sms;
-  }
-  Args a{vinv, rows, o, o_hi, o_lo, ldo, N, heads, (int)items, scale * 1.4426950408889634f / qk_plane_scale};
-  const dim3 grid(items < resident[dev] ? (int)items : resident[dev]);
-  OMT_CUDA(launch_k(attn_f16_kernel, grid, dim3(THREADS), SMEM, (cudaStream_t)stream, tmQh, tmQl, tmKh, tmKl, tmVh, tmVl, a));
-  OMT_LAUNCH_CHECK();
-  return OMT_OK;
+  return af16::launch<false>("omt_attn_spatial_h", q_hi, q_lo, ldq, k_hi, k_lo, ldk, v_hi, v_lo, ldv, vinv, qk_plane_scale,
+                             o, o_hi, o_lo, ldo, n_seq, N, heads, scale, (cudaStream_t)stream);
 }
+
+extern "C" int omt_attn_spatial_h1(const uint16_t* q_hi, int ldq, const uint16_t* k_hi, int ldk, const uint16_t* v_hi,
+                                   int ldv, const float* vinv, float qk_plane_scale, float* o, uint16_t* o_hi, int ldo,
+                                   int n_seq, int N, int heads, float scale, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(q_hi && k_hi && v_hi && vinv && (o || o_hi), "omt_attn_spatial_h1: null pointer");
+  return af16::launch<true>("omt_attn_spatial_h1", q_hi, nullptr, ldq, k_hi, nullptr, ldk, v_hi, nullptr, ldv, vinv,
+                            qk_plane_scale, o, o_hi, nullptr, ldo, n_seq, N, heads, scale, (cudaStream_t)stream);
+}
+

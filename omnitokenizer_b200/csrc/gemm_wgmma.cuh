@@ -8,6 +8,9 @@
 //                NACC = 2: lo planes carry 2^11, the cross products go to a second accumulator folded in as main + cross * 2^-11;
 //                NACC = 1: row-scaled planes, all three products share one accumulator, the epilogue multiplies by the exact
 //                inverse scales (a_rs[row] * w_scale).
+//   H1 = true   (f16x1, gemm_f16.cu omt_linear_h1): the throughput form.  A stage holds only A_hi and W_hi and each
+//                16-deep k-step issues ONE wgmma per 64-row half into the single accumulator; the epilogue applies the same
+//                row-scaled factor (the 2^11 form launches with both factors 1) and writes only the hi planes.
 //
 // Warp-specialised and persistent:
 //   * one producer warpgroup (one thread) issues every TMA load; two consumer warpgroups hold the accumulators in
@@ -43,12 +46,15 @@ constexpr int THREADS = 384;                  // warpgroup 0: producer; 1, 2: co
 constexpr int ORDER_BAR = 3;                  // ping-pong: named barriers 3, 4 ("consumer 0 / 1 may issue"); 1, 2 are wg_bar
 constexpr int STAGE_BYTES = 4 * 16384;        // A (hi), A_lo, W_hi, W_lo: 128 rows x 128 bytes each
 constexpr int STAGES = 3;
+// H1: a stage is A_hi | W_hi, half the bytes, so the ring holds twice as many 128-byte k-slabs in the same shared memory
+template <bool H1> __host__ __device__ constexpr int stage_bytes() { return H1 ? 2 * 16384 : STAGE_BYTES; }
+template <bool H1> __host__ __device__ constexpr int stages() { return H1 ? 2 * STAGES : STAGES; }
 // f16 GEGLU epilogue: per consumer warpgroup, the U planes of one 64-row half of a tile (64 rows x 64 columns x 2 planes)
 // staged in shared memory so that they leave as whole 128-byte rows.  Only those instantiations reserve it: the others
 // keep the larger L1 for their epilogue's loads.
 constexpr int EPI_STAGE_BYTES = 2 * 64 * 128;
-template <bool TF32, int EPI>
-constexpr int smem_bytes() { return STAGES * STAGE_BYTES + (!TF32 && EPI == OMT_EPI_GEGLU ? 2 * EPI_STAGE_BYTES : 0) + 1024; }
+template <bool TF32, int EPI, bool H1 = false>
+constexpr int smem_bytes() { return stages<H1>() * stage_bytes<H1>() + (!TF32 && EPI == OMT_EPI_GEGLU ? 2 * EPI_STAGE_BYTES : 0) + 1024; }
 // __launch_bounds__(384, 1) caps the kernel at 168 registers a thread: 40 * 128 + 232 * 256 == 168 * 384
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
@@ -73,7 +79,7 @@ struct Args {
 
 // Epilogue of one 64-row half of a tile on a consumer warpgroup's fragments (rows [m0 + 64 half, +64), columns [n0, +128)).
 // `stage` is the warpgroup's EPI_STAGE_BYTES of shared memory, `bar` its named barrier.
-template <bool TF32, int NACC, int EPI>
+template <bool TF32, int NACC, int EPI, bool H1>
 __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 2], const float (&crs)[NACC == 2 ? BN / 2 : 1],
                                          int m0, int n0, bool second, int half, int warp, int lane, uint8_t* stage, int bar) {
   const int qd = lane & 3;                      // column pair 8 j + 2 qd inside every 8-column block
@@ -164,7 +170,7 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
               uint32_t hw, lw;
               split2u(x[2 * j] * sc, x[2 * j + 1] * sc, hw, lw);
               *reinterpret_cast<uint32_t*>(g.u_hi + off + 8 * j) = hw;
-              *reinterpret_cast<uint32_t*>(g.u_lo + off + 8 * j) = lw;
+              if (!H1) *reinterpret_cast<uint32_t*>(g.u_lo + off + 8 * j) = lw;
             }
           }
         }
@@ -197,7 +203,7 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
           const int b = 8 * j + 2 * qd;             // byte of U column (8 j + 2 qd) / 2 in the row
           const int off = r * 128 + ((((b >> 4) ^ (r & 7)) << 4) | (b & 15));
           *reinterpret_cast<uint32_t*>(stage + off) = hw;
-          *reinterpret_cast<uint32_t*>(stage + 64 * 128 + off) = lw;
+          if (!H1) *reinterpret_cast<uint32_t*>(stage + 64 * 128 + off) = lw;
         }
       }
     }
@@ -213,7 +219,7 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
           const size_t off = (size_t)map_row(m, g.c_seg, g.c_seg_stride, g.c_seg_off) * g.ldu + uc + 8 * c;
           const int so = r * 128 + ((c ^ (r & 7)) << 4);
           *reinterpret_cast<uint4*>(g.u_hi + off) = *reinterpret_cast<const uint4*>(stage + so);
-          *reinterpret_cast<uint4*>(g.u_lo + off) = *reinterpret_cast<const uint4*>(stage + 64 * 128 + so);
+          if (!H1) *reinterpret_cast<uint4*>(g.u_lo + off) = *reinterpret_cast<const uint4*>(stage + 64 * 128 + so);
         }
       }
     }
@@ -245,7 +251,7 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
   }
 }
 
-template <bool TF32, int NACC, int EPI>
+template <bool TF32, int NACC, int EPI, bool H1 = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAl,
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmA2l,
@@ -254,10 +260,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   constexpr bool PINGPONG = !TF32 && NACC == 1;
   constexpr int HALVES = PINGPONG ? 2 : 1;    // 64-row halves of a tile one consumer warpgroup computes
   constexpr int A_BYTES = BM * 128, W_BYTES = BN * 128;
-  constexpr uint32_t TX_BYTES = TF32 ? A_BYTES + 2 * W_BYTES : 2 * A_BYTES + 2 * W_BYTES;
+  constexpr uint32_t TX_BYTES = H1 ? A_BYTES + W_BYTES : TF32 ? A_BYTES + 2 * W_BYTES : 2 * A_BYTES + 2 * W_BYTES;
+  constexpr int NS = stages<H1>(), SB = stage_bytes<H1>();
+  constexpr int W_OFF = H1 ? A_BYTES : 2 * A_BYTES;   // W_hi in a stage (W_lo follows it)
+  static_assert(!H1 || (!TF32 && NACC == 1), "the single-product form is the single-accumulator f16 kernel");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t full[STAGES], empty[STAGES];
+  __shared__ __align__(8) uint64_t full[NS], empty[NS];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int num_kb = g.K / BK;
@@ -265,9 +274,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int num_tiles = g.num_m_blk * num_n_blk;
 
   if (tid == 0) {
-    prefetch_map(&tmA); prefetch_map(&tmA2); prefetch_map(&tmWh); prefetch_map(&tmWl);
-    if (!TF32) { prefetch_map(&tmAl); prefetch_map(&tmA2l); }
-    for (int s = 0; s < STAGES; ++s) {
+    prefetch_map(&tmA); prefetch_map(&tmA2); prefetch_map(&tmWh);
+    if (!H1) prefetch_map(&tmWl);
+    if (!TF32 && !H1) { prefetch_map(&tmAl); prefetch_map(&tmA2l); }
+    for (int s = 0; s < NS; ++s) {
       mbar_init(&full[s], 1);                   // the producer's expect_tx
       mbar_init(&empty[s], PINGPONG ? 1 : 2);   // the warpgroup that owns the tile / both consumer warpgroups
     }
@@ -277,7 +287,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   pdl_sync();
 
   // Producer and consumers walk the same (tile, k-block) sequence; the running k-block count `it` alone gives the stage
-  // (it % STAGES) and the phase parity ((it / STAGES) & 1) of its full barrier.  The producer waits on the phase before
+  // (it % NS) and the phase parity ((it / NS) & 1) of its full barrier.  The producer waits on the phase before
   // it: a fresh empty barrier counts as released.
   // n fastest: W (at most a few MB of planes) stays in L2 while the CTAs running at the same time share the rows of A,
   // so A is read from HBM about once.  (m fastest re-reads all of A per n block once A outgrows L2.)
@@ -301,18 +311,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const CUtensorMap* mah = second ? &tmA2 : &tmA;
         const CUtensorMap* mal = second ? &tmA2l : &tmAl;
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % STAGES;
-          uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
-          mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
+          const int s = it % NS;
+          uint8_t* sp = smem + (size_t)s * SB;
+          mbar_wait(&empty[s], ((it / NS) & 1) ^ 1);
           mbar_expect_tx(&full[s], TX_BYTES);
           tma_load_3d(mah, &full[s], sp, kb * BK, c1[0], c2[0]);
           tma_load_3d(mah, &full[s], sp + A_BYTES / 2, kb * BK, c1[1], c2[1]);
-          if (!TF32) {
+          if (!TF32 && !H1) {
             tma_load_3d(mal, &full[s], sp + A_BYTES, kb * BK, c1[0], c2[0]);
             tma_load_3d(mal, &full[s], sp + A_BYTES + A_BYTES / 2, kb * BK, c1[1], c2[1]);
           }
-          tma_load_2d(&tmWh, &full[s], sp + 2 * A_BYTES, kb * BK, n0);
-          tma_load_2d(&tmWl, &full[s], sp + 2 * A_BYTES + W_BYTES, kb * BK, n0);
+          tma_load_2d(&tmWh, &full[s], sp + W_OFF, kb * BK, n0);
+          if (!H1) tma_load_2d(&tmWl, &full[s], sp + W_OFF + W_BYTES, kb * BK, n0);
         }
       }
     }
@@ -322,7 +332,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // every tile
     const int wg = (warp >> 2) - 1;
     auto release = [&](uint32_t i) {            // the wgmmas of k-block i have retired: free its stage
-      if ((tid & 127) == 0) mbar_arrive(&empty[i % STAGES]);
+      if ((tid & 127) == 0) mbar_arrive(&empty[i % NS]);
     };
     // Ping-pong order: before each tile but the CTA's first, a warpgroup waits on its barrier ORDER_BAR + wg; the owner
     // of the previous tile arrives on it once it has issued that tile's last k-block, and only if a next tile exists, so
@@ -342,9 +352,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (PINGPONG && tile != (int)blockIdx.x) named_bar_sync(ORDER_BAR + wg, 256);
 
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
-        const int s = it % STAGES;
-        uint8_t* sp = smem + (size_t)s * STAGE_BYTES;
-        mbar_wait(&full[s], (it / STAGES) & 1);
+        const int s = it % NS;
+        uint8_t* sp = smem + (size_t)s * SB;
+        mbar_wait(&full[s], (it / NS) & 1);
         if (TF32) {
           // this warpgroup's 64 rows of A (one 8 KiB box): tf32 hi in place, lo into the A_lo slot
           float4* a = reinterpret_cast<float4*>(sp + wg * (A_BYTES / 2));
@@ -364,7 +374,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           wg_bar(1 + wg);
         }
         const uint32_t sa = smem_u32(sp);
-        const uint64_t d_whi = desc_sw128(sa + 2 * A_BYTES), d_wlo = desc_sw128(sa + 2 * A_BYTES + W_BYTES);
+        const uint64_t d_whi = desc_sw128(sa + W_OFF), d_wlo = desc_sw128(sa + W_OFF + W_BYTES);
         wg_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {             // 32 bytes of the 128-byte row per MMA
@@ -373,7 +383,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           for (int h = 0; h < HALVES; ++h) {      // rows [64 r, +64) of the tile
             const int r = PINGPONG ? h : wg;
             const uint64_t d_ahi = desc_sw128(sa + r * (A_BYTES / 2)), d_alo = desc_sw128(sa + A_BYTES + r * (A_BYTES / 2));
-            if constexpr (TF32) {
+            if constexpr (H1) {
+              wgmma_f16_n128(acc[h], d_ahi + adv, d_whi + adv, 1);
+            } else if constexpr (TF32) {
               wgmma_tf32_n128(acc[h], d_alo + adv, d_whi + adv, 1);
               wgmma_tf32_n128(acc[h], d_ahi + adv, d_wlo + adv, 1);
               wgmma_tf32_n128(acc[h], d_ahi + adv, d_whi + adv, 1);
@@ -399,8 +411,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (PINGPONG) it += num_kb;               // the k-blocks of the other warpgroup's tile
 #pragma unroll
       for (int h = 0; h < HALVES; ++h)
-        epilogue<TF32, NACC, EPI>(g, acc[h], crs, m0, n0, second, PINGPONG ? h : wg, warp, lane,
-                                  smem + STAGES * STAGE_BYTES + wg * EPI_STAGE_BYTES, 1 + wg);
+        epilogue<TF32, NACC, EPI, H1>(g, acc[h], crs, m0, n0, second, PINGPONG ? h : wg, warp, lane,
+                                      smem + NS * SB + wg * EPI_STAGE_BYTES, 1 + wg);
     }
   }
 }
@@ -448,10 +460,10 @@ static inline int w_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const
   return encode_map(m, dt, ptr, 2, dims, strides, box);
 }
 
-template <bool TF32, int NACC, int EPI>
+template <bool TF32, int NACC, int EPI, bool H1 = false>
 static int launch(const CUtensorMap* maps, const Args& g, cudaStream_t st) {
-  auto kern = gemm_wgmma_kernel<TF32, NACC, EPI>;
-  constexpr int SMEM = smem_bytes<TF32, EPI>();
+  auto kern = gemm_wgmma_kernel<TF32, NACC, EPI, H1>;
+  constexpr int SMEM = smem_bytes<TF32, EPI, H1>();
   static int resident[64];     // CTAs of this kernel resident at once, per device (0: not queried yet)
   int dev = 0;
   OMT_CUDA(cudaGetDevice(&dev));

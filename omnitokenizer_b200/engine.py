@@ -21,8 +21,10 @@ import torch
 from . import _cabi
 from . import layout as L
 
-MATH_MODES = {"fp32": _cabi.MATH_FP32, "3xtf32": _cabi.MATH_3XTF32, "f16x3": _cabi.MATH_F16X3}
+# f16x1 is the opt-in throughput mode: one fp16 product per tensor-core product, NOT reference-exact (INTEGRATION.md)
+MATH_MODES = {"fp32": _cabi.MATH_FP32, "3xtf32": _cabi.MATH_3XTF32, "f16x3": _cabi.MATH_F16X3, "f16x1": _cabi.MATH_F16X1}
 DEFAULT_MATH = "f16x3"
+PLANE_MATHS = (_cabi.MATH_F16X3, _cabi.MATH_F16X1)    # modes whose GEMM operands are fp16 planes (shared weight packing)
 # largest codebook of the VQ search kernel (csrc/vq.cu): an eighth of the table (36 B per code) and the z rows of a 512-row
 # block (16 KB) share 200 KB of shared memory.  Launches of few rows take 256-row blocks and would fit 43 648 codes, but a
 # codebook must not work for small batches and fail for large ones.
@@ -47,7 +49,8 @@ class Planes:
 
 
 class PackedLinear:
-    """nn.Linear weight in GEMM layout: rows padded to 128, K padded, optional tf32 hi/lo split."""
+    """nn.Linear weight in GEMM layout: rows padded to 128, K padded, optional tf32 hi/lo split.  f16x1 packs the f16x3
+    planes and scales and keeps only the hi plane."""
 
     def __init__(self, weight: torch.Tensor, bias: Optional[torch.Tensor], device, math: int,
                  k_pad: Optional[int] = None, geglu: Optional[Tuple[int, int]] = None, row_scaled: bool = False):
@@ -59,19 +62,21 @@ class PackedLinear:
         if k_pad is not None:
             w = L.pad_cols(w, k_pad)
         self.k = w.shape[1]
-        w = L.pad_rows(w, 256 if math == _cabi.MATH_F16X3 else 128)
+        w = L.pad_rows(w, 256 if math in PLANE_MATHS else 128)
         if math == _cabi.MATH_3XTF32:
             hi = L.tf32_round(w)
             self.w, self.w_lo = hi, (w - hi).contiguous()
-        elif math == _cabi.MATH_F16X3 and row_scaled:
+        elif math in PLANE_MATHS and row_scaled:
             self.w, self.w_lo, self.w_scale = L.split_f16_rs(w)      # fp16 planes, one scale per matrix (single-accumulator GEMM)
-        elif math == _cabi.MATH_F16X3:
+        elif math in PLANE_MATHS:
             self.w, self.w_lo = L.split_f16(w)          # fp16 operand planes, lo scaled by 2^11 (two-accumulator GEMM)
         else:
             self.w, self.w_lo = w, None
+        if math == _cabi.MATH_F16X1:
+            self.w_lo = None                            # the single-product GEMM reads the hi plane only
         self.bias = None if bias is None else bias.detach().to(device=device, dtype=torch.float32).contiguous()
         self.math = math
-        self.row_scaled = row_scaled and math == _cabi.MATH_F16X3
+        self.row_scaled = row_scaled and math in PLANE_MATHS
 
 
 class Workspace:
@@ -197,7 +202,9 @@ class Engine:
         if not self.use_vae and self.cd != 8:
             raise NotImplementedError(f"--codebook_dim {self.cd}: the VQ search / post_vq kernels are specialised for "
                                       "codebook_dim 8 (every shipped config); VAE mode takes 8 latent channels as well")
-        self.planes = self.math == _cabi.MATH_F16X3
+        self.planes = self.math in PLANE_MATHS
+        # f16x1: every GEMM and the f16 spatial core take their single-product forms (omt_linear_h1, omt_attn_spatial_h1)
+        self.h1 = self.math == _cabi.MATH_F16X1
         # spatial attention core on fp16 operand planes (attention_f16.cu, default); OMT_ATTN_F16=0 = the 3xTF32 core on the fp32 QKV buffer
         self.attn_f16 = self.planes and os.environ.get("OMT_ATTN_F16", "1") == "1"
         # GEGLU output planes with a static (pack-time) scale -> the second FF GEMM takes the single-accumulator form (default).
@@ -363,7 +370,8 @@ class Engine:
     def _linear_h(self, A: Planes, lin: PackedLinear, M, *, C=None, ldc=0, U: Optional[Planes] = None, A2: Optional[Planes] = None,
                   n_split=0, a_map=(0, 0, 0), c_map=(0, 0, 0), residual=None, ldr=0, epi=_cabi.EPI_NONE, qk=None,
                   planes=None, a_uniform=0.0, u_scale=0.0):
-        """nn.Linear on operand planes (wgmma f16x3).  U: GEGLU output planes; qk: (q_scale, k_scale, cos, sin, qk_cols, tokens)."""
+        """nn.Linear on operand planes (wgmma f16x3, or f16x1: hi planes only).  U: GEGLU output planes;
+        qk: (q_scale, k_scale, cos, sin, qk_cols, tokens)."""
         if ((A.rs is not None) or a_uniform > 0.0) != lin.row_scaled:
             raise RuntimeError("operand planes and weight planes are in different f16x3 forms (row-scaled vs 2^11-scaled lo)")
         kw = dict(a_hi=A.hi, a_lo=A.lo, lda=A.ld, a_seg=a_map[0], a_seg_stride=a_map[1], a_seg_off=a_map[2],
@@ -383,7 +391,11 @@ class Engine:
             kw.update(q_scale=qk[0], k_scale=qk[1], rope_cos=qk[2], rope_sin=qk[3], qk_cols=qk[4], tokens=qk[5])
         if planes is not None:      # EPI_QKV_PLANES: U = the q | k | v planes, (q plane scale, k plane scale, vinv)
             kw.update(q_plane_scale=planes[0], k_plane_scale=planes[1], vinv=planes[2])
-        _cabi.linear_h(**kw)
+        if self.h1:
+            kw.update(a_lo=None, a2_lo=None, w_lo=None, u_lo=None)
+            _cabi.linear_h("omt_linear_h1", **kw)
+        else:
+            _cabi.linear_h(**kw)
 
     def _ln(self, x, y, g, b, M, C=None, seg=(0, 0, 0)):
         C = C or self.C
@@ -471,7 +483,11 @@ class Engine:
                                    None, None, None, None, 0, 0)
                         _cabi.call("omt_qk_prep", q_ptr, ld3, k_ptr, ld3, lyr["q_scale"], lyr["k_scale"], cos, sin, M, N,
                                    self.heads)
-                if f16_core:
+                if f16_core and self.h1:
+                    ph = ws.QKVp.hi.data_ptr()
+                    _cabi.call("omt_attn_spatial_h1", ph, ld3, ph + 2 * C, ld3, ph + 4 * C, ld3, ws.vinv, lyr["q_ps"] * lyr["k_ps"],
+                               None, o_hi, C, F, N, self.heads, 8.0)
+                elif f16_core:
                     ph, pl = ws.QKVp.hi.data_ptr(), ws.QKVp.lo.data_ptr()
                     _cabi.call("omt_attn_spatial_h", ph, pl, ld3, ph + 2 * C, pl + 2 * C, ld3, ph + 4 * C, pl + 4 * C, ld3,
                                ws.vinv, lyr["q_ps"] * lyr["k_ps"], None, o_hi, o_lo, C, F, N, self.heads, 8.0)

@@ -7,8 +7,8 @@
                                                        of every build are compared bit for bit with the first one's
 
 Forms: "rs" = the row-scaled single-accumulator f16x3 GEMM (LayerNorm / patch-gather fed), "2^11" = the two-accumulator
-f16x3 GEMM (2^11-scaled lo planes), "3xtf32" = the fp32-operand GEMM.  These are the three gemm_wgmma_kernel forms the
-engine launches.  In the K sweep the intercept a is the per-launch cost that does not grow with K: with a persistent grid
+f16x3 GEMM (2^11-scaled lo planes), "3xtf32" = the fp32-operand GEMM, "rs-h1" / "2^11-h1" = the single-product f16x1
+GEMM (omt_linear_h1) on the hi planes of the same operands.  These are the gemm_wgmma_kernel forms the engine launches.  In the K sweep the intercept a is the per-launch cost that does not grow with K: with a persistent grid
 it is mostly the per-tile work that the mainloop does not hide (the epilogue) plus the pipeline fill."""
 import argparse
 import ctypes
@@ -37,8 +37,9 @@ flush = torch.zeros(64 * 1024 * 1024, device=dev)
 def load_lib(path):
     lib = ctypes.CDLL(os.path.abspath(path))
     for name, (res, argtypes) in _cabi.SIGNATURES.items():
-        fn = getattr(lib, name)
-        fn.restype, fn.argtypes = res, argtypes
+        fn = getattr(lib, name, None)     # an older build lacks the newer entry points; its forms are timed without them
+        if fn is not None:
+            fn.restype, fn.argtypes = res, argtypes
     assert lib.omt_abi_version() == _cabi.ABI_VERSION, f"{path}: ABI version mismatch"
     return lib
 
@@ -79,29 +80,35 @@ def make(kind, form, M, K, g):
             Cq = torch.empty(M, Np, device=dev)
             return lambda: _cabi.call("omt_linear", A, Kp, 0, 0, 0, hi, lo, Cq, Np, 0, 0, 0, M, Np, Kp, None, None, 0, _cabi.EPI_NONE, _cabi.MATH_3XTF32), Np, [Cq]
         return lambda: _cabi.call("omt_linear", A, Kp, 0, 0, 0, hi, lo, R, C, 0, 0, 0, M, Np, Kp, None, R, C, _cabi.EPI_NONE, _cabi.MATH_3XTF32), Np, [R]
-    if form == "rs":
+    h1 = form.endswith("-h1")
+    if form.startswith("rs"):
         ah, al, ars = L.split_rows_rs(A); wh, wl, wsc = L.split_f16_rs(L.pad_rows(W, 256)); kw = dict(a_rs=ars, w_scale=wsc)
     else:
         ah, al = L.split_f16(A); wh, wl = L.split_f16(L.pad_rows(W, 256)); kw = {}
     kw.update(a_hi=ah, a_lo=al, lda=Kp, w_hi=wh, w_lo=wl, M=M, N=Np, K=Kp)
+
+    def linear_h(**k):     # omt_linear_h, or omt_linear_h1 with the lo planes left out
+        if h1:
+            return _cabi.linear_h("omt_linear_h1", **{f: v for f, v in k.items() if f not in ("a_lo", "a2_lo", "w_lo", "u_lo")})
+        return _cabi.linear_h(**k)
     if kind == "ff1+geglu":
         U = torch.empty(2, M, Np // 2, dtype=torch.int16, device=dev)
-        return lambda: _cabi.linear_h(u_hi=U[0], u_lo=U[1], ldu=Np // 2, epilogue=_cabi.EPI_GEGLU, **kw), Np, [U]
+        return lambda: linear_h(u_hi=U[0], u_lo=U[1], ldu=Np // 2, epilogue=_cabi.EPI_GEGLU, **kw), Np, [U]
     if kind == "qkv-planes":
         # the spatial-attention layer's launch: q from the normalised rows, k / v from the raw rows (dual A), rope +
         # l2norm + scale on q / k, q | k | v written as operand planes, N = 1024 tokens per frame
-        a2h, a2l, a2rs = (L.split_rows_rs(A.flip(1)) if form == "rs" else L.split_f16(A.flip(1)) + (None,))
+        a2h, a2l, a2rs = (L.split_rows_rs(A.flip(1)) if form.startswith("rs") else L.split_f16(A.flip(1)) + (None,))
         cos, sin = (t.to(dev).contiguous() for t in L.rope_tables(1024, C // HEADS))
         qs = torch.rand(C // HEADS, device=dev, generator=g) + 0.5; ks = torch.rand(C // HEADS, device=dev, generator=g) + 0.5
         U = torch.empty(2, M, Np, dtype=torch.int16, device=dev); vinv = torch.empty(HEADS, M, device=dev)
-        return lambda: _cabi.linear_h(a2_hi=a2h, a2_lo=a2l, a2_rs=a2rs, n_split=C, u_hi=U[0], u_lo=U[1], ldu=Np,
+        return lambda: linear_h(a2_hi=a2h, a2_lo=a2l, a2_rs=a2rs, n_split=C, u_hi=U[0], u_lo=U[1], ldu=Np,
                                       epilogue=_cabi.EPI_QKV_PLANES, q_scale=qs, k_scale=ks, rope_cos=cos, rope_sin=sin,
                                       qk_cols=2 * C, tokens=1024, q_plane_scale=2.0 ** 13, k_plane_scale=2.0 ** 13, vinv=vinv,
                                       **kw), Np, [U, vinv]
     if kind == "qkv":
         Cq = torch.empty(M, Np, device=dev)
-        return lambda: _cabi.linear_h(c=Cq, ldc=Np, epilogue=_cabi.EPI_NONE, **kw), Np, [Cq]
-    return lambda: _cabi.linear_h(c=R, ldc=C, residual=R, ldr=C, epilogue=_cabi.EPI_NONE, **kw), Np, [R]
+        return lambda: linear_h(c=Cq, ldc=Np, epilogue=_cabi.EPI_NONE, **kw), Np, [Cq]
+    return lambda: linear_h(c=R, ldc=C, residual=R, ldr=C, epilogue=_cabi.EPI_NONE, **kw), Np, [R]
 
 
 def run(kind, form, M, N, K):
@@ -146,7 +153,7 @@ else:
     SHAPES = [("qkv", 3 * C, C), ("qkv-planes", 3 * C, C), ("out+res", C, C), ("ff1+geglu", 2 * INNER, C), ("ff2+res", C, INNER)]
     for M in args.M:
         for kind, N, K in SHAPES:
-            for form in ("rs", "2^11", "3xtf32"):
+            for form in ("rs", "rs-h1", "2^11", "2^11-h1", "3xtf32"):
                 if kind == "qkv-planes" and form == "3xtf32":
                     continue
                 run(kind, form, M, N, K)

@@ -1,11 +1,12 @@
 """Device time per kernel of one warmed bench step, from torch.profiler (CUDA activities):
-   python scripts/kernel_breakdown.py [--math f16x3|3xtf32|fp32] [--workload cfg3|cfg2|cfg4|cfg5] [--top N]
+   python scripts/kernel_breakdown.py [--math f16x3|f16x1|3xtf32|fp32] [--workload cfg3|cfg2|cfg4|cfg5] [--top N]
 
 CUDA graphs are turned off (OMT_CUDA_GRAPH=0) so that every launch is its own event.  Kernels are grouped by name with
 the template arguments kept (they tell the GEMM instantiations apart) and the parameter list dropped; each line gives
 the launches, the device time, and the share of the step's summed device time.  For the f16x3 wgmma GEMM the script also
 records the shape of every omt_linear_h call and prints the achieved f16 tensor rate, 3 x 2MNK (three f16 products per
-fp32-grade product, launched N) over device time, next to the H100 SXM data-sheet dense f16 figure of 989 TFLOP/s."""
+fp32-grade product, launched N; 1 x 2MNK for the single-product f16x1 GEMM) over device time, next to the H100 SXM
+data-sheet dense f16 figure of 989 TFLOP/s."""
 import argparse
 import collections
 import os
@@ -67,10 +68,10 @@ def main():
     shapes = []                          # (M, N, K) of every omt_linear_h call of the profiled step, in launch order
     linear_h = _cabi.linear_h
 
-    def recording_linear_h(**kw):
+    def recording_linear_h(*a, **kw):
         if kw["M"] > 0:                  # M == 0 launches nothing
             shapes.append((kw["M"], kw["N"], kw["K"]))
-        return linear_h(**kw)
+        return linear_h(*a, **kw)
 
     _cabi.linear_h = recording_linear_h
     start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -93,7 +94,7 @@ def main():
         r[1] += e.time_range.elapsed_us()
     if rates:
         for e, (M, N, K) in zip(gemms, shapes):
-            by_name[kernel_name(e.name)][2] += 3 * 2.0 * M * N * K
+            by_name[kernel_name(e.name)][2] += (1 if args.math == "f16x1" else 3) * 2.0 * M * N * K
     print(f"device: {torch.cuda.get_device_name(dev)}   workload {args.workload}   math {args.math}")
     print(f"step (CUDA events, profiler on): {start.elapsed_time(end):.2f} ms   summed kernel time: {total_us / 1e3:.2f} ms"
           f"   launches: {len(kernels)}")
@@ -104,7 +105,7 @@ def main():
         rate = f"{fl / (us * 1e-6) / 1e12:7.1f} ({fl / (us * 1e-6) / 1e12 / F16_DATASHEET_TFLOPS:4.0%})" if fl else ""
         print(f"{us / 1e3:9.3f} {us / total_us:6.1%} {n:8d} {rate:>12}  {name}")
     if rates:
-        print(f"f16 TFLOP/s: 3 x 2MNK over device time; (%) of the {F16_DATASHEET_TFLOPS:.0f} TFLOP/s H100 SXM data-sheet "
+        print(f"f16 TFLOP/s: {1 if args.math == 'f16x1' else 3} x 2MNK over device time; (%) of the {F16_DATASHEET_TFLOPS:.0f} TFLOP/s H100 SXM data-sheet "
               f"dense f16 rate")
 
 

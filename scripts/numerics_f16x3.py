@@ -1,13 +1,15 @@
 """CPU numerics model of the fp16 hi/lo-split tensor-core path (OMT_MATH=f16x3) inside the oracle: every tensor-core
 product a.b is replaced by  hi(a).hi(b) + 2^-11 (hi(a).lo'(b) + lo'(a).hi(b)),  hi = fp16(x), lo' = fp16((x - hi) * 2^11),
 products exact, fp32 accumulation.  Prints flipped code indices and decoder pixel error per golden case, next to the
-3xTF32 model the shipped kernels implement."""
+3xTF32 model the shipped kernels implement and the single-product f16x1 model (tests/f16x1_model.py: row-scaled fp16 hi
+operands, one product, fp32 accumulation)."""
 import sys, os
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 from oracle import omni_oracle as oo
 from util import load_golden, golden_setup, check_sub
+from f16x1_model import mm_f16x1
 
 
 def _tf32_rna(x):
@@ -37,7 +39,7 @@ for name in names:
     if "idx" not in fx:
         continue
     with torch.no_grad():
-        for label, model in (("3xtf32", mm_3xtf32), ("f16x3", mm_f16x3), ("f16x2", mm_f16x2)):
+        for label, model in (("3xtf32", mm_3xtf32), ("f16x3", mm_f16x3), ("f16x2", mm_f16x2), ("f16x1", mm_f16x1)):
             oo.MATMUL_MODEL = model
             emb, idx = oo.encode(sd, cfg, x, include_embeddings=True)
             rec = oo.decode(sd, cfg, fx["idx"].long(), is_image)
