@@ -224,27 +224,43 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
       }
     }
   } else {
-    // plain: (+bias)(+residual); residual may alias C (each element is read and written by the same thread)
+    // plain: (+bias)(+residual).  residual may alias C, so the compiler may not move a residual load above a store to C:
+    // a load after a store waits out its own round trip to L2.  Every load of the half is therefore issued before its
+    // first store; that stays correct in place because each element is read and written by the same thread.  The sums
+    // go into v row by row, so a row's residual needs registers only until it is added (no spills in ping-pong, where
+    // the other half's accumulators are live).
+    const bool bias = g.bias != nullptr, res = g.residual != nullptr;
+    float2 bb[BN / 8];
+    long long prow[2];
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int n = n0 + 8 * j + 2 * qd;
+      bb[j] = bias && n < g.N ? __ldg(reinterpret_cast<const float2*>(g.bias + n)) : make_float2(0.f, 0.f);
+    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int m = mrow[h];
-      if (m < g.M) {
-        const long long prow = map_row(m, g.c_seg, g.c_seg_stride, g.c_seg_off);
+      prow[h] = map_row(m < g.M ? m : 0, g.c_seg, g.c_seg_stride, g.c_seg_off);
+      float2 rr[BN / 8];
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * qd;
+        rr[j] = res && m < g.M && n < g.N ? *reinterpret_cast<const float2*>(g.residual + prow[h] * g.ldr + n)
+                                          : make_float2(0.f, 0.f);
+      }
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        if (bias) { v[h][2 * j] += bb[j].x; v[h][2 * j + 1] += bb[j].y; }
+        if (res) { v[h][2 * j] += rr[j].x; v[h][2 * j + 1] += rr[j].y; }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (mrow[h] < g.M) {
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           const int n = n0 + 8 * j + 2 * qd;
-          if (n < g.N) {
-            float2 o = make_float2(v[h][2 * j], v[h][2 * j + 1]);
-            if (g.bias != nullptr) {
-              const float2 bb = __ldg(reinterpret_cast<const float2*>(g.bias + n));
-              o.x += bb.x; o.y += bb.y;
-            }
-            if (g.residual != nullptr) {
-              const float2 r = *reinterpret_cast<const float2*>(g.residual + prow * g.ldr + n);
-              o.x += r.x; o.y += r.y;
-            }
-            *reinterpret_cast<float2*>(g.c + prow * g.ldc + n) = o;
-          }
+          if (n < g.N) *reinterpret_cast<float2*>(g.c + prow[h] * g.ldc + n) = make_float2(v[h][2 * j], v[h][2 * j + 1]);
         }
       }
     }
