@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
+#include <initializer_list>
 #include "../../include/omnitok_b200.h"
 
 namespace omt {
@@ -29,6 +30,14 @@ int sm_count();
       return OMT_E_CUDA;                                                          \
     }                                                                             \
   } while (0)
+
+// Host check of the pointers a kernel reads or writes with vector accesses: every non-NULL one is a multiple of `bytes`.
+// A misaligned vector access is a device fault, so the entry points refuse such pointers before any launch.
+inline bool aligned_to(size_t bytes, std::initializer_list<const void*> ptrs) {
+  for (const void* p : ptrs)
+    if (reinterpret_cast<uintptr_t>(p) % bytes != 0) return false;
+  return true;
+}
 
 #define OMT_ENTER()                      \
   do {                                   \

@@ -591,7 +591,7 @@ __global__ void __launch_bounds__(256) peg_tile_kernel(const float* __restrict__
 //     temporal  f -> (f % T, f / T)  split is a multiply-shift on the in-row offset;
 //   * the 3x3x3 register window rotates by renaming (w loop unrolled by 3) instead of 36 MOVs per output;
 //   * channel pairs (float2) per thread: one 8-byte shared-memory load per pair and tap.
-// Requires T <= 64, w <= 254 (multiply-shift range) and 16-byte aligned x; the host falls back to v3 otherwise.
+// Requires T <= 64 and w <= 254 (multiply-shift range); the host falls back to v3 otherwise (x is 16-byte aligned for both).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float2 lds_f2(uint32_t addr) {
   float2 v;
@@ -797,6 +797,7 @@ static int layernorm_impl(const char* who, const float* x, int ldx, float* y, in
   OMT_REQUIRE(x && w && (y || pl.y_hi), "%s: null pointer", who);
   OMT_REQUIRE(M >= 0 && C > 0 && C % 4 == 0 && C <= 1024, "%s: C=%d must be a multiple of 4, <= 1024", who, C);
   OMT_REQUIRE(ldx % 4 == 0 && ldx >= C && (y == nullptr || (ldy % 4 == 0 && ldy >= C)), "%s: bad leading dims", who);
+  OMT_REQUIRE(aligned_to(16, {x, y, w, b}), "%s: x, y, w and b must be 16-byte aligned", who);
   OMT_REQUIRE((pl.y_hi == nullptr) == (pl.y_lo == nullptr) && (pl.x_hi == nullptr) == (pl.x_lo == nullptr), "%s: planes come in hi / lo pairs", who);
   if (pl.y_hi != nullptr || pl.x_hi != nullptr) {
     OMT_REQUIRE(pl.lds % 4 == 0 && pl.lds >= C, "%s: plane leading dimension %d", who, pl.lds);
@@ -848,6 +849,7 @@ extern "C" int omt_patchify_ln(const float* video, float* A, uint16_t* A_hi, uin
   OMT_ENTER();
   OMT_REQUIRE(video && (A || A_hi) && ((ln_w == nullptr) == (ln_b == nullptr)) && ((A_hi == nullptr) == (A_lo == nullptr)),
               "omt_patchify_ln: null pointer");
+  OMT_REQUIRE(aligned_to(16, {video, A, ln_w, ln_b}), "omt_patchify_ln: video, A, ln_w and ln_b must be 16-byte aligned");
   OMT_REQUIRE(((uintptr_t)A_hi | (uintptr_t)A_lo) % 8 == 0, "omt_patchify_ln: planes must be 8-byte aligned");
   OMT_REQUIRE(A_rs == nullptr || A_hi != nullptr, "omt_patchify_ln: row scales without planes");
   OMT_REQUIRE(p % 4 == 0 && H % p == 0 && W % p == 0, "omt_patchify_ln: patch %d must be a multiple of 4 dividing %dx%d", p, H, W);
@@ -876,6 +878,7 @@ extern "C" int omt_patchify_ln_u8(const uint8_t* frames, const float* lut, const
   OMT_ENTER();
   OMT_REQUIRE(frames && lut && (A || A_hi) && ((ln_w == nullptr) == (ln_b == nullptr)) && ((A_hi == nullptr) == (A_lo == nullptr)),
               "omt_patchify_ln_u8: null pointer");
+  OMT_REQUIRE(aligned_to(16, {A, ln_w, ln_b}), "omt_patchify_ln_u8: A, ln_w and ln_b must be 16-byte aligned");
   OMT_REQUIRE(((uintptr_t)A_hi | (uintptr_t)A_lo) % 8 == 0, "omt_patchify_ln_u8: planes must be 8-byte aligned");
   OMT_REQUIRE((uintptr_t)frames % 4 == 0, "omt_patchify_ln_u8: frames must be 4-byte aligned");
   OMT_REQUIRE(A_rs == nullptr || A_hi != nullptr, "omt_patchify_ln_u8: row scales without planes");
@@ -924,6 +927,7 @@ extern "C" int omt_unpatchify(const float* P, float* video, int B, int Cin, int 
                               int pt, int first, omt_stream_t stream) {
   OMT_ENTER();
   OMT_REQUIRE(P && video, "omt_unpatchify: null pointer");
+  OMT_REQUIRE(aligned_to(16, {P, video}), "omt_unpatchify: P and video must be 16-byte aligned");
   OMT_REQUIRE(p % 4 == 0 && H % p == 0 && W % p == 0, "omt_unpatchify: bad patch size");
   OMT_REQUIRE(first || (T > 1 && (T - 1) % pt == 0), "omt_unpatchify: (T-1) %% pt != 0");
   const int PT = first ? 1 : pt;
@@ -941,6 +945,7 @@ extern "C" int omt_unpatchify_u8(const float* P, uint8_t* out, int B, int Cin, i
                                  int first, float mul, float add, float lo, float hi, float post, omt_stream_t stream) {
   OMT_ENTER();
   OMT_REQUIRE(P && out, "omt_unpatchify_u8: null pointer");
+  OMT_REQUIRE(aligned_to(16, {P}), "omt_unpatchify_u8: P must be 16-byte aligned");
   OMT_REQUIRE(p % 4 == 0 && H % p == 0 && W % p == 0, "omt_unpatchify_u8: bad patch size");
   OMT_REQUIRE(first || (T > 1 && (T - 1) % pt == 0), "omt_unpatchify_u8: (T-1) %% pt != 0");
   OMT_REQUIRE(lo >= 0.f && hi * post < 256.f, "omt_unpatchify_u8: clamp range [%g, %g] x %g does not fit a byte", lo, hi, post);
@@ -961,6 +966,7 @@ extern "C" int omt_peg(const float* x, float* y, const float* w27, const float* 
   OMT_ENTER();
   OMT_REQUIRE(x && y && w27 && bias && nbr, "omt_peg: null pointer");
   OMT_REQUIRE(x != y, "omt_peg: in-place is not supported (stencil)");
+  OMT_REQUIRE(aligned_to(16, {x, y, w27, bias}), "omt_peg: x, y, w27 and bias must be 16-byte aligned");
   OMT_REQUIRE(C % 4 == 0 && C / 4 <= 128, "omt_peg: C=%d unsupported (need C %% 4 == 0, C <= 512)", C);
   const long long M = (long long)B * rows_per_b;
   if (M == 0) return OMT_OK;
@@ -985,6 +991,9 @@ static int peg_volume_launch(const char* who, const float* x, float* y, const fl
                              omt_stream_t stream) {
   OMT_REQUIRE(x && y && w27 && bias, "%s: null pointer", who);
   OMT_REQUIRE(x != y, "%s: in-place is not supported (stencil)", who);
+  // both tile kernels gather x in 16-byte chunks and read w27 / bias and write y in channel pairs
+  OMT_REQUIRE(aligned_to(16, {x}), "%s: x must be 16-byte aligned", who);
+  OMT_REQUIRE(aligned_to(8, {y, w27, bias}), "%s: y, w27 and bias must be 8-byte aligned", who);
   OMT_REQUIRE(C % PEG_CC == 0 && C / PEG_CC <= 65535 && B <= 65535, "%s: C=%d must be a multiple of 16", who, C);
   OMT_REQUIRE(T >= 1 && h >= 1 && w >= 1, "%s: bad volume", who);
   if (B == 0) return OMT_OK;
@@ -1006,7 +1015,7 @@ static int peg_volume_launch(const char* who, const float* x, float* y, const fl
   }
   const int threads = ((TT * HB * 8 + 31) / 32) * 32;
   dim3 grid(((T + TT - 1) / TT) * ((h + HB - 1) / HB), C / PEG_CC, B);
-  const bool fast_ok = T <= 64 && w <= 254 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
+  const bool fast_ok = T <= 64 && w <= 254;
   const bool v4 = g_peg_kernel == 4 && fast_ok;
   if (v4) {
     // planes of a tile that lie inside the volume (the others are one shared zero row): the maximum over the t-blocks
@@ -1055,6 +1064,7 @@ extern "C" int omt_qk_prep(float* q, int ldq, float* k, int ldk, const float* q_
   OMT_REQUIRE(q && k && q_scale && k_scale, "omt_qk_prep: null pointer");
   OMT_REQUIRE((rope_cos == nullptr) == (rope_sin == nullptr), "omt_qk_prep: cos/sin must both be given");
   OMT_REQUIRE(ldq % 2 == 0 && ldk % 2 == 0 && N > 0, "omt_qk_prep: bad leading dims");
+  OMT_REQUIRE(aligned_to(8, {q, k, q_scale, k_scale}), "omt_qk_prep: q, k, q_scale and k_scale must be 8-byte aligned");
   if (M == 0) return OMT_OK;
   OMT_CUDA(launch_k(qk_prep_kernel, dim3((M + 7) / 8), dim3(256), 0, (cudaStream_t)stream, q, ldq, k, ldk, q_scale, k_scale,
                     rope_cos, rope_sin, M, N, heads));

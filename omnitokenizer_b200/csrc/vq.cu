@@ -322,6 +322,7 @@ extern "C" int omt_pre_vq(const float* x, int ldx, const float* Wt, const float*
   OMT_ENTER();
   OMT_REQUIRE(x && Wt && b && z, "omt_pre_vq: null pointer");
   OMT_REQUIRE(C % 4 == 0 && ldx % 4 == 0 && C <= 1024, "omt_pre_vq: bad C/ldx");
+  OMT_REQUIRE(aligned_to(16, {x, Wt}), "omt_pre_vq: x and Wt must be 16-byte aligned");
   OMT_REQUIRE(cd == 8 || cd == 16, "omt_pre_vq: codebook_dim %d unsupported (8 or 16)", cd);
   if (M == 0) return OMT_OK;
   cudaStream_t st = (cudaStream_t)stream;
@@ -384,6 +385,7 @@ extern "C" int omt_vq_search(const float* z, const float* E, const float* e2, in
                              int64_t* idx, int32_t* counts, omt_stream_t stream) {
   OMT_ENTER();
   OMT_REQUIRE(z && E && e2 && idx, "omt_vq_search: null pointer");
+  OMT_REQUIRE(aligned_to(16, {z, E}), "omt_vq_search: z and E must be 16-byte aligned");
   if (M == 0) return OMT_OK;
   return vq_launch(false, nullptr, 0, nullptr, nullptr, 0, 0, z, nullptr, E, e2, M, n_codes, idx, counts, (cudaStream_t)stream);
 }
@@ -394,6 +396,7 @@ extern "C" int omt_vq_fused(const float* x, int ldx, const float* Wt, const floa
   OMT_ENTER();
   OMT_REQUIRE(x && Wt && b && E && e2 && idx, "omt_vq_fused: null pointer");
   OMT_REQUIRE(C % 4 == 0 && ldx % 4 == 0 && C <= 1024, "omt_vq_fused: bad C/ldx");
+  OMT_REQUIRE(aligned_to(16, {x, Wt, z, E}), "omt_vq_fused: x, Wt, z and E must be 16-byte aligned");
   if (M == 0) return OMT_OK;
   return vq_launch(true, x, ldx, Wt, b, C, l2, nullptr, z, E, e2, M, n_codes, idx, counts, (cudaStream_t)stream);
 }
@@ -405,6 +408,7 @@ extern "C" int omt_post_vq(const int64_t* idx, const float* E, const float* zc, 
   OMT_REQUIRE(Wt && b && X, "omt_post_vq: null pointer");
   OMT_REQUIRE((idx != nullptr && E != nullptr) || zc != nullptr, "omt_post_vq: need idx+E or zc");
   OMT_REQUIRE(C % 4 == 0 && C <= 512, "omt_post_vq: C=%d unsupported", C);
+  OMT_REQUIRE(aligned_to(16, {X, b}), "omt_post_vq: X and b must be 16-byte aligned");
   OMT_REQUIRE(cd == 8, "omt_post_vq: codebook_dim %d unsupported (8)", cd);
   if (M == 0) return OMT_OK;
   OMT_CUDA(launch_k(post_vq_kernel<8>, dim3((M + POSTVQ_ROWS - 1) / POSTVQ_ROWS), dim3(128), 0, (cudaStream_t)stream,
