@@ -115,6 +115,31 @@ int omt_patchify_ln_u8(const uint8_t* frames, const float* lut, const int32_t* s
  * no host sync): two launches, safe inside a captured CUDA graph. */
 int omt_u8_norm_select(const uint8_t* frames, int B, long long per_sample, int32_t* sel, omt_stream_t stream);
 
+/* One image of omt_resample_u8.  Offsets into tab count int32 entries. */
+typedef struct {
+  long long src;          /* byte offset of the image's (H, W, 3) bytes in src */
+  int H, W;               /* source size */
+  int rh, rw;             /* size after the resize */
+  int y0, x0;             /* crop origin in the resized image (0, 0 without a crop) */
+  int flip;               /* 1: the output is mirrored left-right */
+  int need_h, need_v;     /* 0: that axis keeps its size and Pillow skips the pass (rw == W / rh == H) */
+  int hb, hc, hk;         /* horizontal: (xmin, n) bounds [rw][2] at tab + hb, coefficients [rw][hk] at tab + hc */
+  int vb, vc, vk;         /* vertical: the same over rh */
+  int v_first;            /* 1: vertical pass first (Pillow's Image.resize for H > 100 W shrinking in height); needs both passes */
+} omt_resample_desc;
+
+/* Pillow's 8-bit resize (libImaging/Resample.c, horizontal then vertical int32 pass, 22-bit fixed point, clip8 after
+ * each pass) of a ragged batch of (H_i, W_i, 3) uint8 images, then the loaders' RandomCrop / RandomHorizontalFlip as
+ * index maps: out (B, oh, ow, 3) uint8, image b = crop(resize(image b))[y0 : y0 + oh, x0 : x0 + ow], mirrored if flip.
+ * The bounds and coefficients come from the host (Resample.c precompute_coeffs + normalize_coeffs_8bpc in float64), so
+ * the bytes equal Pillow's.  src: packed source bytes (src_bytes of them); desc [B]: device table; tab [tab_len] int32.
+ * desc_host / tab_host: the same two tables in host memory, checked before the launch (every image inside src, every
+ * table inside tab, every tap inside its source axis, the crop inside the resized image); they must equal the device
+ * copies.  tab == tab_host == NULL with tab_len == 0 when no image needs a pass. */
+int omt_resample_u8(const uint8_t* src, long long src_bytes, const omt_resample_desc* desc,
+                    const omt_resample_desc* desc_host, const int32_t* tab, const int32_t* tab_host, long long tab_len,
+                    int B, int oh, int ow, uint8_t* out, omt_stream_t stream);
+
 /* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W). */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,
                    int first, omt_stream_t stream);

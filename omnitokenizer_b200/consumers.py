@@ -10,11 +10,11 @@ OmniTokenizer_VQGAN API; with this package's module the uint8 conversions run fu
 """
 from __future__ import annotations
 
-from typing import Optional, Tuple
+from typing import Optional, Sequence, Tuple
 
 import torch
 
-from .layout import U8Norm, u8_normalize
+from .layout import U8Norm, U8Resize, dit_resize, resize_params, resize_u8, u8_normalize
 
 LATENT_SCALE = 0.18215            # Diffusion/DiT/train.py:242, Diffusion/Latte/train.py:216
 
@@ -192,3 +192,48 @@ def latte_encode_latents_u8(vae, clips: torch.Tensor, norm: U8Norm = LATTE_NORM)
     scaled latents 'b f c h w'."""
     z = _encode_u8(vae, clips, False, norm).mul_(LATENT_SCALE)
     return z.permute(0, 2, 1, 3, 4).contiguous()              # 'b c f h w -> b f c h w'
+
+
+# ----------------------------------------------------------------------------------------------- decoded images, any size
+# The image callers' loaders resize every decoded image with Pillow before ToTensor (U8Resize presets in layout.py).  With
+# this package's module that transform runs on the device (encode_images_u8 / forward_images_u8: omt_resample_u8, byte for
+# byte Pillow's); any other object gets the same bytes from the host twin layout.resize_u8, then the uint8 path above.
+def _host_transform(images: Sequence[torch.Tensor], resize: U8Resize) -> torch.Tensor:
+    images = list(images)
+    params = resize_params(len(images), resize)
+    return torch.stack([resize_u8(im, resize, p) for im, p in zip(images, params)])
+
+
+@torch.no_grad()
+def eval_step_images_u8(vqgan, images: Sequence[torch.Tensor], resize: U8Resize, total_usage: Optional[torch.Tensor] = None,
+                        norm: U8Norm = IMAGE_NORM):
+    """eval_step_u8 over the decoded images of vqgan_eval.py's image loop (ImageDataset, OmniTokenizer/data.py:93-99:
+    resize = layout.image_resize(resolution)), ragged (H_i, W_i, 3) uint8 host tensors.  Returns (frames uint8
+    (B, 1, h, w, 3), vq_output)."""
+    if hasattr(vqgan, "forward_images_u8"):
+        out, vq_output = vqgan.forward_images_u8(images, resize, norm, EVAL_U8)
+        if total_usage is not None and vq_output is not None:
+            total_usage += vq_output["batch_usage"]
+        return out, vq_output
+    return eval_step_u8(vqgan, _host_transform(images, resize), total_usage, norm)
+
+
+@torch.no_grad()
+def encode_to_z_images_u8(vqgan, images: Sequence[torch.Tensor], resize: U8Resize,
+                          norm: U8Norm = IMAGE_NORM) -> Tuple[torch.Tensor, torch.Tensor]:
+    """encode_to_z (lm_transformer.py:258-268) of the LM's image stage from its decoded images (ImageDataset transform)."""
+    if hasattr(vqgan, "encode_images_u8"):
+        emb, targets = vqgan.encode_images_u8(images, resize, norm, include_embeddings=True)
+    else:
+        emb, targets = _encode_u8(vqgan, _host_transform(images, resize), True, norm, include_embeddings=True)
+    return _z_wire_format(emb, targets, 0)
+
+
+@torch.no_grad()
+def dit_encode_latents_images_u8(vae, images: Sequence[torch.Tensor], image_size: int, norm: U8Norm = IMAGE_NORM) -> torch.Tensor:
+    """dit_encode_latents from DiT's decoded images with the OmniTokenizer VAE (Diffusion/DiT/train.py:192-198:
+    Resize((s, s)) bilinear, RandomHorizontalFlip, ToTensor, Normalize(.5, 1) = IMAGE_NORM; then :242)."""
+    resize = dit_resize(image_size)
+    if hasattr(vae, "encode_images_u8"):
+        return vae.encode_images_u8(images, resize, norm).mul_(LATENT_SCALE)
+    return _encode_u8(vae, _host_transform(images, resize), True, norm).mul_(LATENT_SCALE)

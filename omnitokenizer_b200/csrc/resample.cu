@@ -1,0 +1,208 @@
+// omt_resample_u8: Pillow's 8-bit resize (libImaging/Resample.c, ImagingResampleHorizontal_8bpc / _Vertical_8bpc) of a
+// ragged batch of uint8 RGB images, with the loaders' random crop and horizontal flip as output index maps.
+//
+// Pillow resizes in two int32 passes over 22-bit fixed-point coefficients: horizontal (source rows -> an 8-bit
+// intermediate image, clip8 per byte), then vertical.  The coefficients are computed on the host in float64 exactly as
+// precompute_coeffs + normalize_coeffs_8bpc do (layout.resample_coeffs); this kernel only does the integer arithmetic,
+// so its bytes are Pillow's.  Each CTA owns an RS_TW x RS_TH output tile of one image: the horizontal pass covers only the
+// source rows the tile's vertical taps reach and lands in shared memory as clip8'ed bytes (Pillow's intermediate image),
+// in chunks of RS_CHUNK rows, so any tap count (5 for a bicubic upscale, 65 for a 16x downscale, hundreds beyond) fits.
+// Integer sums are exact, so splitting a column's vertical taps across chunks changes nothing.  Pillow's Image.resize
+// runs the vertical pass first for images taller than 100x their width (v_first); those few go byte by byte.
+#include "omt_common.cuh"
+#include <limits.h>
+
+using namespace omt;
+
+namespace {
+
+constexpr int RS_TW = 64;        // output columns per tile (one per thread of a row group)
+constexpr int RS_TH = 16;        // output rows per tile
+constexpr int RS_THREADS = 256;  // 4 row groups of 64 threads
+constexpr int RS_GROUPS = RS_THREADS / RS_TW;
+constexpr int RS_CHUNK = 128;    // intermediate rows in shared memory at a time: 128 x 64 x 3 B = 24 KB
+constexpr int RS_PREC = 22;      // Resample.c PRECISION_BITS (32 - 8 - 2)
+
+__device__ __forceinline__ int clip8(int v) {   // Resample.c clip8
+  return v >= (1 << RS_PREC << 8) ? 255 : (v <= 0 ? 0 : (v >> RS_PREC));
+}
+
+__global__ void __launch_bounds__(RS_THREADS)
+resample_u8_kernel(const uint8_t* __restrict__ src, const omt_resample_desc* __restrict__ desc,
+                   const int32_t* __restrict__ tab, uint8_t* __restrict__ out, int oh, int ow) {
+  __shared__ uint8_t inter[RS_CHUNK][RS_TW * 3];
+  pdl_sync();
+  const omt_resample_desc d = desc[blockIdx.z];
+  const int ox0 = blockIdx.x * RS_TW, oy0 = blockIdx.y * RS_TH;
+  const int th = min(RS_TH, oh - oy0);
+  const int lc = threadIdx.x % RS_TW, rg = threadIdx.x / RS_TW;
+  const int ox = ox0 + lc;
+  const bool col_ok = ox < ow;
+  const uint8_t* img = src + d.src;
+
+  // source rows [ys, ye) the tile's vertical taps reach (the crop shifts rows; a flip only mirrors columns)
+  int ys = INT_MAX, ye = 0;
+  for (int i = 0; i < th; ++i) {
+    const int ry = d.y0 + oy0 + i;
+    const int a = d.need_v ? __ldg(tab + d.vb + 2 * ry) : ry;
+    const int n = d.need_v ? __ldg(tab + d.vb + 2 * ry + 1) : 1;
+    ys = min(ys, a);
+    ye = max(ye, a + n);
+  }
+
+  // this thread's column of the resized image and its horizontal taps
+  const int rx = d.flip ? d.x0 + (ow - 1 - ox) : d.x0 + ox;
+  int hx = rx, hn = 1;
+  const int32_t* hk = nullptr;
+  if (col_ok && d.need_h) {
+    hx = __ldg(tab + d.hb + 2 * rx);
+    hn = __ldg(tab + d.hb + 2 * rx + 1);
+    hk = tab + d.hc + (long long)rx * d.hk;
+  }
+
+  constexpr int RPT = RS_TH / RS_GROUPS;
+  if (d.v_first) {   // tall images (H > 100 W): vertical, clip8, then horizontal, per output byte straight from the source
+    if (!col_ok) return;
+    for (int j = 0; j < RPT; ++j) {
+      const int i = rg + j * RS_GROUPS;
+      if (i >= th) break;
+      const int ry = d.y0 + oy0 + i;
+      const int a = __ldg(tab + d.vb + 2 * ry), n = __ldg(tab + d.vb + 2 * ry + 1);
+      const int32_t* vk = tab + d.vc + (long long)ry * d.vk;
+      int s[3] = {1 << (RS_PREC - 1), 1 << (RS_PREC - 1), 1 << (RS_PREC - 1)};
+      for (int x = 0; x < hn; ++x) {
+        const uint8_t* p = img + ((long long)a * d.W + hx + x) * 3;
+        int v[3] = {1 << (RS_PREC - 1), 1 << (RS_PREC - 1), 1 << (RS_PREC - 1)};
+        for (int y = 0; y < n; ++y, p += (long long)d.W * 3) {
+          const int k = __ldg(vk + y);
+#pragma unroll
+          for (int c = 0; c < 3; ++c) v[c] += __ldg(p + c) * k;
+        }
+        const int k = __ldg(hk + x);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) s[c] += clip8(v[c]) * k;
+      }
+      uint8_t* o = out + (((long long)blockIdx.z * oh + oy0 + i) * ow + ox) * 3;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) o[c] = (uint8_t)clip8(s[c]);
+    }
+    return;
+  }
+
+  // rows rg, rg + 4, ... of the tile: vertical accumulators (or, without a vertical pass, the copied bytes)
+  int acc[RPT][3];
+#pragma unroll
+  for (int j = 0; j < RPT; ++j) acc[j][0] = acc[j][1] = acc[j][2] = d.need_v ? 1 << (RS_PREC - 1) : 0;
+
+  for (int c0 = ys; c0 < ye; c0 += RS_CHUNK) {
+    const int c1 = min(ye, c0 + RS_CHUNK);
+    __syncthreads();                                   // the previous chunk has been read
+    if (col_ok) {
+      for (int r = c0 + rg; r < c1; r += RS_GROUPS) {
+        const uint8_t* row = img + (long long)r * d.W * 3;
+        uint8_t* o = &inter[r - c0][lc * 3];
+        if (d.need_h) {
+          int s0 = 1 << (RS_PREC - 1), s1 = s0, s2 = s0;
+          const uint8_t* p = row + hx * 3;
+          for (int x = 0; x < hn; ++x, p += 3) {
+            const int k = __ldg(hk + x);
+            s0 += __ldg(p) * k;
+            s1 += __ldg(p + 1) * k;
+            s2 += __ldg(p + 2) * k;
+          }
+          o[0] = (uint8_t)clip8(s0);
+          o[1] = (uint8_t)clip8(s1);
+          o[2] = (uint8_t)clip8(s2);
+        } else {
+          o[0] = __ldg(row + rx * 3);
+          o[1] = __ldg(row + rx * 3 + 1);
+          o[2] = __ldg(row + rx * 3 + 2);
+        }
+      }
+    }
+    __syncthreads();
+    if (col_ok) {
+#pragma unroll
+      for (int j = 0; j < RPT; ++j) {
+        const int i = rg + j * RS_GROUPS;
+        if (i >= th) continue;
+        const int ry = d.y0 + oy0 + i;
+        if (d.need_v) {
+          const int a = __ldg(tab + d.vb + 2 * ry), n = __ldg(tab + d.vb + 2 * ry + 1);
+          const int32_t* vk = tab + d.vc + (long long)ry * d.vk;
+          const int y1 = min(a + n, c1);
+          for (int y = max(a, c0); y < y1; ++y) {
+            const int k = __ldg(vk + (y - a));
+            const uint8_t* p = &inter[y - c0][lc * 3];
+            acc[j][0] += p[0] * k;
+            acc[j][1] += p[1] * k;
+            acc[j][2] += p[2] * k;
+          }
+        } else if (ry >= c0 && ry < c1) {
+          const uint8_t* p = &inter[ry - c0][lc * 3];
+          acc[j][0] = p[0];
+          acc[j][1] = p[1];
+          acc[j][2] = p[2];
+        }
+      }
+    }
+  }
+
+  if (!col_ok) return;
+#pragma unroll
+  for (int j = 0; j < RPT; ++j) {
+    const int i = rg + j * RS_GROUPS;
+    if (i >= th) continue;
+    uint8_t* o = out + (((long long)blockIdx.z * oh + oy0 + i) * ow + ox) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = (uint8_t)(d.need_v ? clip8(acc[j][c]) : acc[j][c]);
+  }
+}
+
+// One axis of a descriptor: its (xmin, n) bounds [out][2] at `b` and coefficients [out][k] at `c` lie inside the table,
+// and every output index's taps lie inside the source axis of length `in`.
+bool axis_ok(const int32_t* tab_host, long long tab_len, int b, int c, int k, int out, int in) {
+  if (b < 0 || c < 0 || k < 1 || b + 2LL * out > tab_len || c + (long long)out * k > tab_len) return false;
+  for (int i = 0; i < out; ++i) {
+    const int xmin = tab_host[b + 2 * i], n = tab_host[b + 2 * i + 1];
+    if (xmin < 0 || n < 0 || n > k || (long long)xmin + n > in) return false;
+  }
+  return true;
+}
+
+}  // namespace
+
+extern "C" int omt_resample_u8(const uint8_t* src, long long src_bytes, const omt_resample_desc* desc,
+                               const omt_resample_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
+                               long long tab_len, int B, int oh, int ow, uint8_t* out, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(src && desc && desc_host && out && ((tab == nullptr) == (tab_host == nullptr)) && ((tab == nullptr) == (tab_len == 0)),
+              "omt_resample_u8: null pointer");
+  OMT_REQUIRE(B >= 1 && B <= 65535 && oh >= 1 && ow >= 1 && src_bytes >= 0 && tab_len >= 0,
+              "omt_resample_u8: B=%d, output %dx%d, src_bytes=%lld, tab_len=%lld", B, oh, ow, src_bytes, tab_len);
+  OMT_REQUIRE((uintptr_t)desc % 8 == 0 && (uintptr_t)tab % 4 == 0, "omt_resample_u8: desc must be 8-byte and tab 4-byte aligned");
+  for (int b = 0; b < B; ++b) {
+    const omt_resample_desc& d = desc_host[b];
+    OMT_REQUIRE(d.H >= 1 && d.W >= 1 && d.rh >= 1 && d.rw >= 1,
+                "omt_resample_u8: image %d: source %dx%d, resized %dx%d", b, d.H, d.W, d.rh, d.rw);
+    OMT_REQUIRE(d.src >= 0 && d.src + (long long)d.H * d.W * 3 <= src_bytes,
+                "omt_resample_u8: image %d: bytes [%lld, +%lld) outside the %lld source bytes", b, d.src,
+                (long long)d.H * d.W * 3, src_bytes);
+    OMT_REQUIRE(d.y0 >= 0 && d.x0 >= 0 && (long long)d.y0 + oh <= d.rh && (long long)d.x0 + ow <= d.rw,
+                "omt_resample_u8: image %d: crop %dx%d at (%d, %d) outside the resized %dx%d image", b, oh, ow, d.y0,
+                d.x0, d.rh, d.rw);
+    OMT_REQUIRE((d.flip | d.need_h | d.need_v | d.v_first) >= 0 && (d.flip | d.need_h | d.need_v | d.v_first) <= 1,
+                "omt_resample_u8: image %d: flip / need_h / need_v / v_first must be 0 or 1", b);
+    OMT_REQUIRE(!d.v_first || (d.need_h && d.need_v), "omt_resample_u8: image %d: v_first without both passes", b);
+    OMT_REQUIRE(d.need_h || d.rw == d.W, "omt_resample_u8: image %d: no horizontal pass but width %d -> %d", b, d.W, d.rw);
+    OMT_REQUIRE(d.need_v || d.rh == d.H, "omt_resample_u8: image %d: no vertical pass but height %d -> %d", b, d.H, d.rh);
+    OMT_REQUIRE(!d.need_h || axis_ok(tab_host, tab_len, d.hb, d.hc, d.hk, d.rw, d.W),
+                "omt_resample_u8: image %d: horizontal table outside the table or taps outside the source", b);
+    OMT_REQUIRE(!d.need_v || axis_ok(tab_host, tab_len, d.vb, d.vc, d.vk, d.rh, d.H),
+                "omt_resample_u8: image %d: vertical table outside the table or taps outside the source", b);
+  }
+  dim3 grid((ow + RS_TW - 1) / RS_TW, (oh + RS_TH - 1) / RS_TH, B);
+  OMT_CUDA(launch_k(resample_u8_kernel, grid, dim3(RS_THREADS), 0, (cudaStream_t)stream, src, desc, tab, out, oh, ow));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}

@@ -16,6 +16,7 @@ import math
 import os
 from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import _cabi
@@ -32,6 +33,8 @@ VQ_MAX_CODES = 41856
 # longest latent sequence of the temporal attention core (csrc/attention_fp32.cu attn_temporal_kernel keeps the K / V of
 # one pixel's T' frames in registers, one template instance per T'): 17 latent frames, 65 frames at temporal patch 4
 TEMPORAL_MAX_FRAMES = 17
+# int32 words of one omt_resample_desc (include/omnitok_b200.h): the int64 source offset, then 16 int32 fields
+DESC_WORDS = 18
 
 
 def default_math() -> str:
@@ -215,6 +218,8 @@ class Engine:
             raise NotImplementedError("non-zero dropout reaches SDPA even in eval in the reference (attention.py:451); rejected")
         self._ws: Dict[Tuple, Workspace] = {}
         self._tables: Dict[Tuple, torch.Tensor] = {}
+        # omt_resample_u8 input: grow-only pinned staging buffer, its device copy, and the event of the last copy out of it
+        self._stage = self._stage_dev = self._stage_done = None
         sd = {k: v for k, v in model.state_dict().items()}
         self._pack(sd, a)
 
@@ -667,15 +672,27 @@ class Engine:
         With norm.max_test the table is picked per sample on the device (omt_u8_norm_select), inside the graph."""
         if frames.dtype != torch.uint8 or frames.ndim != 5:
             raise TypeError(f"encode_u8 takes (B, T, H, W, C) uint8 frames, got {tuple(frames.shape)} {frames.dtype}")
-        Bf, Tf, Hf, Wf, Cf = frames.shape
+        return self._encode_u8_input(tuple(frames.shape), mode, norm, lambda buf: buf.copy_(frames))
+
+    def encode_images_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params, mode: str, norm: L.U8Norm):
+        """encode_u8() of the images the loader's transform `resize` (with params[i] = (top, left, flip)) makes of a ragged
+        list of (H_i, W_i, 3) uint8 images in host memory: omt_resample_u8 writes the transformed bytes into encode_u8's
+        input buffer (eagerly: the source geometry changes every batch), then encode_u8's body or graph of that shape runs."""
+        oh, ow = resize.out_size
+        return self._encode_u8_input((len(images), 1, oh, ow, self.cin), mode, norm,
+                                     lambda buf: self.resample_u8(images, resize, params, buf))
+
+    def _encode_u8_input(self, shape, mode: str, norm: L.U8Norm, fill):
+        """encode_u8 of the (B,T,H,W,C) uint8 frames fill(buf) writes into the static input buffer buf."""
+        Bf, Tf, Hf, Wf, Cf = shape
         dims = self._shape((Bf, Cf, Tf, Hf, Wf))
         B, T, H, W, Tp, h, w = dims
         ws = self._workspace(B * Tp * h * w)
-        if ws.u8_in is None or ws.u8_in.shape != frames.shape:
-            ws.u8_in = torch.empty(frames.shape, device=self.device, dtype=torch.uint8)
+        if ws.u8_in is None or tuple(ws.u8_in.shape) != shape:
+            ws.u8_in = torch.empty(shape, device=self.device, dtype=torch.uint8)
             ws.u8_sel = torch.empty(B, device=self.device, dtype=torch.int32)
             ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("enc_u8")}
-        ws.u8_in.copy_(frames)
+        fill(ws.u8_in)
         lut = self._table(("u8norm", norm), lambda: L.u8_norm_table(norm, self.cin))
         sel = ws.u8_sel if norm.max_test else None
 
@@ -689,8 +706,75 @@ class Engine:
                 _cabi.call("omt_u8_norm_select", ws.u8_in, B, T * H * W * self.cin, sel)
             self._encode_body(ws, gather, lay, mode)
 
-        self._run(ws, ("enc_u8:" + mode, tuple(frames.shape), norm), body)
+        self._run(ws, ("enc_u8:" + mode, shape, norm), body)
         return ws, (B, Tp, h, w)
+
+    def stage_images_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params) -> tuple:
+        """Packs a ragged list of (H_i, W_i, 3) uint8 host images for omt_resample_u8 -- descriptors, the batch's distinct
+        coefficient tables (layout.resample_coeffs), source bytes -- into the grow-only pinned staging buffer and copies it
+        to the device asynchronously on the current stream.  Returns the entry point's arguments up to the output."""
+        if self.cin != 3:
+            raise NotImplementedError(f"omt_resample_u8 resizes RGB images; the model takes {self.cin} channels")
+        rh, rw = resize.size
+        B = len(images)
+        desc = torch.zeros(B, DESC_WORDS, dtype=torch.int32)
+        tables, parts, tab_len, src_len = {}, [], 0, 0
+
+        def axis(n_in, n_out):
+            nonlocal tab_len
+            key = (n_in, n_out)
+            if key not in tables:
+                bounds, coeffs = L.resample_coeffs(n_in, n_out, resize.filter)
+                tables[key] = (tab_len, tab_len + bounds.size, coeffs.shape[1])
+                parts.extend((bounds.reshape(-1), coeffs.reshape(-1)))
+                tab_len += bounds.size + coeffs.size
+            return tables[key]
+
+        srcs = []
+        for b, (im, (i, j, flip)) in enumerate(zip(images, params)):
+            H, W = int(im.shape[0]), int(im.shape[1])
+            need_h, need_v = W != rw, H != rh
+            hb, hc, hk = axis(W, rw) if need_h else (0, 0, 0)
+            vb, vc, vk = axis(H, rh) if need_v else (0, 0, 0)
+            desc[b, 2:] = torch.tensor([H, W, rh, rw, i, j, int(flip), int(need_h), int(need_v), hb, hc, hk, vb, vc, vk,
+                                        int(L.vertical_first(H, W, rh, rw))], dtype=torch.int32)
+            srcs.append((src_len, im))
+            src_len += H * W * 3
+        desc[:, :2] = torch.tensor([s for s, _ in srcs], dtype=torch.int64).view(torch.int32).view(B, 2)
+        o_tab = L.round_up(B * DESC_WORDS * 4, 16)
+        o_src = L.round_up(o_tab + tab_len * 4, 16)
+        total = o_src + src_len
+        if self._stage is None or self._stage.numel() < total:
+            if self._stage_done is not None:
+                self._stage_done.synchronize()
+            cap = max(total, 3 * (0 if self._stage is None else self._stage.numel()) // 2)
+            self._stage = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
+            self._stage_dev = torch.empty(cap, dtype=torch.uint8, device=self.device)
+        elif self._stage_done is not None:
+            self._stage_done.synchronize()       # the previous batch's copy has read the staging buffer
+        st = self._stage
+        st[:o_tab].view(torch.int32)[: B * DESC_WORDS].copy_(desc.view(-1))
+        if tab_len:
+            st[o_tab:o_tab + tab_len * 4].view(torch.int32).copy_(torch.from_numpy(np.concatenate(parts)))
+        for off, im in srcs:
+            st[o_src + off:o_src + off + im.numel()].view(im.shape).copy_(im)
+        self._stage_dev[:total].copy_(st[:total], non_blocking=True)
+        if self._stage_done is None:
+            self._stage_done = torch.cuda.Event()
+        self._stage_done.record()
+        dev, host = self._stage_dev.data_ptr(), st.data_ptr()
+        return (dev + o_src, src_len, dev, host, dev + o_tab if tab_len else None, host + o_tab if tab_len else None,
+                tab_len, B) + tuple(resize.out_size)
+
+    def resample_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params, out: torch.Tensor) -> torch.Tensor:
+        """The loader's transform `resize` (params[i] = (top, left, flip)) of a ragged list of (H_i, W_i, 3) uint8 host images,
+        on the device: out (B, oh, ow, 3) uint8 (any shape of that size), equal byte for byte to layout.resize_u8 / Pillow."""
+        oh, ow = resize.out_size
+        if out.dtype != torch.uint8 or out.device != self.device or not out.is_contiguous() or out.numel() != len(images) * oh * ow * 3:
+            raise ValueError(f"resample_u8 writes {len(images)} x {oh} x {ow} x 3 contiguous uint8 bytes on {self.device}, "
+                             f"got {tuple(out.shape)} {out.dtype} on {out.device}")
+        _cabi.call("omt_resample_u8", *self.stage_images_u8(images, resize, params), out)
+        return out
 
     def z_view(self, ws: Workspace) -> torch.Tensor:
         return self._dense(ws.z, ws.M, self.pre_w.shape[0])

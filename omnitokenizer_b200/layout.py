@@ -5,9 +5,11 @@ the per-token arithmetic all happens in the CUDA kernels.
 """
 from __future__ import annotations
 
+import functools
 import math
-from typing import NamedTuple, Tuple
+from typing import List, NamedTuple, Tuple
 
+import numpy as np
 import torch
 
 
@@ -48,6 +50,167 @@ def u8_normalize(frames: torch.Tensor, norm: U8Norm) -> torch.Tensor:
         sel = (frames.reshape(B, -1).amax(dim=1) <= 1).long()
     x = frames.permute(0, 4, 1, 2, 3).long()
     return tab[sel.view(B, 1, 1, 1, 1), torch.arange(C, device=frames.device).view(1, C, 1, 1, 1), x]
+
+
+class U8Resize(NamedTuple):
+    """An image loader's geometric transform before ToTensor: torchvision Resize(size, filter) on the PIL image (Pillow's
+    8-bit resize), then optionally RandomCrop(crop) and RandomHorizontalFlip(0.5), in that order."""
+    size: Tuple[int, int]          # (height, width) after the resize
+    filter: str = "bicubic"        # Pillow filter: "bicubic", "bilinear" or "box"
+    crop: int = 0                  # side of the square random crop of the resized image; 0: none
+    flip: bool = False
+
+    @property
+    def out_size(self) -> Tuple[int, int]:
+        return (self.crop, self.crop) if self.crop else (int(self.size[0]), int(self.size[1]))
+
+
+def image_resize(resolution: int) -> U8Resize:
+    """ImageDataset without --resizecrop (OmniTokenizer/data.py:93-99): Resize((res, res), BICUBIC)."""
+    return U8Resize((resolution, resolution), "bicubic")
+
+
+def resizecrop_resize(resolution: int) -> U8Resize:
+    """ImageDataset with --resizecrop (OmniTokenizer/data.py:84-90): Resize((1.5 res, 1.5 res), BICUBIC), RandomCrop(res)."""
+    side = int(resolution * 1.5)
+    return U8Resize((side, side), "bicubic", crop=resolution)
+
+
+def dit_resize(image_size: int) -> U8Resize:
+    """DiT with the OmniTokenizer VAE (Diffusion/DiT/train.py:192-198): Resize((s, s)) -- torchvision's default filter,
+    BILINEAR -- then RandomHorizontalFlip."""
+    return U8Resize((image_size, image_size), "bilinear", flip=True)
+
+
+def check_resize(resize: U8Resize):
+    if not isinstance(resize, U8Resize):
+        raise TypeError(f"expected a layout.U8Resize, got {type(resize).__name__}")
+    if resize.filter not in _FILTERS:
+        raise ValueError(f"unknown resize filter {resize.filter!r}; choose from {sorted(_FILTERS)}")
+    h, w = resize.size
+    if h < 1 or w < 1 or resize.crop < 0 or resize.crop > min(h, w):
+        raise ValueError(f"resize to {h}x{w} with a crop of {resize.crop}: the crop must fit the resized image")
+
+
+# Resample.c's filters (bicubic a = -0.5) and supports, in its float64 operation order
+def _bicubic(x):
+    x = np.abs(x)
+    a = -0.5
+    return np.where(x < 1.0, ((a + 2.0) * x - (a + 3.0)) * x * x + 1,
+                    np.where(x < 2.0, (((x - 5) * x + 8) * x - 4) * a, 0.0))
+
+
+def _bilinear(x):
+    x = np.abs(x)
+    return np.where(x < 1.0, 1.0 - x, 0.0)
+
+
+def _box(x):
+    return np.where((x > -0.5) & (x <= 0.5), 1.0, 0.0)
+
+
+_FILTERS = {"bicubic": (_bicubic, 2.0), "bilinear": (_bilinear, 1.0), "box": (_box, 0.5)}
+RESAMPLE_BITS = 22       # Resample.c PRECISION_BITS for 8-bit images
+
+
+@functools.lru_cache(maxsize=1024)
+def resample_coeffs(in_size: int, out_size: int, filter: str) -> Tuple[np.ndarray, np.ndarray]:
+    """Pillow's per-axis tables for resizing an axis of in_size to out_size: (bounds int32 [out, 2] = (xmin, n) per output
+    index, coefficients int32 [out, ksize], zero past n).  libImaging/Resample.c precompute_coeffs + normalize_coeffs_8bpc
+    in float64, operation for operation: the weights of an output are summed tap by tap in order (numpy's pairwise sum
+    rounds differently), then rounded to 22-bit fixed point with +-0.5 and truncation.  Computed on the host: a device
+    compiler would contract these multiply-adds into FMAs and change the float64 results."""
+    fn, support = _FILTERS[filter]
+    scale = filterscale = in_size / out_size
+    if filterscale < 1.0:
+        filterscale = 1.0
+    support = support * filterscale
+    ksize = int(math.ceil(support)) * 2 + 1
+    center = 0.0 + (np.arange(out_size, dtype=np.float64) + 0.5) * scale
+    ss = 1.0 / filterscale
+    xmin = np.maximum(np.trunc(center - support + 0.5), 0).astype(np.int64)
+    xmax = np.minimum(np.trunc(center + support + 0.5), in_size).astype(np.int64)
+    n = xmax - xmin
+    x = np.arange(ksize, dtype=np.int64)[None, :]
+    live = x < n[:, None]
+    w = np.where(live, fn(((x + xmin[:, None]).astype(np.float64) - center[:, None] + 0.5) * ss), 0.0)
+    ww = np.zeros(out_size, dtype=np.float64)
+    for j in range(ksize):
+        ww = ww + w[:, j]
+    k = np.where(ww[:, None] != 0.0, w / np.where(ww == 0.0, 1.0, ww)[:, None], w)
+    fixed = np.where(k < 0, np.trunc(-0.5 + k * (1 << RESAMPLE_BITS)), np.trunc(0.5 + k * (1 << RESAMPLE_BITS)))
+    coeffs = np.where(live, fixed, 0).astype(np.int32)
+    bounds = np.stack([xmin, n], axis=1).astype(np.int32)
+    bounds.flags.writeable = False
+    coeffs.flags.writeable = False
+    return bounds, coeffs
+
+
+def resize_params(n: int, resize: U8Resize) -> List[Tuple[int, int, bool]]:
+    """(top, left, flip) of n images, drawn from torch's default CPU generator exactly as the loader's transforms draw them
+    image after image: RandomCrop.get_params (torch.randint for the top, then the left; nothing when the crop is the
+    whole image), then RandomHorizontalFlip (torch.rand(1) < 0.5)."""
+    h, w = resize.size
+    out = []
+    for _ in range(n):
+        i = j = 0
+        if resize.crop and not (h == resize.crop and w == resize.crop):
+            i = torch.randint(0, h - resize.crop + 1, size=(1,)).item()
+            j = torch.randint(0, w - resize.crop + 1, size=(1,)).item()
+        flip = bool(torch.rand(1) < 0.5) if resize.flip else False
+        out.append((int(i), int(j), flip))
+    return out
+
+
+def check_resize_params(params, n: int, resize: U8Resize):
+    if len(params) != n:
+        raise ValueError(f"{len(params)} resize parameters for {n} images")
+    (h, w), (oh, ow) = resize.size, resize.out_size
+    for b, (i, j, flip) in enumerate(params):
+        if not (0 <= i <= h - oh and 0 <= j <= w - ow) or (flip and not resize.flip) or ((i or j) and not resize.crop):
+            raise ValueError(f"resize parameters of image {b} ({i}, {j}, {flip}) are not a draw of {resize}")
+
+
+def _resample_axis(x: torch.Tensor, dim: int, out_size: int, filter: str) -> torch.Tensor:
+    """One Pillow pass over axis `dim` of int64 bytes, tap by tap: 2^21 + sum of byte * coefficient, then clip8."""
+    in_size = x.shape[dim]
+    bounds, coeffs = resample_coeffs(in_size, out_size, filter)
+    xmin = torch.from_numpy(bounds[:, 0].astype(np.int64))
+    k = torch.from_numpy(coeffs.astype(np.int64))
+    shape = [1] * x.ndim
+    shape[dim] = out_size
+    out_shape = list(x.shape)
+    out_shape[dim] = out_size
+    acc = torch.full(out_shape, 1 << (RESAMPLE_BITS - 1), dtype=torch.int64)
+    for t in range(k.shape[1]):            # past n the coefficient is 0 (the clamped index is never counted)
+        acc += x.index_select(dim, (xmin + t).clamp(max=in_size - 1)) * k[:, t].view(shape)
+    return (acc >> RESAMPLE_BITS).clamp(0, 255)
+
+
+def vertical_first(H: int, W: int, h: int, w: int) -> bool:
+    """Pillow's Image.resize runs the vertical pass first (as a resize of its own) for an image taller than 100 times its
+    width that shrinks in height; the two passes round differently in that order."""
+    return H > W * 100 and h < H and w != W
+
+
+def resize_u8(image: torch.Tensor, resize: U8Resize, param: Tuple[int, int, bool] = (0, 0, False)) -> torch.Tensor:
+    """Host twin of omt_resample_u8 for one (H, W, C) uint8 image: Pillow's horizontal pass (skipped when the width stays),
+    then its vertical pass (skipped when the height stays) -- swapped for vertical_first images --, then the crop at
+    (top, left) and the flip -> (oh, ow, C) uint8, byte for byte what the loader's transforms make of the PIL image."""
+    h, w = resize.size
+    x = image.long()
+    v_first = vertical_first(x.shape[0], x.shape[1], h, w)
+    if v_first:
+        x = _resample_axis(x, 0, h, resize.filter)
+    if x.shape[1] != w:
+        x = _resample_axis(x, 1, w, resize.filter)
+    if x.shape[0] != h:
+        x = _resample_axis(x, 0, h, resize.filter)
+    (oh, ow), (i, j, flip) = resize.out_size, param
+    x = x[i:i + oh, j:j + ow]
+    if flip:
+        x = x.flip(1)
+    return x.to(torch.uint8).contiguous()
 
 
 def peg_neighbour_table(T: int, h: int, w: int, temporal: bool, causal: bool) -> torch.Tensor:

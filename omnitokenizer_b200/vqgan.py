@@ -23,7 +23,8 @@ from typing import Optional
 import torch
 import torch.nn as nn
 
-from .consumers import EVAL_U8, VIDEO_NORM
+from . import layout as L
+from .consumers import EVAL_U8, IMAGE_NORM, VIDEO_NORM
 from .engine import Engine
 
 
@@ -361,6 +362,46 @@ class OmniTokenizer_VQGAN(nn.Module):
             ws, dims = eng.encode_u8(f, "raw" if self.use_vae else "vq", norm)
             return self._encode_result(eng, ws.idx, eng.z_view(ws), ws.counts, dims, is_image, include_embeddings)
 
+    def _images_u8(self, images, resize, params):
+        """Checks a ragged list of decoded uint8 images (H_i, W_i, C) in host memory, the transform and its parameters, and
+        the output size against encode's shape rules (with encode's messages) -- all before any launch.  Returns (list,
+        params), drawing the parameters from the CPU generator as the loader's transforms would when params is None."""
+        images = list(images)
+        L.check_resize(resize)
+        C = self.args.image_channels
+        for i, im in enumerate(images):
+            if not isinstance(im, torch.Tensor) or im.dtype != torch.uint8:
+                raise TypeError(f"image {i}: expected a uint8 tensor, got {getattr(im, 'dtype', type(im))}")
+            if im.ndim != 3 or im.shape[2] != C or im.shape[0] < 1 or im.shape[1] < 1:
+                raise ValueError(f"image {i}: expected (H, W, {C}) with H, W >= 1, got {tuple(im.shape)}")
+            if im.device.type != "cpu":
+                raise ValueError(f"image {i}: expected a decoded image in host memory, got one on {im.device}")
+        h, w = resize.out_size
+        eng = self.engine()
+        eng._shape((max(len(images), 1), C, 1, h, w))
+        if params is None:
+            params = L.resize_params(len(images), resize)
+        L.check_resize_params(params, len(images), resize)
+        return images, params
+
+    @torch.no_grad()
+    def encode_images_u8(self, images, resize, norm=IMAGE_NORM, include_embeddings=False, params=None):
+        """encode_u8(images after the loader's transform, is_image=True) from the decoded images themselves: a ragged list of
+        (H_i, W_i, C) uint8 tensors in host memory, any sizes.  `resize` (a layout.U8Resize, e.g. layout.image_resize(res))
+        is the loader's Pillow resize + random crop + flip; omt_resample_u8 applies it on the device byte for byte as Pillow
+        and torchvision do, so the result -- codes, embeddings, VAE latents, usage statistics, CPU RNG draws -- equals
+        encode_u8 of the stacked host-transformed images.  params: per image (top, left, flip); None draws them from the
+        CPU generator as RandomCrop / RandomHorizontalFlip would (layout.resize_params), before the VAE noise."""
+        images, params = self._images_u8(images, resize, params)
+        if not images:
+            h, w = resize.out_size
+            return self.encode_u8(torch.empty((0, h, w, self.args.image_channels), dtype=torch.uint8), True,
+                                  include_embeddings, norm)
+        eng = self.engine()
+        with torch.cuda.device(self.device):
+            ws, dims = eng.encode_images_u8(images, resize, params, "raw" if self.use_vae else "vq", norm)
+            return self._encode_result(eng, ws.idx, eng.z_view(ws), ws.counts, dims, True, include_embeddings)
+
     def _encode_result(self, eng, idx, z, counts, dims, is_image, include_embeddings):
         """What encode() returns (omnitokenizer.py:247-266), with Codebook.forward's usage side effects, from the encoder's
         rows of the dims (B,T',h,w) batch: idx [M] codes, z [M, cd] (VQ) or [M, 2 cd] moments (VAE), counts the code histogram."""
@@ -632,6 +673,22 @@ class OmniTokenizer_VQGAN(nn.Module):
             if not is_image:
                 torch.randint(0, f.shape[1], [f.shape[0]])                      # forward's random-frame draw (omnitokenizer.py:401)
             return x_recon, vq_output
+
+    @torch.no_grad()
+    def forward_images_u8(self, images, resize, norm=IMAGE_NORM, out_affine=EVAL_U8, params=None):
+        """forward_u8 of the images the loader's transform `resize` makes of a ragged list of decoded (H_i, W_i, C) uint8
+        host images (see encode_images_u8): returns (x_recon uint8 (B, 1, h, w, C), vq_output), equal to forward_u8 on the
+        stacked host-transformed images, with the same CPU RNG draws (the transform's parameters first when params is None)."""
+        if self.resolution_scale is not None:
+            raise NotImplementedError("resolution_scale resizes the fp32 frames between the / 255 and the shift "
+                                      "(omnitokenizer.py:334-355); no byte table expresses that -- use forward()")
+        images, params = self._images_u8(images, resize, params)
+        if not images:
+            raise ValueError("forward_images_u8 needs at least one image")
+        eng = self.engine()
+        with torch.cuda.device(self.device):
+            ws, dims = eng.encode_images_u8(images, resize, params, "raw" if self.use_vae else "vq", norm)
+            return self._forward_decode(eng, ws, dims, u8=tuple(float(v) for v in out_affine))
 
     # ---------------------------------------------------------------- CLI surface
     @staticmethod
