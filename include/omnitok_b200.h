@@ -140,6 +140,38 @@ int omt_resample_u8(const uint8_t* src, long long src_bytes, const omt_resample_
                     const omt_resample_desc* desc_host, const int32_t* tab, const int32_t* tab_host, long long tab_len,
                     int B, int oh, int ow, uint8_t* out, omt_stream_t stream);
 
+/* One clip of omt_resample_clips.  Table offsets count int32 words; each table entry is 4 words. */
+typedef struct {
+  long long src;          /* byte offset of the clip's (F, H, W, 3) bytes in src */
+  int H, W;               /* source frame size */
+  int y0, x0;             /* origin of the window the resize reads, in the (flipped) source frame */
+  int wh, ww;             /* window size: the input length of the vertical / horizontal table */
+  int rh, rw;             /* resized size: the output length of the vertical / horizontal table */
+  int cy, cx;             /* crop origin in the resized frame */
+  int flip;               /* 1: the source frame is mirrored left-right before the window is taken */
+  int tv, th;             /* vertical table [rh][4] at tab + tv, horizontal table [rw][4] at tab + th */
+  int form;               /* 0: torch's separable bilinear kernel, 1: its channels-last four-weight kernel */
+} omt_clip_desc;
+
+/* The Latte video loaders' transform of a ragged batch of (F, H_i, W_i, 3) uint8 clips (Diffusion/Latte/datasets:
+ * ToTensorVideo, RandomHorizontalFlipVideo, UCFCenterCropVideo / CenterCropResizeVideo, Normalize), torch's fp32 CPU
+ * arithmetic bit for bit.  out (B, 3, F, oh, ow) fp32, channel-planar:
+ *   v = lut[byte]                                                       (to_tensor: u / 255, from the host)
+ *   source column of window column c: x0 + c, or W - 1 - (x0 + c) when flipped; row: y0 + r
+ *   axis entries (i0, i1, l0, l1) of output indices cy + y and cx + x, x_ab = v[i_a h][i_b w]; F.interpolate bilinear:
+ *     form 0: t_a = fma(x_a0, l0w, x_a1 * l1w), then fma(t_0, l0h, t_1 * l1h)
+ *     form 1: w_ab = l_a h * l_b w, then fma(x_11, w_11, fma(x_10, w_10, fma(x_00, w_00, x_01 * w_01)))
+ *   (value - mean_c) / std_c, true division                          (Normalize)
+ * The axis tables are int32 [n_out][4] = (i0, i1, l0 bits, l1 bits), built on the host in fp32 without contraction.
+ * norm: fp32 [262] on the device: the 256-entry byte table, then mean[3], then std[3].  src: packed source bytes
+ * (src_bytes of them); desc [B]: device table, 8-byte aligned; tab [tab_len] int32, 16-byte aligned.  desc_host /
+ * tab_host: the same tables in host memory, checked before the launch (every clip inside src, every window inside its
+ * frame, every table inside tab, every index inside its axis, the crop inside the resized size); they must equal the
+ * device copies.  One launch for the batch. */
+int omt_resample_clips(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc, const omt_clip_desc* desc_host,
+                       const int32_t* tab, const int32_t* tab_host, long long tab_len, const float* norm, int B, int F,
+                       int oh, int ow, float* out, omt_stream_t stream);
+
 /* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W). */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,
                    int first, omt_stream_t stream);

@@ -57,6 +57,8 @@ SIGNATURES = {
     "omt_u8_norm_select": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p]),
     "omt_resample_u8": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int,
                                 c_void_p, c_void_p]),
+    "omt_resample_clips": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int,
+                                   c_int, c_int, c_int, c_void_p, c_void_p]),
     "omt_unpatchify": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_void_p]),
     "omt_unpatchify_u8": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float] * 5 + [c_void_p]),
     "omt_peg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

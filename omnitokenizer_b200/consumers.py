@@ -14,7 +14,8 @@ from typing import Optional, Sequence, Tuple
 
 import torch
 
-from .layout import U8Norm, U8Resize, dit_resize, resize_params, resize_u8, u8_normalize
+from .layout import (ClipResize, U8Norm, U8Resize, clip_params, dit_resize, resize_clip, resize_params, resize_u8,
+                     u8_normalize)
 
 LATENT_SCALE = 0.18215            # Diffusion/DiT/train.py:242, Diffusion/Latte/train.py:216
 
@@ -237,3 +238,22 @@ def dit_encode_latents_images_u8(vae, images: Sequence[torch.Tensor], image_size
     if hasattr(vae, "encode_images_u8"):
         return vae.encode_images_u8(images, resize, norm).mul_(LATENT_SCALE)
     return _encode_u8(vae, _host_transform(images, resize), True, norm).mul_(LATENT_SCALE)
+
+
+# ----------------------------------------------------------------------------------------------- decoded clips, any size
+# Latte's video loaders turn read_video's frames into fp32 before they resize (ClipResize presets in layout.py), so no
+# uint8 clip of the model's size ever exists.  With this package's module the whole transform runs on the device
+# (encode_clips_u8: omt_resample_clips, bit for bit torch's CPU arithmetic); any other object gets the fp32 clips from the
+# host twin layout.resize_clip.
+@torch.no_grad()
+def latte_encode_latents_clips_u8(vae, clips: Sequence[torch.Tensor], resize: ClipResize,
+                                  norm: U8Norm = LATTE_NORM) -> torch.Tensor:
+    """latte_encode_latents of the clips Latte's loader makes of decoded (F, H_i, W_i, 3) uint8 frames (e.g.
+    layout.ucf_clip_resize(256) for ucf101 / ffs: ToTensorVideo, RandomHorizontalFlipVideo, UCFCenterCropVideo,
+    Normalize(.5, .5)): scaled latents 'b f c h w'."""
+    if hasattr(vae, "encode_clips_u8"):
+        z = vae.encode_clips_u8(clips, resize, norm).mul_(LATENT_SCALE)
+        return z.permute(0, 2, 1, 3, 4).contiguous()          # 'b c f h w -> b f c h w'
+    clips = list(clips)
+    flips = clip_params(len(clips), resize)
+    return latte_encode_latents(vae, torch.stack([resize_clip(c, resize, f, norm) for c, f in zip(clips, flips)]))

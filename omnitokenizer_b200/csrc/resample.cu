@@ -159,6 +159,74 @@ resample_u8_kernel(const uint8_t* __restrict__ src, const omt_resample_desc* __r
   }
 }
 
+// omt_resample_clips: the Latte video loaders' ToTensorVideo -> flip -> bilinear F.interpolate (+ centre crop) ->
+// Normalize, in torch's fp32 CPU arithmetic (either of its two bilinear kernels, per clip: desc.form).  Its own kernel:
+// nothing here is shared with Pillow's integer resize.
+// Each CTA owns RC_TW output columns (one per thread) x RC_TH rows of one frame of one clip; a thread's horizontal table
+// entry is loaded once, and each output row reads exactly two source rows.  Stores run along w within a channel plane.
+constexpr int RC_TW = 128;
+constexpr int RC_TH = 8;
+
+__global__ void __launch_bounds__(RC_TW)
+resample_clips_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
+                      const int4* __restrict__ tab, const float* __restrict__ norm, float* __restrict__ out, int F,
+                      int oh, int ow) {
+  __shared__ float lut[256];
+  pdl_sync();
+  const int b = blockIdx.z / F, f = blockIdx.z % F;
+  const omt_clip_desc d = desc[b];
+  for (int i = threadIdx.x; i < 256; i += RC_TW) lut[i] = __ldg(norm + i);
+  __syncthreads();
+  const int ox = blockIdx.x * RC_TW + threadIdx.x;
+  if (ox >= ow) return;
+  float mean[3], stdv[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    mean[c] = __ldg(norm + 256 + c);
+    stdv[c] = __ldg(norm + 259 + c);
+  }
+  const int4 ew = __ldg(tab + d.th / 4 + d.cx + ox);
+  const int x0 = d.flip ? d.W - 1 - (d.x0 + ew.x) : d.x0 + ew.x;   // the flip comes before the resize: mirror the source
+  const int x1 = d.flip ? d.W - 1 - (d.x0 + ew.y) : d.x0 + ew.y;
+  const float l0w = __int_as_float(ew.z), l1w = __int_as_float(ew.w);
+  const uint8_t* frame = src + d.src + (long long)f * d.H * d.W * 3;
+  const long long plane = (long long)oh * ow;
+  float* o = out + ((long long)b * 3 * F + f) * plane + ox;        // channel c at + c * F * plane
+  const int y_end = min(oh, (int)blockIdx.y * RC_TH + RC_TH);
+  for (int oy = blockIdx.y * RC_TH; oy < y_end; ++oy) {
+    const int4 eh = __ldg(tab + d.tv / 4 + d.cy + oy);
+    const float l0h = __int_as_float(eh.z), l1h = __int_as_float(eh.w);
+    const uint8_t* r0 = frame + (long long)(d.y0 + eh.x) * d.W * 3;
+    const uint8_t* r1 = frame + (long long)(d.y0 + eh.y) * d.W * 3;
+    // torch's CPU kernels: each fma rounds once; the products and the division are never contracted or reassociated
+    const float w00 = __fmul_rn(l0h, l0w), w01 = __fmul_rn(l0h, l1w), w10 = __fmul_rn(l1h, l0w), w11 = __fmul_rn(l1h, l1w);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float x00 = lut[__ldg(r0 + x0 * 3 + c)], x01 = lut[__ldg(r0 + x1 * 3 + c)];
+      const float x10 = lut[__ldg(r1 + x0 * 3 + c)], x11 = lut[__ldg(r1 + x1 * 3 + c)];
+      float v;
+      if (d.form) {
+        v = __fmaf_rn(x11, w11, __fmaf_rn(x10, w10, __fmaf_rn(x00, w00, __fmul_rn(x01, w01))));
+      } else {
+        const float t0 = __fmaf_rn(x00, l0w, __fmul_rn(x01, l1w));
+        const float t1 = __fmaf_rn(x10, l0w, __fmul_rn(x11, l1w));
+        v = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
+      }
+      o[c * F * plane + (long long)oy * ow] = __fdiv_rn(__fsub_rn(v, mean[c]), stdv[c]);
+    }
+  }
+}
+
+// One axis table of a clip: [n_out][4] entries at word `off` inside the table, every (i0, i1) inside an axis of n_in.
+bool clip_axis_ok(const int32_t* tab_host, long long tab_len, int off, int n_out, int n_in) {
+  if (off < 0 || off % 4 != 0 || off + 4LL * n_out > tab_len) return false;
+  for (int i = 0; i < n_out; ++i) {
+    const int i0 = tab_host[off + 4 * i], i1 = tab_host[off + 4 * i + 1];
+    if (i0 < 0 || i1 < i0 || i1 >= n_in) return false;
+  }
+  return true;
+}
+
 // One axis of a descriptor: its (xmin, n) bounds [out][2] at `b` and coefficients [out][k] at `c` lie inside the table,
 // and every output index's taps lie inside the source axis of length `in`.
 bool axis_ok(const int32_t* tab_host, long long tab_len, int b, int c, int k, int out, int in) {
@@ -203,6 +271,44 @@ extern "C" int omt_resample_u8(const uint8_t* src, long long src_bytes, const om
   }
   dim3 grid((ow + RS_TW - 1) / RS_TW, (oh + RS_TH - 1) / RS_TH, B);
   OMT_CUDA(launch_k(resample_u8_kernel, grid, dim3(RS_THREADS), 0, (cudaStream_t)stream, src, desc, tab, out, oh, ow));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_resample_clips(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc,
+                                  const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
+                                  long long tab_len, const float* norm, int B, int F, int oh, int ow, float* out,
+                                  omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(src && desc && desc_host && tab && tab_host && norm && out, "omt_resample_clips: null pointer");
+  OMT_REQUIRE(B >= 1 && F >= 1 && (long long)B * F <= 65535 && oh >= 1 && ow >= 1 && src_bytes >= 0 && tab_len >= 0,
+              "omt_resample_clips: B=%d, F=%d, output %dx%d, src_bytes=%lld, tab_len=%lld", B, F, oh, ow, src_bytes,
+              tab_len);
+  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab}) && aligned_to(4, {norm, out}),
+              "omt_resample_clips: desc must be 8-byte, tab 16-byte and norm / out 4-byte aligned");
+  for (int b = 0; b < B; ++b) {
+    const omt_clip_desc& d = desc_host[b];
+    OMT_REQUIRE(d.H >= 1 && d.W >= 1 && d.wh >= 1 && d.ww >= 1 && d.rh >= 1 && d.rw >= 1,
+                "omt_resample_clips: clip %d: source %dx%d, window %dx%d, resized %dx%d", b, d.H, d.W, d.wh, d.ww, d.rh,
+                d.rw);
+    OMT_REQUIRE(d.src >= 0 && d.src + (long long)F * d.H * d.W * 3 <= src_bytes,
+                "omt_resample_clips: clip %d: bytes [%lld, +%lld) outside the %lld source bytes", b, d.src,
+                (long long)F * d.H * d.W * 3, src_bytes);
+    OMT_REQUIRE(d.y0 >= 0 && d.x0 >= 0 && (long long)d.y0 + d.wh <= d.H && (long long)d.x0 + d.ww <= d.W,
+                "omt_resample_clips: clip %d: window %dx%d at (%d, %d) outside the %dx%d frame", b, d.wh, d.ww, d.y0,
+                d.x0, d.H, d.W);
+    OMT_REQUIRE(d.cy >= 0 && d.cx >= 0 && (long long)d.cy + oh <= d.rh && (long long)d.cx + ow <= d.rw,
+                "omt_resample_clips: clip %d: crop %dx%d at (%d, %d) outside the resized %dx%d frame", b, oh, ow, d.cy,
+                d.cx, d.rh, d.rw);
+    OMT_REQUIRE((d.flip | d.form) >= 0 && (d.flip | d.form) <= 1, "omt_resample_clips: clip %d: flip / form must be 0 or 1", b);
+    OMT_REQUIRE(clip_axis_ok(tab_host, tab_len, d.tv, d.rh, d.wh),
+                "omt_resample_clips: clip %d: vertical table outside the table or indices outside the window", b);
+    OMT_REQUIRE(clip_axis_ok(tab_host, tab_len, d.th, d.rw, d.ww),
+                "omt_resample_clips: clip %d: horizontal table outside the table or indices outside the window", b);
+  }
+  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
+  OMT_CUDA(launch_k(resample_clips_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
+                    reinterpret_cast<const int4*>(tab), norm, out, F, oh, ow));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

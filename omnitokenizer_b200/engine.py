@@ -35,6 +35,8 @@ VQ_MAX_CODES = 41856
 TEMPORAL_MAX_FRAMES = 17
 # int32 words of one omt_resample_desc (include/omnitok_b200.h): the int64 source offset, then 16 int32 fields
 DESC_WORDS = 18
+# int32 words of one omt_clip_desc: the int64 source offset, then 14 int32 fields
+CLIP_DESC_WORDS = 16
 
 
 def default_math() -> str:
@@ -622,19 +624,32 @@ class Engine:
         """x (B,C,T,H,W) fp32 on the device.  mode 'vq': returns (ws, dims) with ws.z (l2-normalised z),
         ws.idx, ws.counts filled; mode 'raw': ws.z = pre_vq output (VAE moments).  Results live in the
         workspace until the next call of the same shape."""
-        dims = self._shape(tuple(x.shape))
+        return self._encode_input(tuple(x.shape), mode, lambda buf: buf.copy_(x))
+
+    def encode_clips_u8(self, clips: Sequence[torch.Tensor], resize: L.ClipResize, flips, mode: str, norm: L.U8Norm):
+        """encode() of the (B, 3, F, oh, ow) fp32 clips the Latte loader's transform `resize` (flips[i]: clip i mirrored)
+        and Normalize `norm` make of a ragged list of (F, H_i, W_i, 3) uint8 clips in host memory: omt_resample_clips
+        writes encode's input buffer (eagerly: the source geometry changes every batch), then encode's body or graph of
+        that shape runs -- the same graph a later encode() of that shape replays."""
+        F, H, W = (int(v) for v in clips[0].shape[:3])
+        shape = (len(clips), self.cin, F) + L.clip_out_size(H, W, resize)
+        return self._encode_input(shape, mode, lambda buf: self.resample_clips(clips, resize, flips, norm, buf))
+
+    def _encode_input(self, shape, mode: str, fill):
+        """encode of the (B,C,T,H,W) fp32 video fill(buf) writes into the static input buffer buf."""
+        dims = self._shape(shape)
         B, T, H, W, Tp, h, w = dims
         ws = self._workspace(B * Tp * h * w)
-        if ws.x_in is None or ws.x_in.shape != x.shape:
-            ws.x_in = torch.empty_like(x, memory_format=torch.contiguous_format)
+        if ws.x_in is None or tuple(ws.x_in.shape) != shape:
+            ws.x_in = torch.empty(shape, device=self.device, dtype=torch.float32)
             ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("enc")}
-        ws.x_in.copy_(x)
+        fill(ws.x_in)
 
         def gather(gi, first, *out):
             _cabi.call("omt_patchify_ln", ws.x_in, *out, B, self.cin, T, H, W, self.p, self.pt, first, 1e-5)
 
         lay = BatchLayout((Tp,) * B, h, w)
-        self._run(ws, ("enc:" + mode, tuple(x.shape)), lambda: self._encode_body(ws, gather, lay, mode))
+        self._run(ws, ("enc:" + mode, shape), lambda: self._encode_body(ws, gather, lay, mode))
         return ws, (B, Tp, h, w)
 
     def encode_batch(self, xs: Sequence[torch.Tensor], mode: str):
@@ -740,8 +755,19 @@ class Engine:
                                         int(L.vertical_first(H, W, rh, rw))], dtype=torch.int32)
             srcs.append((src_len, im))
             src_len += H * W * 3
+        dev, host, o_tab, o_src = self._stage_upload(desc, parts, srcs, src_len)
+        return (dev + o_src, src_len, dev, host, dev + o_tab if tab_len else None, host + o_tab if tab_len else None,
+                tab_len, B) + tuple(resize.out_size)
+
+    def _stage_upload(self, desc: torch.Tensor, parts, srcs, src_len: int):
+        """Packs descriptors (int32 [B, words], the int64 source offset in words 0-1), int32 table parts and the source
+        tensors (srcs: (byte offset, uint8 tensor)) into the grow-only pinned staging buffer, 16-byte aligned sections,
+        and copies it to the device asynchronously on the current stream.  An event guards the pinned buffer's reuse.
+        Returns (device base, host base, table offset, source offset) in bytes."""
+        B = desc.shape[0]
         desc[:, :2] = torch.tensor([s for s, _ in srcs], dtype=torch.int64).view(torch.int32).view(B, 2)
-        o_tab = L.round_up(B * DESC_WORDS * 4, 16)
+        tab_len = sum(p.size for p in parts)
+        o_tab = L.round_up(desc.numel() * 4, 16)
         o_src = L.round_up(o_tab + tab_len * 4, 16)
         total = o_src + src_len
         if self._stage is None or self._stage.numel() < total:
@@ -753,18 +779,63 @@ class Engine:
         elif self._stage_done is not None:
             self._stage_done.synchronize()       # the previous batch's copy has read the staging buffer
         st = self._stage
-        st[:o_tab].view(torch.int32)[: B * DESC_WORDS].copy_(desc.view(-1))
+        st[:o_tab].view(torch.int32)[: desc.numel()].copy_(desc.view(-1))
         if tab_len:
             st[o_tab:o_tab + tab_len * 4].view(torch.int32).copy_(torch.from_numpy(np.concatenate(parts)))
-        for off, im in srcs:
-            st[o_src + off:o_src + off + im.numel()].view(im.shape).copy_(im)
+        for off, t in srcs:
+            st[o_src + off:o_src + off + t.numel()].view(t.shape).copy_(t)
         self._stage_dev[:total].copy_(st[:total], non_blocking=True)
         if self._stage_done is None:
             self._stage_done = torch.cuda.Event()
         self._stage_done.record()
-        dev, host = self._stage_dev.data_ptr(), st.data_ptr()
-        return (dev + o_src, src_len, dev, host, dev + o_tab if tab_len else None, host + o_tab if tab_len else None,
-                tab_len, B) + tuple(resize.out_size)
+        return self._stage_dev.data_ptr(), st.data_ptr(), o_tab, o_src
+
+    def stage_clips_u8(self, clips: Sequence[torch.Tensor], resize: L.ClipResize, flips) -> tuple:
+        """Packs a ragged list of (F, H_i, W_i, 3) uint8 host clips for omt_resample_clips -- descriptors, the batch's
+        distinct axis tables (layout.clip_axis_table), source bytes -- through the staging buffer (_stage_upload).
+        Returns the entry point's arguments up to the normalisation table, then (B, F, oh, ow)."""
+        if self.cin != 3:
+            raise NotImplementedError(f"omt_resample_clips resizes RGB clips; the model takes {self.cin} channels")
+        B = len(clips)
+        F = int(clips[0].shape[0])
+        desc = torch.zeros(B, CLIP_DESC_WORDS, dtype=torch.int32)
+        tables, parts, tab_len, src_len, srcs = {}, [], 0, 0, []
+
+        def axis(n_in, n_out, scale):
+            nonlocal tab_len
+            key = (n_in, n_out, scale)
+            if key not in tables:
+                tables[key] = tab_len
+                parts.append(L.clip_axis_table(n_in, n_out, scale).reshape(-1))
+                tab_len += 4 * n_out
+            return tables[key]
+
+        for b, (clip, flip) in enumerate(zip(clips, flips)):
+            H, W = int(clip.shape[1]), int(clip.shape[2])
+            g = L.clip_geometry(H, W, resize)
+            tv, th = axis(g.wh, g.rh, g.scale_h), axis(g.ww, g.rw, g.scale_w)
+            desc[b, 2:] = torch.tensor([H, W, g.y0, g.x0, g.wh, g.ww, g.rh, g.rw, g.cy, g.cx, int(flip), tv, th,
+                                        L.clip_interp_form(g, resize.in_workers)], dtype=torch.int32)
+            srcs.append((src_len, clip))
+            src_len += clip.numel()
+        oh, ow = L.clip_out_size(int(clips[0].shape[1]), int(clips[0].shape[2]), resize)
+        dev, host, o_tab, o_src = self._stage_upload(desc, parts, srcs, src_len)
+        return (dev + o_src, src_len, dev, host, dev + o_tab, host + o_tab, tab_len), (B, F, oh, ow)
+
+    def resample_clips(self, clips: Sequence[torch.Tensor], resize: L.ClipResize, flips, norm: L.U8Norm,
+                       out: torch.Tensor) -> torch.Tensor:
+        """The Latte loader's transform `resize` (flips[i]: clip i mirrored) and Normalize `norm` of a ragged list of
+        (F, H_i, W_i, 3) uint8 host clips, on the device in one launch: out (B, 3, F, oh, ow) fp32 contiguous, equal bit
+        for bit to layout.resize_clip / the loader's torch CPU pipeline."""
+        B, (F, H, W) = len(clips), tuple(int(v) for v in clips[0].shape[:3])
+        shape = (B, 3, F) + L.clip_out_size(H, W, resize)
+        if out.dtype != torch.float32 or out.device != self.device or not out.is_contiguous() or tuple(out.shape) != shape:
+            raise ValueError(f"resample_clips writes a contiguous fp32 {shape} tensor on {self.device}, "
+                             f"got {tuple(out.shape)} {out.dtype} on {out.device}")
+        lut = self._table(("clipnorm", norm), lambda: L.clip_norm_table(norm))
+        args, (B, F, oh, ow) = self.stage_clips_u8(clips, resize, flips)
+        _cabi.call("omt_resample_clips", *args, lut, B, F, oh, ow, out)
+        return out
 
     def resample_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params, out: torch.Tensor) -> torch.Tensor:
         """The loader's transform `resize` (params[i] = (top, left, flip)) of a ragged list of (H_i, W_i, 3) uint8 host images,

@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import functools
 import math
+import random
 from typing import List, NamedTuple, Tuple
 
 import numpy as np
@@ -211,6 +212,197 @@ def resize_u8(image: torch.Tensor, resize: U8Resize, param: Tuple[int, int, bool
     if flip:
         x = x.flip(1)
     return x.to(torch.uint8).contiguous()
+
+
+class ClipResize(NamedTuple):
+    """A Latte video loader's geometric transform of a ToTensorVideo'd clip (Diffusion/Latte/datasets/__init__.py,
+    video_transforms.py), bilinear F.interpolate with align_corners=False on the fp32 clip:
+    - "scale_crop": UCFCenterCropVideo(size): scale_factor size / min(H, W), then a centre size x size crop;
+    - "crop_resize": CenterCropResizeVideo(size): centre crop of the short edge, then resize to size x size;
+    - "none": the clip keeps its H x W.
+    flip: RandomHorizontalFlipVideo before the resize (Python's random.random() < 0.5, once per clip).
+    in_workers: the transform runs where torch.get_num_threads() == 1, as in the DataLoader worker processes of Latte's
+    configs (num_workers > 0); torch's CPU bilinear kernel picks its arithmetic by that (clip_interp_form)."""
+    mode: str
+    size: int = 0
+    flip: bool = False
+    in_workers: bool = True
+
+
+def ucf_clip_resize(size: int) -> ClipResize:
+    """ucf101 and ffs: ToTensorVideo, RandomHorizontalFlipVideo, UCFCenterCropVideo(size), Normalize."""
+    return ClipResize("scale_crop", size, True)
+
+
+def sky_clip_resize(size: int) -> ClipResize:
+    """sky: ToTensorVideo, CenterCropResizeVideo(size), Normalize (no flip)."""
+    return ClipResize("crop_resize", size, False)
+
+
+def taichi_clip_resize() -> ClipResize:
+    """taichi: ToTensorVideo, RandomHorizontalFlipVideo, Normalize (no resize)."""
+    return ClipResize("none", 0, True)
+
+
+_CLIP_MODES = ("scale_crop", "crop_resize", "none")
+
+
+def check_clip_resize(resize: ClipResize):
+    if not isinstance(resize, ClipResize):
+        raise TypeError(f"expected a layout.ClipResize, got {type(resize).__name__}")
+    if resize.mode not in _CLIP_MODES:
+        raise ValueError(f"unknown clip resize mode {resize.mode!r}; choose from {list(_CLIP_MODES)}")
+    if (resize.mode == "none") != (resize.size == 0) or resize.size < 0:
+        raise ValueError(f"clip resize {resize.mode!r} with size {resize.size}: 'none' takes size 0, the others a size >= 1")
+
+
+class ClipGeometry(NamedTuple):
+    """Where one clip's transform reads and writes: the window (y0, x0, wh, ww) of the (flipped) source frame the resize
+    reads, the resized size (rh, rw), the crop origin (cy, cx) in it, and the fp32 coordinate scale of each axis."""
+    y0: int
+    x0: int
+    wh: int
+    ww: int
+    rh: int
+    rw: int
+    cy: int
+    cx: int
+    scale_h: float
+    scale_w: float
+
+
+@functools.lru_cache(maxsize=4096)
+def scaled_size(H: int, W: int, size: int) -> Tuple[int, int]:
+    """Output size of UCFCenterCropVideo's F.interpolate(scale_factor=size / min(H, W)), from torch's own shape rule."""
+    x = torch.empty(1, 1, H, W, device="meta")
+    y = torch.nn.functional.interpolate(x, scale_factor=size / min(H, W), mode="bilinear", align_corners=False)
+    return int(y.shape[-2]), int(y.shape[-1])
+
+
+def clip_geometry(H: int, W: int, resize: ClipResize) -> ClipGeometry:
+    """The transform's geometry for an H x W source frame.  Raises center_crop's ValueError (video_transforms.py:85-86)
+    where the reference does: UCFCenterCropVideo's scaled short side can come out one pixel short of the size."""
+    if resize.mode == "none":
+        return ClipGeometry(0, 0, H, W, H, W, 0, 0, 1.0, 1.0)
+    s = resize.size
+    if resize.mode == "scale_crop":
+        rh, rw = scaled_size(H, W, s)
+        if rh < s or rw < s:
+            raise ValueError("height and width must be no smaller than crop_size")
+        inv = float(np.float32(1.0 / (s / min(H, W))))     # torch: static_cast<float>(1.0 / scale_factor)
+        # center_crop's offsets are Python's round-half-to-even of (h - th) / 2
+        return ClipGeometry(0, 0, H, W, rh, rw, int(round((rh - s) / 2.0)), int(round((rw - s) / 2.0)), inv, inv)
+    if H < W:                                                # center_crop_using_short_edge
+        y0, x0, n = 0, int(round((W - H) / 2.0)), H
+    else:
+        y0, x0, n = int(round((H - W) / 2.0)), 0, W
+    sc = float(np.float32(n) / np.float32(s))                # torch: (float)input_size / output_size
+    return ClipGeometry(y0, x0, n, n, s, s, 0, 0, sc, sc)
+
+
+def clip_out_size(H: int, W: int, resize: ClipResize) -> Tuple[int, int]:
+    return (H, W) if resize.mode == "none" else (resize.size, resize.size)
+
+
+INTERP_SEPARABLE, INTERP_WEIGHTS = 0, 1
+
+
+def clip_interp_form(g: ClipGeometry, in_workers: bool) -> int:
+    """Which of torch's CPU bilinear kernels (x86-64 with FMA) runs for a 3-channel clip resized to g.rh x g.rw:
+    - INTERP_WEIGHTS, the channels-last kernel, when the output is small (rh + rw <= 128) or torch runs on one thread:
+      w_ab = lambda_h_a * lambda_w_b, out = fma(x11, w11, fma(x10, w10, fma(x00, w00, x01 * w01)));
+    - INTERP_SEPARABLE, the generic kernel, otherwise: t_r = fma(x_r0, l0w, x_r1 * l1w), out = fma(t_0, l0h, t_1 * l1h)."""
+    return INTERP_WEIGHTS if in_workers or g.rh + g.rw <= 128 else INTERP_SEPARABLE
+
+
+@functools.lru_cache(maxsize=1024)
+def clip_axis_table(n_in: int, n_out: int, scale: float) -> np.ndarray:
+    """int32 [n_out, 4]: (i0, i1, lambda0 bits, lambda1 bits) of every output index of one axis of torch's bilinear
+    interpolation (align_corners=False), in fp32 as torch's CPU kernel computes them: src = max(fma(scale, d + 0.5,
+    -0.5), 0) (the compiler contracts it); i0 = min(floor(src), n_in - 1); i1 = i0 + (i0 < n_in - 1);
+    lambda1 = clamp(src - i0, 0, 1); lambda0 = 1 - lambda1.  Built on the host: the device must see these exact bits."""
+    f32 = np.float32
+    d = np.arange(n_out).astype(f32)
+    src = np.maximum(fma32(f32(scale), d + f32(0.5), f32(-0.5)), f32(0))
+    i0 = np.minimum(np.floor(src).astype(np.int64), n_in - 1)
+    i1 = i0 + (i0 < n_in - 1)
+    l1 = np.minimum(np.maximum(src - i0.astype(f32), f32(0)), f32(1))
+    l0 = f32(1) - l1
+    t = np.stack([i0.astype(np.int32), i1.astype(np.int32), l0.view(np.int32), l1.view(np.int32)], axis=1)
+    t.flags.writeable = False
+    return t
+
+
+def fma32(a, b, c) -> np.ndarray:
+    """fp32 a * b + c rounded once, elementwise (the CPU kernel's vector FMA; Python 3.12 has no math.fma).  The product
+    is exact in fp64 and TwoSum gives the sum's exact error, so the fp64 sum is rounded to fp32 correctly except when it
+    lands exactly on a midpoint between two fp32 values: there the sign of the error picks the side."""
+    a, b, c = (np.asarray(t, dtype=np.float32) for t in (a, b, c))
+    p = a.astype(np.float64) * b.astype(np.float64)
+    c = c.astype(np.float64)
+    s = p + c
+    bb = s - p
+    err = (p - (s - bb)) + (c - bb)
+    r = s.astype(np.float32)
+    r64 = r.astype(np.float64)
+    other = np.nextafter(r, np.where(s > r64, np.float32(np.inf), np.float32(-np.inf))).astype(np.float32)
+    tie = (s != r64) & ((r64 + other.astype(np.float64)) * 0.5 == s) & (err != 0)
+    return np.where(tie, np.where(err > 0, np.maximum(r, other), np.minimum(r, other)), r)
+
+
+def byte_table() -> torch.Tensor:
+    """fp32 [256]: to_tensor's clip.float() / 255.0 of every byte (video_transforms.py:143), computed by torch."""
+    return torch.arange(256, dtype=torch.uint8).float() / 255.0
+
+
+def clip_norm_table(norm: U8Norm) -> torch.Tensor:
+    """fp32 [262] for omt_resample_clips: the 256 byte values, then mean[3], then std[3] as fp32."""
+    if norm.max_test:
+        raise ValueError(f"normalisation {norm.name!r} tests each clip's largest byte; the video loaders' Normalize does not")
+    if len(norm.mean) != 3 or len(norm.std) != 3:
+        raise ValueError(f"normalisation {norm.name!r} has {len(norm.mean)} channels, clips have 3")
+    return torch.cat([byte_table(), torch.tensor(norm.mean, dtype=torch.float32), torch.tensor(norm.std, dtype=torch.float32)])
+
+
+def clip_params(n: int, resize: ClipResize) -> List[bool]:
+    """The flips of n clips, drawn as RandomHorizontalFlipVideo draws them clip after clip: random.random() < 0.5 from
+    Python's generator (torch's generator is not touched); nothing is drawn without a flip."""
+    return [random.random() < 0.5 for _ in range(n)] if resize.flip else [False] * n
+
+
+def check_clip_params(params, n: int, resize: ClipResize):
+    if len(params) != n:
+        raise ValueError(f"{len(params)} clip parameters for {n} clips")
+    for b, flip in enumerate(params):
+        if not isinstance(flip, (bool, np.bool_)) or (flip and not resize.flip):
+            raise ValueError(f"clip parameter {b} ({flip!r}) is not a draw of {resize}")
+
+
+def resize_clip(clip: torch.Tensor, resize: ClipResize, flip: bool = False, norm: U8Norm = None) -> torch.Tensor:
+    """Host twin of omt_resample_clips for one (F, H, W, 3) uint8 clip -> (F, 3, oh, ow) fp32: to_tensor, the flip, the
+    window, the bilinear interpolation through clip_axis_table in the arithmetic of clip_interp_form, the crop, and
+    (value - mean) / std when norm is given."""
+    F_, H, W = (int(v) for v in clip.shape[:3])
+    g = clip_geometry(H, W, resize)
+    oh, ow = clip_out_size(H, W, resize)
+    v = byte_table().numpy()[clip.numpy()]                 # (F, H, W, 3)
+    if flip:
+        v = v[:, :, ::-1]
+    v = v[:, g.y0:g.y0 + g.wh, g.x0:g.x0 + g.ww]
+    th = clip_axis_table(g.wh, g.rh, g.scale_h)[g.cy:g.cy + oh]
+    tw = clip_axis_table(g.ww, g.rw, g.scale_w)[g.cx:g.cx + ow]
+    l0h, l1h = (th[:, k].view(np.float32)[None, :, None, None] for k in (2, 3))
+    l0w, l1w = (tw[:, k].view(np.float32)[None, None, :, None] for k in (2, 3))
+
+    r0, r1 = v[:, th[:, 0]], v[:, th[:, 1]]
+    x00, x01, x10, x11 = r0[:, :, tw[:, 0]], r0[:, :, tw[:, 1]], r1[:, :, tw[:, 0]], r1[:, :, tw[:, 1]]
+    if clip_interp_form(g, resize.in_workers) == INTERP_WEIGHTS:
+        out = fma32(x11, l1h * l1w, fma32(x10, l1h * l0w, fma32(x00, l0h * l0w, x01 * (l0h * l1w))))
+    else:
+        out = fma32(fma32(x00, l0w, x01 * l1w), l0h, fma32(x10, l0w, x11 * l1w) * l1h)
+    if norm is not None:
+        out = (out - np.asarray(norm.mean, np.float32)) / np.asarray(norm.std, np.float32)
+    return torch.from_numpy(np.ascontiguousarray(out.transpose(0, 3, 1, 2)))
 
 
 def peg_neighbour_table(T: int, h: int, w: int, temporal: bool, causal: bool) -> torch.Tensor:

@@ -24,7 +24,7 @@ import torch
 import torch.nn as nn
 
 from . import layout as L
-from .consumers import EVAL_U8, IMAGE_NORM, VIDEO_NORM
+from .consumers import EVAL_U8, IMAGE_NORM, LATTE_NORM, VIDEO_NORM
 from .engine import Engine
 
 
@@ -401,6 +401,46 @@ class OmniTokenizer_VQGAN(nn.Module):
         with torch.cuda.device(self.device):
             ws, dims = eng.encode_images_u8(images, resize, params, "raw" if self.use_vae else "vq", norm)
             return self._encode_result(eng, ws.idx, eng.z_view(ws), ws.counts, dims, True, include_embeddings)
+
+    @torch.no_grad()
+    def encode_clips_u8(self, clips, resize, norm=LATTE_NORM, include_embeddings=False, params=None):
+        """encode(x, is_image=False) of the clips Latte's video loaders make of their decoded frames, from the decoded
+        frames themselves: a list of (F, H_i, W_i, C) uint8 tensors in host memory (read_video's frames, channels last),
+        the same F for every clip, any frame sizes.  `resize` (a layout.ClipResize, e.g. layout.ucf_clip_resize(256)) is
+        the loader's flip + bilinear resize + centre crop and `norm` its Normalize; omt_resample_clips applies them on the
+        device bit for bit as torch does on the CPU, so the result -- codes, embeddings, VAE latents, usage statistics,
+        CPU RNG draws -- equals encode of the stacked pipeline output rearranged 'b f c h w -> b c f h w'.  params: per
+        clip, whether it is flipped; None draws them from Python's random as RandomHorizontalFlipVideo does
+        (layout.clip_params).  Everything is checked, with encode's messages, before any launch."""
+        clips = list(clips)
+        L.check_clip_resize(resize)
+        C = self.args.image_channels
+        if not clips:
+            raise ValueError("encode_clips_u8 needs at least one clip")
+        for i, c in enumerate(clips):
+            if not isinstance(c, torch.Tensor) or c.dtype != torch.uint8:
+                raise TypeError(f"clip {i}: expected a uint8 tensor, got {getattr(c, 'dtype', type(c))}")
+            if c.ndim != 4 or c.shape[3] != C or min(c.shape[:3]) < 1:
+                raise ValueError(f"clip {i}: expected (F, H, W, {C}) with F, H, W >= 1, got {tuple(c.shape)}")
+            if c.device.type != "cpu":
+                raise ValueError(f"clip {i}: expected decoded frames in host memory, got a clip on {c.device}")
+            if c.shape[0] != clips[0].shape[0]:
+                raise ValueError(f"every clip must have the same number of frames: {clips[0].shape[0]} and {c.shape[0]}")
+        sizes = {tuple(L.clip_out_size(int(c.shape[1]), int(c.shape[2]), resize)) for c in clips}
+        if len(sizes) > 1:
+            raise ValueError(f"the clips come out at different sizes {sorted(sizes)}: without a resize every clip must "
+                             f"have the same frame size")
+        for c in clips:
+            L.clip_geometry(int(c.shape[1]), int(c.shape[2]), resize)      # the reference's center_crop ValueError
+        L.clip_norm_table(norm)
+        eng = self.engine()
+        eng._shape((len(clips), C, int(clips[0].shape[0])) + sizes.pop())
+        if params is None:
+            params = L.clip_params(len(clips), resize)
+        L.check_clip_params(params, len(clips), resize)
+        with torch.cuda.device(self.device):
+            ws, dims = eng.encode_clips_u8(clips, resize, params, "raw" if self.use_vae else "vq", norm)
+            return self._encode_result(eng, ws.idx, eng.z_view(ws), ws.counts, dims, False, include_embeddings)
 
     def _encode_result(self, eng, idx, z, counts, dims, is_image, include_embeddings):
         """What encode() returns (omnitokenizer.py:247-266), with Codebook.forward's usage side effects, from the encoder's
