@@ -33,6 +33,12 @@ VQ_MAX_CODES = 41856
 # longest latent sequence of the temporal attention core (csrc/attention_fp32.cu attn_temporal_kernel keeps the K / V of
 # one pixel's T' frames in registers, one template instance per T'): 17 latent frames, 65 frames at temporal patch 4
 TEMPORAL_MAX_FRAMES = 17
+# longest patch vector (C * pt * p * p features) of the patch gather + LayerNorm (csrc/rowwise.cu omt_patchify_ln, _u8)
+PATCH_MAX_K = 1024
+# k-block of each math mode's GEMM (csrc/gemm_fp32.cu, gemm_tc2.cu, gemm_f16.cu): a patch vector is a whole number of them
+PATCH_K_BLOCK = {_cabi.MATH_FP32: 8, _cabi.MATH_3XTF32: 32, _cabi.MATH_F16X3: 64, _cabi.MATH_F16X1: 64}
+# window side of the window attention kernel (csrc/attention_fp32.cu omt_attn_window: 64-token windows)
+WINDOW_SIZE = 8
 # int32 words of one omt_resample_desc (include/omnitok_b200.h): the int64 source offset, then 16 int32 fields
 DESC_WORDS = 18
 # int32 words of one omt_clip_desc: the int64 source offset, then 14 int32 fields
@@ -198,6 +204,10 @@ class Engine:
             raise NotImplementedError("omnitok_b200 kernels are specialised for embedding_dim=512, heads x dim_head = 8 x 64")
         self.p, self.pt, self.cin = a.patch_size, a.temporal_patch_size, a.image_channels
         self.ws = a.twod_window_size
+        self.has_window = "w" in (a.enc_block + a.dec_block)
+        if self.has_window and self.ws != WINDOW_SIZE:
+            raise NotImplementedError(f"--twod_window_size {self.ws}: omt_attn_window is specialised for "
+                                      f"{WINDOW_SIZE}x{WINDOW_SIZE} windows (enc_block {a.enc_block!r}, dec_block {a.dec_block!r})")
         self.causal_attn = bool(a.causal_in_temporal_transformer)
         self.causal_peg = bool(a.causal_in_peg)
         self.rope = a.spatial_pos == "rope"
@@ -208,6 +218,12 @@ class Engine:
             raise NotImplementedError(f"--codebook_dim {self.cd}: the VQ search / post_vq kernels are specialised for "
                                       "codebook_dim 8 (every shipped config); VAE mode takes 8 latent channels as well")
         self.planes = self.math in PLANE_MATHS
+        # a first-frame patch vector is K of the encoder's patch GEMM and N of the decoder's to_pixels GEMM (the other
+        # frames' vectors are whole multiples of it): it must be a whole k-block of the mode's GEMM
+        k_block = PATCH_K_BLOCK[self.math]
+        if (self.cin * self.p * self.p) % k_block:
+            raise NotImplementedError(f"--patch_size {self.p}: a patch vector of {self.cin * self.p * self.p} features is not "
+                                      f"a whole {k_block}-wide k-block of the {self.math_name} GEMM")
         # f16x1: every GEMM and the f16 spatial core take their single-product forms (omt_linear_h1, omt_attn_spatial_h1)
         self.h1 = self.math == _cabi.MATH_F16X1
         # spatial attention core on fp16 operand planes (attention_f16.cu, default); OMT_ATTN_F16=0 = the 3xTF32 core on the fp32 QKV buffer
@@ -292,7 +308,6 @@ class Engine:
         self.dec_temporal = transformer("decoder.dec_temporal_transformer", tb)
         self.dec_spatial = transformer("decoder.dec_spatial_transformer", a.dec_block)
 
-        self.has_window = "w" in (a.enc_block + a.dec_block)
         self.pe = {}
         self.cnn = getattr(a, "patch_embed", "linear") == "cnn"
         if self.cnn:
@@ -543,9 +558,13 @@ class Engine:
                                         f"patch size ({self.pt})")
         if H != W or H % self.p != 0:
             raise ValueError(f"frames must be square with side a multiple of the patch size {self.p} (got {H}x{W})")
-        if self.has_window and (self.ws * self.ws != 64 or (H // self.p) % self.ws != 0):
-            raise ValueError(f"window blocks need twod_window_size 8 and a token grid divisible by it (got window "
-                             f"{self.ws}, grid {H // self.p}x{W // self.p}): omt_attn_window is specialised for 8x8 windows")
+        if self.has_window and (H // self.p) % self.ws != 0:
+            raise ValueError(f"window blocks need a token grid divisible by the window (got window {self.ws}, grid "
+                             f"{H // self.p}x{W // self.p})")
+        k = self.cin * (self.pt if T > 1 else 1) * self.p * self.p
+        if k > PATCH_MAX_K:
+            raise NotImplementedError(f"--patch_size {self.p} with --temporal_patch_size {self.pt}: a patch vector of {k} "
+                                      f"features is longer than the {PATCH_MAX_K} the patch gather takes")
         if ((H // self.p) * (W // self.p)) % 64 != 0:
             raise ValueError(f"tokens per frame ({(H // self.p) * (W // self.p)}) must be a multiple of 64 (attention tiles)")
         Tp = 1 + (T - 1) // self.pt

@@ -786,18 +786,26 @@ class OmniTokenizer_VQGAN(nn.Module):
 VQGAN = OmniTokenizer_VQGAN   # the reference's class name inside omnitokenizer.py
 
 
-def canonical_args(extra=()):
-    """argparse Namespace of the canonical config used by every shipped eval script
-    (scripts/recons/eval_video.sh:1-9)."""
+CANONICAL_ARGV = ("--patch_embed linear --patch_size 8 --temporal_patch_size 4 --spatial_depth 4 --temporal_depth 4 "
+                  "--embedding_dim 512 --disc_layers 3 --enc_block ttww --dec_block tttt --twod_window_size 8 "
+                  "--causal_in_temporal_transformer --causal_in_peg --dim_head 64 --heads 8 --apply_noise --apply_blur "
+                  "--spatial_pos rope --n_codes 8192 --codebook_dim 8 --l2_code --commitment_weight 1.0 "
+                  "--no_random_restart --resolution 256 --sequence_length 17 --norm_type batch").split()
+
+
+def parse_args(argv):
+    """argparse Namespace of a command line as vqgan_eval.py parses it (base.VQGAN's, this module's and VideoData's
+    flags), without the canonical flags: store_true flags absent from argv stay False."""
     p = argparse.ArgumentParser()
     p = OmniTokenizer_VQGAN.add_base_model_args(p)
     p = OmniTokenizer_VQGAN.add_model_specific_args(p)
     for f, d in (("--resolution", 256), ("--sequence_length", 17), ("--image_channels", 3),
                  ("--sample_every_n_frames", 1)):
         p.add_argument(f, type=int, default=d)
-    argv = ("--patch_embed linear --patch_size 8 --temporal_patch_size 4 --spatial_depth 4 --temporal_depth 4 "
-            "--embedding_dim 512 --disc_layers 3 --enc_block ttww --dec_block tttt --twod_window_size 8 "
-            "--causal_in_temporal_transformer --causal_in_peg --dim_head 64 --heads 8 --apply_noise --apply_blur "
-            "--spatial_pos rope --n_codes 8192 --codebook_dim 8 --l2_code --commitment_weight 1.0 "
-            "--no_random_restart --resolution 256 --sequence_length 17 --norm_type batch").split()
-    return p.parse_args(argv + list(extra))
+    return p.parse_args(list(argv))
+
+
+def canonical_args(extra=()):
+    """argparse Namespace of the canonical config used by every shipped eval script
+    (scripts/recons/eval_video.sh:1-9)."""
+    return parse_args(CANONICAL_ARGV + list(extra))

@@ -81,6 +81,8 @@ class Config:
 
     @staticmethod
     def from_args(args) -> "Config":
+        """An old checkpoint's Namespace lacks the newer flags: they take the reference's back-fills
+        (omnitokenizer.py:70-125), not this class's canonical defaults."""
         c = Config()
         for k in c.__dataclass_fields__:
             if hasattr(args, k) and getattr(args, k) is not None:
@@ -89,6 +91,12 @@ class Config:
             c.enc_block = "t" * args.spatial_depth
         if not hasattr(args, "dec_block"):
             c.dec_block = "t" * args.spatial_depth
+        if not hasattr(args, "twod_window_size"):
+            c.twod_window_size = 4
+        if not hasattr(args, "spatial_pos"):
+            c.spatial_pos = "rel"
+        if not hasattr(args, "use_vae"):
+            c.use_vae = False
         return c
 
 

@@ -1,4 +1,5 @@
 """Shared helpers for the parity tests (oracle = oracle/omni_oracle.py, test infrastructure)."""
+import dataclasses
 import os
 
 import torch
@@ -55,6 +56,30 @@ def namespace_from_cfg(cfg: oo.Config, **over):
     for k, v in over.items():
         setattr(a, k, v)
     return a
+
+
+def flags_namespace(row):
+    """A fresh argparse Namespace of a tests/golden/flags.pt row: its command line, minus the keys an old checkpoint's
+    Namespace lacks (the model back-fills them in place, so every model gets its own)."""
+    from omnitokenizer_b200.vqgan import parse_args
+    a = parse_args(row["argv"])
+    for k in row["drop"]:
+        delattr(a, k)
+    return a
+
+
+def flags_setup(row):
+    """(cfg, state_dict, [input, ...]) of a tests/golden/flags.pt row, proven to be the ones the reference run used."""
+    cfg = oo.Config.from_args(flags_namespace(row))
+    assert dataclasses.asdict(cfg) == row["cfg"], "the Namespace reads as a different model than the reference built"
+    sd = W.make_state_dict(cfg, row["wseed"])
+    assert W.fingerprint(sd) == row["fingerprint"], "synthetic checkpoint differs from the one the golden run used"
+    xs = []
+    for inp in row["inputs"]:
+        x = W.synthetic_input(inp["shape"], inp["xseed"])
+        assert float(x.double().sum()) == inp["x_sum64"]
+        xs.append(x)
+    return cfg, sd, xs
 
 
 def build_model(cfg, sd, device, math=None):
