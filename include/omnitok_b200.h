@@ -73,7 +73,7 @@ int omt_linear(const float* A, int lda, int a_seg, int a_seg_stride, int a_seg_o
 /* Dual-A form: C[:, :n_split] = A1 . W[:n_split]^T and C[:, n_split:] = A2 . W[n_split:]^T in ONE launch.
  * Attention.forward projects q from the LayerNormed input and k, v from the RAW input
  * (attention.py:407-412); stacking [Wq; Wkv] and switching the A tensor map per output tile fuses the two
- * nn.Linear calls without changing either result.  n_split % 256 == 0; same lda for A1 and A2. */
+ * nn.Linear calls without changing either result.  n_split % 128 == 0 (a whole output tile); same lda for A1 and A2. */
 int omt_linear2(const float* A1, const float* A2, int n_split, int lda, const float* W, const float* W_lo,
                 float* C, int ldc, int M, int N, int K, int math,
                 /* optional fused q/k preparation (what omt_qk_prep does), q_scale == NULL disables it:
@@ -284,7 +284,7 @@ int omt_vq_fused(const float* x, int ldx, const float* Wt, const float* b, int C
                  omt_stream_t stream);
 
 /* Decode-side lookup: F.embedding gather (omnitokenizer.py:270) + post_vq_conv Linear(cd, C) (:156-160).
- * If idx != NULL rows come from E[idx[r]]; else from zc[M, cd].  X[M, C] = row . Wt^T + b.
+ * If idx != NULL rows come from E[idx[r]]; else from zc[M, cd].  X[M, C] = row . Wt^T + b, C % 4 == 0, C <= 1024.
  * When z_st_from != NULL (forward(): straight-through, codebook.py:120) the row is (E[idx]-z)+z and is
  * also written to zq_out[M, cd] (may be NULL). */
 int omt_post_vq(const int64_t* idx, const float* E, const float* zc, const float* z_st_from,
@@ -304,7 +304,7 @@ typedef struct omt_linear_h_args {
   const float* a_rs; const float* a2_rs;           /* non-NULL: ROW-SCALED planes (below): inverse row scales [rows of A] */
   float w_scale;                                   /* row-scaled form: inverse of the per-matrix scale of the W planes */
   const uint16_t* a2_hi; const uint16_t* a2_lo;    /* optional second A (dual-A form, columns >= n_split), same lda / row map */
-  int n_split;                                     /* multiple of 256 */
+  int n_split;                                     /* multiple of 128 (a whole output tile) */
   int lda, a_seg, a_seg_stride, a_seg_off;         /* lda % 8 == 0; row map as in omt_linear (segments of 64 rows) */
   const uint16_t* w_hi; const uint16_t* w_lo;      /* W planes [N rounded up to 256, K], K % 64 == 0 */
   float* c; int ldc, c_seg, c_seg_stride, c_seg_off;   /* fp32 output (OMT_EPI_NONE / OMT_EPI_QKV); row map segments of 32 rows */

@@ -37,7 +37,7 @@ static int launch_gemm_f16(const omt_linear_h_args& a, cudaStream_t st, const ch
   if (a.c_seg > 0)
     OMT_REQUIRE(a.c_seg % 32 == 0 && a.M % a.c_seg == 0, "%s: C row-map segment %d must be a multiple of 32 dividing M=%d", who, a.c_seg, a.M);
   OMT_REQUIRE(a.N % 32 == 0, "%s: N=%d must be a multiple of 32", who, a.N);
-  if (a.a2_hi != nullptr) OMT_REQUIRE(a.n_split > 0 && a.n_split % 256 == 0, "%s: n_split=%d must be a multiple of 256", who, a.n_split);
+  if (a.a2_hi != nullptr) OMT_REQUIRE(a.n_split > 0 && a.n_split % 128 == 0, "%s: n_split=%d must be a multiple of 128", who, a.n_split);
   const int n_pad = (a.N + 255) / 256 * 256;
   const CUtensorMapDataType f16 = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const bool dual = a.a2_hi != nullptr;

@@ -15,7 +15,7 @@ int launch_gemm_tc2(const GemmArgs& g, const float* W_lo, int epilogue, cudaStre
   if (g.a_seg > 0) {
     OMT_REQUIRE(g.a_seg % 64 == 0 && g.M % g.a_seg == 0, "omt_linear(wgmma 3xTF32): A row-map segment %d must be a multiple of 64 dividing M=%d", g.a_seg, g.M);
   }
-  if (A2 != nullptr) OMT_REQUIRE(n_split > 0 && n_split % 256 == 0, "omt_linear2: n_split=%d must be a multiple of 256", n_split);
+  if (A2 != nullptr) OMT_REQUIRE(n_split > 0 && n_split % 128 == 0, "omt_linear2: n_split=%d must be a multiple of 128", n_split);
   const int n_pad = (g.N + 127) / 128 * 128;
   const CUtensorMapDataType f32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUtensorMap maps[6];

@@ -53,7 +53,7 @@ struct LnPlanes {          // optional fp16 hi / lo operand planes (omt_layernor
   float* y_rs; float* x_rs;          // non-NULL: row-scaled planes (omt_common.cuh), the inverse row scale goes here
 };
 
-// PAIR (C a multiple of 256, NV even): a lane owns 8 consecutive columns per 256-column block (two adjacent float4 chunks), so
+// PAIR (C a multiple of 256, NV = C / 128: 2, 4, 6 or 8): a lane owns 8 consecutive columns per 256-column block (two adjacent float4 chunks), so
 // the row-scaled planes leave as 16-byte stores (512 B per warp instruction) instead of 8-byte ones.
 template <int NV, bool PAIR>   // float4 chunks per lane
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, int ldx,
@@ -820,6 +820,14 @@ static int layernorm_impl(const char* who, const float* x, int ldx, float* y, in
     case 4:
       if (pair) OMT_CUDA(launch_k(layernorm_kernel<4, true>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
       else OMT_CUDA(launch_k(layernorm_kernel<4, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
+      break;
+    case 6:      // C = 768 paired; every other width of 6 chunks takes <8, false>
+      if (pair) OMT_CUDA(launch_k(layernorm_kernel<6, true>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
+      else OMT_CUDA(launch_k(layernorm_kernel<8, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
+      break;
+    case 8:      // C = 1024 paired
+      if (pair) OMT_CUDA(launch_k(layernorm_kernel<8, true>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
+      else OMT_CUDA(launch_k(layernorm_kernel<8, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
       break;
     default: OMT_CUDA(launch_k(layernorm_kernel<8, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl)); break;
   }

@@ -256,20 +256,16 @@ vq_fused_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ 
 
 // ---------------------------------------------------------------------------------------
 // post_vq: X[M, C] = zrow[M, CD] . W[C, CD]^T + b, zrow = E[idx] | zc | (E[idx]-z)+z.
-// Block = C/4 threads, thread owns 4 output channels (its 4 x CD weights live in registers).
+// Block = C/4 threads rounded up to 128 (C <= 512) or 256 (C <= 1024, the wide kernel); a thread owns 4 output channels
+// (its 4 x CD weights live in registers).  Both kernels run the same body: only the launch bounds differ.
 // ---------------------------------------------------------------------------------------
 constexpr int POSTVQ_ROWS = 32;
 
 template <int CD>
-__global__ void __launch_bounds__(128) post_vq_kernel(const int64_t* __restrict__ idx,
-                                                      const float* __restrict__ E,
-                                                      const float* __restrict__ zc,
-                                                      const float* __restrict__ zst,
-                                                      float* __restrict__ zq_out,
-                                                      const float* __restrict__ Wt,
-                                                      const float* __restrict__ b,
-                                                      float* __restrict__ X, int M, int C) {
-  pdl_sync();
+__device__ __forceinline__ void post_vq_rows(const int64_t* __restrict__ idx, const float* __restrict__ E,
+                                             const float* __restrict__ zc, const float* __restrict__ zst,
+                                             float* __restrict__ zq_out, const float* __restrict__ Wt,
+                                             const float* __restrict__ b, float* __restrict__ X, int M, int C) {
   __shared__ float rows[POSTVQ_ROWS][CD];
   const int r0 = blockIdx.x * POSTVQ_ROWS;
   for (int i = threadIdx.x; i < POSTVQ_ROWS * CD; i += blockDim.x) {
@@ -311,6 +307,33 @@ __global__ void __launch_bounds__(128) post_vq_kernel(const int64_t* __restrict_
     *reinterpret_cast<float4*>(X + (size_t)r * C + c) =
         make_float4(o[0] + bb.x, o[1] + bb.y, o[2] + bb.z, o[3] + bb.w);
   }
+}
+
+template <int CD>
+__global__ void __launch_bounds__(128) post_vq_kernel(const int64_t* __restrict__ idx,
+                                                      const float* __restrict__ E,
+                                                      const float* __restrict__ zc,
+                                                      const float* __restrict__ zst,
+                                                      float* __restrict__ zq_out,
+                                                      const float* __restrict__ Wt,
+                                                      const float* __restrict__ b,
+                                                      float* __restrict__ X, int M, int C) {
+  pdl_sync();
+  post_vq_rows<CD>(idx, E, zc, zst, zq_out, Wt, b, X, M, C);
+}
+
+// C in (512, 1024]: 256 threads
+template <int CD>
+__global__ void __launch_bounds__(256) post_vq_wide_kernel(const int64_t* __restrict__ idx,
+                                                           const float* __restrict__ E,
+                                                           const float* __restrict__ zc,
+                                                           const float* __restrict__ zst,
+                                                           float* __restrict__ zq_out,
+                                                           const float* __restrict__ Wt,
+                                                           const float* __restrict__ b,
+                                                           float* __restrict__ X, int M, int C) {
+  pdl_sync();
+  post_vq_rows<CD>(idx, E, zc, zst, zq_out, Wt, b, X, M, C);
 }
 
 }  // namespace omt
@@ -407,12 +430,15 @@ extern "C" int omt_post_vq(const int64_t* idx, const float* E, const float* zc, 
   OMT_ENTER();
   OMT_REQUIRE(Wt && b && X, "omt_post_vq: null pointer");
   OMT_REQUIRE((idx != nullptr && E != nullptr) || zc != nullptr, "omt_post_vq: need idx+E or zc");
-  OMT_REQUIRE(C % 4 == 0 && C <= 512, "omt_post_vq: C=%d unsupported", C);
+  OMT_REQUIRE(C % 4 == 0 && C <= 1024, "omt_post_vq: C=%d unsupported (C %% 4 == 0, C <= 1024)", C);
   OMT_REQUIRE(aligned_to(16, {X, b}), "omt_post_vq: X and b must be 16-byte aligned");
   OMT_REQUIRE(cd == 8, "omt_post_vq: codebook_dim %d unsupported (8)", cd);
   if (M == 0) return OMT_OK;
-  OMT_CUDA(launch_k(post_vq_kernel<8>, dim3((M + POSTVQ_ROWS - 1) / POSTVQ_ROWS), dim3(128), 0, (cudaStream_t)stream,
-                    idx, E, zc, z_st_from, zq_out, Wt, b, X, M, C));
+  const dim3 grid((M + POSTVQ_ROWS - 1) / POSTVQ_ROWS);
+  if (C <= 512)
+    OMT_CUDA(launch_k(post_vq_kernel<8>, grid, dim3(128), 0, (cudaStream_t)stream, idx, E, zc, z_st_from, zq_out, Wt, b, X, M, C));
+  else
+    OMT_CUDA(launch_k(post_vq_wide_kernel<8>, grid, dim3(256), 0, (cudaStream_t)stream, idx, E, zc, z_st_from, zq_out, Wt, b, X, M, C));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

@@ -39,6 +39,14 @@ PATCH_MAX_K = 1024
 PATCH_K_BLOCK = {_cabi.MATH_FP32: 8, _cabi.MATH_3XTF32: 32, _cabi.MATH_F16X3: 64, _cabi.MATH_F16X1: 64}
 # window side of the window attention kernel (csrc/attention_fp32.cu omt_attn_window: 64-token windows)
 WINDOW_SIZE = 8
+# model widths C (--embedding_dim) the kernels take: LayerNorm holds a row of at most 1024 channels in one warp's registers,
+# post_vq / pre_vq / the VQ lookup take C <= 1024, and every width here is a whole number of 256-column GEMM tiles
+MODEL_WIDTHS = (256, 512, 768, 1024)
+# head dimension of every attention core (AD = 64, the wgmma tiles)
+HEAD_DIM = 64
+# attention width A = 64 * heads: the fused QKV GEMM switches from the normalised to the raw input at column A, which must
+# start a 128-column output tile, so heads is even; 2..16 heads give A = 128..1024
+MAX_HEADS = 16
 # int32 words of one omt_resample_desc (include/omnitok_b200.h): the int64 source offset, then 16 int32 fields
 DESC_WORDS = 18
 # int32 words of one omt_clip_desc: the int64 source offset, then 14 int32 fields
@@ -91,23 +99,26 @@ class PackedLinear:
 
 
 class Workspace:
-    def __init__(self, device, M: int, C: int, ku: int, kmax: int, cd: int, planes: bool):
+    """Per-shape buffers.  C: model width; A: attention width (q | k | v and the attention output; a window layer, whose
+    width is C, runs only in models with C == A)."""
+
+    def __init__(self, device, M: int, C: int, A: int, ku: int, kmax: int, cd: int, planes: bool):
         f = dict(device=device, dtype=torch.float32)
         self.M = M
         self.buf0 = torch.empty(M, C, **f)
         self.buf1 = torch.empty(M, C, **f)
         self.X, self.Y = self.buf0, self.buf1
-        self.QKV = torch.empty(M, 3 * C, **f)
+        self.QKV = torch.empty(M, 3 * A, **f)
         self.P = torch.empty(M, kmax, **f)       # patch matrix (pixels side), rows x K
         if planes:     # f16x3: every GEMM A operand lives as fp16 hi / lo planes written by its producer
             self.XNp, self.XSp = Planes(device, M, C, True), Planes(device, M, C, True)     # LayerNorm sees whole rows
-            self.Op, self.Up = Planes(device, M, C), Planes(device, M, ku)                  # attention heads / GEGLU tiles do not
+            self.Op, self.Up = Planes(device, M, A), Planes(device, M, ku)                  # attention heads / GEGLU tiles do not
             self.Pp = Planes(device, M, kmax, True)
-            self.QKVp = Planes(device, M, 3 * C)     # q | k | v operand planes for the f16 attention core (QKV GEMM epilogue)
-            self.vinv = torch.empty(C // 64, M, device=device, dtype=torch.float32)   # inverse (row, head) scales of the v planes
+            self.QKVp = Planes(device, M, 3 * A)     # q | k | v operand planes for the f16 attention core (QKV GEMM epilogue)
+            self.vinv = torch.empty(A // 64, M, device=device, dtype=torch.float32)   # inverse (row, head) scales of the v planes
         else:
             self.XN = torch.empty(M, C, **f)
-            self.O = torch.empty(M, C, **f)
+            self.O = torch.empty(M, A, **f)
             self.U = torch.empty(M, ku, **f)
         self.z = torch.empty(M, cd, **f)
         self.idx = torch.empty(M, device=device, dtype=torch.int64)
@@ -198,16 +209,30 @@ class Engine:
             raise ValueError(f"unknown OMT_MATH mode {self.math_name!r}; choose from {sorted(MATH_MODES)}")
         self.math = MATH_MODES[self.math_name]
         a = model.args
+        # C: the model width (LayerNorm, PEG, FF, residual stream); A: the attention width of the temporal / spatial
+        # attention blocks, heads x dim_head, independent of C (to_q C -> A, to_kv C -> 2A, to_out A -> C, attention.py:395-486)
         self.C = a.embedding_dim
         self.heads, self.dh = a.heads, a.dim_head
-        if self.C != 512 or self.dh != 64 or self.heads * self.dh != self.C:
-            raise NotImplementedError("omnitok_b200 kernels are specialised for embedding_dim=512, heads x dim_head = 8 x 64")
+        self.A = self.heads * self.dh
+        if self.dh != HEAD_DIM:
+            raise NotImplementedError(f"--dim_head {self.dh}: every attention core is built on {HEAD_DIM}-wide heads")
+        if self.heads % 2 or not 2 <= self.heads <= MAX_HEADS:
+            raise NotImplementedError(f"--heads {self.heads}: the kernels take an even number of heads from 2 to {MAX_HEADS} "
+                                      f"(the fused QKV GEMM switches its input at column {HEAD_DIM} x heads, which must start "
+                                      "a 128-column output tile)")
+        if self.C not in MODEL_WIDTHS:
+            raise NotImplementedError(f"--embedding_dim {self.C}: the kernels take model widths {', '.join(map(str, MODEL_WIDTHS))}")
         self.p, self.pt, self.cin = a.patch_size, a.temporal_patch_size, a.image_channels
         self.ws = a.twod_window_size
         self.has_window = "w" in (a.enc_block + a.dec_block)
         if self.has_window and self.ws != WINDOW_SIZE:
             raise NotImplementedError(f"--twod_window_size {self.ws}: omt_attn_window is specialised for "
                                       f"{WINDOW_SIZE}x{WINDOW_SIZE} windows (enc_block {a.enc_block!r}, dec_block {a.dec_block!r})")
+        # window attention splits the model width itself into heads of C / heads (attention.py:254-293)
+        if self.has_window and self.C != HEAD_DIM * self.heads:
+            raise NotImplementedError(f"--heads {self.heads} with --embedding_dim {self.C}: window blocks (enc_block "
+                                      f"{a.enc_block!r}, dec_block {a.dec_block!r}) take heads of C / heads = "
+                                      f"{self.C / self.heads:g} channels; omt_attn_window takes {HEAD_DIM}")
         self.causal_attn = bool(a.causal_in_temporal_transformer)
         self.causal_peg = bool(a.causal_in_peg)
         self.rope = a.spatial_pos == "rope"
@@ -367,7 +392,7 @@ class Engine:
         ws = self._ws.get(M)
         if ws is None:
             kmax = self.cin * self.pt * self.p * self.p
-            ws = Workspace(self.device, M, self.C, self.ku, kmax, max(self.cd, 16), self.planes)
+            ws = Workspace(self.device, M, self.C, self.A, self.ku, kmax, max(self.cd, 16), self.planes)
             if ws.counts.numel() < self.n_codes:
                 ws.counts = torch.zeros(self.n_codes, device=self.device, dtype=torch.int32)
             while len(self._ws) >= 3:  # keep a few shapes (and their graphs) resident
@@ -461,13 +486,14 @@ class Engine:
 
     def _transformer(self, tr, ws: Workspace, lay: BatchLayout, temporal: bool, out_planes: Optional[Planes] = None):
         """modules/attention.py:655-689.  out_planes: norm_out goes to operand planes (decoder -> to_pixels GEMMs)."""
-        C, N, M = self.C, lay.N, ws.M
+        C, A, N, M = self.C, self.A, lay.N, ws.M
         h, w, F = lay.h, lay.w, lay.frames
         B, T = lay.B, lay.groups[0].tp
         H = self.planes
+        # q | k | v [M, 3A] and the attention output [M, A]; a window layer's are 3C / C wide, and C == A in a model with one
         q_ptr = ws.QKV.data_ptr()
-        k_ptr, v_ptr = q_ptr + C * 4, q_ptr + 2 * C * 4
-        ld3 = 3 * C
+        k_ptr, v_ptr = q_ptr + A * 4, q_ptr + 2 * A * 4
+        ld3 = 3 * A
         o, o_hi, o_lo = (None, ws.Op.hi, ws.Op.lo) if H else (ws.O, None, None)
         t_off = None if lay.uniform else self._layout_tables(ws, lay)[:2]
         for lyr in tr["layers"]:
@@ -488,39 +514,39 @@ class Engine:
                 f16_core = H and self.attn_f16 and (not temporal) and N % 128 == 0
                 if f16_core:
                     self._ln_h(ws.X, ws.XNp, lyr["norm_g"], lyr["norm_b"], M, xp=ws.XSp)
-                    self._linear_h(ws.XNp, wq, M, U=ws.QKVp, A2=ws.XSp, n_split=C, epi=_cabi.EPI_QKV_PLANES,
-                                   qk=(lyr["q_scale"], lyr["k_scale"], cos, sin, 2 * C, N),
+                    self._linear_h(ws.XNp, wq, M, U=ws.QKVp, A2=ws.XSp, n_split=A, epi=_cabi.EPI_QKV_PLANES,
+                                   qk=(lyr["q_scale"], lyr["k_scale"], cos, sin, 2 * A, N),
                                    planes=(lyr["q_ps"], lyr["k_ps"], ws.vinv))
                 elif H:
                     self._ln_h(ws.X, ws.XNp, lyr["norm_g"], lyr["norm_b"], M, xp=ws.XSp)
-                    self._linear_h(ws.XNp, wq, M, C=q_ptr, ldc=ld3, A2=ws.XSp, n_split=C, epi=_cabi.EPI_QKV,
-                                   qk=(lyr["q_scale"], lyr["k_scale"], cos, sin, 2 * C, N))
+                    self._linear_h(ws.XNp, wq, M, C=q_ptr, ldc=ld3, A2=ws.XSp, n_split=A, epi=_cabi.EPI_QKV,
+                                   qk=(lyr["q_scale"], lyr["k_scale"], cos, sin, 2 * A, N))
                 else:
                     self._ln(ws.X, ws.XN, lyr["norm_g"], lyr["norm_b"], M)
                     if self.fuse_qkprep(M):
-                        _cabi.call("omt_linear2", ws.XN, ws.X, C, C, wq.w, wq.w_lo, q_ptr, ld3, M, wq.n, wq.k, wq.math,
-                                   lyr["q_scale"], lyr["k_scale"], cos, sin, 2 * C, N)
+                        _cabi.call("omt_linear2", ws.XN, ws.X, A, C, wq.w, wq.w_lo, q_ptr, ld3, M, wq.n, wq.k, wq.math,
+                                   lyr["q_scale"], lyr["k_scale"], cos, sin, 2 * A, N)
                     else:
-                        _cabi.call("omt_linear2", ws.XN, ws.X, C, C, wq.w, wq.w_lo, q_ptr, ld3, M, wq.n, wq.k, wq.math,
+                        _cabi.call("omt_linear2", ws.XN, ws.X, A, C, wq.w, wq.w_lo, q_ptr, ld3, M, wq.n, wq.k, wq.math,
                                    None, None, None, None, 0, 0)
                         _cabi.call("omt_qk_prep", q_ptr, ld3, k_ptr, ld3, lyr["q_scale"], lyr["k_scale"], cos, sin, M, N,
                                    self.heads)
                 if f16_core and self.h1:
                     ph = ws.QKVp.hi.data_ptr()
-                    _cabi.call("omt_attn_spatial_h1", ph, ld3, ph + 2 * C, ld3, ph + 4 * C, ld3, ws.vinv, lyr["q_ps"] * lyr["k_ps"],
-                               None, o_hi, C, F, N, self.heads, 8.0)
+                    _cabi.call("omt_attn_spatial_h1", ph, ld3, ph + 2 * A, ld3, ph + 4 * A, ld3, ws.vinv, lyr["q_ps"] * lyr["k_ps"],
+                               None, o_hi, A, F, N, self.heads, 8.0)
                 elif f16_core:
                     ph, pl = ws.QKVp.hi.data_ptr(), ws.QKVp.lo.data_ptr()
-                    _cabi.call("omt_attn_spatial_h", ph, pl, ld3, ph + 2 * C, pl + 2 * C, ld3, ph + 4 * C, pl + 4 * C, ld3,
-                               ws.vinv, lyr["q_ps"] * lyr["k_ps"], None, o_hi, o_lo, C, F, N, self.heads, 8.0)
+                    _cabi.call("omt_attn_spatial_h", ph, pl, ld3, ph + 2 * A, pl + 2 * A, ld3, ph + 4 * A, pl + 4 * A, ld3,
+                               ws.vinv, lyr["q_ps"] * lyr["k_ps"], None, o_hi, o_lo, A, F, N, self.heads, 8.0)
                 elif temporal and lay.uniform:
-                    _cabi.call("omt_attn_temporal", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, B, T, N,
+                    _cabi.call("omt_attn_temporal", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, A, B, T, N,
                                self.heads, 8.0, int(self.causal_attn))
                 elif temporal:
-                    _cabi.call("omt_attn_temporal_varlen", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, *t_off, B,
+                    _cabi.call("omt_attn_temporal_varlen", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, A, *t_off, B,
                                M, N, self.heads, 8.0, int(self.causal_attn))
                 else:
-                    _cabi.call("omt_attn_spatial", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, F, N,
+                    _cabi.call("omt_attn_spatial", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, A, F, N,
                                self.heads, 8.0)
                 proj = lyr["to_out"]
             else:
@@ -530,8 +556,9 @@ class Engine:
                 else:
                     self._ln(ws.X, ws.XN, lyr["norm_g"], lyr["norm_b"], M)
                     self._linear(ws.XN, C, lyr["qkv"], q_ptr, ld3, M)
-                _cabi.call("omt_attn_window", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, C, lyr["bias"], F, h,
-                           w, self.ws, self.heads, float(self.dh) ** -0.5)
+                # C == A here (Engine.__init__): the window qkv is 3C wide with heads of C / heads = 64; scale (C / heads)^-0.5
+                _cabi.call("omt_attn_window", q_ptr, ld3, k_ptr, ld3, v_ptr, ld3, o, o_hi, o_lo, A, lyr["bias"], F, h,
+                           w, self.ws, self.heads, float(C // self.heads) ** -0.5)
                 proj = lyr["proj"]
             if H:
                 self._linear_h(ws.Op, proj, M, C=ws.X, ldc=C, residual=ws.X, ldr=C)
@@ -540,7 +567,7 @@ class Engine:
                 self._linear_h(ws.XNp, lyr["ff1"], M, U=ws.Up, epi=_cabi.EPI_GEGLU, u_scale=us)
                 self._linear_h(ws.Up, lyr["ff2"], M, C=ws.X, ldc=C, residual=ws.X, ldr=C, a_uniform=(1.0 / us if us > 0 else 0.0))
             else:
-                self._linear(ws.O, C, proj, ws.X, C, M, residual=ws.X, ldr=C)
+                self._linear(ws.O, A, proj, ws.X, C, M, residual=ws.X, ldr=C)
                 self._ln(ws.X, ws.XN, lyr["ff_g"], lyr["ff_b"], M)
                 self._linear(ws.XN, C, lyr["ff1"], ws.U, self.ku, M, epi=_cabi.EPI_GEGLU)
                 self._linear(ws.U, self.ku, lyr["ff2"], ws.X, C, M, residual=ws.X, ldr=C)
