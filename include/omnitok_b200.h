@@ -172,6 +172,40 @@ int omt_resample_clips(const uint8_t* src, long long src_bytes, const omt_clip_d
                        const int32_t* tab, const int32_t* tab_host, long long tab_len, const float* norm, int B, int F,
                        int oh, int ow, float* out, omt_stream_t stream);
 
+/* The FVD metric's preprocess (OmniTokenizer/fvd/fvd.py:18-29) of B clips of F frames: the same tables, descriptors and
+ * checks as omt_resample_clips (form 0 for the multi-threaded F.interpolate, no flip, no window, no crop), but
+ *   v = lut[byte]  (lut: fp32 [256], float(byte) or the value a byte map sends the byte to; with sel != NULL, lut is
+ *                   fp32 [2][256] and clip b reads table sel[b], 0 or 1 -- omt_u8_norm_select writes it on the device)
+ *   out = 2 * y / 255 - 1 in that order, true division,
+ * written channels-last: out (B, F, oh, ow, 4) fp32, 16-byte aligned, channel 3 zero (the I3D input of omt_conv3d). */
+int omt_fvd_preprocess(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc, const omt_clip_desc* desc_host,
+                       const int32_t* tab, const int32_t* tab_host, long long tab_len, const float* lut,
+                       const int32_t* sel, int B, int F, int oh, int ow, float* out, omt_stream_t stream);
+
+/* Unit3D of the FVD I3D (fvd/pytorch_i3d.py:59-131) as an implicit GEMM in 3xTF32 on sm_90a wgmma:
+ *   y[m, n] = act(sum_k A[m, k] W[n, k] + bias[n]),  m = ((b To + to) Ho + ho) Wo + wo,  n < N,  act = ReLU if relu
+ *   A[m, (dt, dh, dw, c)] = x[b][to st - pt + dt][ho sh - ph + dh][wo sw - pw + dw][c], zero outside the volume
+ * x: fp32 channels-last [B][T][H][W][Cs], 16-byte aligned; Cs a multiple of 32, or 4 (the network input: a k-block of
+ * 32 values then holds 8 taps).  K = kt kh kw Cs, rounded up to a multiple of 32 when Cs == 4.
+ * w_hi / w_lo: fp32 [round_up(N, 128)][K] (hi = tf32(W), lo = W - hi, BatchNorm folded in, rows >= N zero), 16-byte
+ * aligned; bias: fp32 [N].  (pt, ph, pw): the front padding (SAME: pad // 2); the back padding is implied by To, Ho, Wo.
+ * y: row m at y + m * ldy, N columns written and no others (N even, ldy >= N even, 8-byte aligned), so a branch of an
+ * Inception block writes its slice of the block's concat buffer in place.  The wgmma accumulator is added into an fp32
+ * sum on the CUDA cores every 64 values of K, so the tensor core's accumulation error does not grow with K. */
+int omt_conv3d(const float* x, int Cs, int B, int T, int H, int W, const float* w_hi, const float* w_lo, int K,
+               const float* bias, int N, int kt, int kh, int kw, int st, int sh, int sw, int pt, int ph, int pw,
+               int To, int Ho, int Wo, float* y, int ldy, int relu, omt_stream_t stream);
+
+/* MaxPool3dSamePadding (fvd/pytorch_i3d.py:24-56) on channels-last fp32 [B][T][H][W][Cs] -> [B][To][Ho][Wo][Cs] (Cs a
+ * multiple of 4, both 16-byte aligned): taps outside the volume are F.pad's zeros; max_pool3d's CPU rule, exact. */
+int omt_maxpool3d(const float* x, int Cs, int B, int T, int H, int W, int kt, int kh, int kw, int st, int sh, int sw,
+                  int pt, int ph, int pw, int To, int Ho, int Wo, float* y, omt_stream_t stream);
+
+/* The I3D head (fvd/pytorch_i3d.py:319-365): x [B][T][7][7][Cs] fp32 -> AvgPool3d([2, 7, 7], stride 1) over the first C
+ * channels -> logits[t] = W[N][C] . p[t] + bias -> out [B][N] = the mean over the T - 1 steps.  T >= 2. */
+int omt_i3d_head(const float* x, int Cs, int C, int B, int T, const float* w, const float* bias, int N, float* out,
+                 omt_stream_t stream);
+
 /* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W). */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,
                    int first, omt_stream_t stream);

@@ -174,6 +174,24 @@ def eval_step_u8(vqgan, frames: torch.Tensor, total_usage: Optional[torch.Tensor
 
 
 @torch.no_grad()
+def eval_step_fvd(vqgan, frames: torch.Tensor, i3d, total_usage: Optional[torch.Tensor] = None,
+                  norm: U8Norm = VIDEO_NORM):
+    """The body of vqgan_eval.py's video loop (:114-152) from the loader's uint8 clips (B, T, H, W, 3) on the device:
+    forward_u8 (eval_step_u8) for the reconstruction's bytes, and the FVD logits of both sides on the device
+    (fvd.I3D).  The real side sees the bytes the script makes of the normalised clip, shift_dim((video + 0.5) * 255,
+    1, -1).byte(), as a per-byte map with norm's branch picked per clip.  Returns (real_logits, fake_logits,
+    vq_output); no frame crosses to the host."""
+    from .fvd import real_byte_table
+    _check_u8(frames, (5,), "eval_step_fvd")
+    i3d.check_frames(frames)                 # every refusal before the first launch
+    real_byte_table(norm)
+    fake, vq_output = eval_step_u8(vqgan, frames, total_usage, norm)
+    real_logits = i3d.logits(frames, real_norm=norm).clone()
+    fake_logits = i3d.logits(fake).clone()
+    return real_logits, fake_logits, vq_output
+
+
+@torch.no_grad()
 def encode_to_z_u8(vqgan, frames: torch.Tensor, is_image: bool, sample_every_n_latent_frames: int = 0,
                    norm: U8Norm = VIDEO_NORM) -> Tuple[torch.Tensor, torch.Tensor]:
     """encode_to_z (lm_transformer.py:258-268) from the uint8 frames of the LM's VideoNorm data loader."""

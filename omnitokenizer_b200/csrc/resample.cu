@@ -164,26 +164,35 @@ resample_u8_kernel(const uint8_t* __restrict__ src, const omt_resample_desc* __r
 // nothing here is shared with Pillow's integer resize.
 // Each CTA owns RC_TW output columns (one per thread) x RC_TH rows of one frame of one clip; a thread's horizontal table
 // entry is loaded once, and each output row reads exactly two source rows.  Stores run along w within a channel plane.
+// FVD = true (omt_fvd_preprocess): fvd.py's preprocess instead of the loaders' Normalize.  The byte table holds the
+// value each byte stands for (table sel[b] of two when sel is given), the result is 2 y / 255 - 1 in that order, and a
+// frame leaves channels-last as [oh][ow][4] with channel 3 zero (the I3D input layout).
 constexpr int RC_TW = 128;
 constexpr int RC_TH = 8;
 
-__global__ void __launch_bounds__(RC_TW)
-resample_clips_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
-                      const int4* __restrict__ tab, const float* __restrict__ norm, float* __restrict__ out, int F,
-                      int oh, int ow) {
+template <bool FVD>
+__device__ __forceinline__ void resample_clips_body(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
+                                                    const int4* __restrict__ tab, const float* __restrict__ norm,
+                                                    float* __restrict__ out, int F, int oh, int ow,
+                                                    const int32_t* __restrict__ sel) {
   __shared__ float lut[256];
   pdl_sync();
   const int b = blockIdx.z / F, f = blockIdx.z % F;
   const omt_clip_desc d = desc[b];
+  if constexpr (FVD) {
+    if (sel != nullptr) norm += 256 * __ldg(sel + b);
+  }
   for (int i = threadIdx.x; i < 256; i += RC_TW) lut[i] = __ldg(norm + i);
   __syncthreads();
   const int ox = blockIdx.x * RC_TW + threadIdx.x;
   if (ox >= ow) return;
   float mean[3], stdv[3];
+  if constexpr (!FVD) {
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    mean[c] = __ldg(norm + 256 + c);
-    stdv[c] = __ldg(norm + 259 + c);
+    for (int c = 0; c < 3; ++c) {
+      mean[c] = __ldg(norm + 256 + c);
+      stdv[c] = __ldg(norm + 259 + c);
+    }
   }
   const int4 ew = __ldg(tab + d.th / 4 + d.cx + ox);
   const int x0 = d.flip ? d.W - 1 - (d.x0 + ew.x) : d.x0 + ew.x;   // the flip comes before the resize: mirror the source
@@ -200,6 +209,7 @@ resample_clips_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __re
     const uint8_t* r1 = frame + (long long)(d.y0 + eh.y) * d.W * 3;
     // torch's CPU kernels: each fma rounds once; the products and the division are never contracted or reassociated
     const float w00 = __fmul_rn(l0h, l0w), w01 = __fmul_rn(l0h, l1w), w10 = __fmul_rn(l1h, l0w), w11 = __fmul_rn(l1h, l1w);
+    float y[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const float x00 = lut[__ldg(r0 + x0 * 3 + c)], x01 = lut[__ldg(r0 + x1 * 3 + c)];
@@ -212,9 +222,26 @@ resample_clips_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __re
         const float t1 = __fmaf_rn(x10, l0w, __fmul_rn(x11, l1w));
         v = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
       }
-      o[c * F * plane + (long long)oy * ow] = __fdiv_rn(__fsub_rn(v, mean[c]), stdv[c]);
+      if constexpr (FVD) y[c] = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, v), 255.f), 1.f);
+      else o[c * F * plane + (long long)oy * ow] = __fdiv_rn(__fsub_rn(v, mean[c]), stdv[c]);
     }
+    if constexpr (FVD)
+      reinterpret_cast<float4*>(out)[((long long)blockIdx.z * oh + oy) * ow + ox] = make_float4(y[0], y[1], y[2], 0.f);
   }
+}
+
+__global__ void __launch_bounds__(RC_TW)
+resample_clips_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
+                      const int4* __restrict__ tab, const float* __restrict__ norm, float* __restrict__ out, int F,
+                      int oh, int ow) {
+  resample_clips_body<false>(src, desc, tab, norm, out, F, oh, ow, nullptr);
+}
+
+__global__ void __launch_bounds__(RC_TW)
+fvd_preprocess_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
+                      const int4* __restrict__ tab, const float* __restrict__ lut, const int32_t* __restrict__ sel,
+                      float* __restrict__ out, int F, int oh, int ow) {
+  resample_clips_body<true>(src, desc, tab, lut, out, F, oh, ow, sel);
 }
 
 // One axis table of a clip: [n_out][4] entries at word `off` inside the table, every (i0, i1) inside an axis of n_in.
@@ -275,40 +302,63 @@ extern "C" int omt_resample_u8(const uint8_t* src, long long src_bytes, const om
   return OMT_OK;
 }
 
+// The checks both clip entry points make before their launch (`who` names the entry point in the message).
+static int check_clips(const char* who, const uint8_t* src, long long src_bytes, const omt_clip_desc* desc,
+                       const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host, long long tab_len,
+                       const float* norm, int B, int F, int oh, int ow, float* out) {
+  OMT_REQUIRE(src && desc && desc_host && tab && tab_host && norm && out, "%s: null pointer", who);
+  OMT_REQUIRE(B >= 1 && F >= 1 && (long long)B * F <= 65535 && oh >= 1 && ow >= 1 && src_bytes >= 0 && tab_len >= 0,
+              "%s: B=%d, F=%d, output %dx%d, src_bytes=%lld, tab_len=%lld", who, B, F, oh, ow, src_bytes, tab_len);
+  for (int b = 0; b < B; ++b) {
+    const omt_clip_desc& d = desc_host[b];
+    OMT_REQUIRE(d.H >= 1 && d.W >= 1 && d.wh >= 1 && d.ww >= 1 && d.rh >= 1 && d.rw >= 1,
+                "%s: clip %d: source %dx%d, window %dx%d, resized %dx%d", who, b, d.H, d.W, d.wh, d.ww, d.rh, d.rw);
+    OMT_REQUIRE(d.src >= 0 && d.src + (long long)F * d.H * d.W * 3 <= src_bytes,
+                "%s: clip %d: bytes [%lld, +%lld) outside the %lld source bytes", who, b, d.src,
+                (long long)F * d.H * d.W * 3, src_bytes);
+    OMT_REQUIRE(d.y0 >= 0 && d.x0 >= 0 && (long long)d.y0 + d.wh <= d.H && (long long)d.x0 + d.ww <= d.W,
+                "%s: clip %d: window %dx%d at (%d, %d) outside the %dx%d frame", who, b, d.wh, d.ww, d.y0, d.x0, d.H, d.W);
+    OMT_REQUIRE(d.cy >= 0 && d.cx >= 0 && (long long)d.cy + oh <= d.rh && (long long)d.cx + ow <= d.rw,
+                "%s: clip %d: crop %dx%d at (%d, %d) outside the resized %dx%d frame", who, b, oh, ow, d.cy, d.cx, d.rh,
+                d.rw);
+    OMT_REQUIRE((d.flip | d.form) >= 0 && (d.flip | d.form) <= 1, "%s: clip %d: flip / form must be 0 or 1", who, b);
+    OMT_REQUIRE(clip_axis_ok(tab_host, tab_len, d.tv, d.rh, d.wh),
+                "%s: clip %d: vertical table outside the table or indices outside the window", who, b);
+    OMT_REQUIRE(clip_axis_ok(tab_host, tab_len, d.th, d.rw, d.ww),
+                "%s: clip %d: horizontal table outside the table or indices outside the window", who, b);
+  }
+  return OMT_OK;
+}
+
 extern "C" int omt_resample_clips(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc,
                                   const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
                                   long long tab_len, const float* norm, int B, int F, int oh, int ow, float* out,
                                   omt_stream_t stream) {
   OMT_ENTER();
-  OMT_REQUIRE(src && desc && desc_host && tab && tab_host && norm && out, "omt_resample_clips: null pointer");
-  OMT_REQUIRE(B >= 1 && F >= 1 && (long long)B * F <= 65535 && oh >= 1 && ow >= 1 && src_bytes >= 0 && tab_len >= 0,
-              "omt_resample_clips: B=%d, F=%d, output %dx%d, src_bytes=%lld, tab_len=%lld", B, F, oh, ow, src_bytes,
-              tab_len);
   OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab}) && aligned_to(4, {norm, out}),
               "omt_resample_clips: desc must be 8-byte, tab 16-byte and norm / out 4-byte aligned");
-  for (int b = 0; b < B; ++b) {
-    const omt_clip_desc& d = desc_host[b];
-    OMT_REQUIRE(d.H >= 1 && d.W >= 1 && d.wh >= 1 && d.ww >= 1 && d.rh >= 1 && d.rw >= 1,
-                "omt_resample_clips: clip %d: source %dx%d, window %dx%d, resized %dx%d", b, d.H, d.W, d.wh, d.ww, d.rh,
-                d.rw);
-    OMT_REQUIRE(d.src >= 0 && d.src + (long long)F * d.H * d.W * 3 <= src_bytes,
-                "omt_resample_clips: clip %d: bytes [%lld, +%lld) outside the %lld source bytes", b, d.src,
-                (long long)F * d.H * d.W * 3, src_bytes);
-    OMT_REQUIRE(d.y0 >= 0 && d.x0 >= 0 && (long long)d.y0 + d.wh <= d.H && (long long)d.x0 + d.ww <= d.W,
-                "omt_resample_clips: clip %d: window %dx%d at (%d, %d) outside the %dx%d frame", b, d.wh, d.ww, d.y0,
-                d.x0, d.H, d.W);
-    OMT_REQUIRE(d.cy >= 0 && d.cx >= 0 && (long long)d.cy + oh <= d.rh && (long long)d.cx + ow <= d.rw,
-                "omt_resample_clips: clip %d: crop %dx%d at (%d, %d) outside the resized %dx%d frame", b, oh, ow, d.cy,
-                d.cx, d.rh, d.rw);
-    OMT_REQUIRE((d.flip | d.form) >= 0 && (d.flip | d.form) <= 1, "omt_resample_clips: clip %d: flip / form must be 0 or 1", b);
-    OMT_REQUIRE(clip_axis_ok(tab_host, tab_len, d.tv, d.rh, d.wh),
-                "omt_resample_clips: clip %d: vertical table outside the table or indices outside the window", b);
-    OMT_REQUIRE(clip_axis_ok(tab_host, tab_len, d.th, d.rw, d.ww),
-                "omt_resample_clips: clip %d: horizontal table outside the table or indices outside the window", b);
-  }
+  int rc = check_clips("omt_resample_clips", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, norm, B, F, oh, ow, out);
+  if (rc != OMT_OK) return rc;
   dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
   OMT_CUDA(launch_k(resample_clips_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
                     reinterpret_cast<const int4*>(tab), norm, out, F, oh, ow));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_fvd_preprocess(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc,
+                                  const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
+                                  long long tab_len, const float* lut, const int32_t* sel, int B, int F, int oh,
+                                  int ow, float* out, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(aligned_to(4, {sel}), "omt_fvd_preprocess: sel must be 4-byte aligned");
+  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && aligned_to(4, {lut}),
+              "omt_fvd_preprocess: desc must be 8-byte, tab / out 16-byte and lut 4-byte aligned");
+  int rc = check_clips("omt_fvd_preprocess", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, lut, B, F, oh, ow, out);
+  if (rc != OMT_OK) return rc;
+  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
+  OMT_CUDA(launch_k(fvd_preprocess_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
+                    reinterpret_cast<const int4*>(tab), lut, sel, out, F, oh, ow));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

@@ -98,6 +98,29 @@ class PackedLinear:
         self.row_scaled = row_scaled and math in PLANE_MATHS
 
 
+def run_graphed(graphs: dict, device, key, body):
+    """Run ``body`` (a fixed launch sequence over static buffers): the first call of a shape runs eagerly
+    (sets function attributes, builds tables), the second captures a CUDA graph, later calls replay it --
+    ~170 launches per encode+decode collapse into one submission.  ``graphs``: the workspace's key -> graph state."""
+    if not Engine.graphs_enabled():
+        return body()
+    g = graphs.get(key)
+    if g is None:
+        body()
+        graphs[key] = "warm"
+    elif g == "warm":
+        graph = torch.cuda.CUDAGraph()
+        torch.cuda.synchronize(device)
+        n0 = _cabi.launch_count
+        with torch.cuda.graph(graph):
+            body()
+        graphs[key] = (graph, _cabi.launch_count - n0)
+        graph.replay()
+    else:
+        g[0].replay()
+        _cabi.launch_count += g[1]        # kernels inside the replayed graph (bench.py accounting)
+
+
 class Workspace:
     """Per-shape buffers.  C: model width; A: attention width (q | k | v and the attention output; a window layer, whose
     width is C, runs only in models with C == A)."""
@@ -610,26 +633,7 @@ class Engine:
         return os.environ.get("OMT_CUDA_GRAPH", "1") != "0"
 
     def _run(self, ws: Workspace, key, body):
-        """Run ``body`` (a fixed launch sequence over static buffers): the first call of a shape runs eagerly
-        (sets function attributes, builds tables), the second captures a CUDA graph, later calls replay it --
-        ~170 launches per encode+decode collapse into one submission."""
-        if not self.graphs_enabled():
-            return body()
-        g = ws.graphs.get(key)
-        if g is None:
-            body()
-            ws.graphs[key] = "warm"
-        elif g == "warm":
-            graph = torch.cuda.CUDAGraph()
-            torch.cuda.synchronize(self.device)
-            n0 = _cabi.launch_count
-            with torch.cuda.graph(graph):
-                body()
-            ws.graphs[key] = (graph, _cabi.launch_count - n0)
-            graph.replay()
-        else:
-            g[0].replay()
-            _cabi.launch_count += g[1]        # kernels inside the replayed graph (bench.py accounting)
+        run_graphed(ws.graphs, self.device, key, body)
 
     # ------------------------------------------------------------------ encoder side
     def _encode_body(self, ws: Workspace, gather, lay: BatchLayout, mode: str):

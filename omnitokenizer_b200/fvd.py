@@ -1,0 +1,312 @@
+"""The FVD metric's feature network on the device: OmniTokenizer/fvd/fvd.py's preprocess and InceptionI3d
+(fvd/pytorch_i3d.py) from device uint8 clips, on the sm_90a kernels of csrc/i3d.cu and csrc/resample.cu.
+
+Drop-in names for vqgan_eval.py:18 (`from OmniTokenizer.fvd.fvd import load_fvd_model, frechet_distance,
+get_fvd_logits`): load_fvd_model(device, path), get_fvd_logits(videos, i3d, device), frechet_distance(x1, x2).
+
+Activations are channels-last fp32 [B][T][H][W][Cs], Cs the channel count rounded up to a multiple of 32 (4 for the
+network input); the pad columns are zero.  Every Unit3D is one omt_conv3d launch (3xTF32, BatchNorm folded into the
+weights at pack time), and each Inception branch writes its slice of the block's concat buffer in place.
+"""
+from __future__ import annotations
+
+from typing import Dict, List, Optional, Tuple
+
+import numpy as np
+import torch
+
+from . import _cabi
+from . import layout as L
+from .engine import CLIP_DESC_WORDS, run_graphed
+
+TARGET_RESOLUTION = (224, 224)
+BN_EPS = 1e-5            # pytorch_i3d.py:91
+
+# pytorch_i3d.py:247-328: (endpoint, kind, spec); unit: (cin, cout, kernel, stride); pool: (kernel, stride);
+# mixed: (cin, branch widths b0, b1a, b1b, b2a, b2b, b3b)
+ARCH = [
+    ("Conv3d_1a_7x7", "unit", (3, 64, 7, 2)),
+    ("MaxPool3d_2a_3x3", "pool", ((1, 3, 3), (1, 2, 2))),
+    ("Conv3d_2b_1x1", "unit", (64, 64, 1, 1)),
+    ("Conv3d_2c_3x3", "unit", (64, 192, 3, 1)),
+    ("MaxPool3d_3a_3x3", "pool", ((1, 3, 3), (1, 2, 2))),
+    ("Mixed_3b", "mixed", (192, (64, 96, 128, 16, 32, 32))),
+    ("Mixed_3c", "mixed", (256, (128, 128, 192, 32, 96, 64))),
+    ("MaxPool3d_4a_3x3", "pool", ((3, 3, 3), (2, 2, 2))),
+    ("Mixed_4b", "mixed", (480, (192, 96, 208, 16, 48, 64))),
+    ("Mixed_4c", "mixed", (512, (160, 112, 224, 24, 64, 64))),
+    ("Mixed_4d", "mixed", (512, (128, 128, 256, 24, 64, 64))),
+    ("Mixed_4e", "mixed", (512, (112, 144, 288, 32, 64, 64))),
+    ("Mixed_4f", "mixed", (528, (256, 160, 320, 32, 128, 128))),
+    ("MaxPool3d_5a_2x2", "pool", ((2, 2, 2), (2, 2, 2))),
+    ("Mixed_5b", "mixed", (832, (256, 160, 320, 32, 128, 128))),
+    ("Mixed_5c", "mixed", (832, (384, 192, 384, 48, 128, 128))),
+]
+# branch unit -> (width index, kernel, input: the block input "x", the pooled input "p" or another branch unit)
+BRANCHES = {"b0": (0, 1, "x"), "b1a": (1, 1, "x"), "b1b": (2, 3, "b1a"), "b2a": (3, 1, "x"), "b2b": (4, 3, "b2a"),
+            "b3b": (5, 1, "p")}
+
+
+def cpad(c: int) -> int:
+    """Channel stride of an activation with c channels: 4 for the RGB input, else a multiple of 32."""
+    return 4 if c <= 4 else L.round_up(c, 32)
+
+
+def compute_pad(k: int, s: int, n: int) -> int:
+    """pytorch_i3d.py:26-30 / 93-97: the total SAME padding of one axis (pad // 2 goes in front)."""
+    return max(k - s, 0) if n % s == 0 else max(k - n % s, 0)
+
+
+def same_geometry(kernel, stride, dims) -> Tuple[Tuple[int, ...], Tuple[int, ...]]:
+    """(front padding, output size) per axis of a SAME-padded conv / pool over dims."""
+    front, out = [], []
+    for k, s, n in zip(kernel, stride, dims):
+        p = compute_pad(k, s, n)
+        front.append(p // 2)
+        out.append((n + p - k) // s + 1)
+    return tuple(front), tuple(out)
+
+
+def unit_names() -> List[Tuple[str, int, int, int, int]]:
+    """Every Unit3D with BatchNorm: (prefix, cin, cout, kernel, stride), in the reference's order."""
+    out = []
+    for name, kind, spec in ARCH:
+        if kind == "unit":
+            out.append((name,) + spec)
+        elif kind == "mixed":
+            cin, w = spec
+            for b, (wi, k, src) in BRANCHES.items():
+                out.append((f"{name}.{b}", cin if src in ("x", "p") else w[BRANCHES[src][0]], w[wi], k, 1))
+    return out
+
+
+def expected_keys(num_classes: int = 400) -> Dict[str, tuple]:
+    keys = {}
+    for prefix, cin, cout, k, _ in unit_names():
+        keys[prefix + ".conv3d.weight"] = (cout, cin, k, k, k)
+        for f in ("weight", "bias", "running_mean", "running_var"):
+            keys[f"{prefix}.bn.{f}"] = (cout,)
+    keys["logits.conv3d.weight"] = (num_classes, 1024, 1, 1, 1)
+    keys["logits.conv3d.bias"] = (num_classes,)
+    return keys
+
+
+def fold_bn(w: torch.Tensor, gamma, beta, mean, var) -> Tuple[torch.Tensor, torch.Tensor]:
+    """BatchNorm (running statistics, eps 1e-5) folded into a conv weight (cout, cin, k, k, k), in float64:
+    (W s, beta - mean s) with s = gamma / sqrt(var + eps), rounded to fp32."""
+    s = gamma.double() / torch.sqrt(var.double() + BN_EPS)
+    return (w.double() * s.view(-1, 1, 1, 1, 1)).float(), (beta.double() - mean.double() * s).float()
+
+
+def pack_weight(w: torch.Tensor) -> Tuple[torch.Tensor, int]:
+    """A conv weight (cout, cin, kt, kh, kw) as omt_conv3d's W: rows of K = (dt, dh, dw, c) with c padded to cpad(cin)
+    (K rounded up to 32 for the RGB input), cout padded to a multiple of 128.  Returns (W [n_pad, K] fp32, K)."""
+    cout, cin = int(w.shape[0]), int(w.shape[1])
+    wk = torch.zeros(cout, *w.shape[2:], cpad(cin))
+    wk[..., :cin] = w.float().permute(0, 2, 3, 4, 1)
+    wk = wk.reshape(cout, -1)
+    K = L.round_up(wk.shape[1], 32)
+    packed = torch.zeros(L.round_up(cout, 128), K)
+    packed[:cout, :wk.shape[1]] = wk
+    return packed, K
+
+
+class _Unit:
+    """One Unit3D packed for omt_conv3d: tf32 hi / lo planes of W, the folded bias, its geometry."""
+
+    def __init__(self, w, K, bias, cout, k, s, device):
+        hi = L.tf32_round(w)
+        self.w_hi, self.w_lo = hi.to(device), (w - hi).to(device)
+        self.bias, self.K, self.cout, self.k, self.s = bias.to(device), K, cout, k, s
+
+
+class _Workspace:
+    """Buffers, launch list and CUDA graph state of one (B, T, H, W)."""
+
+    def __init__(self, net: "I3D", B: int, T: int, H: int, W: int, real_norm: Optional[L.U8Norm] = None):
+        dev = net.device
+        self.graphs = {}
+        self.u8 = torch.empty(B, T, H, W, 3, dtype=torch.uint8, device=dev)
+        # byte -> value table: float(byte), or the real-byte map of real_norm, picked per clip with VideoNorm's test
+        self.lut = net.byte_lut if real_norm is None else real_byte_table(real_norm).float().to(dev)
+        self.sel = torch.empty(B, dtype=torch.int32, device=dev) if real_norm is not None and real_norm.max_test else None
+        self.out = torch.empty(B, net.num_classes, device=dev)
+        # preprocess tables (fvd.py:24: F.interpolate to 224 x 224 from the multi-threaded script: the separable kernel)
+        oh, ow = TARGET_RESOLUTION
+        tv = L.clip_axis_table(H, oh, float(np.float32(H) / np.float32(oh))).reshape(-1)
+        th = L.clip_axis_table(W, ow, float(np.float32(W) / np.float32(ow))).reshape(-1)
+        self.tab_host = torch.from_numpy(np.concatenate([tv, th]).astype(np.int32))
+        desc = torch.zeros(B, CLIP_DESC_WORDS, dtype=torch.int32)
+        desc[:, :2] = (torch.arange(B, dtype=torch.int64) * (T * H * W * 3)).view(torch.int32).view(B, 2)
+        desc[:, 2:] = torch.tensor([H, W, 0, 0, H, W, oh, ow, 0, 0, 0, 0, tv.size, L.INTERP_SEPARABLE], dtype=torch.int32)
+        self.desc_host = desc
+        self.desc, self.tab = desc.to(dev), self.tab_host.to(dev)
+        self.ops = []
+        f = dict(device=dev, dtype=torch.float32)
+
+        def act(T_, H_, W_, c):
+            return torch.zeros(B, T_, H_, W_, cpad(c), **f)       # pad columns stay zero: no kernel writes them
+
+        x = act(T, oh, ow, 3)
+        shape = (T, oh, ow)
+        if self.sel is not None:
+            self.ops.append(lambda: _cabi.call("omt_u8_norm_select", self.u8, B, T * H * W * 3, self.sel))
+        self.ops.append(lambda x=x: _cabi.call(
+            "omt_fvd_preprocess", self.u8, self.u8.numel(), self.desc, self.desc_host, self.tab, self.tab_host,
+            self.tab_host.numel(), self.lut, self.sel, B, T, oh, ow, x))
+        cur, c_cur = x, 3
+        for name, kind, spec in ARCH:
+            if kind == "unit":
+                y, yshape = self._conv(net.units[name], cur, shape, act)
+                cur, c_cur, shape = y, spec[1], yshape
+            elif kind == "pool":
+                cur, shape = self._pool(cur, shape, spec[0], spec[1], act, c_cur)
+            else:
+                cin, w = spec
+                cout = w[0] + w[2] + w[4] + w[5]
+                y = act(*shape, cout)
+                offs = {"b0": 0, "b1b": w[0], "b2b": w[0] + w[2], "b3b": w[0] + w[2] + w[4]}
+                pooled, _ = self._pool(cur, shape, (3, 3, 3), (1, 1, 1), act, cin)
+                mids = {}
+                for b in ("b0", "b1a", "b1b", "b2a", "b2b", "b3b"):
+                    wi, k, src = BRANCHES[b]
+                    inp = {"x": cur, "p": pooled}.get(src, mids.get(src))
+                    if b in offs:
+                        self._conv(net.units[f"{name}.{b}"], inp, shape, act, out=(y, offs[b]))
+                    else:
+                        mids[b], _ = self._conv(net.units[f"{name}.{b}"], inp, shape, act)
+                cur, c_cur = y, cout
+        T5 = shape[0]
+        if shape[1:] != (7, 7) or T5 < 2:
+            raise ValueError(f"the I3D head needs [>= 2, 7, 7] features, got {shape}")
+        self.ops.append(lambda cur=cur, T5=T5: _cabi.call(
+            "omt_i3d_head", cur, cur.shape[-1], 1024, B, T5, net.head_w, net.head_b, net.num_classes, self.out))
+
+    def _conv(self, u: _Unit, x, shape, act, out=None):
+        k, s = (u.k,) * 3, (u.s,) * 3
+        front, o = same_geometry(k, s, shape)
+        if out is None:
+            y, col = act(*o, u.cout), 0
+        else:
+            y, col = out
+        B = x.shape[0]
+        ypt = y.data_ptr() + 4 * col
+        self.ops.append(lambda: _cabi.call(
+            "omt_conv3d", x, x.shape[-1], B, shape[0], shape[1], shape[2], u.w_hi, u.w_lo, u.K, u.bias, u.cout,
+            *k, *s, *front, *o, ypt, y.shape[-1], 1))
+        return y, o
+
+    def _pool(self, x, shape, k, s, act, c):
+        front, o = same_geometry(k, s, shape)
+        y = act(*o, c)
+        B = x.shape[0]
+        self.ops.append(lambda: _cabi.call("omt_maxpool3d", x, x.shape[-1], B, *shape, *k, *s, *front, *o, y))
+        return y, o
+
+    def run(self):
+        for op in self.ops:
+            op()
+
+
+class I3D:
+    """InceptionI3d (pytorch_i3d.py:163-365) in eval mode from a state_dict in the reference's layout
+    (`Conv3d_1a_7x7.conv3d.weight`, `Mixed_4e.b1b.bn.running_var`, ..., `logits.conv3d.{weight,bias}`).  BatchNorm is
+    folded and the weights packed once, on `device`; every (B, T, H, W) gets its own buffers and CUDA graph."""
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda"):
+        sd = {k: v for k, v in state_dict.items() if not k.endswith(".num_batches_tracked")}
+        lw = sd.get("logits.conv3d.weight")
+        self.num_classes = int(lw.shape[0]) if lw is not None and lw.dim() == 5 else 400
+        want = expected_keys(self.num_classes)
+        missing, unexpected = sorted(set(want) - set(sd)), sorted(set(sd) - set(want))
+        if missing or unexpected:
+            raise KeyError(f"I3D state_dict: missing keys {missing}, unexpected keys {unexpected}")
+        for k, shape in want.items():
+            if tuple(sd[k].shape) != shape:
+                raise ValueError(f"I3D state_dict: {k} has shape {tuple(sd[k].shape)}, expected {shape}")
+        self.device = torch.device(device)
+        if self.device.type == "cuda" and self.device.index is None:      # vqgan_eval.py:59 passes torch.device('cuda')
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        sd = {k: v.detach().float().cpu() for k, v in sd.items()}
+        self.units = {}
+        for prefix, cin, cout, k, s in unit_names():
+            w, b = fold_bn(sd[prefix + ".conv3d.weight"],
+                           *(sd[f"{prefix}.bn.{f}"] for f in ("weight", "bias", "running_mean", "running_var")))
+            self.units[prefix] = _Unit(*pack_weight(w), b, cout, k, s, self.device)
+        self.head_w = sd["logits.conv3d.weight"].reshape(self.num_classes, 1024).contiguous().to(self.device)
+        self.head_b = sd["logits.conv3d.bias"].contiguous().to(self.device)
+        self.byte_lut = torch.arange(256, dtype=torch.float32).to(self.device)     # torch.FloatTensor(videos)
+        self._ws = {}
+
+    @staticmethod
+    def check_frames(frames: torch.Tensor):
+        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+            raise TypeError(f"I3D.logits takes a uint8 tensor, got {getattr(frames, 'dtype', type(frames))}")
+        if frames.dim() != 5 or frames.shape[-1] != 3:
+            raise ValueError(f"I3D.logits takes (B, T, H, W, 3) frames, got {tuple(frames.shape)}")
+        if frames.shape[1] < 9:
+            raise ValueError(f"I3D needs T >= 9 frames (its AvgPool3d spans 2 time steps after 8x temporal "
+                             f"downsampling), got T={frames.shape[1]}")
+        if min(frames.shape[:4]) < 1:
+            raise ValueError(f"empty clip batch {tuple(frames.shape)}")
+
+    def logits(self, frames_u8: torch.Tensor, real_norm: Optional[L.U8Norm] = None) -> torch.Tensor:
+        """(B, T, H, W, 3) uint8 on this I3D's device -> logits (B, num_classes) fp32: get_fvd_logits of the reference.
+        real_norm: the frames are the loader's bytes, and the network sees the bytes vqgan_eval.py makes of the
+        normalised clip, shift_dim((video + 0.5) * 255, 1, -1).byte() (real_byte_table, its branch picked per clip).
+        The returned tensor is the workspace's static output: clone it before the next call of the same shape."""
+        self.check_frames(frames_u8)
+        if frames_u8.device != self.device:
+            raise ValueError(f"I3D.logits: frames on {frames_u8.device}, the network is on {self.device}")
+        if real_norm is not None:
+            real_byte_table(real_norm)                      # refuses a per-channel normalisation before any launch
+        key = tuple(int(v) for v in frames_u8.shape[:4]) + (real_norm,)
+        ws = self._ws.get(key)
+        if ws is None:
+            ws = self._ws[key] = _Workspace(self, *key)
+        ws.u8.copy_(frames_u8)
+        run_graphed(ws.graphs, self.device, "i3d", ws.run)
+        return ws.out
+
+
+def real_byte_table(norm: L.U8Norm) -> torch.Tensor:
+    """uint8 [n_tab, 256]: the byte vqgan_eval.py feeds I3D for each loader byte u of a real clip,
+    ((v + 0.5) * 255).byte() (:144, :156) of the normalised value v (layout.u8_norm_table, fp32, its own op order).
+    Table 1 (VideoNorm's max <= 1 branch) is only used for clips whose bytes are all 0 or 1."""
+    tab = L.u8_norm_table(norm, 3)                          # [n_tab, 3, 256]
+    if not bool((tab == tab[:, :1]).all()):
+        raise ValueError(f"normalisation {norm.name!r} differs per channel; the FVD byte map is one table per branch")
+    return ((tab[:, 0] + 0.5) * 255).byte()
+
+
+def load_fvd_model(device, path: str) -> I3D:
+    """fvd.py:36-42 with the checkpoint path given (the weights are not shipped): i3d_pretrained_400.pt."""
+    return I3D(torch.load(path, map_location="cpu"), device)
+
+
+def get_fvd_logits(videos, i3d: I3D, device=None) -> torch.Tensor:
+    """fvd.py:31-34: numpy or torch uint8 (b, t, h, w, c) on the CPU or the device -> logits (b, num_classes) on the
+    device.  Host input is copied as uint8 (a quarter of the bytes of the reference's fp32 copy)."""
+    if isinstance(videos, np.ndarray):
+        videos = torch.from_numpy(np.ascontiguousarray(videos))
+    I3D.check_frames(videos)
+    return i3d.logits(videos.to(i3d.device, non_blocking=False)).clone()
+
+
+def frechet_distance(x1: torch.Tensor, x2: torch.Tensor) -> torch.Tensor:
+    """fvd.py:101-112 (with _symmetric_matrix_square_root, trace_sqrt_product and cov, :56-98): the Frechet distance
+    between two sets of embeddings.  Runs once per split in torch; it is not a kernel."""
+    def sqrtm(mat, eps=1e-10):
+        u, s, v = torch.svd(mat)
+        return u @ torch.diag(torch.where(s < eps, s, torch.sqrt(s))) @ v.t()
+
+    def cov(m):
+        m = m.t()
+        c = m - m.mean(dim=1, keepdim=True)
+        return (1.0 / (m.size(1) - 1)) * (c @ c.t()).squeeze()
+
+    x1, x2 = x1.flatten(start_dim=1), x2.flatten(start_dim=1)
+    sigma, sigma_w = cov(x1), cov(x2)
+    r = sqrtm(sigma)
+    trace = torch.trace(sigma + sigma_w) - 2.0 * torch.trace(sqrtm(r @ (sigma_w @ r)))
+    return trace + torch.sum((x1.mean(dim=0) - x2.mean(dim=0)) ** 2)
