@@ -41,8 +41,16 @@ static int launch_gemm_f16(const omt_linear_h_args& a, cudaStream_t st, const ch
   const int n_pad = (a.N + 255) / 256 * 256;
   const CUtensorMapDataType f16 = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const bool dual = a.a2_hi != nullptr;
-  CUtensorMap maps[6];
+  CUtensorMap maps[8];
   int rc;
+  if (a.epilogue == OMT_EPI_GEGLU || a.epilogue == OMT_EPI_QKV_PLANES) {   // output planes, written by TMA stores
+    const bool geglu = a.epilogue == OMT_EPI_GEGLU;
+    const int cols = geglu ? a.N / 2 : a.N;
+    const int seg = geglu ? a.c_seg : 0;
+    if ((rc = row_map(&maps[6], f16, 2, a.u_hi, a.ldu, a.M, cols, seg, a.c_seg_stride, a.c_seg_off, 32))) return rc;
+    if (h1) maps[7] = maps[6];
+    else if ((rc = row_map(&maps[7], f16, 2, a.u_lo, a.ldu, a.M, cols, seg, a.c_seg_stride, a.c_seg_off, 32))) return rc;
+  }
   if ((rc = row_map(&maps[0], f16, 2, a.a_hi, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off))) return rc;
   if ((rc = row_map(&maps[2], f16, 2, dual ? a.a2_hi : a.a_hi, a.lda, a.M, a.K, a.a_seg, a.a_seg_stride, a.a_seg_off))) return rc;
   if ((rc = w_map(&maps[4], f16, 2, a.w_hi, n_pad, a.K))) return rc;

@@ -30,8 +30,9 @@
 //     epilogue together.
 // Both issue the same products in the same k order for every output element, so they give the same bits.
 // The epilogue works on the accumulator fragments in place: a row's 64-column head is spread over the 4 lanes of a quad,
-// so the l2 norm and the v-plane maximum are two-step shuffles.  The f16 GEGLU epilogue, whose fragments hold only 8 bytes
-// of a U-plane row per quad, stages each 64-row half of its U planes in shared memory and stores whole 128-byte rows.
+// so the l2 norm and the v-plane maximum are two-step shuffles.  The f16 epilogues that write operand planes (GEGLU: a
+// quad holds only 8 bytes of a U-plane row; QKV planes: 16 bytes of a head's row) stage 64 rows x 64 columns of the hi /
+// lo planes at a time in shared memory, and one thread of the warpgroup writes them out by TMA stores.
 #pragma once
 #include "omt_common.cuh"
 #include "tc_ptx.cuh"
@@ -49,12 +50,18 @@ constexpr int STAGES = 3;
 // H1: a stage is A_hi | W_hi, half the bytes, so the ring holds twice as many 128-byte k-slabs in the same shared memory
 template <bool H1> __host__ __device__ constexpr int stage_bytes() { return H1 ? 2 * 16384 : STAGE_BYTES; }
 template <bool H1> __host__ __device__ constexpr int stages() { return H1 ? 2 * STAGES : STAGES; }
-// f16 GEGLU epilogue: per consumer warpgroup, the U planes of one 64-row half of a tile (64 rows x 64 columns x 2 planes)
-// staged in shared memory so that they leave as whole 128-byte rows.  Only those instantiations reserve it: the others
-// keep the larger L1 for their epilogue's loads.
+// f16 plane-writing epilogues (GEGLU, QKV planes): per consumer warpgroup, 64 rows x 64 columns of the hi and lo planes
+// (the U planes of one 64-row half, or one head of one) staged in shared memory in the SWIZZLE_128B layout of a TMA box,
+// so that they leave by TMA stores.  Only those instantiations reserve it: the others keep the larger L1.  The f16x1 QKV
+// planes epilogue stores its hi plane from the fragments: behind its single-product mainloop, the per-head hand-off of
+// the stage between the warpgroup and the TMA store measured slower than the per-thread stores.
 constexpr int EPI_STAGE_BYTES = 2 * 64 * 128;
+template <bool TF32, int EPI, bool H1>
+__host__ __device__ constexpr bool tma_planes() {
+  return !TF32 && (EPI == OMT_EPI_GEGLU || (EPI == OMT_EPI_QKV_PLANES && !H1));
+}
 template <bool TF32, int EPI, bool H1 = false>
-constexpr int smem_bytes() { return stages<H1>() * stage_bytes<H1>() + (!TF32 && EPI == OMT_EPI_GEGLU ? 2 * EPI_STAGE_BYTES : 0) + 1024; }
+constexpr int smem_bytes() { return stages<H1>() * stage_bytes<H1>() + (tma_planes<TF32, EPI, H1>() ? 2 * EPI_STAGE_BYTES : 0) + 1024; }
 // __launch_bounds__(384, 1) caps the kernel at 168 registers a thread: 40 * 128 + 232 * 256 == 168 * 384
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 
@@ -77,12 +84,31 @@ struct Args {
   float* vinv;                                // QKV_PLANES: [v heads][M] inverse per-(row, head) scale of the v planes
 };
 
+// One thread writes a warpgroup's staged planes (64 rows from `row`, 64 columns from `col`) by TMA, as two 32-row boxes
+// per plane: a C row-map segment is a multiple of 32 rows, so no box crosses one.  Rows at or past M fall outside the
+// map and are not written.
+template <bool H1>
+__device__ __forceinline__ void store_planes(const CUtensorMap* mh, const CUtensorMap* ml, const uint8_t* stage, int col,
+                                             int row, int seg) {
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int r = row + 32 * i;
+    const int c1 = seg > 0 ? r % seg : r, c2 = seg > 0 ? r / seg : 0;
+    tma_store_3d(mh, stage + i * 32 * 128, col, c1, c2);
+    if (!H1) tma_store_3d(ml, stage + 64 * 128 + i * 32 * 128, col, c1, c2);
+  }
+  bulk_commit();
+}
+
 // Epilogue of one 64-row half of a tile on a consumer warpgroup's fragments (rows [m0 + 64 half, +64), columns [n0, +128)).
-// `stage` is the warpgroup's EPI_STAGE_BYTES of shared memory, `bar` its named barrier.
+// `stage` is the warpgroup's EPI_STAGE_BYTES of shared memory, `bar` its named barrier; tmUh / tmUl map the output planes
+// of the plane-writing f16 epilogues.
 template <bool TF32, int NACC, int EPI, bool H1>
 __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 2], const float (&crs)[NACC == 2 ? BN / 2 : 1],
-                                         int m0, int n0, bool second, int half, int warp, int lane, uint8_t* stage, int bar) {
+                                         int m0, int n0, bool second, int half, int warp, int lane, uint8_t* stage, int bar,
+                                         const CUtensorMap* tmUh, const CUtensorMap* tmUl) {
   const int qd = lane & 3;                      // column pair 8 j + 2 qd inside every 8-column block
+  const bool elected = (warp & 3) == 0 && lane == 0;   // the warpgroup's TMA-store thread
   int mrow[2];
   mrow[0] = m0 + half * 64 + (warp & 3) * 16 + (lane >> 2);
   mrow[1] = mrow[0] + 8;
@@ -108,10 +134,15 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
   }
 
   if constexpr (EPI == OMT_EPI_QKV || EPI == OMT_EPI_QKV_PLANES) {
+    constexpr bool STAGED = tma_planes<TF32, EPI, H1>();
 #pragma unroll
     for (int hd = 0; hd < BN / 64; ++hd) {
       const int nh = n0 + hd * 64;              // first column of this head
-      if (nh >= g.N) break;                     // warp-uniform
+      if (nh >= g.N) break;                     // warpgroup-uniform
+      if constexpr (STAGED) {
+        if (elected) bulk_wait_read<0>();       // the previous TMA store has read the stage
+        wg_bar(bar);
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int m = mrow[h];
@@ -163,7 +194,19 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
             row_scale(mx, sc, inv);
             if (m < g.M && qd == 0) g.vinv[(size_t)((nh - g.qk_cols) >> 6) * g.M + m] = inv;
           }
-          if (m < g.M) {
+          if constexpr (STAGED) {
+            // the head's 64 columns of row r in the stage: 16-byte chunk j at chunk j ^ (r & 7) (the TMA box layout;
+            // the 8 rows of a warp's store land in 8 different bank groups)
+            const int r = (warp & 3) * 16 + (lane >> 2) + 8 * h;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              uint32_t hw, lw;
+              split2u(x[2 * j] * sc, x[2 * j + 1] * sc, hw, lw);
+              const int off = r * 128 + ((j ^ (r & 7)) << 4) + 4 * qd;
+              *reinterpret_cast<uint32_t*>(stage + off) = hw;
+              *reinterpret_cast<uint32_t*>(stage + 64 * 128 + off) = lw;
+            }
+          } else if (m < g.M) {
             const size_t off = (size_t)m * g.ldu + nh + 2 * qd;
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
@@ -175,53 +218,101 @@ __device__ __forceinline__ void epilogue(const Args& g, const float (&acc)[BN / 
           }
         }
       }
+      if constexpr (STAGED) {
+        fence_async_smem();                     // this thread's stage writes -> visible to the TMA store
+        wg_bar(bar);
+        if (elected) store_planes<false>(tmUh, tmUl, stage, nh, m0 + half * 64, 0);
+      }
     }
   } else if constexpr (EPI == OMT_EPI_GEGLU) {
     // packed columns (2i, 2i+1) = (value_i, gate_i): U[:, i] = gelu_erf(gate) * value; lanes qd and qd ^ 1 hold neighbouring
-    // outputs, so the even lane takes both.  f16: the 64 x 64 U values of the half go to the planes in `stage` (row r at
-    // r * 128 bytes, its 16-byte chunk c at chunk c ^ (r & 7): the 8 rows of a store land in 8 different bank groups),
-    // then every thread of the warpgroup copies whole 16-byte chunks out, 8 threads per 128-byte row.
-    if (!TF32) wg_bar(bar);                     // the previous half's copy-out has read the stage
+    // outputs.
+    if constexpr (TF32) {
+      // the even lane stores both
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = mrow[h];
-      const long long prow = map_row(m < g.M ? m : 0, g.c_seg, g.c_seg_stride, g.c_seg_off);
+      for (int h = 0; h < 2; ++h) {
+        const int m = mrow[h];
+        const long long prow = map_row(m < g.M ? m : 0, g.c_seg, g.c_seg_stride, g.c_seg_off);
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int n = n0 + 8 * j + 2 * qd;
-        float val = v[h][2 * j], gate = v[h][2 * j + 1];
-        if (g.bias != nullptr && n < g.N) { val += __ldg(g.bias + n); gate += __ldg(g.bias + n + 1); }
-        const float o = gelu_erf(gate) * val;
-        const float o1 = __shfl_xor_sync(0xffffffffu, o, 1);
-        if (TF32 && (qd & 1) == 0 && m < g.M && n < g.N) {
-          *reinterpret_cast<float2*>(g.c + prow * g.ldc + (n >> 1)) = make_float2(o, o1);
-        } else if (!TF32 && (qd & 1) == 0) {
-          uint32_t hw, lw;
-          if (g.u_scale > 0.f) split2u(o * g.u_scale, o1 * g.u_scale, hw, lw);
-          else split2(o, o1, hw, lw);
+        for (int j = 0; j < BN / 8; ++j) {
+          const int n = n0 + 8 * j + 2 * qd;
+          float val = v[h][2 * j], gate = v[h][2 * j + 1];
+          if (g.bias != nullptr && n < g.N) { val += __ldg(g.bias + n); gate += __ldg(g.bias + n + 1); }
+          const float o = gelu_erf(gate) * val;
+          const float o1 = __shfl_xor_sync(0xffffffffu, o, 1);
+          if ((qd & 1) == 0 && m < g.M && n < g.N) *reinterpret_cast<float2*>(g.c + prow * g.ldc + (n >> 1)) = make_float2(o, o1);
+        }
+      }
+    } else {
+      // f16: the 64 x 64 U values of the half go to the planes in `stage` (row r at r * 128 bytes, its 16-byte chunk c
+      // at chunk c ^ (r & 7): the 8 rows of a store land in 8 different bank groups), then one thread writes them out
+      // by TMA stores.
+      if constexpr (!H1) {
+        // The pair of 8-column blocks (2k, 2k + 1) is split between the lanes of a pair: the even lane packs the U pair
+        // of block 2k, the odd lane that of block 2k + 1, each after one exchange.  So every lane splits 8 pairs a row
+        // and the four lanes of a quad fill one 16-byte chunk.  The whole half is packed before the warpgroup waits for
+        // the stage, which the previous half's TMA store may still be reading.
+        const bool odd = (qd & 1) != 0;
+        uint32_t hw[2][BN / 16], lw[2][BN / 16];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int k = 0; k < BN / 16; ++k) {
+            float o[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int j = 2 * k + e;
+              const int n = n0 + 8 * j + 2 * qd;
+              float val = v[h][2 * j], gate = v[h][2 * j + 1];
+              if (g.bias != nullptr && n < g.N) { val += __ldg(g.bias + n); gate += __ldg(g.bias + n + 1); }
+              o[e] = gelu_erf(gate) * val;
+            }
+            const float got = __shfl_xor_sync(0xffffffffu, odd ? o[0] : o[1], 1);   // the partner's o of my block
+            const float a = odd ? got : o[0], b = odd ? o[1] : got;                  // U columns i, i + 1
+            if (g.u_scale > 0.f) split2u(a * g.u_scale, b * g.u_scale, hw[h][k], lw[h][k]);
+            else split2(a, b, hw[h][k], lw[h][k]);
+          }
+        }
+        if (elected) bulk_wait_read<0>();     // the previous half's TMA store has read the stage
+        wg_bar(bar);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
           const int r = (warp & 3) * 16 + (lane >> 2) + 8 * h;
-          const int b = 8 * j + 2 * qd;             // byte of U column (8 j + 2 qd) / 2 in the row
-          const int off = r * 128 + ((((b >> 4) ^ (r & 7)) << 4) | (b & 15));
-          *reinterpret_cast<uint32_t*>(stage + off) = hw;
-          if (!H1) *reinterpret_cast<uint32_t*>(stage + 64 * 128 + off) = lw;
-        }
-      }
-    }
-    if (!TF32) {
-      wg_bar(bar);
-      const int t = (warp & 3) * 32 + lane;
-      const int uc = n0 >> 1;                   // first U column of the tile
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int r = (t >> 3) + 16 * i, c = t & 7;
-        const int m = m0 + half * 64 + r;
-        if (m < g.M && 2 * (uc + 8 * c) < g.N) {   // N % 32 == 0: a 16-byte chunk is wholly inside or outside
-          const size_t off = (size_t)map_row(m, g.c_seg, g.c_seg_stride, g.c_seg_off) * g.ldu + uc + 8 * c;
-          const int so = r * 128 + ((c ^ (r & 7)) << 4);
-          *reinterpret_cast<uint4*>(g.u_hi + off) = *reinterpret_cast<const uint4*>(stage + so);
-          if (!H1) *reinterpret_cast<uint4*>(g.u_lo + off) = *reinterpret_cast<const uint4*>(stage + 64 * 128 + so);
+          for (int k = 0; k < BN / 16; ++k) {
+            // U column (8 (2k + odd) + 2 (qd & ~1)) / 2: byte 16 k + 8 odd + 4 (qd >> 1) of the row
+            const int off = r * 128 + ((k ^ (r & 7)) << 4) + 8 * (qd & 1) + 4 * (qd >> 1);
+            *reinterpret_cast<uint32_t*>(stage + off) = hw[h][k];
+            *reinterpret_cast<uint32_t*>(stage + 64 * 128 + off) = lw[h][k];
+          }
+        }
+      } else {
+        // f16x1 (hi plane only; the paired form spills here): the even lane packs both outputs of each block
+        if (elected) bulk_wait_read<0>();     // the previous half's TMA store has read the stage
+        wg_bar(bar);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = (warp & 3) * 16 + (lane >> 2) + 8 * h;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int n = n0 + 8 * j + 2 * qd;
+            float val = v[h][2 * j], gate = v[h][2 * j + 1];
+            if (g.bias != nullptr && n < g.N) { val += __ldg(g.bias + n); gate += __ldg(g.bias + n + 1); }
+            const float o = gelu_erf(gate) * val;
+            const float o1 = __shfl_xor_sync(0xffffffffu, o, 1);
+            if ((qd & 1) == 0) {
+              uint32_t hw, lw;
+              if (g.u_scale > 0.f) split2u(o * g.u_scale, o1 * g.u_scale, hw, lw);
+              else split2(o, o1, hw, lw);
+              const int b = 8 * j + 2 * qd;         // byte of U column (8 j + 2 qd) / 2 in the row
+              *reinterpret_cast<uint32_t*>(stage + r * 128 + ((((b >> 4) ^ (r & 7)) << 4) | (b & 15))) = hw;
+            }
+          }
         }
       }
+      fence_async_smem();                       // this thread's stage writes -> visible to the TMA store
+      wg_bar(bar);
+      if (elected) store_planes<H1>(tmUh, tmUl, stage, n0 >> 1, m0 + half * 64, g.c_seg);
     }
   } else {
     // plain: (+bias)(+residual).  residual may alias C, so the compiler may not move a residual load above a store to C:
@@ -271,7 +362,8 @@ template <bool TF32, int NACC, int EPI, bool H1 = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAl,
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmA2l,
-                  const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const Args g) {
+                  const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl,
+                  const __grid_constant__ CUtensorMap tmUh, const __grid_constant__ CUtensorMap tmUl, const Args g) {
   constexpr int BK = TF32 ? 32 : 64;          // elements per 128-byte row
   constexpr bool PINGPONG = !TF32 && NACC == 1;
   constexpr int HALVES = PINGPONG ? 2 : 1;    // 64-row halves of a tile one consumer warpgroup computes
@@ -428,8 +520,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
       for (int h = 0; h < HALVES; ++h)
         epilogue<TF32, NACC, EPI, H1>(g, acc[h], crs, m0, n0, second, PINGPONG ? h : wg, warp, lane,
-                                      smem + NS * SB + wg * EPI_STAGE_BYTES, 1 + wg);
+                                      smem + NS * SB + wg * EPI_STAGE_BYTES, 1 + wg, &tmUh, &tmUl);
     }
+    // the warpgroup's TMA stores must be done before its shared memory goes away with the CTA
+    if (tma_planes<TF32, EPI, H1>() && (tid & 127) == 0) bulk_wait<0>();
   }
 }
 
@@ -455,15 +549,15 @@ static inline int encode_map(CUtensorMap* m, CUtensorMapDataType dt, const void*
   return OMT_OK;
 }
 
-// [K, seg, n_seg] map over a row-mapped matrix of 16-bit (esize 2) or fp32 (esize 4) elements, 128-byte x 64-row boxes
+// [K, seg, n_seg] map over a row-mapped matrix of 16-bit (esize 2) or fp32 (esize 4) elements, 128-byte x box_rows boxes
 static inline int row_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const void* ptr, int ld, int rows, int cols,
-                          int seg, int seg_stride, int seg_off) {
+                          int seg, int seg_stride, int seg_off, int box_rows = 64) {
   const int s = seg > 0 ? seg : rows;
   const int nseg = seg > 0 ? rows / seg : 1;
   const long long sstride = seg > 0 ? seg_stride : rows;
   cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)s, (cuuint64_t)nseg};
   cuuint64_t strides[2] = {(cuuint64_t)ld * esize, (cuuint64_t)sstride * ld * esize};
-  cuuint32_t box[3] = {(cuuint32_t)(128 / esize), 64, 1};
+  cuuint32_t box[3] = {(cuuint32_t)(128 / esize), (cuuint32_t)box_rows, 1};
   const uint8_t* base = static_cast<const uint8_t*>(ptr) + (size_t)(seg > 0 ? seg_off : 0) * ld * esize;
   return encode_map(m, dt, base, 3, dims, strides, box);
 }
@@ -476,6 +570,8 @@ static inline int w_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const
   return encode_map(m, dt, ptr, 2, dims, strides, box);
 }
 
+// maps: A, A_lo, A2, A2_lo, W_hi, W_lo, and for the plane-writing f16 epilogues the output planes hi, lo (row_map with
+// 32-row boxes); the other epilogues take six maps
 template <bool TF32, int NACC, int EPI, bool H1 = false>
 static int launch(const CUtensorMap* maps, const Args& g, cudaStream_t st) {
   auto kern = gemm_wgmma_kernel<TF32, NACC, EPI, H1>;
@@ -494,7 +590,9 @@ static int launch(const CUtensorMap* maps, const Args& g, cudaStream_t st) {
   }
   const int tiles = g.num_m_blk * ((g.N + BN - 1) / BN);
   const dim3 grid(tiles < resident[dev] ? tiles : resident[dev]);
-  OMT_CUDA(launch_k(kern, grid, dim3(THREADS), SMEM, st, maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], g));
+  const CUtensorMap& uh = tma_planes<TF32, EPI, H1>() ? maps[6] : maps[0];
+  const CUtensorMap& ul = tma_planes<TF32, EPI, H1>() ? maps[7] : maps[0];
+  OMT_CUDA(launch_k(kern, grid, dim3(THREADS), SMEM, st, maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], uh, ul, g));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }
