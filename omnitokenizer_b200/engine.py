@@ -146,21 +146,34 @@ class Workspace:
         self.z = torch.empty(M, cd, **f)
         self.idx = torch.empty(M, device=device, dtype=torch.int64)
         self.counts = torch.zeros(8192, device=device, dtype=torch.int32)
-        # static I/O buffers + captured CUDA graphs of this shape
-        self.x_in = None
-        self.u8_in, self.u8_sel = None, None      # encode_u8: uint8 frames, per-sample table index
-        self.video_u8 = None
         self.idx_in = torch.empty(M, device=device, dtype=torch.int64)
         self.zc_in = torch.empty(M, cd, **f)
         self.zq = torch.empty(M, cd, **f)
-        self.video = None
-        # packed batches: encode_batch's (layout key, per-group static input videos); decode_batch's static outputs per
-        # dtype {uint8?: (layout key, per-group videos)}; the layout tables of those layouts (Engine._layout_tables)
-        self.batch_in, self.batch_out, self.layout_tables = None, {}, {}
-        self.graphs = {}
+        # static I/O buffers per slot {slot: (layout key, buffers)} (static()), the layout tables of the layouts they hold
+        # (Engine._layout_tables), and the captured CUDA graphs {(slot, layout key, mode, extra): graph state}
+        self.sets, self.layout_tables, self.graphs = {}, {}, {}
 
     def reset(self):
         self.X, self.Y = self.buf0, self.buf1
+
+    def static(self, slot: str, lay_key, make):
+        """The static buffers of `slot` for the layout lay_key.  A slot holds one set: a set of another layout replaces
+        it (make() builds the new one), which drops exactly the graphs captured over the slot and the layout tables no
+        held set uses any more."""
+        held = self.sets.get(slot)
+        if held is not None and held[0] == lay_key:
+            return held[1]
+        bufs = make()
+        self.sets[slot] = (lay_key, bufs)
+        for k in self.graphs_of(slot):
+            del self.graphs[k]
+        live = {k for k, _ in self.sets.values()}
+        self.layout_tables = {k: v for k, v in self.layout_tables.items() if k in live}
+        return bufs
+
+    def graphs_of(self, slot: str) -> dict:
+        """The graph states captured over the static buffers of `slot`, by graph key."""
+        return {k: v for k, v in self.graphs.items() if k[0] == slot}
 
 
 class Group(NamedTuple):
@@ -209,7 +222,8 @@ class BatchLayout:
                 i = self.order[g.s0 + k]
                 self.slot[i] = (gi, k)
                 self.f_in[i] = g.f0 + k * g.tp
-        # graphs and static I/O buffers are keyed on this: two layouts with the same M differ here
+        # graphs and static I/O buffers are keyed on this (with cin, p, pt it fixes every input and output shape): two
+        # layouts with the same M differ here
         self.key = (tuple(sorted_tp), h, w)
 
     def rows(self, i: int) -> slice:
@@ -480,8 +494,8 @@ class Engine:
     # ------------------------------------------------------------------ transformer
     def _layout_tables(self, ws: Workspace, lay: BatchLayout):
         """(t_off host copy, t_off device copy, int64 [M] sorted position of the sample each row belongs to) of a packed
-        layout.  They live in the workspace for as long as a static buffer set of that layout does (_keep_layouts), and
-        with it every graph that reads them; the copy to the device is asynchronous (pinned host memory)."""
+        layout.  They live in the workspace for as long as a static buffer set of that layout does (Workspace.static),
+        and with it every graph that reads them; the copy to the device is asynchronous (pinned host memory)."""
         t = ws.layout_tables.get(lay.key)
         if t is None:
             host = torch.tensor(lay.t_off, dtype=torch.int32).pin_memory()
@@ -489,12 +503,6 @@ class Engine:
             frame = torch.arange(lay.M, device=self.device, dtype=torch.int32) // lay.N
             t = ws.layout_tables[lay.key] = (host, dev, torch.searchsorted(dev, frame, right=True) - 1)
         return t
-
-    @staticmethod
-    def _keep_layouts(ws: Workspace):
-        """Drop the layout tables of layouts no static buffer set of the workspace holds any more (their graphs are gone)."""
-        live = {v[0] for v in ws.batch_out.values()} | ({ws.batch_in[0]} if ws.batch_in is not None else set())
-        ws.layout_tables = {k: v for k, v in ws.layout_tables.items() if k in live}
 
     def row_sample(self, ws: Workspace, lay: BatchLayout) -> torch.Tensor:
         """int64 [M] on the device: sorted position (lay.pos) of the sample each canonical row of the layout belongs to."""
@@ -674,7 +682,7 @@ class Engine:
         """x (B,C,T,H,W) fp32 on the device.  mode 'vq': returns (ws, dims) with ws.z (l2-normalised z),
         ws.idx, ws.counts filled; mode 'raw': ws.z = pre_vq output (VAE moments).  Results live in the
         workspace until the next call of the same shape."""
-        return self._encode_input(tuple(x.shape), mode, lambda buf: buf.copy_(x))
+        return self._encode_input(tuple(x.shape), mode, lambda bufs: bufs[0].copy_(x))
 
     def encode_clips_u8(self, clips: Sequence[torch.Tensor], resize: L.ClipResize, flips, mode: str, norm: L.U8Norm):
         """encode() of the (B, 3, F, oh, ow) fp32 clips the Latte loader's transform `resize` (flips[i]: clip i mirrored)
@@ -683,24 +691,29 @@ class Engine:
         that shape runs -- the same graph a later encode() of that shape replays."""
         F, H, W = (int(v) for v in clips[0].shape[:3])
         shape = (len(clips), self.cin, F) + L.clip_out_size(H, W, resize)
-        return self._encode_input(shape, mode, lambda buf: self.resample_clips(clips, resize, flips, norm, buf))
+        return self._encode_input(shape, mode, lambda bufs: self.resample_clips(clips, resize, flips, norm, bufs[0]))
 
     def _encode_input(self, shape, mode: str, fill):
-        """encode of the (B,C,T,H,W) fp32 video fill(buf) writes into the static input buffer buf."""
-        dims = self._shape(shape)
-        B, T, H, W, Tp, h, w = dims
-        ws = self._workspace(B * Tp * h * w)
-        if ws.x_in is None or tuple(ws.x_in.shape) != shape:
-            ws.x_in = torch.empty(shape, device=self.device, dtype=torch.float32)
-            ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("enc")}
-        fill(ws.x_in)
+        """encode of the (B,C,T,H,W) fp32 video fill(bufs) writes into bufs[0], encode's static input buffer."""
+        B, T, H, W, Tp, h, w = self._shape(shape)
+        return self._encode_pass("encode", BatchLayout((Tp,) * B, h, w), mode, fill), (B, Tp, h, w)
+
+    def _encode_pass(self, slot: str, lay: BatchLayout, mode: str, fill) -> Workspace:
+        """One encode of the layout lay from the static fp32 input buffers of `slot`, one (n,C,T,H,W) video per group,
+        which fill(bufs) writes."""
+        ws = self._workspace(lay.M)
+        bufs = ws.static(slot, lay.key, lambda: [
+            torch.empty(self._video_shape(g.n, g.tp, lay.h, lay.w, False), device=self.device, dtype=torch.float32)
+            for g in lay.groups])
+        fill(bufs)
+        H, W = lay.h * self.p, lay.w * self.p
 
         def gather(gi, first, *out):
-            _cabi.call("omt_patchify_ln", ws.x_in, *out, B, self.cin, T, H, W, self.p, self.pt, first, 1e-5)
+            g, x = lay.groups[gi], bufs[gi]
+            _cabi.call("omt_patchify_ln", x, *out, g.n, self.cin, x.shape[2], H, W, self.p, self.pt, first, 1e-5)
 
-        lay = BatchLayout((Tp,) * B, h, w)
-        self._run(ws, ("enc:" + mode, shape), lambda: self._encode_body(ws, gather, lay, mode))
-        return ws, (B, Tp, h, w)
+        self._run(ws, (slot, lay.key, mode, None), lambda: self._encode_body(ws, gather, lay, mode))
+        return ws
 
     def encode_batch(self, xs: Sequence[torch.Tensor], mode: str):
         """encode() of a list of single videos xs[i] (C, T_i, H, W) fp32 on the device, all with the same C, H, W, in ONE pass:
@@ -713,23 +726,12 @@ class Engine:
                 raise ValueError(f"every element of a batch must have the same frame size: {H}x{W} and {d[2]}x{d[3]}")
         self._check_packed([d[4] for d in dims])
         lay = BatchLayout([d[4] for d in dims], dims[0][5], dims[0][6])
-        ws = self._workspace(lay.M)
-        if ws.batch_in is None or ws.batch_in[0] != lay.key:
-            ws.batch_in = (lay.key, [torch.empty((g.n, self.cin, 1 + (g.tp - 1) * self.pt, H, W), device=self.device)
-                                     for g in lay.groups])
-            ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("encb")}
-            self._keep_layouts(ws)
-        bufs = ws.batch_in[1]
-        for g, buf in zip(lay.groups, bufs):
-            torch.stack([xs[i].to(device=self.device, dtype=torch.float32) for i in lay.order[g.s0:g.s0 + g.n]], out=buf)
 
-        def gather(gi, first, *out):
-            g = lay.groups[gi]
-            _cabi.call("omt_patchify_ln", bufs[gi], *out, g.n, self.cin, bufs[gi].shape[2], H, W, self.p, self.pt, first,
-                       1e-5)
+        def fill(bufs):
+            for g, buf in zip(lay.groups, bufs):
+                torch.stack([xs[i].to(device=self.device, dtype=torch.float32) for i in lay.order[g.s0:g.s0 + g.n]], out=buf)
 
-        self._run(ws, ("encb:" + mode, lay.key), lambda: self._encode_body(ws, gather, lay, mode))
-        return ws, lay
+        return self._encode_pass("encode_batch", lay, mode, fill), lay
 
     def encode_u8(self, frames: torch.Tensor, mode: str, norm: L.U8Norm):
         """encode() from uint8 frames (B,T,H,W,C) on the device: the patch gather maps every byte through the host-built
@@ -750,28 +752,25 @@ class Engine:
     def _encode_u8_input(self, shape, mode: str, norm: L.U8Norm, fill):
         """encode_u8 of the (B,T,H,W,C) uint8 frames fill(buf) writes into the static input buffer buf."""
         Bf, Tf, Hf, Wf, Cf = shape
-        dims = self._shape((Bf, Cf, Tf, Hf, Wf))
-        B, T, H, W, Tp, h, w = dims
-        ws = self._workspace(B * Tp * h * w)
-        if ws.u8_in is None or tuple(ws.u8_in.shape) != shape:
-            ws.u8_in = torch.empty(shape, device=self.device, dtype=torch.uint8)
-            ws.u8_sel = torch.empty(B, device=self.device, dtype=torch.int32)
-            ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("enc_u8")}
-        fill(ws.u8_in)
+        B, T, H, W, Tp, h, w = self._shape((Bf, Cf, Tf, Hf, Wf))
+        lay = BatchLayout((Tp,) * B, h, w)
+        ws = self._workspace(lay.M)
+        frames, sel = ws.static("encode_u8", lay.key, lambda: (
+            torch.empty(shape, device=self.device, dtype=torch.uint8),
+            torch.empty(B, device=self.device, dtype=torch.int32)))      # per-sample table index (omt_u8_norm_select)
+        fill(frames)
         lut = self._table(("u8norm", norm), lambda: L.u8_norm_table(norm, self.cin))
-        sel = ws.u8_sel if norm.max_test else None
+        sel = sel if norm.max_test else None
 
         def gather(gi, first, *out):
-            _cabi.call("omt_patchify_ln_u8", ws.u8_in, lut, sel, *out, B, self.cin, T, H, W, self.p, self.pt, first, 1e-5)
-
-        lay = BatchLayout((Tp,) * B, h, w)
+            _cabi.call("omt_patchify_ln_u8", frames, lut, sel, *out, B, self.cin, T, H, W, self.p, self.pt, first, 1e-5)
 
         def body():
             if sel is not None:
-                _cabi.call("omt_u8_norm_select", ws.u8_in, B, T * H * W * self.cin, sel)
+                _cabi.call("omt_u8_norm_select", frames, B, T * H * W * self.cin, sel)
             self._encode_body(ws, gather, lay, mode)
 
-        self._run(ws, ("enc_u8:" + mode, shape, norm), body)
+        self._run(ws, ("encode_u8", lay.key, mode, norm), body)
         return ws, (B, Tp, h, w)
 
     def stage_images_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params) -> tuple:
@@ -956,23 +955,9 @@ class Engine:
         with u8 = (mul, add, lo, hi, post) a fresh uint8 (B,T,H,W,C) tensor (fused consumer conversion)."""
         B, Tp, h, w = dims
         self._check_latent_frames(Tp)
-        ws = self._workspace(B * Tp * h * w)
-        vshape = self._video_shape(B, Tp, h, w, False)
-        if ws.video is None or tuple(ws.video.shape) != vshape:
-            ws.video = torch.empty(vshape, device=self.device, dtype=torch.float32)
-            ws.video_u8 = torch.empty(self._video_shape(B, Tp, h, w, True), device=self.device, dtype=torch.uint8)
-            ws.graphs = {k: v for k, v in ws.graphs.items() if not k[0].startswith("dec:")}
-        if idx is not None:
-            ws.idx_in.copy_(idx.reshape(-1))
-            mode = "idx_st" if straight_through else "idx"
-        else:
-            self._dense(ws.zc_in, ws.M, zc.shape[1]).copy_(zc)
-            mode = "zc"
-        u8 = None if u8 is None else tuple(float(v) for v in u8)
-        lay = BatchLayout((Tp,) * B, h, w)
-        outs = [ws.video if u8 is None else ws.video_u8]
-        self._run(ws, ("dec:" + mode, dims, u8), lambda: self._decode_body(ws, lay, mode, outs, u8))
-        return ws.video.clone() if u8 is None else ws.video_u8.clone()
+        outs = self._decode_pass("decode", BatchLayout((Tp,) * B, h, w), None if idx is None else idx.reshape(-1), zc, u8,
+                                 straight_through)
+        return outs[0].clone()
 
     def decode_batch(self, tps: Sequence[int], h: int, w: int, *, idx=None, zc=None, u8=None) -> List[torch.Tensor]:
         """decode() of a list of single samples in ONE pass.  tps[i]: latent frames of sample i; idx: list of int64 codes
@@ -982,22 +967,28 @@ class Engine:
             self._check_latent_frames(tp)
         self._check_packed(tps)
         lay = BatchLayout(tps, h, w)
-        ws = self._workspace(lay.M)
-        u8 = None if u8 is None else tuple(float(v) for v in u8)
-        is_u8 = u8 is not None
-        if is_u8 not in ws.batch_out or ws.batch_out[is_u8][0] != lay.key:      # one static output set per dtype
-            dt = torch.uint8 if is_u8 else torch.float32
-            ws.batch_out[is_u8] = (lay.key, [torch.empty(self._video_shape(g.n, g.tp, h, w, is_u8), device=self.device, dtype=dt)
-                                             for g in lay.groups])
-            ws.graphs = {k: v for k, v in ws.graphs.items() if not (k[0].startswith("decb") and (k[2] is not None) == is_u8)}
-            self._keep_layouts(ws)
-        outs = ws.batch_out[is_u8][1]
         if idx is not None:
-            ws.idx_in.copy_(torch.cat([idx[i].reshape(-1) for i in lay.order]))
-            mode = "idx"
+            idx = torch.cat([idx[i].reshape(-1) for i in lay.order])
         else:
-            cdp = zc[0].shape[-1]
-            self._dense(ws.zc_in, ws.M, cdp).copy_(torch.cat([zc[i].reshape(-1, cdp) for i in lay.order]))
-            mode = "zc"
-        self._run(ws, ("decb:" + mode, lay.key, u8), lambda: self._decode_body(ws, lay, mode, outs, u8))
+            zc = torch.cat([zc[i].reshape(-1, zc[0].shape[-1]) for i in lay.order])
+        outs = self._decode_pass("decode_batch", lay, idx, zc, u8)
         return [outs[gi][k].clone() for gi, k in lay.slot]
+
+    def _decode_pass(self, slot: str, lay: BatchLayout, idx, zc, u8, straight_through=False) -> List[torch.Tensor]:
+        """One decode of the layout lay from the codes idx (int64 [M]) or latents zc (fp32 [M, cd]) in its row order, into
+        the static output videos of `slot` (fp32), or of slot + "_u8" with u8 = (mul, add, lo, hi, post): one per group."""
+        ws = self._workspace(lay.M)
+        if u8 is not None:
+            u8, slot = tuple(float(v) for v in u8), slot + "_u8"
+        dt = torch.float32 if u8 is None else torch.uint8
+        outs = ws.static(slot, lay.key, lambda: [
+            torch.empty(self._video_shape(g.n, g.tp, lay.h, lay.w, u8 is not None), device=self.device, dtype=dt)
+            for g in lay.groups])
+        if idx is not None:
+            ws.idx_in.copy_(idx)
+            mode = "idx_st" if straight_through else "idx"
+        else:
+            self._dense(ws.zc_in, ws.M, zc.shape[1]).copy_(zc)
+            mode = "zc"
+        self._run(ws, (slot, lay.key, mode, u8), lambda: self._decode_body(ws, lay, mode, outs, u8))
+        return outs

@@ -149,7 +149,7 @@ def test_ucf_config_full_size(cuda):
     assert got.shape[:2] == (5, 5) and _eq(got, want)
 
 
-def test_second_batch_of_other_sizes_reuses_graph(model, cuda):
+def test_second_batch_of_other_sizes_reuses_encode_slot_graph(model, cuda):
     rz = L.ucf_clip_resize(64)
     batches = [[_clip(5, h, w, 300 + 10 * b + k) for k, (h, w) in enumerate(sz)]
                for b, sz in enumerate([[(240, 320), (80, 90)], [(17, 23), (640, 480)], [(64, 64), (1, 1)], [(200, 70), (3, 300)]])]
@@ -159,8 +159,8 @@ def test_second_batch_of_other_sizes_reuses_graph(model, cuda):
         want = model.encode(_host_stack(clips, rz).to(cuda), False)
         random.seed(1)
         assert torch.equal(model.encode_clips_u8(clips, rz), want)
-        ws = next(w for w in model.engine()._ws.values() if w.x_in is not None and tuple(w.x_in.shape) == (2, 3, 5, 64, 64))
-        graphs.append({k: v for k, v in ws.graphs.items() if k[0].startswith("enc:")})
+        ws = model.engine()._workspace(2 * 2 * 8 * 8)            # 2 clips of T' = 2 on the 8 x 8 token grid
+        graphs.append(ws.graphs_of("encode"))
     assert len(graphs[-1]) == 1
     g = next(iter(graphs[-1].values()))
     assert not isinstance(g, str) and next(iter(graphs[2].values())) is g

@@ -272,7 +272,7 @@ def test_vae_batch_equals_sequential_calls(cuda, math):
     check_sub(fx["rec"], m.decode_batch([z.permute(1, 2, 3, 0)])[0][None], PIX_TOL, "vae reconstruction")
 
 
-def test_graph_replay_and_layouts_with_equal_rows(cuda):
+def test_encode_batch_slot_replay_and_layouts_with_equal_rows(cuda):
     cfg, sd, _ = golden_setup(load_golden("img64"))
     m = build_model(cfg, sd, cuda, "f16x3")
     eng = m.engine()
@@ -280,7 +280,7 @@ def test_graph_replay_and_layouts_with_equal_rows(cuda):
           W.synthetic_input((1, 3, 9, 64, 64), 23)[0]]                     # T' = 2, 1, 3: 6 frames
     runs = [m.encode_batch(xs) for _ in range(3)]
     ws = eng._workspace(6 * 64)
-    graphs = [v for k, v in ws.graphs.items() if k[0] == "encb:vq"]
+    graphs = list(ws.graphs_of("encode_batch").values())
     assert graphs and isinstance(graphs[0], tuple), "the second call of a layout captures a graph, the third replays it"
     for r in runs[1:]:
         assert all(torch.equal(a, b) for a, b in zip(runs[0], r))
@@ -328,7 +328,7 @@ def test_errors_raise_before_launch(cuda):
     assert m.codebook.call_cnt == 0 and torch.equal(m.codebook.codebook_usage, usage)
 
 
-def test_layout_state_stays_bounded(cuda):
+def test_layout_state_and_decode_batch_slots_stay_bounded(cuda):
     """The same lengths in other orders reuse one layout (no engine-wide table grows); decode_batch and decode_u8_batch
     alternating on one layout each keep their own outputs and reach graph replay."""
     cfg, sd, _ = golden_setup(load_golden("img64"))
@@ -351,9 +351,31 @@ def test_layout_state_stays_bounded(cuda):
         recs8.append(m.decode_u8_batch(first))
     for r, r8 in zip(recs[1:], recs8[1:]):
         assert all(torch.equal(a, b) for a, b in zip(recs[0], r)) and all(torch.equal(a, b) for a, b in zip(recs8[0], r8))
-    dec = {k[2] is not None: v for k, v in ws.graphs.items() if k[0].startswith("decb")}
-    assert set(dec) == {False, True} and all(isinstance(v, tuple) for v in dec.values()), "both output forms replay a graph"
+    dec = [ws.graphs_of(slot) for slot in ("decode_batch", "decode_batch_u8")]
+    assert all(len(g) == 1 and all(isinstance(v, tuple) for v in g.values()) for g in dec), "both output forms replay a graph"
     assert len(ws.layout_tables) == 1
+
+
+def test_encode_batch_graph_survives_other_encode_inputs(cuda):
+    """encode and encode_u8 at other shapes of the same row count replace only their own static inputs: encode_batch
+    keeps replaying the graph it captured."""
+    cfg, sd, _ = golden_setup(load_golden("img64"))
+    m = build_model(cfg, sd, cuda, "f16x3")
+    eng = m.engine()
+    xs = [W.synthetic_input((1, 3, 5, 64, 64), 41)[0], W.synthetic_input((1, 3, 64, 64), 42)[0],
+          W.synthetic_input((1, 3, 9, 64, 64), 43)[0]]                     # T' = 2, 1, 3: 6 frames
+    runs = [m.encode_batch(xs) for _ in range(3)]
+    ws = eng._workspace(6 * 64)
+    (g,) = ws.graphs_of("encode_batch").values()
+    assert isinstance(g, tuple)
+    m.encode(W.synthetic_input((2, 3, 9, 64, 64), 44).to(cuda), False)      # 2 x T' = 3: 6 frames
+    frames = torch.randint(0, 256, (6, 64, 64, 3), dtype=torch.uint8, generator=torch.Generator().manual_seed(45))
+    m.encode_u8(frames.to(cuda), True)                                      # 6 images
+    assert len(eng._ws) == 1 and ws.graphs_of("encode") and ws.graphs_of("encode_u8")
+    runs.append(m.encode_batch(xs))
+    (g_after,) = ws.graphs_of("encode_batch").values()
+    assert g_after is g, "encode_batch captured its graph again"
+    assert all(torch.equal(a, b) for a, b in zip(runs[0], runs[-1]))
 
 
 def test_long_clip_in_a_packed_batch_without_temporal_blocks(cuda):

@@ -139,7 +139,7 @@ def test_encode_and_forward_images_u8_equal_u8_path(cuda, math, vae):
         assert _eq(C.encode_to_z_images_u8(m, imgs, L.image_resize(64)), want)
 
 
-def test_second_batch_of_other_sizes_reuses_graph(model, cuda):
+def test_second_batch_of_other_sizes_reuses_encode_u8_slot_graph(model, cuda):
     """Batches of different source sizes at the same output shape share encode_u8's graph of that shape and stay exact."""
     rz = L.image_resize(64)
     batches = [[_img(h, w, 300 + 10 * b + k) for k, (h, w) in enumerate(sz)]
@@ -148,8 +148,8 @@ def test_second_batch_of_other_sizes_reuses_graph(model, cuda):
     for imgs in batches:
         want = model.encode_u8(_host_stack(imgs, rz).to(cuda), True, norm=C.IMAGE_NORM)
         assert torch.equal(model.encode_images_u8(imgs, rz), want)
-        ws = next(w for w in model.engine()._ws.values() if w.u8_in is not None and w.u8_in.shape[0] == 2)
-        graphs.append({k: v for k, v in ws.graphs.items() if k[0].startswith("enc_u8")})
+        ws = model.engine()._workspace(2 * 8 * 8)                # 2 images on the 8 x 8 token grid
+        graphs.append(ws.graphs_of("encode_u8"))
     assert len(graphs[-1]) == 1
     g = next(iter(graphs[-1].values()))
     assert not isinstance(g, str) and next(iter(graphs[2].values())) is g

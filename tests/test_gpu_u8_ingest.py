@@ -155,7 +155,7 @@ def test_encode_u8_and_forward_u8_equal_fp32_path(cuda, name, math):
     assert torch.equal(torch.get_rng_state(), rng_want)
 
 
-def test_encode_u8_graphs_interleave_with_encode(cuda):
+def test_encode_u8_slot_graphs_interleave_with_encode_slot(cuda):
     """Same shape through encode and encode_u8: each call path runs eagerly, then captures, then replays a graph."""
     cfg = oo.Config(resolution=64)
     m = build_model(cfg, W.make_state_dict(cfg, 2), cuda, default_math())
@@ -170,8 +170,7 @@ def test_encode_u8_graphs_interleave_with_encode(cuda):
         assert torch.equal(a, b)
     assert not torch.equal(outs[0][0], outs[2][0])
     ws = next(iter(m.engine()._ws.values()))
-    kinds = {k[0] for k in ws.graphs}
-    assert {"enc:vq", "enc_u8:vq"} <= kinds and all(not isinstance(v, str) for v in ws.graphs.values())
+    assert ws.graphs_of("encode") and ws.graphs_of("encode_u8") and all(not isinstance(v, str) for v in ws.graphs.values())
 
 
 def test_fullsize_cfg3_codes(cuda):
