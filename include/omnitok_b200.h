@@ -206,6 +206,28 @@ int omt_maxpool3d(const float* x, int Cs, int B, int T, int H, int W, int kt, in
 int omt_i3d_head(const float* x, int Cs, int C, int B, int T, const float* w, const float* bias, int N, float* out,
                  omt_stream_t stream);
 
+/* pytorch-fid's InceptionV3 preprocess (inception.py:147-151, after fid_score.py's ToTensor) of B images of H x W: the
+ * tables, descriptors and checks of omt_fvd_preprocess with F = 1, but the division comes before the resize:
+ *   v = lut[byte]  (lut: fp32 [256], byte / 255 or the value a byte map sends the byte to; with sel != NULL, lut is
+ *                   fp32 [2][256] and image b reads table sel[b])
+ *   out = 2 * y - 1, two roundings,
+ * written channels-last: out (B, oh, ow, 4) fp32, 16-byte aligned, channel 3 zero (the input of the first conv). */
+int omt_fid_preprocess(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc, const omt_clip_desc* desc_host,
+                       const int32_t* tab, const int32_t* tab_host, long long tab_len, const float* lut,
+                       const int32_t* sel, int B, int oh, int ow, float* out, omt_stream_t stream);
+
+/* 2-D pooling of the FID InceptionV3 on channels-last fp32 [B][H][W][Cs] -> y, output pixel p = (b Ho + ho) Wo + wo,
+ * channel c < C at y[p * ldy + c] (C, Cs, ldy multiples of 4; x and y 16-byte aligned), so a pool branch writes its
+ * slice of the concat buffer in place.  Window (kh, kw), stride (sh, sw), symmetric padding (ph, pw) <= half the window;
+ * only taps inside the image take part, in (h, w) order, as torch's CPU kernels visit them:
+ *   OMT_POOL_MAX: max_pool2d (the padding never wins; NaN propagates);
+ *   OMT_POOL_AVG: avg_pool2d(count_include_pad=False): the fp32 sum, then one true division by the count of taps.
+ * Both exact.  The global AdaptiveAvgPool2d(1) of an 8 x 8 map is OMT_POOL_AVG with an 8 x 8 window. */
+#define OMT_POOL_MAX 0
+#define OMT_POOL_AVG 1
+int omt_pool2d(const float* x, int Cs, int C, int B, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw,
+               int Ho, int Wo, float* y, int ldy, int mode, omt_stream_t stream);
+
 /* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W). */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,
                    int first, omt_stream_t stream);

@@ -65,6 +65,9 @@ SIGNATURES = {
                    + [c_int] * 13 + [c_void_p, c_int, c_int, c_void_p]),
     "omt_maxpool3d": (c_int, [c_void_p] + [c_int] * 17 + [c_void_p, c_void_p]),
     "omt_i3d_head": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "omt_fid_preprocess": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                   c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "omt_pool2d": (c_int, [c_void_p] + [c_int] * 13 + [c_void_p, c_int, c_int, c_void_p]),
     "omt_unpatchify": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_void_p]),
     "omt_unpatchify_u8": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float] * 5 + [c_void_p]),
     "omt_peg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

@@ -238,6 +238,35 @@ def eval_step_images_u8(vqgan, images: Sequence[torch.Tensor], resize: U8Resize,
 
 
 @torch.no_grad()
+def eval_step_fid(vqgan, images: Sequence[torch.Tensor], resize: U8Resize, inception,
+                  total_usage: Optional[torch.Tensor] = None, norm: U8Norm = IMAGE_NORM):
+    """The body of vqgan_eval.py's image loop (:185-220) from the decoded ragged host images of ImageDataset, with the
+    PNG round trip and the pytorch-fid run replaced by FID features on the device (fid.FIDInception): forward_images_u8
+    for the reconstruction's bytes and vq_output, and the pool3 features of both sides.  The real side reads the
+    transformed input bytes that call wrote into the encode_u8 slot (the random crop and flip are drawn once) and sees
+    the bytes the script saves of the normalised input, ((x + 0.5) * 255).astype(uint8), as a per-byte map.  Returns
+    (real_features, fake_features, vq_output), each features (B, 2048) fp32; no image crosses to the host.
+    --infer_downsample (a PIL ANTIALIAS resize before saving) is not supported."""
+    from .fvd import real_byte_table
+    images = list(images)
+    if not images:
+        raise ValueError("eval_step_fid needs at least one image")
+    real_byte_table(norm)                    # refuses a per-channel normalisation before the first launch
+    if hasattr(vqgan, "forward_images_u8"):
+        fake, vq_output = vqgan.forward_images_u8(images, resize, norm, EVAL_U8)
+        if total_usage is not None and vq_output is not None:
+            total_usage += vq_output["batch_usage"]
+        real = vqgan.engine().encode_u8_frames(tuple(fake.shape))
+    else:
+        real = _host_transform(images, resize).to(inception.device)
+        fake, vq_output = eval_step_u8(vqgan, real, total_usage, norm)
+        real = real.unsqueeze(1)
+    real_features = inception.features(real[:, 0], real_norm=norm).clone()
+    fake_features = inception.features(fake[:, 0].contiguous()).clone()
+    return real_features, fake_features, vq_output
+
+
+@torch.no_grad()
 def encode_to_z_images_u8(vqgan, images: Sequence[torch.Tensor], resize: U8Resize,
                           norm: U8Norm = IMAGE_NORM) -> Tuple[torch.Tensor, torch.Tensor]:
     """encode_to_z (lm_transformer.py:258-268) of the LM's image stage from its decoded images (ImageDataset transform)."""

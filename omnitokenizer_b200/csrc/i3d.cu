@@ -316,6 +316,46 @@ i3d_head_kernel(const float* __restrict__ x, int Cs, int C, int T, const float* 
   for (int n = tid; n < N; n += HEAD_THREADS) out[(size_t)b * N + n] = acc[n] / (float)(T - 1);
 }
 
+// 2-D pooling of the FID InceptionV3 (pytorch-fid inception.py) on channels-last fp32 [B][H][W][Cs]: one thread per 4
+// channels of an output pixel.  Only taps inside the image take part (max: padding never wins; average: the count
+// excludes it, count_include_pad=False), in (h, w) order as torch's CPU kernels visit them: max_pool2d's rule (maxval
+// from -inf, replaced when val > maxval or val is NaN); avg_pool2d's fp32 sum from 0, then one true division by the count.
+// Output pixel p, channel c at y[p * ldy + c]: a pool branch writes its slice of the concat buffer in place.
+__global__ void __launch_bounds__(256)
+pool2d_kernel(const float4* __restrict__ x, float* __restrict__ y, int Cs4, int C4, int ldy, long long total, int H,
+              int W, int Ho, int Wo, int kh, int kw, int sh, int sw, int ph, int pw, int avg) {
+  pdl_sync();
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C4);
+    const long long p = i / C4;                   // output pixel (b, ho, wo)
+    const int wo = (int)(p % Wo);
+    const long long r = p / Wo;
+    const int ho = (int)(r % Ho);
+    const long long b = r / Ho;
+    const int h0 = ho * sh - ph, w0 = wo * sw - pw;
+    const int hs = max(h0, 0), he = min(h0 + kh, H), ws = max(w0, 0), we = min(w0 + kw, W);
+    const float init = avg ? 0.f : -INFINITY;
+    float m[4] = {init, init, init, init};
+    for (int hi = hs; hi < he; ++hi) {
+      for (int wi = ws; wi < we; ++wi) {
+        const float4 v = __ldg(x + ((b * H + hi) * W + wi) * Cs4 + c);
+        const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          if (avg) m[k] = __fadd_rn(m[k], e[k]);
+          else if (e[k] > m[k] || isnan(e[k])) m[k] = e[k];
+        }
+      }
+    }
+    if (avg) {
+      const float n = (float)((he - hs) * (we - ws));
+#pragma unroll
+      for (int k = 0; k < 4; ++k) m[k] = __fdiv_rn(m[k], n);
+    }
+    *reinterpret_cast<float4*>(y + p * ldy + 4 * c) = make_float4(m[0], m[1], m[2], m[3]);
+  }
+}
+
 }  // namespace i3d
 }  // namespace omt
 
@@ -381,6 +421,28 @@ extern "C" int omt_i3d_head(const float* x, int Cs, int C, int B, int T, const f
   OMT_REQUIRE(smem <= 48 * 1024, "omt_i3d_head: C=%d + N=%d floats exceed 48 KiB of shared memory", C, N);
   OMT_CUDA(launch_k(i3d::i3d_head_kernel, dim3(B), dim3(i3d::HEAD_THREADS), smem, (cudaStream_t)stream, x, Cs, C, T, w,
                     bias, N, out));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_pool2d(const float* x, int Cs, int C, int B, int H, int W, int kh, int kw, int sh, int sw, int ph,
+                          int pw, int Ho, int Wo, float* y, int ldy, int mode, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(x && y, "omt_pool2d: null pointer");
+  OMT_REQUIRE(mode == OMT_POOL_MAX || mode == OMT_POOL_AVG, "omt_pool2d: mode %d is neither max (0) nor average (1)", mode);
+  OMT_REQUIRE(Cs % 4 == 0 && C >= 4 && C % 4 == 0 && C <= Cs && ldy >= C && ldy % 4 == 0,
+              "omt_pool2d: C=%d channels of stride %d into rows of %d: all multiples of 4, C <= both", C, Cs, ldy);
+  OMT_REQUIRE(B >= 1 && H >= 1 && W >= 1 && Ho >= 1 && Wo >= 1, "omt_pool2d: input %dx%dx%d, output %dx%d", B, H, W, Ho, Wo);
+  OMT_REQUIRE(kh >= 1 && kw >= 1 && sh >= 1 && sw >= 1 && ph >= 0 && pw >= 0 && 2 * ph <= kh && 2 * pw <= kw,
+              "omt_pool2d: window %dx%d, stride %dx%d, padding %dx%d (at most half the window)", kh, kw, sh, sw, ph, pw);
+  OMT_REQUIRE((long long)(Ho - 1) * sh - ph + kh <= H + 2LL * ph && (long long)(Wo - 1) * sw - pw + kw <= W + 2LL * pw,
+              "omt_pool2d: output %dx%d reads past the %dx%d input padded by %dx%d", Ho, Wo, H, W, ph, pw);
+  OMT_REQUIRE(aligned_to(16, {x, y}), "omt_pool2d: x and y (at its column offset) must be 16-byte aligned");
+  const long long total = (long long)B * Ho * Wo * (C / 4);
+  const long long blocks = (total + 255) / 256;
+  const int grid = (int)(blocks < 65536 ? blocks : 65536);
+  OMT_CUDA(launch_k(i3d::pool2d_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, reinterpret_cast<const float4*>(x),
+                    y, Cs / 4, C / 4, ldy, total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, mode == OMT_POOL_AVG ? 1 : 0));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

@@ -164,17 +164,21 @@ resample_u8_kernel(const uint8_t* __restrict__ src, const omt_resample_desc* __r
 // nothing here is shared with Pillow's integer resize.
 // Each CTA owns RC_TW output columns (one per thread) x RC_TH rows of one frame of one clip; a thread's horizontal table
 // entry is loaded once, and each output row reads exactly two source rows.  Stores run along w within a channel plane.
-// FVD = true (omt_fvd_preprocess): fvd.py's preprocess instead of the loaders' Normalize.  The byte table holds the
+// OUT = OUT_FVD (omt_fvd_preprocess): fvd.py's preprocess instead of the loaders' Normalize.  The byte table holds the
 // value each byte stands for (table sel[b] of two when sel is given), the result is 2 y / 255 - 1 in that order, and a
 // frame leaves channels-last as [oh][ow][4] with channel 3 zero (the I3D input layout).
+// OUT = OUT_FID (omt_fid_preprocess): pytorch-fid's ToTensor -> F.interpolate -> 2 x - 1.  The same layout and tables, but
+// the byte table already holds byte / 255 (the division comes before the resize), and the result is 2 y - 1.
 constexpr int RC_TW = 128;
 constexpr int RC_TH = 8;
+enum { OUT_NORMALIZE = 0, OUT_FVD = 1, OUT_FID = 2 };
 
-template <bool FVD>
+template <int OUT>
 __device__ __forceinline__ void resample_clips_body(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
                                                     const int4* __restrict__ tab, const float* __restrict__ norm,
                                                     float* __restrict__ out, int F, int oh, int ow,
                                                     const int32_t* __restrict__ sel) {
+  constexpr bool FVD = OUT != OUT_NORMALIZE;     // a feature network's input: byte table sel[b], [oh][ow][4] out
   __shared__ float lut[256];
   pdl_sync();
   const int b = blockIdx.z / F, f = blockIdx.z % F;
@@ -222,7 +226,8 @@ __device__ __forceinline__ void resample_clips_body(const uint8_t* __restrict__ 
         const float t1 = __fmaf_rn(x10, l0w, __fmul_rn(x11, l1w));
         v = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
       }
-      if constexpr (FVD) y[c] = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, v), 255.f), 1.f);
+      if constexpr (OUT == OUT_FID) y[c] = __fsub_rn(__fmul_rn(2.f, v), 1.f);
+      else if constexpr (FVD) y[c] = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, v), 255.f), 1.f);
       else o[c * F * plane + (long long)oy * ow] = __fdiv_rn(__fsub_rn(v, mean[c]), stdv[c]);
     }
     if constexpr (FVD)
@@ -234,14 +239,21 @@ __global__ void __launch_bounds__(RC_TW)
 resample_clips_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
                       const int4* __restrict__ tab, const float* __restrict__ norm, float* __restrict__ out, int F,
                       int oh, int ow) {
-  resample_clips_body<false>(src, desc, tab, norm, out, F, oh, ow, nullptr);
+  resample_clips_body<OUT_NORMALIZE>(src, desc, tab, norm, out, F, oh, ow, nullptr);
 }
 
 __global__ void __launch_bounds__(RC_TW)
 fvd_preprocess_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
                       const int4* __restrict__ tab, const float* __restrict__ lut, const int32_t* __restrict__ sel,
                       float* __restrict__ out, int F, int oh, int ow) {
-  resample_clips_body<true>(src, desc, tab, lut, out, F, oh, ow, sel);
+  resample_clips_body<OUT_FVD>(src, desc, tab, lut, out, F, oh, ow, sel);
+}
+
+__global__ void __launch_bounds__(RC_TW)
+fid_preprocess_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
+                      const int4* __restrict__ tab, const float* __restrict__ lut, const int32_t* __restrict__ sel,
+                      float* __restrict__ out, int oh, int ow) {
+  resample_clips_body<OUT_FID>(src, desc, tab, lut, out, 1, oh, ow, sel);
 }
 
 // One axis table of a clip: [n_out][4] entries at word `off` inside the table, every (i0, i1) inside an axis of n_in.
@@ -359,6 +371,23 @@ extern "C" int omt_fvd_preprocess(const uint8_t* src, long long src_bytes, const
   dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
   OMT_CUDA(launch_k(fvd_preprocess_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
                     reinterpret_cast<const int4*>(tab), lut, sel, out, F, oh, ow));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_fid_preprocess(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc,
+                                  const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
+                                  long long tab_len, const float* lut, const int32_t* sel, int B, int oh, int ow,
+                                  float* out, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(aligned_to(4, {sel}), "omt_fid_preprocess: sel must be 4-byte aligned");
+  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && aligned_to(4, {lut}),
+              "omt_fid_preprocess: desc must be 8-byte, tab / out 16-byte and lut 4-byte aligned");
+  int rc = check_clips("omt_fid_preprocess", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, lut, B, 1, oh, ow, out);
+  if (rc != OMT_OK) return rc;
+  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B);
+  OMT_CUDA(launch_k(fid_preprocess_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
+                    reinterpret_cast<const int4*>(tab), lut, sel, out, oh, ow));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

@@ -749,6 +749,19 @@ class Engine:
         return self._encode_u8_input((len(images), 1, oh, ow, self.cin), mode, norm,
                                      lambda buf: self.resample_u8(images, resize, params, buf))
 
+    def encode_u8_frames(self, shape) -> torch.Tensor:
+        """The encode_u8 slot's static uint8 input buffer for frames of `shape` (B, T, H, W, C): the bytes the last
+        encode_u8 / encode_images_u8 of that shape encoded (for images, the loader's transform as omt_resample_u8 made
+        it).  Valid until the next call of either; raises LookupError if the slot holds another shape."""
+        Bf, Tf, Hf, Wf, Cf = shape
+        B, T, H, W, Tp, h, w = self._shape((Bf, Cf, Tf, Hf, Wf))
+        lay = BatchLayout((Tp,) * B, h, w)
+        ws = self._ws.get(lay.M)
+        held = None if ws is None else ws.sets.get("encode_u8")
+        if held is None or held[0] != lay.key or tuple(held[1][0].shape) != tuple(shape):
+            raise LookupError(f"the encode_u8 slot holds no {tuple(shape)} frames")
+        return held[1][0]
+
     def _encode_u8_input(self, shape, mode: str, norm: L.U8Norm, fill):
         """encode_u8 of the (B,T,H,W,C) uint8 frames fill(buf) writes into the static input buffer buf."""
         Bf, Tf, Hf, Wf, Cf = shape
