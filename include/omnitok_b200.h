@@ -228,6 +228,41 @@ int omt_fid_preprocess(const uint8_t* src, long long src_bytes, const omt_clip_d
 int omt_pool2d(const float* x, int Cs, int C, int B, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw,
                int Ho, int Wo, float* y, int ldy, int mode, omt_stream_t stream);
 
+/* Frame-pair metrics (evaluation/common_metrics_on_video_quality, OmniTokenizer/modules/lpips.py) take P frames
+ * (P, H, W, 3) channels last in one of two forms:
+ *   OMT_Q_U8:  uint8, each byte standing for lut[t][byte] (fp32 [n_tab][256], or [n_tab][3][256] per channel), with
+ *              t = sel[p] (int32 [P]) or 0 when sel is NULL;
+ *   OMT_Q_F32: fp32 values (no tables).
+ * Every reduction runs in a fixed order (no floating-point atomics): two runs give the same bits. */
+#define OMT_Q_U8 0
+#define OMT_Q_F32 1
+
+/* calculate_psnr.py's img_psnr and calculate_ssim.py's calculate_ssim_function (3 channels) of pairs (a[p], b[p]):
+ *   sse[p]  = sum over C H W of (a - b)^2, the fp32 values widened to fp64 (PSNR follows on the host from
+ *             mse = sse / (3 H W): 100 if mse < 1e-10, else 20 log10(1 / sqrt(mse)));
+ *   ssim[p] = the mean over channels, in channel order, of the mean over the valid (H - 10) x (W - 10) map of
+ *             ((2 mu1 mu2 + C1)(2 s12 + C2)) / ((mu1^2 + mu2^2 + C1)(s1 + s2 + C2)), C1 = 0.01^2, C2 = 0.03^2, from
+ *             the five maps mu1, mu2, E[x^2], E[y^2], E[xy] filtered with taps[11] (fp64; cv2.getGaussianKernel(11,
+ *             1.5)) along w, then along h, in fp64.
+ * H, W >= 11.  sse, ssim: fp64 [P]. */
+int omt_psnr_ssim(const void* a, const float* lut_a, const int32_t* sel_a, const void* b, const float* lut_b,
+                  const int32_t* sel_b, int form, int P, int H, int W, const double* taps, double* sse, double* ssim,
+                  omt_stream_t stream);
+
+/* LPIPS network input of P frames: calculate_lpips.py's x * 2 - 1, then ScalingLayer's (x - shift_c) / scale_c, fp32
+ * rounded after every op, written as out [P][H][W][4] (16-byte aligned, channel 3 zero; the omt_conv3d input layout).
+ * OMT_Q_U8: lut [n_tab][3][256] holds the whole chain per byte (built on the host), sel picks the table per frame;
+ * OMT_Q_F32: shift_scale fp32 [6] = (shift_0..2, scale_0..2) on the device, lut and sel NULL. */
+int omt_lpips_input(const void* x, const float* lut, const int32_t* sel, const float* shift_scale, int form, int P,
+                    int H, int W, float* out, omt_stream_t stream);
+
+/* LPIPS head at one VGG tap (lpips.py:97-108): x fp32 [2P][h][w][Cs], pair p = images p and p + P, C channels; per pair
+ *   taps_out[tap * P + p] = mean over pixels of sum_c lin_w[c] (x_c / (|x| + 1e-10) - y_c / (|y| + 1e-10))^2
+ * with |x| = sqrt(sum_c x_c^2) (fp32 per pixel, the pixel sum in fp64).  If total != NULL, total[p] = taps_out[0][p]
+ * + ... + taps_out[tap][p], added in fp32 in that order (the earlier taps' launches must precede this one). */
+int omt_lpips_head(const float* x, int Cs, int C, int P, int h, int w, const float* lin_w, int tap, float* taps_out,
+                   float* total, omt_stream_t stream);
+
 /* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W). */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,
                    int first, omt_stream_t stream);

@@ -68,6 +68,9 @@ SIGNATURES = {
     "omt_fid_preprocess": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
                                    c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "omt_pool2d": (c_int, [c_void_p] + [c_int] * 13 + [c_void_p, c_int, c_int, c_void_p]),
+    "omt_psnr_ssim": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_void_p] * 4),
+    "omt_lpips_input": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_void_p, c_void_p]),
+    "omt_lpips_head": (c_int, [c_void_p] + [c_int] * 5 + [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "omt_unpatchify": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_void_p]),
     "omt_unpatchify_u8": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float] * 5 + [c_void_p]),
     "omt_peg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

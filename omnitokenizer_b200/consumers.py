@@ -192,6 +192,31 @@ def eval_step_fvd(vqgan, frames: torch.Tensor, i3d, total_usage: Optional[torch.
 
 
 @torch.no_grad()
+def eval_step_quality(vqgan, frames: torch.Tensor, lpips=None, total_usage: Optional[torch.Tensor] = None,
+                      norm: U8Norm = VIDEO_NORM):
+    """vqgan_eval.py's loop body (:114-152) with the per-frame reconstruction metrics of
+    evaluation/common_metrics_on_video_quality on the device: forward_u8 (eval_step_u8) for the reconstruction's bytes,
+    then quality.frame_metrics of the real and reconstructed bytes (PSNR, SSIM and, with a quality.LPIPS model, the VGG
+    LPIPS).  The real side sees the bytes the script makes of the normalised clip, ((video + 0.5) * 255).byte(), as a
+    per-byte map with norm's branch picked per clip.  frames: the loader's uint8 (B, T, H, W, 3) on the device, or
+    images (B, H, W, 3) as T = 1.  Returns (psnr (B, T) fp64, ssim (B, T) fp64, lpips (B, T) fp32 or None,
+    fake_u8 (B, T, H, W, 3), vq_output); fake_u8 can feed i3d.logits as well.  No frame crosses to the host."""
+    from . import quality
+    from .fvd import real_byte_table
+    _check_u8(frames, (4, 5), "eval_step_quality")
+    real = frames.unsqueeze(1) if frames.dim() == 4 else frames
+    quality.check_pair(real, real, torch.uint8, "eval_step_quality")      # every refusal before the first launch
+    quality._check_sizes(int(real.shape[2]), int(real.shape[3]), int(real.shape[4]), "eval_step_quality",
+                         lpips is not None)
+    real_byte_table(norm)
+    fake, vq_output = eval_step_u8(vqgan, frames, total_usage, norm)
+    if fake.dim() == 4:
+        fake = fake.unsqueeze(1)
+    psnr, ssim, lp = quality.frame_metrics(real, fake, lpips, real_norm=norm)
+    return psnr, ssim, lp, fake, vq_output
+
+
+@torch.no_grad()
 def encode_to_z_u8(vqgan, frames: torch.Tensor, is_image: bool, sample_every_n_latent_frames: int = 0,
                    norm: U8Norm = VIDEO_NORM) -> Tuple[torch.Tensor, torch.Tensor]:
     """encode_to_z (lm_transformer.py:258-268) from the uint8 frames of the LM's VideoNorm data loader."""
