@@ -182,6 +182,24 @@ int omt_fvd_preprocess(const uint8_t* src, long long src_bytes, const omt_clip_d
                        const int32_t* tab, const int32_t* tab_host, long long tab_len, const float* lut,
                        const int32_t* sel, int B, int F, int oh, int ow, float* out, omt_stream_t stream);
 
+/* The FVD preprocess of evaluation/common_metrics_on_video_quality (fvd/styleganv and fvd/videogpt preprocess_single)
+ * of B clips of F frames: the descriptors and axis tables of omt_resample_clips (no flip, no window; desc.form picks
+ * torch's bilinear kernel), torch's fp32 CPU arithmetic bit for bit.  Each source sample is read in one of three forms:
+ *   OMT_FVDS_U8:        uint8 (F, H, W, 3) clips, v = (float)byte / 255 (C == 3);
+ *   OMT_FVDS_F32:       fp32 (F, C, H, W) clips, C 1 (grey, every channel reads it) or 3, v used as is (styleganv);
+ *   OMT_FVDS_F32_TRUNC: the same fp32 clips through videogpt's byte round trip, v = (float)(uint8)(x * 255) / 255
+ *                       (the low byte of the truncated int32, as numpy's astype on x86-64);
+ *   out = (y - 0.5) * 2, two roundings,
+ * written channels-last: out (B, F, oh, ow, 4) fp32, 16-byte aligned, channel 3 zero (the I3D input of omt_conv3d).
+ * desc.src and src_elems count elements of src (bytes, or floats); a clip's frames follow each other from desc.src, so
+ * a clip stored with more than F frames is read as its first F. */
+#define OMT_FVDS_U8 0
+#define OMT_FVDS_F32 1
+#define OMT_FVDS_F32_TRUNC 2
+int omt_fvd_suite_preprocess(const void* src, long long src_elems, int form, int C, const omt_clip_desc* desc,
+                             const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
+                             long long tab_len, int B, int F, int oh, int ow, float* out, omt_stream_t stream);
+
 /* Unit3D of the FVD I3D (fvd/pytorch_i3d.py:59-131) as an implicit GEMM in 3xTF32 on sm_90a wgmma:
  *   y[m, n] = act(sum_k A[m, k] W[n, k] + bias[n]),  m = ((b To + to) Ho + ho) Wo + wo,  n < N,  act = ReLU if relu
  *   A[m, (dt, dh, dw, c)] = x[b][to st - pt + dt][ho sh - ph + dh][wo sw - pw + dw][c], zero outside the volume

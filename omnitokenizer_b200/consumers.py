@@ -329,3 +329,41 @@ def latte_encode_latents_clips_u8(vae, clips: Sequence[torch.Tensor], resize: Cl
     clips = list(clips)
     flips = clip_params(len(clips), resize)
     return latte_encode_latents(vae, torch.stack([resize_clip(c, resize, f, norm) for c, f in zip(clips, flips)]))
+
+
+FVD_SAMPLING = ("first", "last", "center")
+
+
+def fvd_external_indices(n: int, frames: int, sampling: str = "center"):
+    """The frames fvd_external.py's load_videos keeps of an n-frame clip (:30-46): all when n == frames, else the first
+    or last `frames`, or range(c - frames // 2, c + frames // 2), one more for odd `frames`, with c = n // 2.  Raises
+    its assertion n >= frames as a ValueError."""
+    if sampling not in FVD_SAMPLING:
+        raise ValueError(f"fvd_external: unknown sampling {sampling!r}; expected one of {FVD_SAMPLING}")
+    if frames < 1 or n < frames:
+        raise ValueError(f"fvd_external: a clip of {n} frames, fewer than frames={frames}")
+    if n == frames or sampling == "first":
+        return range(frames)
+    if sampling == "last":
+        return range(n - frames, n)
+    c = n // 2
+    return range(c - frames // 2, c + frames // 2 + frames % 2)
+
+
+def fvd_external(gt_clips_u8: Sequence[torch.Tensor], gen_clips_u8: Sequence[torch.Tensor], i3d, frames: int = 17,
+                 sampling: str = "center") -> dict:
+    """evaluation/fvd_external.py from decoded clips: each a uint8 (T_i, H, W, 3) tensor of any length T_i >= frames
+    at the target resolution (decoding the videos with decord / ffmpeg and scaling them to --resolution is the
+    caller's job).  Applies load_videos's frame selection and assertion to every clip, stacks each side on the device,
+    and returns calculate_fvd(gt, gen, method="videogpt") from the bytes (i3d: fvd.load_fvd_model's network)."""
+    from .quality import calculate_fvd
+    sides = []
+    for name, clips in (("gt", gt_clips_u8), ("gen", gen_clips_u8)):
+        clips = list(clips)
+        if not clips:
+            raise ValueError(f"fvd_external: no {name} clips")
+        for c in clips:
+            _check_u8(c, (4,), f"fvd_external ({name})")
+        idx = [fvd_external_indices(int(c.shape[0]), frames, sampling) for c in clips]
+        sides.append(torch.stack([c[r.start:r.stop].to(i3d.device) for c, r in zip(clips, idx)]))
+    return calculate_fvd(sides[0], sides[1], i3d.device, method="videogpt", i3d=i3d)

@@ -256,6 +256,67 @@ fid_preprocess_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __re
   resample_clips_body<OUT_FID>(src, desc, tab, lut, out, 1, oh, ow, sel);
 }
 
+// omt_fvd_suite_preprocess: evaluation/common_metrics_on_video_quality's FVD preprocess (styleganv / videogpt
+// preprocess_single) from uint8 channels-last or fp32 channel-planar clips.  The same tile walk and bilinear arithmetic
+// as resample_clips_body, but the value of a source sample is read in one of three forms, and the result is
+// (y - 0.5) * 2 in two roundings.  desc.src counts elements of src (bytes or floats); the frames of a clip follow each
+// other, so a clip stored with a longer time axis is read as its first F frames.
+__device__ __forceinline__ float suite_u8_value(int b) { return __fdiv_rn((float)b, 255.f); }
+
+template <int FORM>
+__device__ __forceinline__ float suite_value(const void* __restrict__ src, long long frame, int C, int H, int W, int y,
+                                             int x, int c) {
+  if constexpr (FORM == OMT_FVDS_U8) {
+    return suite_u8_value(__ldg(static_cast<const uint8_t*>(src) + frame + ((long long)y * W + x) * 3 + c));
+  } else {
+    const float v = __ldg(static_cast<const float*>(src) + frame + ((long long)(C == 1 ? 0 : c) * H + y) * W + x);
+    if constexpr (FORM == OMT_FVDS_F32) return v;
+    // videogpt: (videos * 255).numpy().astype(np.uint8), then .float() / 255.  The cast truncates to int32 and keeps
+    // the low byte, as the x86-64 conversion does for products inside the int32 range.
+    return suite_u8_value(__float2int_rz(__fmul_rn(v, 255.f)) & 255);
+  }
+}
+
+template <int FORM>
+__global__ void __launch_bounds__(RC_TW)
+fvd_suite_preprocess_kernel(const void* __restrict__ src, const omt_clip_desc* __restrict__ desc,
+                            const int4* __restrict__ tab, int C, float* __restrict__ out, int F, int oh, int ow) {
+  pdl_sync();
+  const int b = blockIdx.z / F, f = blockIdx.z % F;
+  const omt_clip_desc d = desc[b];
+  const int ox = blockIdx.x * RC_TW + threadIdx.x;
+  if (ox >= ow) return;
+  const int4 ew = __ldg(tab + d.th / 4 + d.cx + ox);
+  const int x0 = d.x0 + ew.x, x1 = d.x0 + ew.y;
+  const float l0w = __int_as_float(ew.z), l1w = __int_as_float(ew.w);
+  const long long frame = d.src + (long long)f * (FORM == OMT_FVDS_U8 ? 3 : C) * d.H * d.W;
+  const int y_end = min(oh, (int)blockIdx.y * RC_TH + RC_TH);
+  for (int oy = blockIdx.y * RC_TH; oy < y_end; ++oy) {
+    const int4 eh = __ldg(tab + d.tv / 4 + d.cy + oy);
+    const float l0h = __int_as_float(eh.z), l1h = __int_as_float(eh.w);
+    const int r0 = d.y0 + eh.x, r1 = d.y0 + eh.y;
+    const float w00 = __fmul_rn(l0h, l0w), w01 = __fmul_rn(l0h, l1w), w10 = __fmul_rn(l1h, l0w), w11 = __fmul_rn(l1h, l1w);
+    float y[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float x00 = suite_value<FORM>(src, frame, C, d.H, d.W, r0, x0, c);
+      const float x01 = suite_value<FORM>(src, frame, C, d.H, d.W, r0, x1, c);
+      const float x10 = suite_value<FORM>(src, frame, C, d.H, d.W, r1, x0, c);
+      const float x11 = suite_value<FORM>(src, frame, C, d.H, d.W, r1, x1, c);
+      float v;
+      if (d.form) {
+        v = __fmaf_rn(x11, w11, __fmaf_rn(x10, w10, __fmaf_rn(x00, w00, __fmul_rn(x01, w01))));
+      } else {
+        const float t0 = __fmaf_rn(x00, l0w, __fmul_rn(x01, l1w));
+        const float t1 = __fmaf_rn(x10, l0w, __fmul_rn(x11, l1w));
+        v = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
+      }
+      y[c] = __fmul_rn(__fsub_rn(v, 0.5f), 2.f);
+    }
+    reinterpret_cast<float4*>(out)[((long long)blockIdx.z * oh + oy) * ow + ox] = make_float4(y[0], y[1], y[2], 0.f);
+  }
+}
+
 // One axis table of a clip: [n_out][4] entries at word `off` inside the table, every (i0, i1) inside an axis of n_in.
 bool clip_axis_ok(const int32_t* tab_host, long long tab_len, int off, int n_out, int n_in) {
   if (off < 0 || off % 4 != 0 || off + 4LL * n_out > tab_len) return false;
@@ -314,20 +375,21 @@ extern "C" int omt_resample_u8(const uint8_t* src, long long src_bytes, const om
   return OMT_OK;
 }
 
-// The checks both clip entry points make before their launch (`who` names the entry point in the message).
-static int check_clips(const char* who, const uint8_t* src, long long src_bytes, const omt_clip_desc* desc,
+// The checks the clip entry points make before their launch (`who` names the entry point in the message).  A frame
+// holds H W ch elements of src (src_bytes counts elements).
+static int check_clips(const char* who, const void* src, long long src_bytes, const omt_clip_desc* desc,
                        const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host, long long tab_len,
-                       const float* norm, int B, int F, int oh, int ow, float* out) {
-  OMT_REQUIRE(src && desc && desc_host && tab && tab_host && norm && out, "%s: null pointer", who);
+                       int B, int F, int oh, int ow, float* out, int ch = 3) {
+  OMT_REQUIRE(src && desc && desc_host && tab && tab_host && out, "%s: null pointer", who);
   OMT_REQUIRE(B >= 1 && F >= 1 && (long long)B * F <= 65535 && oh >= 1 && ow >= 1 && src_bytes >= 0 && tab_len >= 0,
               "%s: B=%d, F=%d, output %dx%d, src_bytes=%lld, tab_len=%lld", who, B, F, oh, ow, src_bytes, tab_len);
   for (int b = 0; b < B; ++b) {
     const omt_clip_desc& d = desc_host[b];
     OMT_REQUIRE(d.H >= 1 && d.W >= 1 && d.wh >= 1 && d.ww >= 1 && d.rh >= 1 && d.rw >= 1,
                 "%s: clip %d: source %dx%d, window %dx%d, resized %dx%d", who, b, d.H, d.W, d.wh, d.ww, d.rh, d.rw);
-    OMT_REQUIRE(d.src >= 0 && d.src + (long long)F * d.H * d.W * 3 <= src_bytes,
+    OMT_REQUIRE(d.src >= 0 && d.src + (long long)F * d.H * d.W * ch <= src_bytes,
                 "%s: clip %d: bytes [%lld, +%lld) outside the %lld source bytes", who, b, d.src,
-                (long long)F * d.H * d.W * 3, src_bytes);
+                (long long)F * d.H * d.W * ch, src_bytes);
     OMT_REQUIRE(d.y0 >= 0 && d.x0 >= 0 && (long long)d.y0 + d.wh <= d.H && (long long)d.x0 + d.ww <= d.W,
                 "%s: clip %d: window %dx%d at (%d, %d) outside the %dx%d frame", who, b, d.wh, d.ww, d.y0, d.x0, d.H, d.W);
     OMT_REQUIRE(d.cy >= 0 && d.cx >= 0 && (long long)d.cy + oh <= d.rh && (long long)d.cx + ow <= d.rw,
@@ -349,7 +411,8 @@ extern "C" int omt_resample_clips(const uint8_t* src, long long src_bytes, const
   OMT_ENTER();
   OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab}) && aligned_to(4, {norm, out}),
               "omt_resample_clips: desc must be 8-byte, tab 16-byte and norm / out 4-byte aligned");
-  int rc = check_clips("omt_resample_clips", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, norm, B, F, oh, ow, out);
+  OMT_REQUIRE(norm, "omt_resample_clips: null pointer");
+  int rc = check_clips("omt_resample_clips", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, out);
   if (rc != OMT_OK) return rc;
   dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
   OMT_CUDA(launch_k(resample_clips_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
@@ -366,7 +429,8 @@ extern "C" int omt_fvd_preprocess(const uint8_t* src, long long src_bytes, const
   OMT_REQUIRE(aligned_to(4, {sel}), "omt_fvd_preprocess: sel must be 4-byte aligned");
   OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && aligned_to(4, {lut}),
               "omt_fvd_preprocess: desc must be 8-byte, tab / out 16-byte and lut 4-byte aligned");
-  int rc = check_clips("omt_fvd_preprocess", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, lut, B, F, oh, ow, out);
+  OMT_REQUIRE(lut, "omt_fvd_preprocess: null pointer");
+  int rc = check_clips("omt_fvd_preprocess", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, out);
   if (rc != OMT_OK) return rc;
   dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
   OMT_CUDA(launch_k(fvd_preprocess_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
@@ -383,11 +447,45 @@ extern "C" int omt_fid_preprocess(const uint8_t* src, long long src_bytes, const
   OMT_REQUIRE(aligned_to(4, {sel}), "omt_fid_preprocess: sel must be 4-byte aligned");
   OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && aligned_to(4, {lut}),
               "omt_fid_preprocess: desc must be 8-byte, tab / out 16-byte and lut 4-byte aligned");
-  int rc = check_clips("omt_fid_preprocess", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, lut, B, 1, oh, ow, out);
+  OMT_REQUIRE(lut, "omt_fid_preprocess: null pointer");
+  int rc = check_clips("omt_fid_preprocess", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, B, 1, oh, ow, out);
   if (rc != OMT_OK) return rc;
   dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B);
   OMT_CUDA(launch_k(fid_preprocess_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
                     reinterpret_cast<const int4*>(tab), lut, sel, out, oh, ow));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_fvd_suite_preprocess(const void* src, long long src_elems, int form, int C,
+                                        const omt_clip_desc* desc, const omt_clip_desc* desc_host, const int32_t* tab,
+                                        const int32_t* tab_host, long long tab_len, int B, int F, int oh, int ow,
+                                        float* out, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(form == OMT_FVDS_U8 || form == OMT_FVDS_F32 || form == OMT_FVDS_F32_TRUNC,
+              "omt_fvd_suite_preprocess: unknown input form %d", form);
+  OMT_REQUIRE(form == OMT_FVDS_U8 ? C == 3 : (C == 1 || C == 3),
+              "omt_fvd_suite_preprocess: C=%d (uint8 clips have 3 channels, fp32 clips 1 or 3)", C);
+  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && (form == OMT_FVDS_U8 || aligned_to(4, {src})),
+              "omt_fvd_suite_preprocess: desc must be 8-byte, tab / out 16-byte and fp32 src 4-byte aligned");
+  int rc = check_clips("omt_fvd_suite_preprocess", src, src_elems, desc, desc_host, tab, tab_host, tab_len, B, F, oh,
+                       ow, out, form == OMT_FVDS_U8 ? 3 : C);
+  if (rc != OMT_OK) return rc;
+  for (int b = 0; b < B; ++b) {
+    const omt_clip_desc& d = desc_host[b];
+    OMT_REQUIRE(!d.flip && d.y0 == 0 && d.x0 == 0 && d.wh == d.H && d.ww == d.W,
+                "omt_fvd_suite_preprocess: clip %d: the suite's preprocess has no flip and no window", b);
+  }
+  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
+  const int4* t4 = reinterpret_cast<const int4*>(tab);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (form == OMT_FVDS_U8)
+    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_U8>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F, oh, ow));
+  else if (form == OMT_FVDS_F32)
+    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_F32>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F, oh, ow));
+  else
+    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_F32_TRUNC>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F,
+                      oh, ow));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

@@ -4,12 +4,18 @@
 Drop-in names for vqgan_eval.py:18 (`from OmniTokenizer.fvd.fvd import load_fvd_model, frechet_distance,
 get_fvd_logits`): load_fvd_model(device, path), get_fvd_logits(videos, i3d, device), frechet_distance(x1, x2).
 
+The same network also runs evaluation/common_metrics_on_video_quality's StyleGAN-V I3D (fvd/styleganv's
+i3d_torchscript.pt, load_i3d_styleganv): the same topology and widths with its own key names, BatchNorm eps 1e-3 and
+fixed F.pad tables that equal SAME padding at 224 x 224 (checked per clip length, check_styleganv_pads).  I3D.features
+runs either network on one side of quality.calculate_fvd: omt_fvd_suite_preprocess, then the network's CUDA graph.
+
 Activations are channels-last fp32 [B][T][H][W][Cs], Cs the channel count rounded up to a multiple of 32 (4 for the
 network input); the pad columns are zero.  Every Unit3D is one omt_conv3d launch (3xTF32, BatchNorm folded into the
 weights at pack time), and each Inception branch writes its slice of the block's concat buffer in place.
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, List, Optional, Tuple
 
 import numpy as np
@@ -21,6 +27,9 @@ from .engine import CLIP_DESC_WORDS, run_graphed
 
 TARGET_RESOLUTION = (224, 224)
 BN_EPS = 1e-5            # pytorch_i3d.py:91
+VARIANT_EPS = {"videogpt": BN_EPS,      # fvd/videogpt/pytorch_i3d.py: the network of OmniTokenizer/fvd
+               "styleganv": 1e-3}       # i3d_torchscript.pt: batch_norm(..., 0.1, 0.001)
+SUITE_CHUNK_FRAMES = 256  # clip frames per feature launch sequence of I3D.features (about 7 MB of activations each)
 
 # pytorch_i3d.py:247-328: (endpoint, kind, spec); unit: (cin, cout, kernel, stride); pool: (kernel, stride);
 # mixed: (cin, branch widths b0, b1a, b1b, b2a, b2b, b3b)
@@ -91,10 +100,10 @@ def expected_keys(num_classes: int = 400) -> Dict[str, tuple]:
     return keys
 
 
-def fold_bn(w: torch.Tensor, gamma, beta, mean, var) -> Tuple[torch.Tensor, torch.Tensor]:
-    """BatchNorm (running statistics, eps 1e-5) folded into a conv weight (cout, cin, k, k, k), in float64:
-    (W s, beta - mean s) with s = gamma / sqrt(var + eps), rounded to fp32."""
-    s = gamma.double() / torch.sqrt(var.double() + BN_EPS)
+def fold_bn(w: torch.Tensor, gamma, beta, mean, var, eps: float = BN_EPS) -> Tuple[torch.Tensor, torch.Tensor]:
+    """BatchNorm (running statistics, eps 1e-5 unless given) folded into a conv weight (cout, cin, k, k, k), in
+    float64: (W s, beta - mean s) with s = gamma / sqrt(var + eps), rounded to fp32."""
+    s = gamma.double() / torch.sqrt(var.double() + eps)
     return (w.double() * s.view(-1, 1, 1, 1, 1)).float(), (beta.double() - mean.double() * s).float()
 
 
@@ -123,14 +132,32 @@ class _Unit:
 class _Workspace:
     """Buffers, launch list and CUDA graph state of one (B, T, H, W)."""
 
-    def __init__(self, net: "I3D", B: int, T: int, H: int, W: int, real_norm: Optional[L.U8Norm] = None):
+    def __init__(self, net: "I3D", B: int, T: int, H: Optional[int], W: Optional[int],
+                 real_norm: Optional[L.U8Norm] = None):
+        """H = W = None: the network alone; the caller writes the input self.x (I3D.features)."""
         dev = net.device
         self.graphs = {}
+        oh, ow = TARGET_RESOLUTION
+        if net.variant == "styleganv":
+            check_styleganv_pads(T)
+        self.ops = []
+        f = dict(device=dev, dtype=torch.float32)
+
+        def act(T_, H_, W_, c):
+            return torch.zeros(B, T_, H_, W_, cpad(c), **f)       # pad columns stay zero: no kernel writes them
+
+        x = self.x = act(T, oh, ow, 3)
+        self.out = torch.empty(B, net.num_classes, device=dev)
+        if H is not None:
+            self._preprocess(net, B, T, H, W, real_norm, x)
+        self._network(net, B, T, x, act)
+
+    def _preprocess(self, net: "I3D", B: int, T: int, H: int, W: int, real_norm: Optional[L.U8Norm], x):
+        dev = net.device
         self.u8 = torch.empty(B, T, H, W, 3, dtype=torch.uint8, device=dev)
         # byte -> value table: float(byte), or the real-byte map of real_norm, picked per clip with VideoNorm's test
         self.lut = net.byte_lut if real_norm is None else real_byte_table(real_norm).float().to(dev)
         self.sel = torch.empty(B, dtype=torch.int32, device=dev) if real_norm is not None and real_norm.max_test else None
-        self.out = torch.empty(B, net.num_classes, device=dev)
         # preprocess tables (fvd.py:24: F.interpolate to 224 x 224 from the multi-threaded script: the separable kernel)
         oh, ow = TARGET_RESOLUTION
         tv = L.clip_axis_table(H, oh, float(np.float32(H) / np.float32(oh))).reshape(-1)
@@ -141,19 +168,14 @@ class _Workspace:
         desc[:, 2:] = torch.tensor([H, W, 0, 0, H, W, oh, ow, 0, 0, 0, 0, tv.size, L.INTERP_SEPARABLE], dtype=torch.int32)
         self.desc_host = desc
         self.desc, self.tab = desc.to(dev), self.tab_host.to(dev)
-        self.ops = []
-        f = dict(device=dev, dtype=torch.float32)
-
-        def act(T_, H_, W_, c):
-            return torch.zeros(B, T_, H_, W_, cpad(c), **f)       # pad columns stay zero: no kernel writes them
-
-        x = act(T, oh, ow, 3)
-        shape = (T, oh, ow)
         if self.sel is not None:
             self.ops.append(lambda: _cabi.call("omt_u8_norm_select", self.u8, B, T * H * W * 3, self.sel))
         self.ops.append(lambda x=x: _cabi.call(
             "omt_fvd_preprocess", self.u8, self.u8.numel(), self.desc, self.desc_host, self.tab, self.tab_host,
             self.tab_host.numel(), self.lut, self.sel, B, T, oh, ow, x))
+
+    def _network(self, net: "I3D", B: int, T: int, x, act):
+        shape = (T,) + TARGET_RESOLUTION
         cur, c_cur = x, 3
         for name, kind, spec in ARCH:
             if kind == "unit":
@@ -211,9 +233,16 @@ class _Workspace:
 class I3D:
     """InceptionI3d (pytorch_i3d.py:163-365) in eval mode from a state_dict in the reference's layout
     (`Conv3d_1a_7x7.conv3d.weight`, `Mixed_4e.b1b.bn.running_var`, ..., `logits.conv3d.{weight,bias}`).  BatchNorm is
-    folded and the weights packed once, on `device`; every (B, T, H, W) gets its own buffers and CUDA graph."""
+    folded and the weights packed once, on `device`; every (B, T, H, W) gets its own buffers and CUDA graph.
+    variant: "videogpt" (this network, BatchNorm eps 1e-5) or "styleganv" (the StyleGAN-V I3D's weights mapped onto
+    these keys by styleganv_state_dict, eps 1e-3; see load_i3d_styleganv)."""
 
-    def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda"):
+    MAX_SUITE_WORKSPACES = 4
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", variant: str = "videogpt"):
+        if variant not in VARIANT_EPS:
+            raise ValueError(f"unknown I3D variant {variant!r}; expected one of {sorted(VARIANT_EPS)}")
+        self.variant = variant
         sd = {k: v for k, v in state_dict.items() if not k.endswith(".num_batches_tracked")}
         lw = sd.get("logits.conv3d.weight")
         self.num_classes = int(lw.shape[0]) if lw is not None and lw.dim() == 5 else 400
@@ -231,12 +260,14 @@ class I3D:
         self.units = {}
         for prefix, cin, cout, k, s in unit_names():
             w, b = fold_bn(sd[prefix + ".conv3d.weight"],
-                           *(sd[f"{prefix}.bn.{f}"] for f in ("weight", "bias", "running_mean", "running_var")))
+                           *(sd[f"{prefix}.bn.{f}"] for f in ("weight", "bias", "running_mean", "running_var")),
+                           eps=VARIANT_EPS[variant])
             self.units[prefix] = _Unit(*pack_weight(w), b, cout, k, s, self.device)
         self.head_w = sd["logits.conv3d.weight"].reshape(self.num_classes, 1024).contiguous().to(self.device)
         self.head_b = sd["logits.conv3d.bias"].contiguous().to(self.device)
         self.byte_lut = torch.arange(256, dtype=torch.float32).to(self.device)     # torch.FloatTensor(videos)
         self._ws = {}
+        self._suite_ws = {}
 
     @staticmethod
     def check_frames(frames: torch.Tensor):
@@ -256,6 +287,9 @@ class I3D:
         normalised clip, shift_dim((video + 0.5) * 255, 1, -1).byte() (real_byte_table, its branch picked per clip).
         The returned tensor is the workspace's static output: clone it before the next call of the same shape."""
         self.check_frames(frames_u8)
+        if self.variant != "videogpt":
+            raise ValueError(f"I3D.logits runs OmniTokenizer/fvd's preprocess and network; this is the {self.variant} "
+                             f"network (quality.calculate_fvd runs it)")
         if frames_u8.device != self.device:
             raise ValueError(f"I3D.logits: frames on {frames_u8.device}, the network is on {self.device}")
         if real_norm is not None:
@@ -268,6 +302,73 @@ class I3D:
         run_graphed(ws.graphs, self.device, "i3d", ws.run)
         return ws.out
 
+    def features(self, clips: "SuiteClips", t: int) -> torch.Tensor:
+        """The network's features (B, num_classes) fp32 on the device of the first t frames of every clip of one
+        calculate_fvd side, in chunks of at most SUITE_CHUNK_FRAMES frames: each chunk is one omt_fvd_suite_preprocess
+        launch reading the clips in place, then the (chunk, t) workspace's CUDA graph."""
+        if clips.src.device != self.device:
+            raise ValueError(f"I3D.features: clips on {clips.src.device}, the network is on {self.device}")
+        if not 1 <= t <= clips.T:
+            raise ValueError(f"I3D.features: prefix of {t} frames of {clips.T}-frame clips")
+        B = clips.B
+        out = torch.empty(B, self.num_classes, device=self.device)
+        chunk = max(1, min(B, SUITE_CHUNK_FRAMES // t))
+        oh, ow = TARGET_RESOLUTION
+        for b0 in range(0, B, chunk):
+            n = min(chunk, B - b0)
+            key = (n, t)
+            ws = self._suite_ws.get(key)
+            if ws is None:
+                while len(self._suite_ws) >= self.MAX_SUITE_WORKSPACES:
+                    self._suite_ws.pop(next(iter(self._suite_ws)))
+                ws = self._suite_ws[key] = _Workspace(self, n, t, None, None)
+            _cabi.call("omt_fvd_suite_preprocess", clips.src, clips.src.numel(), clips.form, clips.C,
+                       clips.desc.data_ptr() + b0 * 4 * CLIP_DESC_WORDS, clips.desc_host[b0:], clips.tab, clips.tab_host,
+                       clips.tab_host.numel(), n, t, oh, ow, ws.x)
+            run_graphed(ws.graphs, self.device, "i3d", ws.run)
+            out[b0:b0 + n] = ws.out
+        return out
+
+
+FORM_U8, FORM_F32, FORM_F32_TRUNC = 0, 1, 2      # OMT_FVDS_U8 / OMT_FVDS_F32 / OMT_FVDS_F32_TRUNC
+
+
+def suite_geometry(H: int, W: int, resolution: int = 224) -> Tuple[int, int, int, int]:
+    """preprocess_single's resize and crop (fvd/styleganv/fvd.py:38-64, fvd/videogpt/fvd.py:21-49): the shorter side
+    scaled to `resolution` with the longer one's size ceil(n * resolution / min(H, W)) in Python's double, then the
+    centre crop at ((rh - resolution) // 2, (rw - resolution) // 2).  Returns (rh, rw, cy, cx)."""
+    scale = resolution / min(H, W)
+    rh, rw = (resolution, math.ceil(W * scale)) if H < W else (math.ceil(H * scale), resolution)
+    return rh, rw, (rh - resolution) // 2, (rw - resolution) // 2
+
+
+class SuiteClips:
+    """One side of quality.calculate_fvd on the device, read in place by omt_fvd_suite_preprocess: src is uint8
+    (B, T, H, W, 3) (form FORM_U8) or fp32 (B, T, C, H, W) (FORM_F32, FORM_F32_TRUNC), contiguous; the descriptors
+    point at each clip's first frame with the full T stride, so every prefix length reads the same buffer.  Both
+    methods' F.interpolate calls take torch's generic bilinear kernel (layout.INTERP_SEPARABLE): styleganv's
+    (C, t, H, W) view always, videogpt's contiguous (t, 3, H, W) batch whenever torch runs on more than one thread."""
+
+    def __init__(self, src: torch.Tensor, form: int):
+        self.src, self.form = src, form
+        if form == FORM_U8:
+            self.B, self.T, H, W, self.C = (int(v) for v in src.shape)
+            frame = H * W * 3
+        else:
+            self.B, self.T, self.C, H, W = (int(v) for v in src.shape)
+            frame = self.C * H * W
+        self.H, self.W = H, W
+        rh, rw, cy, cx = suite_geometry(H, W)
+        tv = L.clip_axis_table(H, rh, float(np.float32(H) / np.float32(rh))).reshape(-1)
+        th = L.clip_axis_table(W, rw, float(np.float32(W) / np.float32(rw))).reshape(-1)
+        self.tab_host = torch.from_numpy(np.concatenate([tv, th]).astype(np.int32))
+        desc = torch.zeros(self.B, CLIP_DESC_WORDS, dtype=torch.int32)
+        desc[:, :2] = (torch.arange(self.B, dtype=torch.int64) * (self.T * frame)).view(torch.int32).view(self.B, 2)
+        desc[:, 2:] = torch.tensor([H, W, 0, 0, H, W, rh, rw, cy, cx, 0, 0, tv.size, L.INTERP_SEPARABLE],
+                                   dtype=torch.int32)
+        self.desc_host = desc
+        self.desc, self.tab = desc.to(src.device), self.tab_host.to(src.device)
+
 
 def real_byte_table(norm: L.U8Norm) -> torch.Tensor:
     """uint8 [n_tab, 256]: the byte vqgan_eval.py feeds I3D for each loader byte u of a real clip,
@@ -277,6 +378,130 @@ def real_byte_table(norm: L.U8Norm) -> torch.Tensor:
     if not bool((tab == tab[:, :1]).all()):
         raise ValueError(f"normalisation {norm.name!r} differs per channel; the FVD byte map is one table per branch")
     return ((tab[:, 0] + 0.5) * 255).byte()
+
+
+# ------------------------------------------------------------------------------------------------ StyleGAN-V I3D
+# i3d_torchscript.pt's module names -> this network's
+_SGV_UNITS = {"conv3d_1a_7x7": "Conv3d_1a_7x7", "conv3d_2b_1x1": "Conv3d_2b_1x1", "conv3d_2c_3x3": "Conv3d_2c_3x3"}
+_SGV_BRANCHES = {"branch_0": "b0", "branch_1.0": "b1a", "branch_1.1": "b1b", "branch_2.0": "b2a", "branch_2.1": "b2b",
+                 "branch_3.1": "b3b"}
+_SGV_FIELDS = {"conv3d.weight": "conv3d.weight", "batch3d.weight": "bn.weight", "batch3d.bias": "bn.bias",
+               "batch3d.running_mean": "bn.running_mean", "batch3d.running_var": "bn.running_var",
+               "batch3d.num_batches_tracked": "bn.num_batches_tracked"}
+
+# The torchscript's F.pad tables of every strided layer and of the Inception pool branch, as F.pad's
+# (w front, w back, h front, h back, t front, t back): pads[0] when T % stride_t == 0, pads[1] when it is 1.  They are
+# fixed for a 224 x 224 input.  Its stride-1 convs pad k // 2 on every side inside conv3d; its max pools run with
+# ceil_mode=True after the zero F.pad.
+STYLEGANV_PADS = {
+    "Conv3d_1a_7x7": ((7, 7, 7), (2, 2, 2), ((2, 3, 2, 3, 2, 3), (2, 3, 2, 3, 3, 3))),
+    "MaxPool3d_2a_3x3": ((1, 3, 3), (1, 2, 2), ((0, 1, 0, 1, 0, 0), None)),
+    "MaxPool3d_3a_3x3": ((1, 3, 3), (1, 2, 2), ((0, 1, 0, 1, 0, 0), None)),
+    "MaxPool3d_4a_3x3": ((3, 3, 3), (2, 2, 2), ((0, 1, 0, 1, 0, 1), (0, 1, 0, 1, 1, 1))),
+    "MaxPool3d_5a_2x2": ((2, 2, 2), (2, 2, 2), ((0, 0, 0, 0, 0, 0), (0, 0, 0, 0, 0, 1))),
+    "branch_3.0": ((3, 3, 3), (1, 1, 1), ((1, 1, 1, 1, 1, 1), None)),
+}
+
+
+def styleganv_key(key: str) -> str:
+    """One i3d_torchscript.pt state_dict key in this network's layout (KeyError for a key the network does not have)."""
+    if key.startswith("conv3d_0c_1x1.conv3d."):
+        return "logits.conv3d." + key[len("conv3d_0c_1x1.conv3d."):]
+    head, _, rest = key.partition(".")
+    if head in _SGV_UNITS and rest in _SGV_FIELDS:
+        return f"{_SGV_UNITS[head]}.{_SGV_FIELDS[rest]}"
+    if head.startswith("mixed_"):
+        for b, name in _SGV_BRANCHES.items():
+            if rest.startswith(b + ".") and rest[len(b) + 1:] in _SGV_FIELDS:
+                return f"Mixed_{head[len('mixed_'):]}.{name}.{_SGV_FIELDS[rest[len(b) + 1:]]}"
+    raise KeyError(f"StyleGAN-V I3D state_dict: unexpected key {key}")
+
+
+def styleganv_state_dict(state_dict: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """i3d_torchscript.pt's state_dict (`conv3d_1a_7x7.batch3d.running_var`, `mixed_4e.branch_1.1.conv3d.weight`,
+    `conv3d_0c_1x1.conv3d.bias`, ...) under this network's keys."""
+    return {styleganv_key(k): v for k, v in state_dict.items()}
+
+
+def _scripted_pads(module) -> Dict[str, tuple]:
+    """The F.pad tables of a loaded i3d_torchscript.pt, in STYLEGANV_PADS's layout."""
+    names = {"Conv3d_1a_7x7": "conv3d_1a_7x7", "MaxPool3d_2a_3x3": "maxPool3d_2a_3x3",
+             "MaxPool3d_3a_3x3": "maxPool3d_3a_3x3", "MaxPool3d_4a_3x3": "maxPool3d_4a_3x3",
+             "MaxPool3d_5a_2x2": "maxPool3d_5a_2x2"}
+    mods = [(k, getattr(module, v)) for k, v in names.items()]
+    mods += [("branch_3.0", getattr(getattr(module, name.lower()).branch_3, "0")) for name, kind, _ in ARCH
+             if kind == "mixed"]
+    out = {}
+    for k, m in mods:
+        tabs = [getattr(getattr(m.pads, i), "padding", None) for i in ("0", "1")]
+        tabs = tuple(tuple(int(v) for v in p) if p is not None else None for p in tabs)
+        if out.setdefault(k, tabs) != tabs:
+            raise ValueError(f"StyleGAN-V I3D: the Inception pool branches differ in their pad tables ({tabs})")
+    return out
+
+
+def check_styleganv_pads(T: int, H: int = 224, W: int = 224, pads: Optional[Dict[str, tuple]] = None):
+    """pads: {layer: (pads[0], pads[1])} to check instead of STYLEGANV_PADS's tables (e.g. a loaded torchscript's).
+
+    The StyleGAN-V I3D on a (T, H, W) input computes what omt_conv3d / omt_maxpool3d compute with SAME padding
+    (same_geometry): at every strided layer and Inception pool branch, the F.pad table the torchscript picks for the
+    layer's input length equals SAME's front / back padding, ceil_mode adds no window ((n + pad - k) % s == 0 on every
+    axis), and the zero padding of a max pool reads post-ReLU values (>= 0), so it never wins where SAME's does not.
+    Raises ValueError naming the first layer that differs."""
+    pads = {k: v[2] for k, v in STYLEGANV_PADS.items()} if pads is None else pads
+    shape = (T, H, W)
+
+    def check(name, dims):
+        k, s, _ = STYLEGANV_PADS[name]
+        tabs = pads[name]
+        r = dims[0] % s[0]
+        tab = tabs[r] if r < 2 else None
+        if tab is None:
+            raise ValueError(f"StyleGAN-V I3D {name}: no pad table for T % {s[0]} == {r}")
+        fb = [(tab[4], tab[5]), (tab[2], tab[3]), (tab[0], tab[1])]
+        front, out = same_geometry(k, s, dims)
+        for ax, (kk, ss, n) in enumerate(zip(k, s, dims)):
+            p = compute_pad(kk, ss, n)
+            if fb[ax] != (front[ax], p - front[ax]) or (n + p - kk) % ss:
+                raise ValueError(f"StyleGAN-V I3D {name} at input {tuple(dims)}: F.pad {tab} is not SAME padding "
+                                 f"{front} / {p} on axis {ax} or ceil_mode adds a window")
+        return out
+
+    for name, kind, spec in ARCH:
+        if kind == "unit":
+            if name in STYLEGANV_PADS:
+                shape = check(name, shape)
+            else:
+                shape = same_geometry((spec[2],) * 3, (spec[3],) * 3, shape)[1]
+        elif kind == "pool":
+            shape = check(name, shape)
+        else:
+            check("branch_3.0", shape)
+    if shape[1:] != (7, 7) or shape[0] < 2:
+        raise ValueError(f"the I3D head needs [>= 2, 7, 7] features, got {shape} for a {T} x {H} x {W} input")
+
+
+def load_i3d_styleganv(device, path) -> I3D:
+    """The StyleGAN-V I3D of evaluation/common_metrics_on_video_quality/fvd/styleganv (load_i3d_pretrained) from
+    `path`: its i3d_torchscript.pt (read with torch.jit.load; its pad tables are checked against STYLEGANV_PADS), a
+    plain state_dict file in either key layout, or a state_dict.  Nothing is downloaded."""
+    if isinstance(path, dict):
+        sd = path
+    else:
+        try:
+            module = torch.jit.load(path, map_location="cpu")
+        except (RuntimeError, ValueError):
+            module = None
+        if module is not None:
+            scripted = _scripted_pads(module)
+            if scripted != {k: v[2] for k, v in STYLEGANV_PADS.items()}:
+                raise ValueError(f"{path}: pad tables {scripted} are not the StyleGAN-V I3D's")
+            sd = module.state_dict()
+        else:
+            sd = torch.load(path, map_location="cpu")
+    if any(k.startswith(("conv3d_", "mixed_")) for k in sd):
+        sd = styleganv_state_dict(sd)
+    return I3D(sd, device, variant="styleganv")
 
 
 def load_fvd_model(device, path: str) -> I3D:

@@ -7,7 +7,9 @@ trunk on csrc/i3d.cu's omt_conv3d (3x3, pad 1, ReLU, 3xTF32) and omt_pool2d (2 x
   uint8 (B, T, H, W, 3) frames;
 - drop-ins with the suite's signatures and result dicts: calculate_psnr, calculate_ssim (videos (B, T, C, H, W) in
   [0, 1]) and calculate_lpips_vgg (the VGG LPIPS; the suite's calculate_lpips means AlexNet, spatial=True, which is not
-  built here).
+  built here);
+- calculate_fvd(videos1, videos2, device, method, i3d): the suite's FVD at every prefix length, styleganv or videogpt,
+  on fvd.I3D.features (csrc/resample.cu's omt_fvd_suite_preprocess and the I3D kernels).
 
 Activations are channels-last fp32 [2P][h][w][C] (the network input [2P][H][W][4]); pair p is images p (real) and
 p + P (reconstruction).  Each VGG tap's LPIPS head runs right after the tap's conv, so only two ping-pong activation
@@ -26,7 +28,9 @@ from . import _cabi
 from . import layout as L
 from .engine import run_graphed
 from .fid import byte_lut
-from .fvd import pack_weight, real_byte_table
+from .fvd import FORM_F32 as FORM_FVD_F32, FORM_F32_TRUNC as FORM_FVD_F32_TRUNC, FORM_U8 as FORM_FVD_U8
+from .fvd import I3D, SuiteClips, pack_weight, real_byte_table
+from .fvd import frechet_distance as fvd_frechet_distance
 
 FORM_U8, FORM_F32 = 0, 1           # OMT_Q_U8 / OMT_Q_F32
 POOL_MAX = 0                       # omt_pool2d mode
@@ -423,3 +427,108 @@ def calculate_lpips_vgg(videos1, videos2, model: LPIPS) -> dict:
     a, b, (B, T), setting = _videos_f32(videos1, videos2, "calculate_lpips_vgg", True, model.device)
     _, _, lp = _run(a, b, FORM_F32, model, None, None)
     return result_dict(lp.view(B, T).cpu().numpy(), setting)
+
+
+# ------------------------------------------------------------------------------------------------ calculate_fvd
+FVD_METHODS = ("styleganv", "videogpt")
+FVD_MIN_FRAMES = 10                # calculate_fvd.py:43: the first prefix length
+
+
+def sqrtm_disp(a: np.ndarray, disp: bool = False):
+    """scipy.linalg.sqrtm(a, disp=False) -> (root, error estimate) on every scipy: from 1.16 sqrtm takes no disp and
+    returns the root alone (the estimate is then None)."""
+    from scipy.linalg import sqrtm
+    try:
+        return sqrtm(a, disp=False)
+    except TypeError:
+        return sqrtm(a), None
+
+
+def frechet_distance_styleganv(feats_fake: np.ndarray, feats_real: np.ndarray) -> float:
+    """fvd/styleganv/fvd.py:75-90: numpy means and np.cov, scipy.linalg.sqrtm of the product, the real part; the mean
+    term alone for one clip per side."""
+    mu_gen, sigma_gen = feats_fake.mean(axis=0), np.cov(feats_fake, rowvar=False)
+    mu_real, sigma_real = feats_real.mean(axis=0), np.cov(feats_real, rowvar=False)
+    m = np.square(mu_gen - mu_real).sum()
+    if feats_fake.shape[0] > 1:
+        s, _ = sqrtm_disp(np.dot(sigma_gen, sigma_real))
+        return float(np.real(m + np.trace(sigma_gen + sigma_real - s * 2)))
+    return float(np.real(m))
+
+
+def frechet_distance_videogpt(x1: torch.Tensor, x2: torch.Tensor) -> float:
+    """fvd/videogpt/fvd.py:113-125: OmniTokenizer/fvd's torch distance (fvd.frechet_distance), with the mean term
+    alone for one clip per side."""
+    if x1.shape[0] > 1:
+        return float(fvd_frechet_distance(x1, x2))
+    return float(torch.sum((x1.flatten(start_dim=1).mean(dim=0) - x2.flatten(start_dim=1).mean(dim=0)) ** 2))
+
+
+def _fvd_side(v, name: str):
+    """One side of calculate_fvd -> SuiteClips on the device (uploaded once), with the refusals."""
+    if not isinstance(v, torch.Tensor):
+        raise TypeError(f"calculate_fvd: {name} must be a torch tensor, got {type(v)}")
+    if v.dtype == torch.uint8:
+        if v.dim() != 5 or v.shape[-1] != 3:
+            raise ValueError(f"calculate_fvd: uint8 {name} must be (B, T, H, W, 3), got {tuple(v.shape)}")
+        form = FORM_FVD_U8
+    elif v.dtype == torch.float32:
+        if v.dim() != 5 or v.shape[2] not in (1, 3):
+            raise ValueError(f"calculate_fvd: fp32 {name} must be (B, T, C, H, W) with C 1 or 3, got {tuple(v.shape)}")
+        form = FORM_FVD_F32
+    else:
+        raise TypeError(f"calculate_fvd: {name} must be fp32 (B, T, C, H, W) in [0, 1] or uint8 (B, T, H, W, 3), "
+                        f"got {v.dtype}")
+    if min(v.shape) < 1:
+        raise ValueError(f"calculate_fvd: empty {name} {tuple(v.shape)}")
+    return v, form
+
+
+def _video_setting(v: torch.Tensor, form: int) -> torch.Size:
+    """calculate_fvd.trans's shape: (B, 3, T, H, W) (grey repeated to 3 channels)."""
+    if form == FORM_FVD_U8:
+        B, T, H, W, _ = v.shape
+    else:
+        B, T, _, H, W = v.shape
+    return torch.Size([B, 3, T, H, W])
+
+
+@torch.no_grad()
+def calculate_fvd(videos1, videos2, device="cuda", method: str = "styleganv", i3d=None) -> dict:
+    """calculate_fvd.py's calculate_fvd: the FVD between the first t frames of videos1 and of videos2 for every
+    t = 10 ... T (T: videos1's length; T < 10 gives an empty value and runs no network), with the suite's result dict.
+    videos: fp32 (B, T, C, H, W) in [0, 1] (C 1 or 3; host or device) or uint8 (B, T, H, W, 3) standing for byte / 255;
+    the two sides may differ in B and in H x W, and videos2 needs at least T frames.  uint8 clips and fp32 clips of
+    byte / 255 give the same features.
+    method: "styleganv" with i3d = fvd.load_i3d_styleganv(...), or "videogpt" (fvd_external.py's) with
+    i3d = fvd.load_fvd_model(device, "i3d_pretrained_400.pt").  videogpt rounds fp32 clips to bytes first, as its
+    preprocess does.  The features come to the host as float64 and the distance is the method's own host code."""
+    if method not in FVD_METHODS:
+        raise ValueError(f"calculate_fvd: unknown method {method!r}; expected one of {FVD_METHODS}")
+    if not isinstance(i3d, I3D):
+        raise TypeError(f"calculate_fvd needs the method's network as i3d= (fvd.load_i3d_styleganv or "
+                        f"fvd.load_fvd_model), got {type(i3d)}")
+    if i3d.variant != method:
+        raise ValueError(f"calculate_fvd: method {method!r} with the {i3d.variant} network")
+    if torch.device(device).type != "cuda":
+        raise ValueError(f"calculate_fvd runs on a CUDA device, got {device}")
+    sides = [_fvd_side(v, n) for v, n in ((videos1, "videos1"), (videos2, "videos2"))]
+    T1, T2 = int(sides[0][0].shape[1]), int(sides[1][0].shape[1])
+    if T2 < T1:
+        raise ValueError(f"calculate_fvd: videos2 has {T2} frames, fewer than videos1's {T1}")
+    result = {"value": {}, "video_setting": _video_setting(*sides[0]),
+              "video_setting_name": "batch_size, channel, time, heigth, width"}
+    if T1 < FVD_MIN_FRAMES:
+        return result
+    clips = []
+    for v, form in sides:
+        if form == FORM_FVD_F32 and method == "videogpt":
+            form = FORM_FVD_F32_TRUNC
+        clips.append(SuiteClips(v.to(i3d.device).contiguous(), form))
+    for t in range(FVD_MIN_FRAMES, T1 + 1):
+        f1, f2 = (i3d.features(c, t).double().cpu() for c in clips)
+        if method == "styleganv":
+            result["value"][t] = frechet_distance_styleganv(f1.numpy(), f2.numpy())
+        else:
+            result["value"][t] = frechet_distance_videogpt(f1, f2)
+    return result
