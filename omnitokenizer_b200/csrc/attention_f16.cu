@@ -333,29 +333,11 @@ attn_f16_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant_
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 static int encode2d(CUtensorMap* m, const uint16_t* base, int cols, long long rows, int ld) {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  if (fn == nullptr) { set_error("cuTensorMapEncodeTiled entry point not found"); return OMT_E_CUDA; }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
   cuuint32_t box[2] = {64, (cuuint32_t)KT};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<uint16_t*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return OMT_E_CUDA; }
-  return OMT_OK;
+  return encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, base, 2, dims, strides, box);
 }
 
 // Launch of either form: h1 takes the hi planes alone (the lo pointers are NULL and their maps never loaded).
@@ -386,20 +368,11 @@ static int launch(const char* who, const uint16_t* q_hi, const uint16_t* q_lo, i
     if ((rc = encode2d(&tmKl, k_lo, heads * D, rows, ldk))) return rc;
     if ((rc = encode2d(&tmVl, v_lo, heads * D, rows, ldv))) return rc;
   }
-  static int resident[64];     // CTAs of the kernel resident at once, per device (0: not queried yet)
-  int dev = 0;
-  OMT_CUDA(cudaGetDevice(&dev));
-  OMT_REQUIRE(dev >= 0 && dev < 64, "%s: device ordinal %d out of range", who, dev);
-  if (resident[dev] == 0) {
-    OMT_CUDA(cudaFuncSetAttribute(attn_f16_kernel<H1>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM));
-    int per_sm = 0, sms = 0;
-    OMT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attn_f16_kernel<H1>, THREADS, L::SMEM));
-    OMT_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    OMT_REQUIRE(per_sm > 0, "%s: no CTA fits on an SM of device %d", who, dev);
-    resident[dev] = per_sm * sms;
-  }
+  static KernelSetup setup;
+  int resident = 0;
+  if ((rc = setup.resident(attn_f16_kernel<H1>, THREADS, L::SMEM, &resident))) return rc;
   Args a{vinv, rows, o, o_hi, o_lo, ldo, N, heads, (int)items, scale * 1.4426950408889634f / qk_plane_scale};
-  const dim3 grid(items < resident[dev] ? (int)items : resident[dev]);
+  const dim3 grid(items < resident ? (int)items : resident);
   OMT_CUDA(launch_k(attn_f16_kernel<H1>, grid, dim3(THREADS), L::SMEM, stream, tmQh, tmQl, tmKh, tmKl, tmVh, tmVl, a));
   OMT_LAUNCH_CHECK();
   return OMT_OK;

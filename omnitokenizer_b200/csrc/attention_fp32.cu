@@ -269,15 +269,9 @@ int launch_attn_tc3(const float* q, int ldq, const float* k, int ldk, const floa
 int g_attn_kernel = 3;   // N % 128 == 0: 3 = wgmma 3xTF32 core (attention_tc3.cu); 1 = CUDA-core fp32
 
 static int set_flash_smem() {
-  static bool done[64];      // the attribute is per device
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !done[dev]) {
-    OMT_CUDA(cudaFuncSetAttribute(attn_flash_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
-    OMT_CUDA(cudaFuncSetAttribute(attn_flash_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 65536));
-    done[dev] = true;
-  }
-  return OMT_OK;
+  static KernelSetup plain, window;
+  const int rc = plain.smem(attn_flash_kernel<false>, 65536);
+  return rc != OMT_OK ? rc : window.smem(attn_flash_kernel<true>, 65536);
 }
 
 }  // namespace omt

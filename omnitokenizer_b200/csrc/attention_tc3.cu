@@ -197,29 +197,11 @@ attn_tc3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 static int encode2d(CUtensorMap* m, const float* base, int cols, long long rows, int ld, int box_rows) {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  if (fn == nullptr) { set_error("cuTensorMapEncodeTiled entry point not found"); return OMT_E_CUDA; }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
   cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return OMT_E_CUDA; }
-  return OMT_OK;
+  return encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, 2, dims, strides, box);
 }
 
 }  // namespace atc3
@@ -235,13 +217,8 @@ int launch_attn_tc3(const float* q, int ldq, const float* k, int ldk, const floa
   if (rc) return rc;
   rc = encode2d(&tmV, v, heads * D, rows, ldv, KT);
   if (rc) return rc;
-  static bool attr[64];      // the attribute is per device
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && !attr[dev]) {
-    OMT_CUDA(cudaFuncSetAttribute(attn_tc3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    attr[dev] = true;
-  }
+  static KernelSetup setup;
+  if ((rc = setup.smem(attn_tc3_kernel, SMEM))) return rc;
   Args a{o, ldo, o_hi, o_lo, N, scale * 1.4426950408889634f};
   dim3 grid(N / QT, heads, n_seq);
   OMT_CUDA(launch_k(attn_tc3_kernel, grid, dim3(THREADS), SMEM, st, tmQ, tmK, tmV, a));

@@ -114,7 +114,7 @@ int launch_gemm_fp32(const GemmArgs& g, int epilogue, cudaStream_t st) {
   return OMT_OK;
 }
 
-int launch_gemm_tc(const GemmArgs& g, const float* W_lo, int epilogue, int math, cudaStream_t st, const float* A2, int n_split);
+int launch_gemm_tc2(const GemmArgs& g, const float* W_lo, int epilogue, cudaStream_t st, const float* A2, int n_split);
 
 }  // namespace omt
 
@@ -146,7 +146,7 @@ static int linear_impl(const QkPrep* qk, const float* A, const float* A2, int n_
   if (math == OMT_MATH_FP32) return launch_gemm_fp32(g, epilogue == OMT_EPI_QKV ? OMT_EPI_NONE : epilogue, (cudaStream_t)stream);
   if (math == OMT_MATH_3XTF32) {
     OMT_REQUIRE(W_lo != nullptr, "omt_linear: 3xTF32 needs W_lo");
-    return launch_gemm_tc(g, W_lo, epilogue, math, (cudaStream_t)stream, A2, n_split);
+    return launch_gemm_tc2(g, W_lo, epilogue, (cudaStream_t)stream, A2, n_split);
   }
   OMT_REQUIRE(math != OMT_MATH_F16X3, "omt_linear: the f16x3 path takes operand planes (omt_linear_h)");
   set_error("omt_linear: unknown math mode %d", math);
@@ -161,8 +161,6 @@ extern "C" int omt_linear(const float* A, int lda, int a_seg, int a_seg_stride, 
                      M, N, K, bias, residual, ldr, epilogue, math, stream);
 }
 
-namespace omt { int tc_fuses_qkprep(int math); }   // gemm_tc2.cu: does the selected tensor-core kernel apply OMT_EPI_QKV itself?
-
 extern "C" int omt_linear2(const float* A1, const float* A2, int n_split, int lda, const float* W, const float* W_lo,
                            float* C, int ldc, int M, int N, int K, int math, const float* q_scale,
                            const float* k_scale, const float* rope_cos, const float* rope_sin, int qk_cols, int tokens,
@@ -174,7 +172,7 @@ extern "C" int omt_linear2(const float* A1, const float* A2, int n_split, int ld
               "omt_linear2: bad q/k preparation arguments");
   OMT_REQUIRE((rope_cos == nullptr) == (rope_sin == nullptr), "omt_linear2: cos/sin must both be given");
   QkPrep qk{q_scale, k_scale, rope_cos, rope_sin, qk_cols, tokens};
-  const bool fused = tc_fuses_qkprep(math);
+  const bool fused = math == OMT_MATH_3XTF32;   // the wgmma 3xTF32 kernel applies rope + l2norm + scale in its epilogue
   int rc = linear_impl(&qk, A1, A2, n_split, lda, 0, 0, 0, W, W_lo, C, ldc, 0, 0, 0, M, N, K, nullptr, nullptr, 0,
                        fused ? OMT_EPI_QKV : OMT_EPI_NONE, math, stream);
   if (rc != OMT_OK || fused) return rc;

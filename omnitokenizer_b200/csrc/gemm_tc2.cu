@@ -40,12 +40,4 @@ int launch_gemm_tc2(const GemmArgs& g, const float* W_lo, int epilogue, cudaStre
   return launch<true, 1, OMT_EPI_NONE>(maps, a, st);
 }
 
-// the wgmma 3xTF32 kernel applies OMT_EPI_QKV (rope + l2norm + scale) in its own epilogue
-int tc_fuses_qkprep(int math) { return math == OMT_MATH_3XTF32; }
-
-int launch_gemm_tc(const GemmArgs& g, const float* W_lo, int epilogue, int math, cudaStream_t st, const float* A2, int n_split) {
-  OMT_REQUIRE(math == OMT_MATH_3XTF32 && W_lo != nullptr, "omt_linear: the tensor-core fp32-operand path is 3xTF32 (needs W_lo)");
-  return launch_gemm_tc2(g, W_lo, epilogue, st, A2, n_split);
-}
-
 }  // namespace omt

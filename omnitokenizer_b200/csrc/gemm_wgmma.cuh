@@ -527,28 +527,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static inline int encode_map(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const cuuint64_t* dims,
-                             const cuuint64_t* strides, const cuuint32_t* box) {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  if (fn == nullptr) { set_error("cuTensorMapEncodeTiled entry point not found"); return OMT_E_CUDA; }
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(m, dt, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return OMT_E_CUDA; }
-  return OMT_OK;
-}
-
 // [K, seg, n_seg] map over a row-mapped matrix of 16-bit (esize 2) or fp32 (esize 4) elements, 128-byte x box_rows boxes
 static inline int row_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const void* ptr, int ld, int rows, int cols,
                           int seg, int seg_stride, int seg_off, int box_rows = 64) {
@@ -559,7 +537,7 @@ static inline int row_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, con
   cuuint64_t strides[2] = {(cuuint64_t)ld * esize, (cuuint64_t)sstride * ld * esize};
   cuuint32_t box[3] = {(cuuint32_t)(128 / esize), (cuuint32_t)box_rows, 1};
   const uint8_t* base = static_cast<const uint8_t*>(ptr) + (size_t)(seg > 0 ? seg_off : 0) * ld * esize;
-  return encode_map(m, dt, base, 3, dims, strides, box);
+  return encode_tiled(m, dt, base, 3, dims, strides, box);
 }
 
 // W [n_pad, K] (rows padded to a multiple of 128), 128-byte x 128-row boxes
@@ -567,7 +545,7 @@ static inline int w_map(CUtensorMap* m, CUtensorMapDataType dt, int esize, const
   cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)n_pad};
   cuuint64_t strides[1] = {(cuuint64_t)K * esize};
   cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)BN};
-  return encode_map(m, dt, ptr, 2, dims, strides, box);
+  return encode_tiled(m, dt, ptr, 2, dims, strides, box);
 }
 
 // maps: A, A_lo, A2, A2_lo, W_hi, W_lo, and for the plane-writing f16 epilogues the output planes hi, lo (row_map with
@@ -576,20 +554,12 @@ template <bool TF32, int NACC, int EPI, bool H1 = false>
 static int launch(const CUtensorMap* maps, const Args& g, cudaStream_t st) {
   auto kern = gemm_wgmma_kernel<TF32, NACC, EPI, H1>;
   constexpr int SMEM = smem_bytes<TF32, EPI, H1>();
-  static int resident[64];     // CTAs of this kernel resident at once, per device (0: not queried yet)
-  int dev = 0;
-  OMT_CUDA(cudaGetDevice(&dev));
-  OMT_REQUIRE(dev >= 0 && dev < 64, "wgmma GEMM: device ordinal %d out of range", dev);
-  if (resident[dev] == 0) {
-    OMT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    int per_sm = 0, sms = 0;
-    OMT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, THREADS, SMEM));
-    OMT_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    OMT_REQUIRE(per_sm > 0, "wgmma GEMM: no CTA fits on an SM of device %d", dev);
-    resident[dev] = per_sm * sms;
-  }
+  static KernelSetup setup;
+  int resident = 0;
+  const int rc = setup.resident(kern, THREADS, SMEM, &resident);
+  if (rc != OMT_OK) return rc;
   const int tiles = g.num_m_blk * ((g.N + BN - 1) / BN);
-  const dim3 grid(tiles < resident[dev] ? tiles : resident[dev]);
+  const dim3 grid(tiles < resident ? tiles : resident);
   const CUtensorMap& uh = tma_planes<TF32, EPI, H1>() ? maps[6] : maps[0];
   const CUtensorMap& ul = tma_planes<TF32, EPI, H1>() ? maps[7] : maps[0];
   OMT_CUDA(launch_k(kern, grid, dim3(THREADS), SMEM, st, maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], uh, ul, g));

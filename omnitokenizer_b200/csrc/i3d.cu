@@ -220,28 +220,18 @@ template <int BN>
 int launch_conv(const ConvArgs& g, const float* w_hi, const float* w_lo, cudaStream_t st) {
   auto kern = conv3d_kernel<BN>;
   constexpr int SMEM = smem_bytes<BN>();
-  static int resident[64];
-  int dev = 0;
-  OMT_CUDA(cudaGetDevice(&dev));
-  OMT_REQUIRE(dev >= 0 && dev < 64, "omt_conv3d: device ordinal %d out of range", dev);
-  if (resident[dev] == 0) {
-    OMT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    int per_sm = 0, sms = 0;
-    OMT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, THREADS, SMEM));
-    OMT_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    OMT_REQUIRE(per_sm > 0, "omt_conv3d: no CTA fits on an SM of device %d", dev);
-    resident[dev] = per_sm * sms;
-  }
+  static KernelSetup setup;
+  int resident = 0, rc;
+  if ((rc = setup.resident(kern, THREADS, SMEM, &resident))) return rc;
   const int n_pad = (g.N + 127) / 128 * 128;
   CUtensorMap maps[2];
   cuuint64_t dims[2] = {(cuuint64_t)g.K, (cuuint64_t)n_pad};
   cuuint64_t strides[1] = {(cuuint64_t)g.K * 4};
   cuuint32_t box[2] = {32, (cuuint32_t)BN};
-  int rc;
-  if ((rc = wgg::encode_map(&maps[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, w_hi, 2, dims, strides, box))) return rc;
-  if ((rc = wgg::encode_map(&maps[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, w_lo, 2, dims, strides, box))) return rc;
+  if ((rc = encode_tiled(&maps[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, w_hi, 2, dims, strides, box))) return rc;
+  if ((rc = encode_tiled(&maps[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, w_lo, 2, dims, strides, box))) return rc;
   const int tiles = ((g.M + BM - 1) / BM) * ((g.N + BN - 1) / BN);
-  const dim3 grid(tiles < resident[dev] ? tiles : resident[dev]);
+  const dim3 grid(tiles < resident ? tiles : resident);
   OMT_CUDA(launch_k(kern, grid, dim3(THREADS), SMEM, st, maps[0], maps[1], g));
   OMT_LAUNCH_CHECK();
   return OMT_OK;

@@ -1,17 +1,49 @@
 // Shared helpers for the omnitok_b200 kernels (sm_90a only).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
+#include <atomic>
 #include <initializer_list>
 #include "../../include/omnitok_b200.h"
 
 namespace omt {
 
+// ---- host runtime (runtime.cu) ------------------------------------------------------------------------------------------
+constexpr int MAX_DEVICES = 64;   // device ordinals the per-device caches cover
+
 void set_error(const char* fmt, ...);
-int check_device();   // OMT_OK when the current device is sm_90; caches per device
+// OMT_OK when the current device is sm_90 (properties cached per device); it then becomes this thread's launch device,
+// the one sm_count() and KernelSetup work on, until the next check.  Every entry point calls it first (OMT_ENTER).
+int check_device();
 int sm_count();
+
+// A tiled TMA map over `base` with 128-byte swizzle, 256-byte L2 promotion and no out-of-bounds fill; unit element strides.
+int encode_tiled(CUtensorMap* m, CUtensorMapDataType dt, const void* base, int rank, const cuuint64_t* dims,
+                 const cuuint64_t* strides, const cuuint32_t* box);
+
+// Launch setup of one kernel on each device, kept as a function-local static at its launcher (zero-initialised, so there
+// is no constructor to run).  A call that finds the device already set up is one atomic load; first-time setup and
+// growth take one library-wide lock and check again inside it.
+class KernelSetup {
+ public:
+  // Raise the kernel's dynamic shared-memory limit on the launch device to at least `bytes`.
+  template <typename K> int smem(K* kernel, size_t bytes) { return smem_impl(reinterpret_cast<const void*>(kernel), bytes); }
+  // The same, then *ctas = the CTAs of `threads` threads resident at once on the device (occupancy x SMs).  Counted on
+  // the first call per device, so a launcher passes the same `bytes` every time; a kernel no SM can hold is refused.
+  template <typename K> int resident(K* kernel, int threads, size_t bytes, int* ctas) {
+    return resident_impl(reinterpret_cast<const void*>(kernel), threads, bytes, ctas);
+  }
+
+ private:
+  int smem_impl(const void* kernel, size_t bytes);
+  int resident_impl(const void* kernel, int threads, size_t bytes, int* ctas);
+  int grow(const void* kernel, int dev, size_t bytes);   // with the lock held
+  std::atomic<int> smem_[MAX_DEVICES];   // the limit set on each device, 0 before the first call
+  std::atomic<int> ctas_[MAX_DEVICES];   // resident CTAs on each device, 0 before the first resident()
+};
 
 #define OMT_REQUIRE(cond, ...)                  \
   do {                                          \

@@ -239,15 +239,10 @@ extern "C" int omt_psnr_ssim(const void* a, const float* lut_a, const int32_t* s
                   aligned_to(8, {taps, sse, ssim}),
               "omt_psnr_ssim: misaligned pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  static bool attr_set[64];
-  int dev = 0;
-  OMT_CUDA(cudaGetDevice(&dev));
-  OMT_REQUIRE(dev >= 0 && dev < 64, "omt_psnr_ssim: device ordinal %d out of range", dev);
-  if (!attr_set[dev]) {
-    OMT_CUDA(cudaFuncSetAttribute(quality::psnr_ssim_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, quality::SS_SMEM));
-    OMT_CUDA(cudaFuncSetAttribute(quality::psnr_ssim_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, quality::SS_SMEM));
-    attr_set[dev] = true;
-  }
+  static KernelSetup setup_u8, setup_f32;
+  int rc;
+  if ((rc = setup_u8.smem(quality::psnr_ssim_kernel<false>, quality::SS_SMEM))) return rc;
+  if ((rc = setup_f32.smem(quality::psnr_ssim_kernel<true>, quality::SS_SMEM))) return rc;
   if (form == OMT_Q_F32)
     OMT_CUDA(launch_k(quality::psnr_ssim_kernel<true>, dim3(P), dim3(quality::SS_THREADS), quality::SS_SMEM, st, a, lut_a,
                       sel_a, b, lut_b, sel_b, H, W, taps, sse, ssim));

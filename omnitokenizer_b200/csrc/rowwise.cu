@@ -2,46 +2,10 @@
 // LayerNorm, patch gather+LN, un-patchify, PEG gather-stencil, rope+l2norm+scale.
 // All of them stream the canonical X[B][T'][N][C] buffer once with 16-byte accesses.
 #include "omt_common.cuh"
-#include <string.h>
 
 namespace omt {
 
-static thread_local char g_err[512] = "";
-
-void set_error(const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_err, sizeof(g_err), fmt, ap);
-  va_end(ap);
-}
-
 int g_peg_kernel = 4;   // omt_set_option("peg_kernel", 3|4): 4 = peg_tile4_kernel (cp.async gather + FFMA2, default), 3 = peg_tile_kernel
-int g_pdl = 0;   // programmatic dependent launch is opt-in (dependent CTAs hold SM resources during the tail)
-static int g_dev_ok[64];   // 0 unknown, 1 ok, -1 bad
-static int g_sms[64];
-
-int check_device() {
-  int dev = 0;
-  OMT_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64) { set_error("device ordinal %d out of range", dev); return OMT_E_ARG; }
-  if (g_dev_ok[dev] == 0) {
-    cudaDeviceProp p;
-    OMT_CUDA(cudaGetDeviceProperties(&p, dev));
-    g_sms[dev] = p.multiProcessorCount;
-    g_dev_ok[dev] = (p.major == 9 && p.minor == 0) ? 1 : -1;
-  }
-  if (g_dev_ok[dev] < 0) {
-    set_error("omnitok_b200 kernels are built for sm_90a (H100) only (no fallback path)");
-    return OMT_E_ARCH;
-  }
-  return OMT_OK;
-}
-
-int sm_count() {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  return (dev >= 0 && dev < 64 && g_sms[dev] > 0) ? g_sms[dev] : 148;
-}
 
 // ------------------------------------------------------------------------------------------
 // LayerNorm: one warp per row, whole row in registers (C <= 1024), two-pass statistics.
@@ -777,20 +741,6 @@ __global__ void __launch_bounds__(256) qk_prep_kernel(float* __restrict__ q, int
 
 using namespace omt;
 
-extern "C" int omt_abi_version(void) { return OMT_ABI_VERSION; }
-extern "C" const char* omt_last_error(void) { return omt::g_err; }
-
-extern "C" int omt_device_info(int* sms, int* major, int* minor) {
-  int dev = 0;
-  OMT_CUDA(cudaGetDevice(&dev));
-  cudaDeviceProp p;
-  OMT_CUDA(cudaGetDeviceProperties(&p, dev));
-  if (sms) *sms = p.multiProcessorCount;
-  if (major) *major = p.major;
-  if (minor) *minor = p.minor;
-  return OMT_OK;
-}
-
 static int layernorm_impl(const char* who, const float* x, int ldx, float* y, int ldy, const omt::LnPlanes& pl, const float* w,
                           const float* b, int M, int C, float eps, int seg, int seg_stride, int seg_off, omt_stream_t stream) {
   OMT_ENTER();
@@ -978,14 +928,10 @@ extern "C" int omt_peg(const float* x, float* y, const float* w27, const float* 
   OMT_REQUIRE(C % 4 == 0 && C / 4 <= 128, "omt_peg: C=%d unsupported (need C %% 4 == 0, C <= 512)", C);
   const long long M = (long long)B * rows_per_b;
   if (M == 0) return OMT_OK;
-  static bool attr_set[64];          // the attribute is per device
+  static KernelSetup setup;
+  const int rc = setup.smem(peg_kernel, 27 * 512 * 4);   // the widest row (C = 512) once
+  if (rc != OMT_OK) return rc;
   const size_t smem = (size_t)27 * C * sizeof(float);
-  int dev0 = 0;
-  cudaGetDevice(&dev0);
-  if (dev0 >= 0 && dev0 < 64 && !attr_set[dev0]) {
-    OMT_CUDA(cudaFuncSetAttribute(peg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 27 * 512 * 4));
-    attr_set[dev0] = true;
-  }
   const unsigned blocks = (unsigned)((M + PEG_ROWS - 1) / PEG_ROWS);
   peg_kernel<<<blocks, 128, smem, (cudaStream_t)stream>>>(x, y, w27, bias, nbr, rows_per_b, C, M);
   OMT_LAUNCH_CHECK();
@@ -1014,13 +960,9 @@ static int peg_volume_launch(const char* who, const float* x, float* y, const fl
   while (TT > 1 && (smem_of(TT, HB) > 112 * 1024 || TT * HB * 8 > 256)) --TT;
   const size_t smem = smem_of(TT, HB);
   OMT_REQUIRE(smem <= 200 * 1024, "%s: row of %d tokens does not fit the shared-memory tile", who, w);
-  static size_t smem_set[64];        // per device
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && smem > smem_set[dev]) {
-    OMT_CUDA(cudaFuncSetAttribute(peg_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    smem_set[dev] = smem;
-  }
+  static KernelSetup setup3, setup4;
+  int rc = setup3.smem(peg_tile_kernel, smem);
+  if (rc != OMT_OK) return rc;
   const int threads = ((TT * HB * 8 + 31) / 32) * 32;
   dim3 grid(((T + TT - 1) / TT) * ((h + HB - 1) / HB), C / PEG_CC, B);
   const bool fast_ok = T <= 64 && w <= 254;
@@ -1035,11 +977,7 @@ static int peg_volume_launch(const char* who, const float* x, float* y, const fl
     }
     const int zrow = vp * (HB + 2);
     const size_t smem4 = (size_t)(zrow + 1) * RS * sizeof(float);
-    static size_t smem4_set[64];
-    if (dev >= 0 && dev < 64 && smem4 > smem4_set[dev]) {
-      OMT_CUDA(cudaFuncSetAttribute(peg_tile4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4));
-      smem4_set[dev] = smem4;
-    }
+    if ((rc = setup4.smem(peg_tile4_kernel, smem4)) != OMT_OK) return rc;
     OMT_CUDA(launch_k(peg_tile4_kernel, grid, dim3(threads), smem4, (cudaStream_t)stream, x, y, w27, bias, T, h, w, C, temporal, causal, TT, HB, RS, zrow, t_off));
   } else {
     OMT_CUDA(launch_k(peg_tile_kernel, grid, dim3(threads), smem, (cudaStream_t)stream, x, y, w27, bias, T, h, w, C, temporal, causal, TT, HB, RS, t_off));
@@ -1078,33 +1016,4 @@ extern "C" int omt_qk_prep(float* q, int ldq, float* k, int ldk, const float* q_
                     rope_cos, rope_sin, M, N, heads));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
-}
-
-namespace omt { extern int g_attn_kernel; extern int g_f16_bn; extern int g_attn_f16_ctas; }
-
-extern "C" int omt_set_option(const char* name, int value) {
-  if (name == nullptr) return OMT_E_ARG;
-  if (strcmp(name, "pdl") == 0) { omt::g_pdl = value ? 1 : 0; return OMT_OK; }
-  if (strcmp(name, "peg_kernel") == 0) {
-    if (value != 3 && value != 4) { omt::set_error("peg_kernel must be 3 or 4"); return OMT_E_ARG; }
-    omt::g_peg_kernel = value;
-    return OMT_OK;
-  }
-  if (strcmp(name, "attn_kernel") == 0) {
-    if (value != 1 && value != 3) { omt::set_error("attn_kernel must be 1 or 3"); return OMT_E_ARG; }
-    omt::g_attn_kernel = value;
-    return OMT_OK;
-  }
-  if (strcmp(name, "f16_bn") == 0) {
-    if (value != 0 && value != 128 && value != 256) { omt::set_error("f16_bn must be 0, 128 or 256"); return OMT_E_ARG; }
-    omt::g_f16_bn = value;
-    return OMT_OK;
-  }
-  if (strcmp(name, "attn_f16_ctas") == 0) {
-    if (value != 1 && value != 2) { omt::set_error("attn_f16_ctas must be 1 or 2"); return OMT_E_ARG; }
-    omt::g_attn_f16_ctas = value;
-    return OMT_OK;
-  }
-  omt::set_error("unknown option %s", name);
-  return OMT_E_ARG;
 }

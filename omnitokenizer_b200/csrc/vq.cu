@@ -356,13 +356,9 @@ extern "C" int omt_pre_vq(const float* x, int ldx, const float* Wt, const float*
   if (cd == 8) {
     OMT_CUDA(launch_k(pre_vq_kernel<8>, dim3(blocks), dim3(256), smem, st, x, ldx, Wt, b, z, M, C, l2));
   } else {
-    static bool set16[64];           // per device
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < 64 && !set16[dev]) {
-      OMT_CUDA(cudaFuncSetAttribute(pre_vq_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * 1024 * 4));
-      set16[dev] = true;
-    }
+    static KernelSetup setup;
+    const int rc = setup.smem(pre_vq_kernel<16>, 16 * 1024 * 4);   // the widest row (C = 1024) once
+    if (rc != OMT_OK) return rc;
     OMT_CUDA(launch_k(pre_vq_kernel<16>, dim3(blocks), dim3(256), smem, st, x, ldx, Wt, b, z, M, C, l2));
   }
   OMT_LAUNCH_CHECK();
@@ -376,13 +372,9 @@ static int vq_launch_r(const float* x, int ldx, const float* Wt, const float* b,
   const size_t smem = vq_region0_bytes(per, PROJECT, C) + (size_t)R * VQF_THREADS * 32;
   OMT_REQUIRE(smem <= 200 * 1024, "omt_vq: n_codes=%d too large for the shared-memory table slice (C=%d, %d rows per thread)",
               n_codes, C, R);
-  static size_t set[64];
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 64 && smem > set[dev]) {
-    OMT_CUDA(cudaFuncSetAttribute(vq_fused_kernel<PROJECT, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    set[dev] = smem;
-  }
+  static KernelSetup setup;
+  const int rc = setup.smem(vq_fused_kernel<PROJECT, R>, smem);
+  if (rc != OMT_OK) return rc;
   const int rows = R * VQF_THREADS;
   const unsigned blocks = (unsigned)((M + rows - 1) / rows) * VQF_SLICES;
   OMT_CUDA(launch_k(vq_fused_kernel<PROJECT, R>, dim3(blocks), dim3(VQF_THREADS), smem, st, x, ldx, Wt, b, C, l2, z_in, z_out, E, e2,
