@@ -200,6 +200,15 @@ int omt_fvd_suite_preprocess(const void* src, long long src_elems, int form, int
                              const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
                              long long tab_len, int B, int F, int oh, int ow, float* out, omt_stream_t stream);
 
+/* The Inception Score's input (calculate_is.py's nn.Upsample(size=(299, 299), mode='bilinear') on the CPU, or no resize)
+ * of B clips of F frames: the kernel body, descriptors, axis tables and checks of omt_fvd_suite_preprocess in two of its
+ * forms, OMT_FVDS_U8 (uint8 (F, H, W, 3), v = (float)byte / 255) and OMT_FVDS_F32 (fp32 (F, 3, H, W), v as is), and
+ * out = y with no affine, written channels-last: out (B, F, oh, ow, 4) fp32, 16-byte aligned, channel 3 zero.  Axis
+ * tables whose entries are (i, i, 1.0, 0.0) copy the frame bit for bit (the network run at the input's own size). */
+int omt_is_preprocess(const void* src, long long src_elems, int form, const omt_clip_desc* desc,
+                      const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host, long long tab_len,
+                      int B, int F, int oh, int ow, float* out, omt_stream_t stream);
+
 /* Unit3D of the FVD I3D (fvd/pytorch_i3d.py:59-131) as an implicit GEMM in 3xTF32 on sm_90a wgmma:
  *   y[m, n] = act(sum_k A[m, k] W[n, k] + bias[n]),  m = ((b To + to) Ho + ho) Wo + wo,  n < N,  act = ReLU if relu
  *   A[m, (dt, dh, dw, c)] = x[b][to st - pt + dt][ho sh - ph + dh][wo sw - pw + dw][c], zero outside the volume
@@ -234,15 +243,18 @@ int omt_fid_preprocess(const uint8_t* src, long long src_bytes, const omt_clip_d
                        const int32_t* tab, const int32_t* tab_host, long long tab_len, const float* lut,
                        const int32_t* sel, int B, int oh, int ow, float* out, omt_stream_t stream);
 
-/* 2-D pooling of the FID InceptionV3 on channels-last fp32 [B][H][W][Cs] -> y, output pixel p = (b Ho + ho) Wo + wo,
+/* 2-D pooling of the FID and IS InceptionV3s on channels-last fp32 [B][H][W][Cs] -> y, output pixel p = (b Ho + ho) Wo + wo,
  * channel c < C at y[p * ldy + c] (C, Cs, ldy multiples of 4; x and y 16-byte aligned), so a pool branch writes its
  * slice of the concat buffer in place.  Window (kh, kw), stride (sh, sw), symmetric padding (ph, pw) <= half the window;
  * only taps inside the image take part, in (h, w) order, as torch's CPU kernels visit them:
  *   OMT_POOL_MAX: max_pool2d (the padding never wins; NaN propagates);
- *   OMT_POOL_AVG: avg_pool2d(count_include_pad=False): the fp32 sum, then one true division by the count of taps.
- * Both exact.  The global AdaptiveAvgPool2d(1) of an 8 x 8 map is OMT_POOL_AVG with an 8 x 8 window. */
+ *   OMT_POOL_AVG: avg_pool2d(count_include_pad=False): the fp32 sum, then one true division by the count of taps;
+ *   OMT_POOL_AVG_PAD: avg_pool2d(count_include_pad=True): the same sum, then one true division by torch's window size
+ *                     (min(h0 + kh, H + ph) - h0) (min(w0 + kw, W + pw) - w0), h0 = ho sh - ph, w0 = wo sw - pw.
+ * All exact.  The global AdaptiveAvgPool2d(1) of an h x w map is OMT_POOL_AVG with an h x w window. */
 #define OMT_POOL_MAX 0
 #define OMT_POOL_AVG 1
+#define OMT_POOL_AVG_PAD 2
 int omt_pool2d(const float* x, int Cs, int C, int B, int H, int W, int kh, int kw, int sh, int sw, int ph, int pw,
                int Ho, int Wo, float* y, int ldy, int mode, omt_stream_t stream);
 
@@ -280,6 +292,21 @@ int omt_lpips_input(const void* x, const float* lut, const int32_t* sel, const f
  * + ... + taps_out[tap][p], added in fp32 in that order (the earlier taps' launches must precede this one). */
 int omt_lpips_head(const float* x, int Cs, int C, int P, int h, int w, const float* lin_w, int tap, float* taps_out,
                    float* total, omt_stream_t stream);
+
+/* Row softmax of the Inception Score's classifier (calculate_is.py's F.softmax over dim 1), fp32: rows of N logits at
+ * x + r * ldx -> y + r * ldy, per row m = max, e_j = exp(x_j - m) (the difference and exp in fp64, rounded once to fp32),
+ * s = the fp32 sum of e in a fixed order, y_j = e_j / s (true division).  N >= 1, ldx, ldy >= N, 4-byte aligned. */
+int omt_softmax_rows(const float* x, int ldx, int rows, int N, float* y, int ldy, omt_stream_t stream);
+
+/* The split reduction of the Inception Score (calculate_is.py:44-55 with scipy.stats.entropy), in fp64 in a fixed order
+ * (no floating-point atomics: two runs give the same bits).  p: fp32 probabilities, rows of N at p + r * ldp; split k
+ * holds rows [k n, (k + 1) n).  Per split:
+ *   py[k][j]  = (sum over the split's rows of p[r][j]) / n                      (col_mean: fp64 [splits][N])
+ *   kl[k]     = mean over the split's rows of sum_j x_j log(x_j / y_j), x = p[r] / sum(p[r]), y = py[k] / sum(py[k]),
+ *               terms with x_j == 0 contributing 0                           (kl: fp64 [splits])
+ * The score of split k is exp(kl[k]); the host takes it, and the mean and standard deviation over the splits. */
+int omt_inception_score(const float* p, int ldp, int N, int n, int splits, double* col_mean, double* kl,
+                        omt_stream_t stream);
 
 /* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W). */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,

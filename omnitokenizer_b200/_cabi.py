@@ -63,6 +63,8 @@ SIGNATURES = {
                                    c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "omt_fvd_suite_preprocess": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "omt_is_preprocess": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
+                                  c_int, c_int, c_int, c_void_p, c_void_p]),
     "omt_conv3d": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]
                    + [c_int] * 13 + [c_void_p, c_int, c_int, c_void_p]),
     "omt_maxpool3d": (c_int, [c_void_p] + [c_int] * 17 + [c_void_p, c_void_p]),
@@ -73,6 +75,8 @@ SIGNATURES = {
     "omt_psnr_ssim": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_void_p] * 4),
     "omt_lpips_input": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_void_p, c_void_p]),
     "omt_lpips_head": (c_int, [c_void_p] + [c_int] * 5 + [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "omt_softmax_rows": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "omt_inception_score": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "omt_unpatchify": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_void_p]),
     "omt_unpatchify_u8": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float] * 5 + [c_void_p]),
     "omt_peg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

@@ -306,10 +306,11 @@ i3d_head_kernel(const float* __restrict__ x, int Cs, int C, int T, const float* 
   for (int n = tid; n < N; n += HEAD_THREADS) out[(size_t)b * N + n] = acc[n] / (float)(T - 1);
 }
 
-// 2-D pooling of the FID InceptionV3 (pytorch-fid inception.py) on channels-last fp32 [B][H][W][Cs]: one thread per 4
-// channels of an output pixel.  Only taps inside the image take part (max: padding never wins; average: the count
-// excludes it, count_include_pad=False), in (h, w) order as torch's CPU kernels visit them: max_pool2d's rule (maxval
-// from -inf, replaced when val > maxval or val is NaN); avg_pool2d's fp32 sum from 0, then one true division by the count.
+// 2-D pooling of the FID and IS InceptionV3s on channels-last fp32 [B][H][W][Cs]: one thread per 4 channels of an output
+// pixel.  Only taps inside the image take part, in (h, w) order as torch's CPU kernels visit them: max_pool2d's rule
+// (maxval from -inf, replaced when val > maxval or val is NaN; the padding never wins); avg_pool2d's fp32 sum from 0,
+// then one true division by the count of taps (avg 1, count_include_pad=False) or by torch's window size, the window
+// clipped to the padded image (avg 2, count_include_pad=True).
 // Output pixel p, channel c at y[p * ldy + c]: a pool branch writes its slice of the concat buffer in place.
 __global__ void __launch_bounds__(256)
 pool2d_kernel(const float4* __restrict__ x, float* __restrict__ y, int Cs4, int C4, int ldy, long long total, int H,
@@ -338,7 +339,8 @@ pool2d_kernel(const float4* __restrict__ x, float* __restrict__ y, int Cs4, int 
       }
     }
     if (avg) {
-      const float n = (float)((he - hs) * (we - ws));
+      const float n = avg == 2 ? (float)((min(h0 + kh, H + ph) - h0) * (min(w0 + kw, W + pw) - w0))
+                               : (float)((he - hs) * (we - ws));
 #pragma unroll
       for (int k = 0; k < 4; ++k) m[k] = __fdiv_rn(m[k], n);
     }
@@ -419,7 +421,8 @@ extern "C" int omt_pool2d(const float* x, int Cs, int C, int B, int H, int W, in
                           int pw, int Ho, int Wo, float* y, int ldy, int mode, omt_stream_t stream) {
   OMT_ENTER();
   OMT_REQUIRE(x && y, "omt_pool2d: null pointer");
-  OMT_REQUIRE(mode == OMT_POOL_MAX || mode == OMT_POOL_AVG, "omt_pool2d: mode %d is neither max (0) nor average (1)", mode);
+  OMT_REQUIRE(mode == OMT_POOL_MAX || mode == OMT_POOL_AVG || mode == OMT_POOL_AVG_PAD,
+              "omt_pool2d: mode %d is not max (0), average (1) or average counting the padding (2)", mode);
   OMT_REQUIRE(Cs % 4 == 0 && C >= 4 && C % 4 == 0 && C <= Cs && ldy >= C && ldy % 4 == 0,
               "omt_pool2d: C=%d channels of stride %d into rows of %d: all multiples of 4, C <= both", C, Cs, ldy);
   OMT_REQUIRE(B >= 1 && H >= 1 && W >= 1 && Ho >= 1 && Wo >= 1, "omt_pool2d: input %dx%dx%d, output %dx%d", B, H, W, Ho, Wo);
@@ -432,7 +435,7 @@ extern "C" int omt_pool2d(const float* x, int Cs, int C, int B, int H, int W, in
   const long long blocks = (total + 255) / 256;
   const int grid = (int)(blocks < 65536 ? blocks : 65536);
   OMT_CUDA(launch_k(i3d::pool2d_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, reinterpret_cast<const float4*>(x),
-                    y, Cs / 4, C / 4, ldy, total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, mode == OMT_POOL_AVG ? 1 : 0));
+                    y, Cs / 4, C / 4, ldy, total, H, W, Ho, Wo, kh, kw, sh, sw, ph, pw, mode));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

@@ -9,6 +9,9 @@
 //                    op order, into the [P][H][W][4] network input of omt_conv3d (channel 3 zero).
 //   omt_lpips_head   normalize_tensor of both images' features at one VGG tap, the squared difference, NetLinLayer's
 //                    1x1 conv and spatial_average: one CTA per pair, a warp per pixel.
+//   omt_softmax_rows  the Inception Score classifier's softmax: one CTA per row.
+//   omt_inception_score  the IS split reduction in fp64: the split's column means (a thread per column), then one CTA
+//                    per split, a warp per row, for the rows' KL divergences from the split's marginal.
 //
 // Every reduction has a fixed order (per-thread partials in a fixed visiting order, then a fixed tree over the block):
 // no floating-point atomics, so two runs give the same bits.
@@ -219,6 +222,103 @@ lpips_head_kernel(const float* __restrict__ x, int Cs, int C, int P, int hw, con
   }
 }
 
+// Fixed-order warp sum in fp64: the same butterfly in every lane, so every lane holds the same bits.
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// Row r of x -> row r of y: m = max, e = exp(x - m) in fp64 rounded to fp32 (a probability's error then does not grow
+// with its distance from the max), the fp32 sum of e (per-thread partials in column order, the warp butterfly, then the
+// warps in order), one true division per entry.
+constexpr int SM_THREADS = 256, SM_WARPS = SM_THREADS / 32;
+__global__ void __launch_bounds__(SM_THREADS, 1)
+softmax_rows_kernel(const float* __restrict__ x, int ldx, int N, float* __restrict__ y, int ldy) {
+  __shared__ float red[SM_WARPS];
+  pdl_sync();
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const float* xr = x + (size_t)blockIdx.x * ldx;
+  float* yr = y + (size_t)blockIdx.x * ldy;
+  float m = -INFINITY;
+  for (int j = tid; j < N; j += SM_THREADS) m = fmaxf(m, __ldg(xr + j));
+  m = warp_max(m);
+  if (lane == 0) red[warp] = m;
+  __syncthreads();
+  m = red[0];
+#pragma unroll
+  for (int i = 1; i < SM_WARPS; ++i) m = fmaxf(m, red[i]);
+  __syncthreads();
+  float s = 0.f;
+  for (int j = tid; j < N; j += SM_THREADS) {
+    const float e = (float)exp(__dsub_rn((double)__ldg(xr + j), (double)m));
+    yr[j] = e;
+    s = __fadd_rn(s, e);
+  }
+  s = warp_sum(s);
+  if (lane == 0) red[warp] = s;
+  __syncthreads();
+  s = red[0];
+#pragma unroll
+  for (int i = 1; i < SM_WARPS; ++i) s = __fadd_rn(s, red[i]);
+  for (int j = tid; j < N; j += SM_THREADS) yr[j] = __fdiv_rn(yr[j], s);
+}
+
+// py[k][j]: the fp64 sum of column j over split k's rows in row order, over n.
+__global__ void __launch_bounds__(256)
+is_col_mean_kernel(const float* __restrict__ p, int ldp, int N, int n, double* __restrict__ col_mean) {
+  pdl_sync();
+  const int k = blockIdx.y, j = blockIdx.x * 256 + threadIdx.x;
+  if (j >= N) return;
+  const float* pk = p + (size_t)k * n * ldp + j;
+  double s = 0.0;
+  for (int r = 0; r < n; ++r) s = __dadd_rn(s, (double)__ldg(pk + (size_t)r * ldp));
+  col_mean[(size_t)k * N + j] = __ddiv_rn(s, (double)n);
+}
+
+// One CTA per split: y = py / sum(py) in shared memory, then warp w takes rows w, w + KL_WARPS, ... in order; a row's
+// sum and its KL terms are lane partials in column order and the warp butterfly.  The warps' totals are added in order.
+constexpr int KL_THREADS = 512, KL_WARPS = KL_THREADS / 32;
+__global__ void __launch_bounds__(KL_THREADS)
+is_kl_kernel(const float* __restrict__ p, int ldp, int N, int n, const double* __restrict__ col_mean,
+             double* __restrict__ kl) {
+  extern __shared__ double q[];                 // [N]
+  __shared__ double red[KL_WARPS];
+  pdl_sync();
+  const int k = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const double* py = col_mean + (size_t)k * N;
+  double s = 0.0;
+  for (int j = tid; j < N; j += KL_THREADS) s = __dadd_rn(s, py[j]);
+  s = warp_sum_d(s);
+  if (lane == 0) red[warp] = s;
+  __syncthreads();
+  double tot = red[0];
+  for (int i = 1; i < KL_WARPS; ++i) tot = __dadd_rn(tot, red[i]);
+  for (int j = tid; j < N; j += KL_THREADS) q[j] = __ddiv_rn(py[j], tot);
+  __syncthreads();
+  double acc = 0.0;
+  for (int r = warp; r < n; r += KL_WARPS) {
+    const float* row = p + ((size_t)k * n + r) * ldp;
+    double rs = 0.0;
+    for (int j = lane; j < N; j += 32) rs = __dadd_rn(rs, (double)__ldg(row + j));
+    rs = warp_sum_d(rs);
+    double t = 0.0;
+    for (int j = lane; j < N; j += 32) {
+      const double xj = __ddiv_rn((double)__ldg(row + j), rs);
+      // rel_entr: 0 where x == 0; where x > 0 the split's column mean, so y, is positive too
+      if (xj > 0.0) t = __dadd_rn(t, __dmul_rn(xj, log(__ddiv_rn(xj, q[j]))));
+    }
+    acc = __dadd_rn(acc, warp_sum_d(t));
+  }
+  if (lane == 0) red[warp] = acc;
+  __syncthreads();
+  if (tid == 0) {
+    double t = red[0];
+    for (int i = 1; i < KL_WARPS; ++i) t = __dadd_rn(t, red[i]);
+    kl[k] = __ddiv_rn(t, (double)n);
+  }
+}
+
 }  // namespace quality
 }  // namespace omt
 
@@ -287,6 +387,37 @@ extern "C" int omt_lpips_head(const float* x, int Cs, int C, int P, int h, int w
   OMT_REQUIRE(aligned_to(4, {x, lin_w, taps_out, total}), "omt_lpips_head: misaligned pointer");
   OMT_CUDA(launch_k(quality::lpips_head_kernel, dim3(P), dim3(quality::HEAD_THREADS), 0, (cudaStream_t)stream, x, Cs, C, P,
                     h * w, lin_w, tap, taps_out, total));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_softmax_rows(const float* x, int ldx, int rows, int N, float* y, int ldy, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(x && y, "omt_softmax_rows: null pointer");
+  OMT_REQUIRE(rows >= 1 && N >= 1 && ldx >= N && ldy >= N, "omt_softmax_rows: %d rows of %d, ldx=%d, ldy=%d", rows, N,
+              ldx, ldy);
+  OMT_REQUIRE(aligned_to(4, {x, y}), "omt_softmax_rows: x and y must be 4-byte aligned");
+  OMT_CUDA(launch_k(quality::softmax_rows_kernel, dim3(rows), dim3(quality::SM_THREADS), 0, (cudaStream_t)stream, x, ldx,
+                    N, y, ldy));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_inception_score(const float* p, int ldp, int N, int n, int splits, double* col_mean, double* kl,
+                                   omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(p && col_mean && kl, "omt_inception_score: null pointer");
+  OMT_REQUIRE(N >= 1 && ldp >= N && n >= 1 && splits >= 1 && splits <= 65535,
+              "omt_inception_score: %d splits of %d rows of %d, ldp=%d", splits, n, N, ldp);
+  const size_t smem = (size_t)N * sizeof(double);
+  OMT_REQUIRE(smem <= 48 * 1024, "omt_inception_score: N=%d classes exceed 48 KiB of fp64 shared memory", N);
+  OMT_REQUIRE(aligned_to(4, {p}) && aligned_to(8, {col_mean, kl}), "omt_inception_score: misaligned pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  OMT_CUDA(launch_k(quality::is_col_mean_kernel, dim3((N + 255) / 256, splits), dim3(256), 0, st, p, ldp, N, n,
+                    col_mean));
+  OMT_LAUNCH_CHECK();
+  OMT_CUDA(launch_k(quality::is_kl_kernel, dim3(splits), dim3(quality::KL_THREADS), smem, st, p, ldp, N, n,
+                    (const double*)col_mean, kl));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

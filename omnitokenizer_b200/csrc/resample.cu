@@ -261,6 +261,7 @@ fid_preprocess_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __re
 // as resample_clips_body, but the value of a source sample is read in one of three forms, and the result is
 // (y - 0.5) * 2 in two roundings.  desc.src counts elements of src (bytes or floats); the frames of a clip follow each
 // other, so a clip stored with a longer time axis is read as its first F frames.
+// SUITE = false (omt_is_preprocess): the Inception Score's nn.Upsample alone, y written as it is.
 __device__ __forceinline__ float suite_u8_value(int b) { return __fdiv_rn((float)b, 255.f); }
 
 template <int FORM>
@@ -277,7 +278,7 @@ __device__ __forceinline__ float suite_value(const void* __restrict__ src, long 
   }
 }
 
-template <int FORM>
+template <int FORM, bool SUITE>
 __global__ void __launch_bounds__(RC_TW)
 fvd_suite_preprocess_kernel(const void* __restrict__ src, const omt_clip_desc* __restrict__ desc,
                             const int4* __restrict__ tab, int C, float* __restrict__ out, int F, int oh, int ow) {
@@ -311,7 +312,7 @@ fvd_suite_preprocess_kernel(const void* __restrict__ src, const omt_clip_desc* _
         const float t1 = __fmaf_rn(x10, l0w, __fmul_rn(x11, l1w));
         v = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
       }
-      y[c] = __fmul_rn(__fsub_rn(v, 0.5f), 2.f);
+      y[c] = SUITE ? __fmul_rn(__fsub_rn(v, 0.5f), 2.f) : v;
     }
     reinterpret_cast<float4*>(out)[((long long)blockIdx.z * oh + oy) * ow + ox] = make_float4(y[0], y[1], y[2], 0.f);
   }
@@ -457,6 +458,38 @@ extern "C" int omt_fid_preprocess(const uint8_t* src, long long src_bytes, const
   return OMT_OK;
 }
 
+// The checks and launch of omt_fvd_suite_preprocess (SUITE) and omt_is_preprocess (`who` names the entry point).
+template <bool SUITE>
+static int suite_preprocess(const char* who, const void* src, long long src_elems, int form, int C,
+                            const omt_clip_desc* desc, const omt_clip_desc* desc_host, const int32_t* tab,
+                            const int32_t* tab_host, long long tab_len, int B, int F, int oh, int ow, float* out,
+                            omt_stream_t stream) {
+  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && (form == OMT_FVDS_U8 || aligned_to(4, {src})),
+              "%s: desc must be 8-byte, tab / out 16-byte and fp32 src 4-byte aligned", who);
+  int rc = check_clips(who, src, src_elems, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, out,
+                       form == OMT_FVDS_U8 ? 3 : C);
+  if (rc != OMT_OK) return rc;
+  for (int b = 0; b < B; ++b) {
+    const omt_clip_desc& d = desc_host[b];
+    OMT_REQUIRE(!d.flip && d.y0 == 0 && d.x0 == 0 && d.wh == d.H && d.ww == d.W,
+                "%s: clip %d: the suite's preprocess has no flip and no window", who, b);
+  }
+  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
+  const int4* t4 = reinterpret_cast<const int4*>(tab);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (form == OMT_FVDS_U8)
+    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_U8, SUITE>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F,
+                      oh, ow));
+  else if (form == OMT_FVDS_F32)
+    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_F32, SUITE>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F,
+                      oh, ow));
+  else
+    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_F32_TRUNC, true>, grid, dim3(RC_TW), 0, s, src, desc, t4, C,
+                      out, F, oh, ow));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
 extern "C" int omt_fvd_suite_preprocess(const void* src, long long src_elems, int form, int C,
                                         const omt_clip_desc* desc, const omt_clip_desc* desc_host, const int32_t* tab,
                                         const int32_t* tab_host, long long tab_len, int B, int F, int oh, int ow,
@@ -466,26 +499,16 @@ extern "C" int omt_fvd_suite_preprocess(const void* src, long long src_elems, in
               "omt_fvd_suite_preprocess: unknown input form %d", form);
   OMT_REQUIRE(form == OMT_FVDS_U8 ? C == 3 : (C == 1 || C == 3),
               "omt_fvd_suite_preprocess: C=%d (uint8 clips have 3 channels, fp32 clips 1 or 3)", C);
-  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && (form == OMT_FVDS_U8 || aligned_to(4, {src})),
-              "omt_fvd_suite_preprocess: desc must be 8-byte, tab / out 16-byte and fp32 src 4-byte aligned");
-  int rc = check_clips("omt_fvd_suite_preprocess", src, src_elems, desc, desc_host, tab, tab_host, tab_len, B, F, oh,
-                       ow, out, form == OMT_FVDS_U8 ? 3 : C);
-  if (rc != OMT_OK) return rc;
-  for (int b = 0; b < B; ++b) {
-    const omt_clip_desc& d = desc_host[b];
-    OMT_REQUIRE(!d.flip && d.y0 == 0 && d.x0 == 0 && d.wh == d.H && d.ww == d.W,
-                "omt_fvd_suite_preprocess: clip %d: the suite's preprocess has no flip and no window", b);
-  }
-  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
-  const int4* t4 = reinterpret_cast<const int4*>(tab);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (form == OMT_FVDS_U8)
-    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_U8>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F, oh, ow));
-  else if (form == OMT_FVDS_F32)
-    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_F32>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F, oh, ow));
-  else
-    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_F32_TRUNC>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F,
-                      oh, ow));
-  OMT_LAUNCH_CHECK();
-  return OMT_OK;
+  return suite_preprocess<true>("omt_fvd_suite_preprocess", src, src_elems, form, C, desc, desc_host, tab, tab_host,
+                                tab_len, B, F, oh, ow, out, stream);
+}
+
+extern "C" int omt_is_preprocess(const void* src, long long src_elems, int form, const omt_clip_desc* desc,
+                                 const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
+                                 long long tab_len, int B, int F, int oh, int ow, float* out, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(form == OMT_FVDS_U8 || form == OMT_FVDS_F32,
+              "omt_is_preprocess: input form %d is neither uint8 (0) nor fp32 (1)", form);
+  return suite_preprocess<false>("omt_is_preprocess", src, src_elems, form, 3, desc, desc_host, tab, tab_host, tab_len,
+                                 B, F, oh, ow, out, stream);
 }

@@ -29,7 +29,7 @@ from .fvd import cpad, pack_weight, real_byte_table
 TARGET_RESOLUTION = (299, 299)     # inception.py:148
 BN_EPS = 1e-3                      # torchvision BasicConv2d's BatchNorm2d(eps=0.001)
 DIMS = 2048                        # fid_score.py --dims default: the pool3 features; the only width built here
-POOL_MAX, POOL_AVG = 0, 1          # omt_pool2d modes
+POOL_MAX, POOL_AVG, POOL_AVG_PAD = 0, 1, 2   # omt_pool2d modes (POOL_AVG_PAD: avg_pool2d(count_include_pad=True))
 IMAGE_EXTENSIONS = ("bmp", "jpg", "jpeg", "pgm", "png", "ppm", "tif", "tiff", "webp", "JPEG")   # fid_score.py:94
 
 
@@ -67,12 +67,12 @@ STEM = [_c("Conv2d_1a_3x3", "x", 3, 32, 3, s=2), _c("Conv2d_2a_3x3", "x", 32, 32
         _c("Conv2d_3b_1x1", "x", 64, 80, 1), _c("Conv2d_4a_3x3", "x", 80, 192, 3), Pool(POOL_MAX, 3, 2, 0, None)]
 
 
-def _block_a(cin, pool_features):        # FIDInceptionA: the pool averages without the padding
+def _block_a(cin, pool_features, avg):   # FIDInceptionA: the pool averages without the padding (torchvision's with it)
     return ([_c("branch1x1", "x", cin, 64, 1, col=0),
              _c("branch5x5_1", "x", cin, 48, 1), _c("branch5x5_2", "branch5x5_1", 48, 64, 5, p=2, col=64),
              _c("branch3x3dbl_1", "x", cin, 64, 1), _c("branch3x3dbl_2", "branch3x3dbl_1", 64, 96, 3, p=1),
              _c("branch3x3dbl_3", "branch3x3dbl_2", 96, 96, 3, p=1, col=128),
-             _c("branch_pool", "p", cin, pool_features, 1, col=224)], Pool(POOL_AVG, 3, 1, 1, None), 224 + pool_features)
+             _c("branch_pool", "p", cin, pool_features, 1, col=224)], Pool(avg, 3, 1, 1, None), 224 + pool_features)
 
 
 def _block_b(cin):                       # InceptionB (Mixed_6a): the max pool fills the last cin columns
@@ -81,7 +81,7 @@ def _block_b(cin):                       # InceptionB (Mixed_6a): the max pool f
              _c("branch3x3dbl_3", "branch3x3dbl_2", 96, 96, 3, s=2, col=384)], Pool(POOL_MAX, 3, 2, 0, 480), 480 + cin)
 
 
-def _block_c(cin, c7):                   # FIDInceptionC
+def _block_c(cin, c7, avg):              # FIDInceptionC / torchvision's InceptionC
     return ([_c("branch1x1", "x", cin, 192, 1, col=0),
              _c("branch7x7_1", "x", cin, c7, 1), _c("branch7x7_2", "branch7x7_1", c7, c7, (1, 7), p=(0, 3)),
              _c("branch7x7_3", "branch7x7_2", c7, 192, (7, 1), p=(3, 0), col=192),
@@ -89,7 +89,7 @@ def _block_c(cin, c7):                   # FIDInceptionC
              _c("branch7x7dbl_3", "branch7x7dbl_2", c7, c7, (1, 7), p=(0, 3)),
              _c("branch7x7dbl_4", "branch7x7dbl_3", c7, c7, (7, 1), p=(3, 0)),
              _c("branch7x7dbl_5", "branch7x7dbl_4", c7, 192, (1, 7), p=(0, 3), col=384),
-             _c("branch_pool", "p", cin, 192, 1, col=576)], Pool(POOL_AVG, 3, 1, 1, None), 768)
+             _c("branch_pool", "p", cin, 192, 1, col=576)], Pool(avg, 3, 1, 1, None), 768)
 
 
 def _block_d(cin):                       # InceptionD (Mixed_7a)
@@ -100,7 +100,7 @@ def _block_d(cin):                       # InceptionD (Mixed_7a)
              _c("branch7x7x3_4", "branch7x7x3_3", 192, 192, 3, s=2, col=320)], Pool(POOL_MAX, 3, 2, 0, 512), 512 + cin)
 
 
-def _block_e(cin, pool_mode):            # FIDInceptionE_1 (average pool without the padding) / _E_2 (max pool)
+def _block_e(cin, pool_mode):            # FIDInceptionE_1 (average pool without the padding) / _E_2 (max pool); InceptionE
     return ([_c("branch1x1", "x", cin, 320, 1, col=0),
              _c("branch3x3_1", "x", cin, 384, 1),
              _c("branch3x3_2a", "branch3x3_1", 384, 384, (1, 3), p=(0, 1), col=320),
@@ -111,13 +111,20 @@ def _block_e(cin, pool_mode):            # FIDInceptionE_1 (average pool without
              _c("branch_pool", "p", cin, 192, 1, col=1856)], Pool(pool_mode, 3, 1, 1, None), 2048)
 
 
-# pytorch-fid's blocks 2 and 3 (inception.py:104-125, fid_inception_v3 :204-213): (name, convs, pool, output width)
-BLOCKS = [("Mixed_5b",) + _block_a(192, 32), ("Mixed_5c",) + _block_a(256, 64), ("Mixed_5d",) + _block_a(288, 64),
-          ("Mixed_6a",) + _block_b(288),
-          ("Mixed_6b",) + _block_c(768, 128), ("Mixed_6c",) + _block_c(768, 160), ("Mixed_6d",) + _block_c(768, 160),
-          ("Mixed_6e",) + _block_c(768, 192),
-          ("Mixed_7a",) + _block_d(768),
-          ("Mixed_7b",) + _block_e(1280, POOL_AVG), ("Mixed_7c",) + _block_e(2048, POOL_MAX)]
+def blocks(avg: int = POOL_AVG, e2: int = POOL_MAX) -> list:
+    """The Mixed blocks, (name, convs, pool, output width) each: the branch_pool averages of the A, C and E blocks use
+    pool mode `avg` except Mixed_7c's, which uses `e2`.  The defaults are pytorch-fid's blocks 2 and 3 (inception.py:
+    104-125, fid_inception_v3 :204-213); blocks(POOL_AVG_PAD, POOL_AVG_PAD) is torchvision's Inception3."""
+    return [("Mixed_5b",) + _block_a(192, 32, avg), ("Mixed_5c",) + _block_a(256, 64, avg),
+            ("Mixed_5d",) + _block_a(288, 64, avg),
+            ("Mixed_6a",) + _block_b(288),
+            ("Mixed_6b",) + _block_c(768, 128, avg), ("Mixed_6c",) + _block_c(768, 160, avg),
+            ("Mixed_6d",) + _block_c(768, 160, avg), ("Mixed_6e",) + _block_c(768, 192, avg),
+            ("Mixed_7a",) + _block_d(768),
+            ("Mixed_7b",) + _block_e(1280, avg), ("Mixed_7c",) + _block_e(2048, e2)]
+
+
+BLOCKS = blocks()
 
 
 def conv_list() -> List[Conv]:
@@ -159,6 +166,16 @@ class _Unit:
         self.bias, self.conv = bias.to(device), conv
 
 
+def pack_units(sd: Dict[str, torch.Tensor], device) -> Dict[str, _Unit]:
+    """Every BasicConv2d of a float32 CPU state_dict with BatchNorm folded, packed on device, by key prefix."""
+    units = {}
+    for c in conv_list():
+        w, b = fold_bn(sd[c.name + ".conv.weight"], *(sd[f"{c.name}.bn.{f}"]
+                                                      for f in ("weight", "bias", "running_mean", "running_var")))
+        units[c.name] = _Unit(c, w, b, device)
+    return units
+
+
 def byte_lut(real_norm: Optional[L.U8Norm] = None) -> torch.Tensor:
     """fp32 [n_tab, 256]: the value the network's input takes for each byte before the resize: ToTensor's byte / 255
     (fid_score.py:146), or, for the loader's bytes of a real image, / 255 of the byte vqgan_eval.py saves for it,
@@ -167,12 +184,84 @@ def byte_lut(real_norm: Optional[L.U8Norm] = None) -> torch.Tensor:
     return b / 255
 
 
-class _Workspace:
+class Launches:
+    """The launch list of an InceptionV3 trunk over static channels-last buffers of a batch of B (fid._Workspace and
+    iscore's workspaces build theirs with it)."""
+
+    def __init__(self, device, B: int):
+        self.device, self.B = device, B
+        self.graphs = {}
+        self.ops = []
+
+    def trunk(self, units: Dict[str, "_Unit"], x, hw, blocks_=BLOCKS):
+        """The stem and the Mixed blocks from the (B, hw, 4) input x.  Returns (the last block's buffer, its width,
+        its size)."""
+        cur, c_cur = x, 3
+        for layer in STEM:
+            if isinstance(layer, Conv):
+                cur, hw = self._conv(units[layer.name], cur, hw)
+                c_cur = layer.cout
+            else:
+                cur, hw = self._pool(layer, cur, c_cur, hw)
+        for name, convs, pool, cout in blocks_:
+            o = hw
+            if pool.col is not None:                   # strided blocks: the output size is the pool's
+                o = tuple(out_size(n, pool.k, pool.s, pool.p) for n in hw)
+            y = self._act(*o, cout)
+            bufs = {"x": cur}
+            if pool.col is None:
+                bufs["p"], _ = self._pool(pool, cur, c_cur, hw)
+            else:
+                self._pool(pool, cur, c_cur, hw, out=(y, pool.col))
+            for c in convs:
+                u = units[f"{name}.{c.name}"]
+                if c.col is None:
+                    bufs[c.name], _ = self._conv(u, bufs[c.src], hw)
+                else:
+                    _, got = self._conv(u, bufs[c.src], hw, out=(y, c.col))
+                    if got != o:
+                        raise AssertionError(f"{name}.{c.name}: output {got}, the block's is {o}")
+            cur, c_cur, hw = y, cout, o
+        return cur, c_cur, hw
+
+    def _act(self, H_, W_, c):
+        # pad columns stay zero: no kernel writes them
+        return torch.zeros(self.B, H_, W_, cpad(c), device=self.device, dtype=torch.float32)
+
+    def _conv(self, u: _Unit, x, hw, out=None, relu: int = 1):
+        c = u.conv
+        o = tuple(out_size(n, k, c.s, p) for n, k, p in zip(hw, c.k, c.p))
+        y, col = (self._act(*o, c.cout), 0) if out is None else out
+        ypt = y.data_ptr() + 4 * col
+        B = self.B
+        self.ops.append(lambda: _cabi.call(
+            "omt_conv3d", x, x.shape[-1], B, 1, hw[0], hw[1], u.w_hi, u.w_lo, u.K, u.bias, c.cout,
+            1, c.k[0], c.k[1], 1, c.s, c.s, 0, c.p[0], c.p[1], 1, o[0], o[1], ypt, y.shape[-1], relu))
+        return y, o
+
+    def _pool(self, pool: Pool, x, c, hw, out=None, k=None):
+        """k: a (kh, kw) window in place of pool.k's square one."""
+        kh, kw = (pool.k, pool.k) if k is None else k
+        o = (out_size(hw[0], kh, pool.s, pool.p), out_size(hw[1], kw, pool.s, pool.p))
+        y, col = (self._act(*o, c), 0) if out is None else out
+        ypt = y.data_ptr() + 4 * col
+        B = self.B
+        self.ops.append(lambda: _cabi.call(
+            "omt_pool2d", x, x.shape[-1], c, B, hw[0], hw[1], kh, kw, pool.s,
+            pool.s, pool.p, pool.p, o[0], o[1], ypt, y.shape[-1], pool.mode))
+        return y, o
+
+    def run(self):
+        for op in self.ops:
+            op()
+
+
+class _Workspace(Launches):
     """Buffers, launch list and CUDA graph state of one (B, H, W, real_norm)."""
 
     def __init__(self, net: "FIDInception", B: int, H: int, W: int, real_norm: Optional[L.U8Norm] = None):
         dev = net.device
-        self.graphs = {}
+        super().__init__(dev, B)
         self.u8 = torch.empty(B, H, W, 3, dtype=torch.uint8, device=dev)
         self.lut = byte_lut(real_norm).to(dev)
         self.sel = torch.empty(B, dtype=torch.int32, device=dev) if real_norm is not None and real_norm.max_test else None
@@ -187,8 +276,6 @@ class _Workspace:
         desc[:, 2:] = torch.tensor([H, W, 0, 0, H, W, oh, ow, 0, 0, 0, 0, tv.size, L.INTERP_SEPARABLE], dtype=torch.int32)
         self.desc_host = desc
         self.desc, self.tab = desc.to(dev), self.tab_host.to(dev)
-        self.ops = []
-        self.B = B
 
         x = self._act(oh, ow, 3)
         if self.sel is not None:
@@ -196,65 +283,11 @@ class _Workspace:
         self.ops.append(lambda: _cabi.call(
             "omt_fid_preprocess", self.u8, self.u8.numel(), self.desc, self.desc_host, self.tab, self.tab_host,
             self.tab_host.numel(), self.lut, self.sel, B, oh, ow, x))
-        cur, c_cur, hw = x, 3, (oh, ow)
-        for layer in STEM:
-            if isinstance(layer, Conv):
-                cur, hw = self._conv(net.units[layer.name], cur, hw)
-                c_cur = layer.cout
-            else:
-                cur, hw = self._pool(layer, cur, c_cur, hw)
-        for name, convs, pool, cout in BLOCKS:
-            o = hw
-            if pool.col is not None:                   # strided blocks: the output size is the pool's
-                o = tuple(out_size(n, pool.k, pool.s, pool.p) for n in hw)
-            y = self._act(*o, cout)
-            bufs = {"x": cur}
-            if pool.col is None:
-                bufs["p"], _ = self._pool(pool, cur, c_cur, hw)
-            else:
-                self._pool(pool, cur, c_cur, hw, out=(y, pool.col))
-            for c in convs:
-                u = net.units[f"{name}.{c.name}"]
-                if c.col is None:
-                    bufs[c.name], _ = self._conv(u, bufs[c.src], hw)
-                else:
-                    _, got = self._conv(u, bufs[c.src], hw, out=(y, c.col))
-                    if got != o:
-                        raise AssertionError(f"{name}.{c.name}: output {got}, the block's is {o}")
-            cur, c_cur, hw = y, cout, o
+        cur, c_cur, hw = self.trunk(net.units, x, (oh, ow))
         if hw != (8, 8) or c_cur != DIMS:
             raise ValueError(f"the pool3 features need an [8, 8, {DIMS}] map, got {hw + (c_cur,)}")
         # AdaptiveAvgPool2d(1) of the 8 x 8 map (inception.py:123): one 8 x 8 window straight into the (B, 2048) output
         self._pool(Pool(POOL_AVG, 8, 1, 0, 0), cur, c_cur, hw, out=(self.out.view(B, 1, 1, DIMS), 0))
-
-    def _act(self, H_, W_, c):
-        # pad columns stay zero: no kernel writes them
-        return torch.zeros(self.B, H_, W_, cpad(c), device=self.u8.device, dtype=torch.float32)
-
-    def _conv(self, u: _Unit, x, hw, out=None):
-        c = u.conv
-        o = tuple(out_size(n, k, c.s, p) for n, k, p in zip(hw, c.k, c.p))
-        y, col = (self._act(*o, c.cout), 0) if out is None else out
-        ypt = y.data_ptr() + 4 * col
-        B = self.B
-        self.ops.append(lambda: _cabi.call(
-            "omt_conv3d", x, x.shape[-1], B, 1, hw[0], hw[1], u.w_hi, u.w_lo, u.K, u.bias, c.cout,
-            1, c.k[0], c.k[1], 1, c.s, c.s, 0, c.p[0], c.p[1], 1, o[0], o[1], ypt, y.shape[-1], 1))
-        return y, o
-
-    def _pool(self, pool: Pool, x, c, hw, out=None):
-        o = tuple(out_size(n, pool.k, pool.s, pool.p) for n in hw)
-        y, col = (self._act(*o, c), 0) if out is None else out
-        ypt = y.data_ptr() + 4 * col
-        B = self.B
-        self.ops.append(lambda: _cabi.call(
-            "omt_pool2d", x, x.shape[-1], c, B, hw[0], hw[1], pool.k, pool.k, pool.s,
-            pool.s, pool.p, pool.p, o[0], o[1], ypt, y.shape[-1], pool.mode))
-        return y, o
-
-    def run(self):
-        for op in self.ops:
-            op()
 
 
 class FIDInception:
@@ -279,12 +312,7 @@ class FIDInception:
         self.device = torch.device(device)
         if self.device.type == "cuda" and self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
-        sd = {k: v.detach().float().cpu() for k, v in sd.items()}
-        self.units = {}
-        for c in conv_list():
-            w, b = fold_bn(sd[c.name + ".conv.weight"], *(sd[f"{c.name}.bn.{f}"]
-                                                          for f in ("weight", "bias", "running_mean", "running_var")))
-            self.units[c.name] = _Unit(c, w, b, self.device)
+        self.units = pack_units({k: v.detach().float().cpu() for k, v in sd.items()}, self.device)
         self._ws = {}
 
     @staticmethod
