@@ -181,7 +181,7 @@ def eval_step_fvd(vqgan, frames: torch.Tensor, i3d, total_usage: Optional[torch.
     (fvd.I3D).  The real side sees the bytes the script makes of the normalised clip, shift_dim((video + 0.5) * 255,
     1, -1).byte(), as a per-byte map with norm's branch picked per clip.  Returns (real_logits, fake_logits,
     vq_output); no frame crosses to the host."""
-    from .fvd import real_byte_table
+    from .metricnet import real_byte_table
     _check_u8(frames, (5,), "eval_step_fvd")
     i3d.check_frames(frames)                 # every refusal before the first launch
     real_byte_table(norm)
@@ -202,7 +202,7 @@ def eval_step_quality(vqgan, frames: torch.Tensor, lpips=None, total_usage: Opti
     images (B, H, W, 3) as T = 1.  Returns (psnr (B, T) fp64, ssim (B, T) fp64, lpips (B, T) fp32 or None,
     fake_u8 (B, T, H, W, 3), vq_output); fake_u8 can feed i3d.logits as well.  No frame crosses to the host."""
     from . import quality
-    from .fvd import real_byte_table
+    from .metricnet import real_byte_table
     _check_u8(frames, (4, 5), "eval_step_quality")
     real = frames.unsqueeze(1) if frames.dim() == 4 else frames
     quality.check_pair(real, real, torch.uint8, "eval_step_quality")      # every refusal before the first launch
@@ -272,7 +272,7 @@ def eval_step_fid(vqgan, images: Sequence[torch.Tensor], resize: U8Resize, incep
     the bytes the script saves of the normalised input, ((x + 0.5) * 255).astype(uint8), as a per-byte map.  Returns
     (real_features, fake_features, vq_output), each features (B, 2048) fp32; no image crosses to the host.
     --infer_downsample (a PIL ANTIALIAS resize before saving) is not supported."""
-    from .fvd import real_byte_table
+    from .metricnet import real_byte_table
     images = list(images)
     if not images:
         raise ValueError("eval_step_fid needs at least one image")

@@ -12,6 +12,7 @@ attention and both PEG variants go through index maps.
 """
 from __future__ import annotations
 
+import gc
 import math
 import os
 from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
@@ -112,8 +113,16 @@ def run_graphed(graphs: dict, device, key, body):
         graph = torch.cuda.CUDAGraph()
         torch.cuda.synchronize(device)
         n0 = _cabi.launch_count
-        with torch.cuda.graph(graph):
-            body()
+        # An evicted workspace lives on in a reference cycle (its launch closures hold it) until the cyclic collector
+        # frees it; freeing its captured graph inside this capture would reset that graph and invalidate the capture.
+        collecting = gc.isenabled()
+        gc.disable()
+        try:
+            with torch.cuda.graph(graph):
+                body()
+        finally:
+            if collecting:
+                gc.enable()
         graphs[key] = (graph, _cabi.launch_count - n0)
         graph.replay()
     else:

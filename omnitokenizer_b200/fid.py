@@ -8,7 +8,7 @@ fid_given_paths(paths, model, batch_size) for directories of images (the `python
 line of vqgan_eval.py).
 
 Activations are channels-last fp32 [B][H][W][Cs], Cs the channel count rounded up to a multiple of 32 (4 for the
-network input, fvd.cpad); the pad columns are zero.  Every BasicConv2d (conv without bias, BatchNorm2d(eps=0.001),
+network input, metricnet.cpad); the pad columns are zero.  Every BasicConv2d (conv without bias, BatchNorm2d(eps=0.001),
 ReLU) is one omt_conv3d launch with a kernel depth of 1 (3xTF32, BatchNorm folded into the weights at pack time); each
 branch writes its slice of the block's concat buffer in place, and the pools run on omt_pool2d.
 """
@@ -23,8 +23,10 @@ import torch
 
 from . import _cabi
 from . import layout as L
-from .engine import CLIP_DESC_WORDS, run_graphed
-from .fvd import cpad, pack_weight, real_byte_table
+from . import metricnet
+from .engine import run_graphed
+from .metricnet import (MAX_WORKSPACES, PackedConv, axis_tables, bounded, byte_lut, check_state_dict, clip_descs, cpad,
+                        real_byte_table, resolve_device)
 
 TARGET_RESOLUTION = (299, 299)     # inception.py:148
 BN_EPS = 1e-3                      # torchvision BasicConv2d's BatchNorm2d(eps=0.001)
@@ -150,23 +152,16 @@ def expected_keys() -> Dict[str, tuple]:
 
 
 def fold_bn(w: torch.Tensor, gamma, beta, mean, var) -> Tuple[torch.Tensor, torch.Tensor]:
-    """BatchNorm2d (running statistics, eps 1e-3) folded into a conv weight (cout, cin, kh, kw), in float64:
-    (W s, beta - mean s) with s = gamma / sqrt(var + eps), rounded to fp32."""
-    s = gamma.double() / torch.sqrt(var.double() + BN_EPS)
-    return (w.double() * s.view(-1, 1, 1, 1)).float(), (beta.double() - mean.double() * s).float()
+    """metricnet.fold_bn with BasicConv2d's BatchNorm2d eps 1e-3."""
+    return metricnet.fold_bn(w, gamma, beta, mean, var, BN_EPS)
 
 
-class _Unit:
-    """One BasicConv2d packed for omt_conv3d: tf32 hi / lo planes of W, the folded bias, its geometry."""
-
-    def __init__(self, conv: Conv, w, bias, device):
-        packed, self.K = pack_weight(w.unsqueeze(2))        # (cout, cin, 1, kh, kw): K = (dh, dw, c)
-        hi = L.tf32_round(packed)
-        self.w_hi, self.w_lo = hi.to(device), (packed - hi).to(device)
-        self.bias, self.conv = bias.to(device), conv
+def _Unit(conv: Conv, w, bias, device) -> PackedConv:
+    """One BasicConv2d (cout, cin, kh, kw) packed for omt_conv3d, with its geometry."""
+    return PackedConv(w, bias, device, conv, (1, conv.s, conv.s))
 
 
-def pack_units(sd: Dict[str, torch.Tensor], device) -> Dict[str, _Unit]:
+def pack_units(sd: Dict[str, torch.Tensor], device) -> Dict[str, PackedConv]:
     """Every BasicConv2d of a float32 CPU state_dict with BatchNorm folded, packed on device, by key prefix."""
     units = {}
     for c in conv_list():
@@ -174,14 +169,6 @@ def pack_units(sd: Dict[str, torch.Tensor], device) -> Dict[str, _Unit]:
                                                       for f in ("weight", "bias", "running_mean", "running_var")))
         units[c.name] = _Unit(c, w, b, device)
     return units
-
-
-def byte_lut(real_norm: Optional[L.U8Norm] = None) -> torch.Tensor:
-    """fp32 [n_tab, 256]: the value the network's input takes for each byte before the resize: ToTensor's byte / 255
-    (fid_score.py:146), or, for the loader's bytes of a real image, / 255 of the byte vqgan_eval.py saves for it,
-    ((v + 0.5) * 255).astype(uint8) of the normalised value v (:205; fvd.real_byte_table)."""
-    b = torch.arange(256, dtype=torch.float32).view(1, 256) if real_norm is None else real_byte_table(real_norm).float()
-    return b / 255
 
 
 class Launches:
@@ -193,7 +180,7 @@ class Launches:
         self.graphs = {}
         self.ops = []
 
-    def trunk(self, units: Dict[str, "_Unit"], x, hw, blocks_=BLOCKS):
+    def trunk(self, units: Dict[str, PackedConv], x, hw, blocks_=BLOCKS):
         """The stem and the Mixed blocks from the (B, hw, 4) input x.  Returns (the last block's buffer, its width,
         its size)."""
         cur, c_cur = x, 3
@@ -228,15 +215,11 @@ class Launches:
         # pad columns stay zero: no kernel writes them
         return torch.zeros(self.B, H_, W_, cpad(c), device=self.device, dtype=torch.float32)
 
-    def _conv(self, u: _Unit, x, hw, out=None, relu: int = 1):
+    def _conv(self, u: PackedConv, x, hw, out=None, relu: int = 1):
         c = u.conv
         o = tuple(out_size(n, k, c.s, p) for n, k, p in zip(hw, c.k, c.p))
         y, col = (self._act(*o, c.cout), 0) if out is None else out
-        ypt = y.data_ptr() + 4 * col
-        B = self.B
-        self.ops.append(lambda: _cabi.call(
-            "omt_conv3d", x, x.shape[-1], B, 1, hw[0], hw[1], u.w_hi, u.w_lo, u.K, u.bias, c.cout,
-            1, c.k[0], c.k[1], 1, c.s, c.s, 0, c.p[0], c.p[1], 1, o[0], o[1], ypt, y.shape[-1], relu))
+        self.ops.append(u.launch(x, self.B, (1,) + hw, (0,) + c.p, (1,) + o, y, col, relu))
         return y, o
 
     def _pool(self, pool: Pool, x, c, hw, out=None, k=None):
@@ -268,14 +251,8 @@ class _Workspace(Launches):
         self.out = torch.empty(B, DIMS, device=dev)
         # inception.py:148 F.interpolate to 299 x 299 from torch's multi-threaded CPU kernel: the separable form
         oh, ow = TARGET_RESOLUTION
-        tv = L.clip_axis_table(H, oh, float(np.float32(H) / np.float32(oh))).reshape(-1)
-        th = L.clip_axis_table(W, ow, float(np.float32(W) / np.float32(ow))).reshape(-1)
-        self.tab_host = torch.from_numpy(np.concatenate([tv, th]).astype(np.int32))
-        desc = torch.zeros(B, CLIP_DESC_WORDS, dtype=torch.int32)
-        desc[:, :2] = (torch.arange(B, dtype=torch.int64) * (H * W * 3)).view(torch.int32).view(B, 2)
-        desc[:, 2:] = torch.tensor([H, W, 0, 0, H, W, oh, ow, 0, 0, 0, 0, tv.size, L.INTERP_SEPARABLE], dtype=torch.int32)
-        self.desc_host = desc
-        self.desc, self.tab = desc.to(dev), self.tab_host.to(dev)
+        self.tab_host, self.desc_host = axis_tables(H, W, oh, ow), clip_descs(B, H * W * 3, H, W, oh, ow)
+        self.desc, self.tab = self.desc_host.to(dev), self.tab_host.to(dev)
 
         x = self._act(oh, ow, 3)
         if self.sel is not None:
@@ -297,21 +274,11 @@ class FIDInception:
     `num_batches_tracked` are ignored.  BatchNorm is folded and the weights packed once, on `device`; every
     (B, H, W, real_norm) gets its own buffers and CUDA graph (the last few are kept)."""
 
-    MAX_WORKSPACES = 4
-
     def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda"):
         sd = {k: v for k, v in state_dict.items()
               if not (k.endswith(".num_batches_tracked") or k.startswith(("fc.", "AuxLogits.")))}
-        want = expected_keys()
-        missing, unexpected = sorted(set(want) - set(sd)), sorted(set(sd) - set(want))
-        if missing or unexpected:
-            raise KeyError(f"FID InceptionV3 state_dict: missing keys {missing}, unexpected keys {unexpected}")
-        for k, shape in want.items():
-            if tuple(sd[k].shape) != shape:
-                raise ValueError(f"FID InceptionV3 state_dict: {k} has shape {tuple(sd[k].shape)}, expected {shape}")
-        self.device = torch.device(device)
-        if self.device.type == "cuda" and self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
+        check_state_dict(sd, expected_keys(), "FID InceptionV3")
+        self.device = resolve_device(device)
         self.units = pack_units({k: v.detach().float().cpu() for k, v in sd.items()}, self.device)
         self._ws = {}
 
@@ -335,11 +302,7 @@ class FIDInception:
         if real_norm is not None:
             real_byte_table(real_norm)                       # refuses a per-channel normalisation before any launch
         key = tuple(int(v) for v in images_u8.shape[:3]) + (real_norm,)
-        ws = self._ws.get(key)
-        if ws is None:
-            while len(self._ws) >= self.MAX_WORKSPACES:
-                self._ws.pop(next(iter(self._ws)))
-            ws = self._ws[key] = _Workspace(self, *key)
+        ws = bounded(self._ws, MAX_WORKSPACES, key, lambda: _Workspace(self, *key))
         ws.u8.copy_(images_u8)
         run_graphed(ws.graphs, self.device, "fid", ws.run)
         return ws.out

@@ -23,7 +23,12 @@ import torch
 
 from . import _cabi
 from . import layout as L
+from . import metricnet
 from .engine import CLIP_DESC_WORDS, run_graphed
+# cpad, pack_weight and the FORM_* values stay importable from here: the I3D's channel strides, weight layout and
+# SuiteClips forms
+from .metricnet import (FORM_F32, FORM_F32_TRUNC, FORM_U8, MAX_WORKSPACES, PackedConv, axis_tables,  # noqa: F401
+                        bounded, check_state_dict, clip_descs, cpad, pack_weight, real_byte_table, resolve_device)
 
 TARGET_RESOLUTION = (224, 224)
 BN_EPS = 1e-5            # pytorch_i3d.py:91
@@ -56,9 +61,9 @@ BRANCHES = {"b0": (0, 1, "x"), "b1a": (1, 1, "x"), "b1b": (2, 3, "b1a"), "b2a": 
             "b3b": (5, 1, "p")}
 
 
-def cpad(c: int) -> int:
-    """Channel stride of an activation with c channels: 4 for the RGB input, else a multiple of 32."""
-    return 4 if c <= 4 else L.round_up(c, 32)
+def fold_bn(w: torch.Tensor, gamma, beta, mean, var, eps: float = BN_EPS) -> Tuple[torch.Tensor, torch.Tensor]:
+    """metricnet.fold_bn with eps 1e-5 (pytorch_i3d.py:91) unless given."""
+    return metricnet.fold_bn(w, gamma, beta, mean, var, eps)
 
 
 def compute_pad(k: int, s: int, n: int) -> int:
@@ -100,35 +105,6 @@ def expected_keys(num_classes: int = 400) -> Dict[str, tuple]:
     return keys
 
 
-def fold_bn(w: torch.Tensor, gamma, beta, mean, var, eps: float = BN_EPS) -> Tuple[torch.Tensor, torch.Tensor]:
-    """BatchNorm (running statistics, eps 1e-5 unless given) folded into a conv weight (cout, cin, k, k, k), in
-    float64: (W s, beta - mean s) with s = gamma / sqrt(var + eps), rounded to fp32."""
-    s = gamma.double() / torch.sqrt(var.double() + eps)
-    return (w.double() * s.view(-1, 1, 1, 1, 1)).float(), (beta.double() - mean.double() * s).float()
-
-
-def pack_weight(w: torch.Tensor) -> Tuple[torch.Tensor, int]:
-    """A conv weight (cout, cin, kt, kh, kw) as omt_conv3d's W: rows of K = (dt, dh, dw, c) with c padded to cpad(cin)
-    (K rounded up to 32 for the RGB input), cout padded to a multiple of 128.  Returns (W [n_pad, K] fp32, K)."""
-    cout, cin = int(w.shape[0]), int(w.shape[1])
-    wk = torch.zeros(cout, *w.shape[2:], cpad(cin))
-    wk[..., :cin] = w.float().permute(0, 2, 3, 4, 1)
-    wk = wk.reshape(cout, -1)
-    K = L.round_up(wk.shape[1], 32)
-    packed = torch.zeros(L.round_up(cout, 128), K)
-    packed[:cout, :wk.shape[1]] = wk
-    return packed, K
-
-
-class _Unit:
-    """One Unit3D packed for omt_conv3d: tf32 hi / lo planes of W, the folded bias, its geometry."""
-
-    def __init__(self, w, K, bias, cout, k, s, device):
-        hi = L.tf32_round(w)
-        self.w_hi, self.w_lo = hi.to(device), (w - hi).to(device)
-        self.bias, self.K, self.cout, self.k, self.s = bias.to(device), K, cout, k, s
-
-
 class _Workspace:
     """Buffers, launch list and CUDA graph state of one (B, T, H, W)."""
 
@@ -160,14 +136,8 @@ class _Workspace:
         self.sel = torch.empty(B, dtype=torch.int32, device=dev) if real_norm is not None and real_norm.max_test else None
         # preprocess tables (fvd.py:24: F.interpolate to 224 x 224 from the multi-threaded script: the separable kernel)
         oh, ow = TARGET_RESOLUTION
-        tv = L.clip_axis_table(H, oh, float(np.float32(H) / np.float32(oh))).reshape(-1)
-        th = L.clip_axis_table(W, ow, float(np.float32(W) / np.float32(ow))).reshape(-1)
-        self.tab_host = torch.from_numpy(np.concatenate([tv, th]).astype(np.int32))
-        desc = torch.zeros(B, CLIP_DESC_WORDS, dtype=torch.int32)
-        desc[:, :2] = (torch.arange(B, dtype=torch.int64) * (T * H * W * 3)).view(torch.int32).view(B, 2)
-        desc[:, 2:] = torch.tensor([H, W, 0, 0, H, W, oh, ow, 0, 0, 0, 0, tv.size, L.INTERP_SEPARABLE], dtype=torch.int32)
-        self.desc_host = desc
-        self.desc, self.tab = desc.to(dev), self.tab_host.to(dev)
+        self.tab_host, self.desc_host = axis_tables(H, W, oh, ow), clip_descs(B, T * H * W * 3, H, W, oh, ow)
+        self.desc, self.tab = self.desc_host.to(dev), self.tab_host.to(dev)
         if self.sel is not None:
             self.ops.append(lambda: _cabi.call("omt_u8_norm_select", self.u8, B, T * H * W * 3, self.sel))
         self.ops.append(lambda x=x: _cabi.call(
@@ -204,18 +174,10 @@ class _Workspace:
         self.ops.append(lambda cur=cur, T5=T5: _cabi.call(
             "omt_i3d_head", cur, cur.shape[-1], 1024, B, T5, net.head_w, net.head_b, net.num_classes, self.out))
 
-    def _conv(self, u: _Unit, x, shape, act, out=None):
-        k, s = (u.k,) * 3, (u.s,) * 3
-        front, o = same_geometry(k, s, shape)
-        if out is None:
-            y, col = act(*o, u.cout), 0
-        else:
-            y, col = out
-        B = x.shape[0]
-        ypt = y.data_ptr() + 4 * col
-        self.ops.append(lambda: _cabi.call(
-            "omt_conv3d", x, x.shape[-1], B, shape[0], shape[1], shape[2], u.w_hi, u.w_lo, u.K, u.bias, u.cout,
-            *k, *s, *front, *o, ypt, y.shape[-1], 1))
+    def _conv(self, u: PackedConv, x, shape, act, out=None):
+        front, o = same_geometry(u.k, u.stride, shape)
+        y, col = (act(*o, u.cout), 0) if out is None else out
+        self.ops.append(u.launch(x, x.shape[0], shape, front, o, y, col))
         return y, o
 
     def _pool(self, x, shape, k, s, act, c):
@@ -233,11 +195,10 @@ class _Workspace:
 class I3D:
     """InceptionI3d (pytorch_i3d.py:163-365) in eval mode from a state_dict in the reference's layout
     (`Conv3d_1a_7x7.conv3d.weight`, `Mixed_4e.b1b.bn.running_var`, ..., `logits.conv3d.{weight,bias}`).  BatchNorm is
-    folded and the weights packed once, on `device`; every (B, T, H, W) gets its own buffers and CUDA graph.
+    folded and the weights packed once, on `device`; every (B, T, H, W) gets its own buffers and CUDA graph (the last
+    few are kept).
     variant: "videogpt" (this network, BatchNorm eps 1e-5) or "styleganv" (the StyleGAN-V I3D's weights mapped onto
     these keys by styleganv_state_dict, eps 1e-3; see load_i3d_styleganv)."""
-
-    MAX_SUITE_WORKSPACES = 4
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", variant: str = "videogpt"):
         if variant not in VARIANT_EPS:
@@ -246,23 +207,14 @@ class I3D:
         sd = {k: v for k, v in state_dict.items() if not k.endswith(".num_batches_tracked")}
         lw = sd.get("logits.conv3d.weight")
         self.num_classes = int(lw.shape[0]) if lw is not None and lw.dim() == 5 else 400
-        want = expected_keys(self.num_classes)
-        missing, unexpected = sorted(set(want) - set(sd)), sorted(set(sd) - set(want))
-        if missing or unexpected:
-            raise KeyError(f"I3D state_dict: missing keys {missing}, unexpected keys {unexpected}")
-        for k, shape in want.items():
-            if tuple(sd[k].shape) != shape:
-                raise ValueError(f"I3D state_dict: {k} has shape {tuple(sd[k].shape)}, expected {shape}")
-        self.device = torch.device(device)
-        if self.device.type == "cuda" and self.device.index is None:      # vqgan_eval.py:59 passes torch.device('cuda')
-            self.device = torch.device("cuda", torch.cuda.current_device())
+        check_state_dict(sd, expected_keys(self.num_classes), "I3D")
+        self.device = resolve_device(device)
         sd = {k: v.detach().float().cpu() for k, v in sd.items()}
         self.units = {}
-        for prefix, cin, cout, k, s in unit_names():
-            w, b = fold_bn(sd[prefix + ".conv3d.weight"],
-                           *(sd[f"{prefix}.bn.{f}"] for f in ("weight", "bias", "running_mean", "running_var")),
-                           eps=VARIANT_EPS[variant])
-            self.units[prefix] = _Unit(*pack_weight(w), b, cout, k, s, self.device)
+        for prefix, _, _, _, s in unit_names():
+            bn = (sd[f"{prefix}.bn.{f}"] for f in ("weight", "bias", "running_mean", "running_var"))
+            w, b = fold_bn(sd[prefix + ".conv3d.weight"], *bn, eps=VARIANT_EPS[variant])
+            self.units[prefix] = PackedConv(w, b, self.device, stride=(s,) * 3)
         self.head_w = sd["logits.conv3d.weight"].reshape(self.num_classes, 1024).contiguous().to(self.device)
         self.head_b = sd["logits.conv3d.bias"].contiguous().to(self.device)
         self.byte_lut = torch.arange(256, dtype=torch.float32).to(self.device)     # torch.FloatTensor(videos)
@@ -295,9 +247,7 @@ class I3D:
         if real_norm is not None:
             real_byte_table(real_norm)                      # refuses a per-channel normalisation before any launch
         key = tuple(int(v) for v in frames_u8.shape[:4]) + (real_norm,)
-        ws = self._ws.get(key)
-        if ws is None:
-            ws = self._ws[key] = _Workspace(self, *key)
+        ws = bounded(self._ws, MAX_WORKSPACES, key, lambda: _Workspace(self, *key))
         ws.u8.copy_(frames_u8)
         run_graphed(ws.graphs, self.device, "i3d", ws.run)
         return ws.out
@@ -316,21 +266,13 @@ class I3D:
         oh, ow = TARGET_RESOLUTION
         for b0 in range(0, B, chunk):
             n = min(chunk, B - b0)
-            key = (n, t)
-            ws = self._suite_ws.get(key)
-            if ws is None:
-                while len(self._suite_ws) >= self.MAX_SUITE_WORKSPACES:
-                    self._suite_ws.pop(next(iter(self._suite_ws)))
-                ws = self._suite_ws[key] = _Workspace(self, n, t, None, None)
+            ws = bounded(self._suite_ws, MAX_WORKSPACES, (n, t), lambda: _Workspace(self, n, t, None, None))
             _cabi.call("omt_fvd_suite_preprocess", clips.src, clips.src.numel(), clips.form, clips.C,
                        clips.desc.data_ptr() + b0 * 4 * CLIP_DESC_WORDS, clips.desc_host[b0:], clips.tab, clips.tab_host,
                        clips.tab_host.numel(), n, t, oh, ow, ws.x)
             run_graphed(ws.graphs, self.device, "i3d", ws.run)
             out[b0:b0 + n] = ws.out
         return out
-
-
-FORM_U8, FORM_F32, FORM_F32_TRUNC = 0, 1, 2      # OMT_FVDS_U8 / OMT_FVDS_F32 / OMT_FVDS_F32_TRUNC
 
 
 def suite_geometry(H: int, W: int, resolution: int = 224) -> Tuple[int, int, int, int]:
@@ -359,25 +301,9 @@ class SuiteClips:
             frame = self.C * H * W
         self.H, self.W = H, W
         rh, rw, cy, cx = suite_geometry(H, W)
-        tv = L.clip_axis_table(H, rh, float(np.float32(H) / np.float32(rh))).reshape(-1)
-        th = L.clip_axis_table(W, rw, float(np.float32(W) / np.float32(rw))).reshape(-1)
-        self.tab_host = torch.from_numpy(np.concatenate([tv, th]).astype(np.int32))
-        desc = torch.zeros(self.B, CLIP_DESC_WORDS, dtype=torch.int32)
-        desc[:, :2] = (torch.arange(self.B, dtype=torch.int64) * (self.T * frame)).view(torch.int32).view(self.B, 2)
-        desc[:, 2:] = torch.tensor([H, W, 0, 0, H, W, rh, rw, cy, cx, 0, 0, tv.size, L.INTERP_SEPARABLE],
-                                   dtype=torch.int32)
-        self.desc_host = desc
-        self.desc, self.tab = desc.to(src.device), self.tab_host.to(src.device)
-
-
-def real_byte_table(norm: L.U8Norm) -> torch.Tensor:
-    """uint8 [n_tab, 256]: the byte vqgan_eval.py feeds I3D for each loader byte u of a real clip,
-    ((v + 0.5) * 255).byte() (:144, :156) of the normalised value v (layout.u8_norm_table, fp32, its own op order).
-    Table 1 (VideoNorm's max <= 1 branch) is only used for clips whose bytes are all 0 or 1."""
-    tab = L.u8_norm_table(norm, 3)                          # [n_tab, 3, 256]
-    if not bool((tab == tab[:, :1]).all()):
-        raise ValueError(f"normalisation {norm.name!r} differs per channel; the FVD byte map is one table per branch")
-    return ((tab[:, 0] + 0.5) * 255).byte()
+        self.tab_host = axis_tables(H, W, rh, rw)
+        self.desc_host = clip_descs(self.B, self.T * frame, H, W, rh, rw, cy, cx)
+        self.desc, self.tab = self.desc_host.to(src.device), self.tab_host.to(src.device)
 
 
 # ------------------------------------------------------------------------------------------------ StyleGAN-V I3D

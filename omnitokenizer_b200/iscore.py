@@ -22,9 +22,9 @@ import torch
 
 from . import _cabi
 from . import fid
-from . import layout as L
 from .engine import CLIP_DESC_WORDS, run_graphed
-from .fvd import FORM_F32, FORM_U8
+from .metricnet import (FORM_F32, FORM_U8, MAX_WORKSPACES, axis_table, axis_tables, bounded,  # noqa: F401
+                        check_state_dict, clip_descs, resolve_device)
 
 NUM_CLASSES = 1000
 FEATURES = fid.DIMS
@@ -63,17 +63,6 @@ def trunk_size(H: int, W: int) -> Tuple[int, int]:
     return hw
 
 
-def axis_table(n_in: int, n_out: Optional[int]) -> np.ndarray:
-    """int32 [n_out, 4] of one axis: torch's bilinear resize of n_in to n_out (layout.clip_axis_table), or, with n_out
-    None (no resize), the identity [n_in, 4] of entries (i, i, 1.0, 0.0), whose fma chain reproduces each value."""
-    if n_out is None:
-        ident = np.zeros((n_in, 4), dtype=np.int32)
-        ident[:, 0] = ident[:, 1] = np.arange(n_in)
-        ident[:, 2] = np.float32(1).view(np.int32)
-        return ident
-    return L.clip_axis_table(n_in, n_out, float(np.float32(n_in) / np.float32(n_out)))
-
-
 class _Workspace(fid.Launches):
     """Buffers, launch list and CUDA graph state of the network on n frames of oh x ow: the input x (written by
     omt_is_preprocess outside the graph), the trunk, the pool, fc, and the softmax into probs."""
@@ -98,18 +87,10 @@ class ISInception:
     BatchNorm is folded and the weights packed once, on `device` (a CUDA device); every (frames, height, width) of a
     launch sequence gets its own buffers and CUDA graph (the last few are kept)."""
 
-    MAX_WORKSPACES = 4
-
     def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda"):
         sd = {k: v for k, v in state_dict.items()
               if not (k.endswith(".num_batches_tracked") or k.startswith("AuxLogits."))}
-        want = expected_keys()
-        missing, unexpected = sorted(set(want) - set(sd)), sorted(set(sd) - set(want))
-        if missing or unexpected:
-            raise KeyError(f"IS Inception3 state_dict: missing keys {missing}, unexpected keys {unexpected}")
-        for k, shape in want.items():
-            if tuple(sd[k].shape) != shape:
-                raise ValueError(f"IS Inception3 state_dict: {k} has shape {tuple(sd[k].shape)}, expected {shape}")
+        check_state_dict(sd, expected_keys(), "IS Inception3")
         self.device = check_device(device)
         sd = {k: v.detach().float().cpu() for k, v in sd.items()}
         self.units = fid.pack_units(sd, self.device)
@@ -117,26 +98,12 @@ class ISInception:
         self._ws = {}
         self._tables = {}
 
-    def _workspace(self, n: int, oh: int, ow: int) -> _Workspace:
-        key = (n, oh, ow)
-        ws = self._ws.get(key)
-        if ws is None:
-            while len(self._ws) >= self.MAX_WORKSPACES:
-                self._ws.pop(next(iter(self._ws)))
-            ws = self._ws[key] = _Workspace(self, n, oh, ow)
-        return ws
-
     def _table(self, H: int, W: int, resize: bool):
-        """(host, device) int32 axis tables of an H x W frame: vertical at word 0, horizontal at word 4 oh."""
-        key = (H, W, resize)
-        t = self._tables.get(key)
-        if t is None:
-            oh, ow = TARGET_RESOLUTION if resize else (None, None)
-            host = torch.from_numpy(np.concatenate([axis_table(H, oh).reshape(-1), axis_table(W, ow).reshape(-1)]))
-            if len(self._tables) >= self.MAX_WORKSPACES:
-                self._tables.pop(next(iter(self._tables)))
-            t = self._tables[key] = (host, host.to(self.device))
-        return t
+        """(host, device) int32 axis tables of an H x W frame (metricnet.axis_tables), resized or at its own size."""
+        def make():
+            host = axis_tables(H, W, *(TARGET_RESOLUTION if resize else (None, None)))
+            return host, host.to(self.device)
+        return bounded(self._tables, MAX_WORKSPACES, (H, W, resize), make)
 
     def probabilities(self, frames: torch.Tensor, resize: bool = True) -> torch.Tensor:
         """F.softmax(inception_model(up(x))) of calculate_is.py's get_pred for every frame: fp32 (N, 3, H, W) frames
@@ -150,15 +117,12 @@ class ISInception:
         src = frames.contiguous()
         oh, ow = TARGET_RESOLUTION if resize else (H, W)
         tab_host, tab = self._table(H, W, resize)
-        desc = torch.zeros(N, CLIP_DESC_WORDS, dtype=torch.int32)
-        desc[:, :2] = (torch.arange(N, dtype=torch.int64) * (3 * H * W)).view(torch.int32).view(N, 2)
-        desc[:, 2:] = torch.tensor([H, W, 0, 0, H, W, oh, ow, 0, 0, 0, 0, 4 * oh, L.INTERP_SEPARABLE],
-                                   dtype=torch.int32)
+        desc = clip_descs(N, 3 * H * W, H, W, oh, ow)
         desc_dev = desc.to(self.device)
         out = torch.empty(N, NUM_CLASSES, device=self.device)
         for f0 in range(0, N, CHUNK_FRAMES):
             n = min(CHUNK_FRAMES, N - f0)
-            ws = self._workspace(n, oh, ow)
+            ws = bounded(self._ws, MAX_WORKSPACES, (n, oh, ow), lambda: _Workspace(self, n, oh, ow))
             _cabi.call("omt_is_preprocess", src, src.numel(), form, desc_dev.data_ptr() + f0 * 4 * CLIP_DESC_WORDS,
                        desc[f0:], tab, tab_host, tab_host.numel(), n, 1, oh, ow, ws.x)
             run_graphed(ws.graphs, self.device, "is", ws.run)
@@ -167,11 +131,9 @@ class ISInception:
 
 
 def check_device(device) -> torch.device:
-    dev = torch.device(device)
+    dev = resolve_device(device)
     if dev.type != "cuda":
         raise ValueError(f"the Inception Score runs on a CUDA device, got {dev}")
-    if dev.index is None:
-        dev = torch.device("cuda", torch.cuda.current_device())
     return dev
 
 

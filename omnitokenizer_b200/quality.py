@@ -27,10 +27,11 @@ import torch
 from . import _cabi
 from . import layout as L
 from .engine import run_graphed
-from .fid import byte_lut
-from .fvd import FORM_F32 as FORM_FVD_F32, FORM_F32_TRUNC as FORM_FVD_F32_TRUNC, FORM_U8 as FORM_FVD_U8
-from .fvd import I3D, SuiteClips, pack_weight, real_byte_table
+from .fvd import I3D, SuiteClips
 from .fvd import frechet_distance as fvd_frechet_distance
+from .metricnet import FORM_F32 as FORM_FVD_F32, FORM_F32_TRUNC as FORM_FVD_F32_TRUNC, FORM_U8 as FORM_FVD_U8
+from .metricnet import (MAX_WORKSPACES, PackedConv, bounded, byte_lut, check_state_dict, real_byte_table,
+                        resolve_device)
 
 FORM_U8, FORM_F32 = 0, 1           # OMT_Q_U8 / OMT_Q_F32
 POOL_MAX = 0                       # omt_pool2d mode
@@ -154,41 +155,20 @@ def input_table(shift: torch.Tensor, scale: torch.Tensor, real_norm: Optional[L.
     return ((x - shift.float().view(1, 3, 1)) / scale.float().view(1, 3, 1)).contiguous()
 
 
-class _Unit:
-    """One 3x3 conv packed for omt_conv3d: tf32 hi / lo planes of W, its bias and widths."""
-
-    def __init__(self, conv: Conv, w, bias, device):
-        packed, self.K = pack_weight(w.float().unsqueeze(2))
-        hi = L.tf32_round(packed)
-        self.w_hi, self.w_lo = hi.to(device), (packed - hi).to(device)
-        self.bias, self.conv = bias.float().contiguous().to(device), conv
-
-
 class LPIPS:
     """lpips.py's LPIPS (VGG16 trunk, five lin layers, ScalingLayer) in eval mode, from a state_dict (see
     lpips_state_dict for the accepted layouts).  A missing or mis-shaped key is named in the error.  The weights are
     packed once, on `device`.  net / spatial: the lpips package's options; anything but VGG without the spatial map
     raises NotImplementedError."""
 
-    MAX_WORKSPACES = 4
-
     def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", net: str = "vgg", spatial: bool = False):
         check_net(net, spatial)
         sd = lpips_state_dict(state_dict)
-        want = expected_keys()
-        missing = sorted(set(want) - set(sd))
-        unexpected = sorted(set(sd) - set(want))
-        if missing or unexpected:
-            raise KeyError(f"LPIPS state_dict: missing keys {missing}, unexpected keys {unexpected}")
-        for k, shape in want.items():
-            if tuple(sd[k].shape) != shape:
-                raise ValueError(f"LPIPS state_dict: {k} has shape {tuple(sd[k].shape)}, expected {shape}")
-        self.device = torch.device(device)
-        if self.device.type == "cuda" and self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
-        sd = {k: sd[k].detach().float().cpu() for k in want}
-        self.units = [[_Unit(c, sd[f"net.slice{c.slice}.{c.idx}.weight"], sd[f"net.slice{c.slice}.{c.idx}.bias"],
-                             self.device) for c in convs] for convs in SLICES]
+        check_state_dict(sd, expected_keys(), "LPIPS")
+        self.device = resolve_device(device)
+        sd = {k: v.detach().float().cpu() for k, v in sd.items()}
+        self.units = [[PackedConv(sd[f"net.slice{c.slice}.{c.idx}.weight"], sd[f"net.slice{c.slice}.{c.idx}.bias"],
+                                  self.device) for c in convs] for convs in SLICES]
         self.lin = [sd[f"lin{k}.model.1.weight"].reshape(-1).contiguous().to(self.device) for k in range(len(CHNS))]
         self.shift, self.scale = sd["scaling_layer.shift"].reshape(3), sd["scaling_layer.scale"].reshape(3)
         self.shift_scale = torch.cat([self.shift, self.scale]).to(self.device)
@@ -244,13 +224,10 @@ class _Workspace:
                 self.ops.append(lambda x_=cur, y_=y, c=c_cur, h_=h, w_=w, ho_=ho, wo_=wo: _cabi.call(
                     "omt_pool2d", x_, c, c, 2 * P, h_, w_, 2, 2, 2, 2, 0, 0, ho_, wo_, y_, c, POOL_MAX))
                 cur, h, w, nxt = y, ho, wo, 1 - nxt
-            for u in units:
-                co = u.conv.cout
-                y = bufs[nxt][:2 * P * h * w * co].view(2 * P, h, w, co)
-                self.ops.append(lambda x_=cur, y_=y, u=u, cs=cur.shape[-1], h_=h, w_=w: _cabi.call(
-                    "omt_conv3d", x_, cs, 2 * P, 1, h_, w_, u.w_hi, u.w_lo, u.K, u.bias, u.conv.cout,
-                    1, 3, 3, 1, 1, 1, 0, 1, 1, 1, h_, w_, y_, u.conv.cout, 1))
-                cur, c_cur, nxt = y, co, 1 - nxt
+            for u in units:                           # 3 x 3, padding 1, ReLU
+                y = bufs[nxt][:2 * P * h * w * u.cout].view(2 * P, h, w, u.cout)
+                self.ops.append(u.launch(cur, 2 * P, (1, h, w), (0, 1, 1), (1, h, w), y))
+                cur, c_cur, nxt = y, u.cout, 1 - nxt
             last = s == len(lpips.units) - 1
             self.ops.append(lambda x_=cur, c=c_cur, h_=h, w_=w, k=s, tot=(self.lp if last else None): _cabi.call(
                 "omt_lpips_head", x_, c, c, P, h_, w_, lpips.lin[k], k, self.lp_taps, tot))
@@ -261,15 +238,6 @@ class _Workspace:
 
 
 _PLAIN_WS: Dict[tuple, _Workspace] = {}
-
-
-def _workspace(cache: dict, cap: int, key: tuple, make):
-    ws = cache.get(key)
-    if ws is None:
-        while len(cache) >= cap:
-            cache.pop(next(iter(cache)))
-        ws = cache[key] = make()
-    return ws
 
 
 def chunk_pairs(P: int, H: int, W: int, with_lpips: bool) -> int:
@@ -318,9 +286,9 @@ def _run(a: torch.Tensor, b: torch.Tensor, form: int, lpips: Optional[LPIPS], re
         n = min(chunk, P - p0)
         key = (dev, form, n, H, W, real_norm)
         if lpips is None:
-            ws = _workspace(_PLAIN_WS, 8, key, lambda: _Workspace(dev, form, n, H, W, real_norm, None))
+            ws = bounded(_PLAIN_WS, 8, key, lambda: _Workspace(dev, form, n, H, W, real_norm, None))
         else:
-            ws = _workspace(lpips._ws, LPIPS.MAX_WORKSPACES, key, lambda: _Workspace(dev, form, n, H, W, real_norm, lpips))
+            ws = bounded(lpips._ws, MAX_WORKSPACES, key, lambda: _Workspace(dev, form, n, H, W, real_norm, lpips))
         ws.a.copy_(a[p0:p0 + n])
         ws.b.copy_(b[p0:p0 + n])
         if ws.sel is not None:
@@ -338,7 +306,7 @@ def frame_metrics(real_u8: torch.Tensor, fake_u8: torch.Tensor, lpips: Optional[
                   real_norm: Optional[L.U8Norm] = None):
     """Per-frame PSNR, SSIM and (with an LPIPS model) VGG LPIPS of device uint8 frames (B, T, H, W, 3) (images:
     T = 1), each byte standing for byte / 255.  real_norm: the real frames are the loader's bytes, and the metrics see
-    the bytes vqgan_eval.py makes of the normalised clip, ((v + 0.5) * 255).byte() (fvd.real_byte_table), with
+    the bytes vqgan_eval.py makes of the normalised clip, ((v + 0.5) * 255).byte() (metricnet.real_byte_table), with
     real_norm's branch picked per clip on the device.  Returns psnr (B, T) fp64, ssim (B, T) fp64 and lpips (B, T)
     fp32 or None, on the device."""
     what = "frame_metrics"
@@ -379,7 +347,7 @@ def _videos_f32(videos1, videos2, what: str, with_lpips: bool, device=None):
         raise ValueError(f"{what}: empty batch {tuple(v1.shape)}")
     _check_sizes(H, W, C, what, with_lpips)
     if device is None:
-        device = v1.device if v1.device.type == "cuda" else torch.device("cuda", torch.cuda.current_device())
+        device = resolve_device(v1.device if v1.device.type == "cuda" else "cuda")
     out = [t.to(device=device, dtype=torch.float32).permute(0, 1, 3, 4, 2).reshape(B * T, H, W, 3).contiguous()
            for t in (v1, v2)]
     return out[0], out[1], (B, T), v1[0].shape
