@@ -209,6 +209,24 @@ int omt_is_preprocess(const void* src, long long src_elems, int form, const omt_
                       const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host, long long tab_len,
                       int B, int F, int oh, int ow, float* out, omt_stream_t stream);
 
+/* vqgan_eval.py's --infer_downsample (:121-136, then :147-148) of B clips of F frames, torch's fp32 CPU arithmetic bit for
+ * bit: the descriptors and axis tables of omt_resample_clips (no flip, no window, no crop; desc.form picks torch's
+ * bilinear kernel for the call shape and thread count).  Each source sample is read in one of two forms:
+ *   OMT_DS_F32: the decoder's fp32 reconstruction 'b c t h w', (3, F, H, W) per clip from desc.src (floats),
+ *               v = clamp(x + 0.5, 0, 1)   (the reconstruction side);
+ *   OMT_DS_U8:  the loader's uint8 (F, H, W, 3) clips from desc.src (bytes), v = lut[byte] (lut: fp32 [256], e.g.
+ *               VideoNorm(byte) + 0.5; with sel != NULL, lut is fp32 [2][256] and clip b reads table sel[b], 0 or 1 --
+ *               omt_u8_norm_select writes it on the device)   (the real side);
+ *   out = (uint8)(y * 255): the product truncated to int32 and its low byte kept, as .byte() does on x86-64,
+ * written channels-last: out (B, F, oh, ow, 3) uint8, the frames I3D.logits reads.  lut / sel are ignored for
+ * OMT_DS_F32 (NULL allowed).  src_elems counts elements of src. */
+#define OMT_DS_F32 0
+#define OMT_DS_U8 1
+int omt_eval_downsample(const void* src, long long src_elems, int form, const omt_clip_desc* desc,
+                        const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host, long long tab_len,
+                        const float* lut, const int32_t* sel, int B, int F, int oh, int ow, uint8_t* out,
+                        omt_stream_t stream);
+
 /* Unit3D of the FVD I3D (fvd/pytorch_i3d.py:59-131) as an implicit GEMM in 3xTF32 on sm_90a wgmma:
  *   y[m, n] = act(sum_k A[m, k] W[n, k] + bias[n]),  m = ((b To + to) Ho + ho) Wo + wo,  n < N,  act = ReLU if relu
  *   A[m, (dt, dh, dw, c)] = x[b][to st - pt + dt][ho sh - ph + dh][wo sw - pw + dw][c], zero outside the volume

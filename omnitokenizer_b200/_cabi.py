@@ -65,6 +65,8 @@ SIGNATURES = {
                                          c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "omt_is_preprocess": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
                                   c_int, c_int, c_int, c_void_p, c_void_p]),
+    "omt_eval_downsample": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                    c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "omt_conv3d": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]
                    + [c_int] * 13 + [c_void_p, c_int, c_int, c_void_p]),
     "omt_maxpool3d": (c_int, [c_void_p] + [c_int] * 17 + [c_void_p, c_void_p]),

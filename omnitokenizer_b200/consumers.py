@@ -14,6 +14,7 @@ from typing import Optional, Sequence, Tuple
 
 import torch
 
+from . import layout as L
 from .layout import (ClipResize, U8Norm, U8Resize, clip_params, dit_resize, resize_clip, resize_params, resize_u8,
                      u8_normalize)
 
@@ -173,20 +174,61 @@ def eval_step_u8(vqgan, frames: torch.Tensor, total_usage: Optional[torch.Tensor
     return out, vq_output
 
 
+def check_replacewithgt(k, T: int, sequence_length: Optional[int], what: str) -> int:
+    """vqgan_eval.py's --replacewithgt k (type=int): 0 <= k <= T, and the clip as long as --sequence_length (:145)."""
+    if isinstance(k, bool) or not isinstance(k, int):
+        raise TypeError(f"{what}: replacewithgt must be an integer frame count, got {k!r}")
+    if not 0 <= k <= T:
+        raise ValueError(f"{what}: replacewithgt {k} outside [0, {T}] for {T}-frame clips")
+    if sequence_length is not None and T != sequence_length:
+        raise ValueError(f"{what}: replacewithgt needs clips of sequence_length {sequence_length} frames, got T={T}")
+    return k
+
+
 @torch.no_grad()
 def eval_step_fvd(vqgan, frames: torch.Tensor, i3d, total_usage: Optional[torch.Tensor] = None,
-                  norm: U8Norm = VIDEO_NORM):
+                  norm: U8Norm = VIDEO_NORM, infer_downsample: Optional[int] = None, replacewithgt: Optional[int] = None,
+                  sequence_length: Optional[int] = None, one_thread: Optional[bool] = None):
     """The body of vqgan_eval.py's video loop (:114-152) from the loader's uint8 clips (B, T, H, W, 3) on the device:
     forward_u8 (eval_step_u8) for the reconstruction's bytes, and the FVD logits of both sides on the device
     (fvd.I3D).  The real side sees the bytes the script makes of the normalised clip, shift_dim((video + 0.5) * 255,
     1, -1).byte(), as a per-byte map with norm's branch picked per clip.  Returns (real_logits, fake_logits,
-    vq_output); no frame crosses to the host."""
+    vq_output); no frame crosses to the host.
+    infer_downsample d (:121-136): both sides are scored at 1 / d of their size: forward_u8's fp32 reconstruction and
+    the real values go through F.interpolate(scale_factor=1 / d) in torch's CPU arithmetic, then * 255 and .byte()
+    (downsample.clips_u8; one_thread as there).  replacewithgt k (:142-145): the first k reconstructed frames are the
+    real ones; sequence_length, when given, is the script's --sequence_length, which the clips must match."""
     from .metricnet import real_byte_table
     _check_u8(frames, (5,), "eval_step_fvd")
     i3d.check_frames(frames)                 # every refusal before the first launch
     real_byte_table(norm)
-    fake, vq_output = eval_step_u8(vqgan, frames, total_usage, norm)
-    real_logits = i3d.logits(frames, real_norm=norm).clone()
+    if infer_downsample is None and replacewithgt is None:
+        fake, vq_output = eval_step_u8(vqgan, frames, total_usage, norm)
+        real_logits = i3d.logits(frames, real_norm=norm).clone()
+        fake_logits = i3d.logits(fake).clone()
+        return real_logits, fake_logits, vq_output
+
+    from . import downsample
+    d = 1 if infer_downsample is None else L.check_infer_downsample(infer_downsample, "eval_step_fvd")
+    B, T, H, W, _ = (int(v) for v in frames.shape)
+    k = 0 if replacewithgt is None else check_replacewithgt(replacewithgt, T, sequence_length, "eval_step_fvd")
+    downsample.out_size(H, W, d, "eval_step_fvd")
+    downsample.real_value_table(norm)
+    if frames.device.type != "cuda" or frames.device != i3d.device:
+        raise ValueError(f"eval_step_fvd: frames on {frames.device}, the I3D is on {i3d.device}")
+    frames = frames.contiguous()
+    if hasattr(vqgan, "forward_u8"):
+        x_recons, vq_output = vqgan.forward_u8(frames, norm, None)
+    else:
+        _, _, _, x_recons, vq_output = vqgan(u8_normalize(frames, norm), log_image=True)
+    if total_usage is not None and vq_output is not None:
+        total_usage += vq_output["batch_usage"]
+    # with d = 1 (replacewithgt alone) the interpolation is the identity and the launches only map the values to bytes
+    real = downsample.clips_u8(frames, d, real_norm=norm, one_thread=one_thread, what="eval_step_fvd")
+    fake = downsample.clips_u8(x_recons.float().contiguous(), d, one_thread=one_thread, what="eval_step_fvd")
+    if k:
+        fake[:, :k].copy_(real[:, :k])
+    real_logits = i3d.logits(real).clone()
     fake_logits = i3d.logits(fake).clone()
     return real_logits, fake_logits, vq_output
 
@@ -264,19 +306,23 @@ def eval_step_images_u8(vqgan, images: Sequence[torch.Tensor], resize: U8Resize,
 
 @torch.no_grad()
 def eval_step_fid(vqgan, images: Sequence[torch.Tensor], resize: U8Resize, inception,
-                  total_usage: Optional[torch.Tensor] = None, norm: U8Norm = IMAGE_NORM):
+                  total_usage: Optional[torch.Tensor] = None, norm: U8Norm = IMAGE_NORM,
+                  infer_downsample: Optional[int] = None):
     """The body of vqgan_eval.py's image loop (:185-220) from the decoded ragged host images of ImageDataset, with the
     PNG round trip and the pytorch-fid run replaced by FID features on the device (fid.FIDInception): forward_images_u8
     for the reconstruction's bytes and vq_output, and the pool3 features of both sides.  The real side reads the
     transformed input bytes that call wrote into the encode_u8 slot (the random crop and flip are drawn once) and sees
     the bytes the script saves of the normalised input, ((x + 0.5) * 255).astype(uint8), as a per-byte map.  Returns
     (real_features, fake_features, vq_output), each features (B, 2048) fp32; no image crosses to the host.
-    --infer_downsample (a PIL ANTIALIAS resize before saving) is not supported."""
+    infer_downsample d (:207-208, :218-219): both sides' saved bytes are first resized to (h // d, h // d) with
+    Image.ANTIALIAS (Pillow's LANCZOS, downsample.images_u8); the real side's byte map then comes before the resize."""
     from .metricnet import real_byte_table
     images = list(images)
     if not images:
         raise ValueError("eval_step_fid needs at least one image")
     real_byte_table(norm)                    # refuses a per-channel normalisation before the first launch
+    if infer_downsample is not None:
+        return _eval_step_fid_downsample(vqgan, images, resize, inception, total_usage, norm, infer_downsample)
     if hasattr(vqgan, "forward_images_u8"):
         fake, vq_output = vqgan.forward_images_u8(images, resize, norm, EVAL_U8)
         if total_usage is not None and vq_output is not None:
@@ -288,6 +334,34 @@ def eval_step_fid(vqgan, images: Sequence[torch.Tensor], resize: U8Resize, incep
         real = real.unsqueeze(1)
     real_features = inception.features(real[:, 0], real_norm=norm).clone()
     fake_features = inception.features(fake[:, 0].contiguous()).clone()
+    return real_features, fake_features, vq_output
+
+
+def _eval_step_fid_downsample(vqgan, images, resize: U8Resize, inception, total_usage, norm: U8Norm, d):
+    from . import downsample
+    d = L.check_infer_downsample(d, "eval_step_fid")
+    h, w = resize.out_size
+    if h != w:
+        raise ValueError(f"eval_step_fid: infer_downsample resizes square images, the transform makes {h}x{w}")
+    L.eval_downsample_resize(h, d)                       # refuses a factor that leaves no pixel
+    downsample.real_value_table(norm)
+    if inception.device.type != "cuda":
+        raise ValueError(f"eval_step_fid: the FID network is on {inception.device}, not a CUDA device")
+    if hasattr(vqgan, "forward_images_u8"):
+        fake, vq_output = vqgan.forward_images_u8(images, resize, norm, EVAL_U8)
+        if total_usage is not None and vq_output is not None:
+            total_usage += vq_output["batch_usage"]
+        real = vqgan.engine().encode_u8_frames(tuple(fake.shape))
+    else:
+        real = _host_transform(images, resize).to(inception.device)
+        fake, vq_output = eval_step_u8(vqgan, real, total_usage, norm)
+        real = real.unsqueeze(1)
+    # the saved input bytes ((x + 0.5) * 255).astype(uint8): the value map at d = 1 (an identity interpolation)
+    real = downsample.clips_u8(real.contiguous(), 1, real_norm=norm, what="eval_step_fid")
+    real_small = downsample.images_u8(real[:, 0], d, "eval_step_fid")
+    fake_small = downsample.images_u8(fake[:, 0].contiguous(), d, "eval_step_fid")
+    real_features = inception.features(real_small).clone()
+    fake_features = inception.features(fake_small).clone()
     return real_features, fake_features, vq_output
 
 

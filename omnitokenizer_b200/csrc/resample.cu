@@ -318,6 +318,62 @@ fvd_suite_preprocess_kernel(const void* __restrict__ src, const omt_clip_desc* _
   }
 }
 
+// omt_eval_downsample: vqgan_eval.py's --infer_downsample, F.interpolate(scale_factor = 1 / d) of the clamped
+// reconstruction (OMT_DS_F32) or of the real clip's values (OMT_DS_U8, by byte table), then * 255 and .byte(), written
+// channels-last as uint8.  The tile walk and bilinear arithmetic of resample_clips_body; its own kernel, so the loader
+// and metric preprocess kernels above stay as they are.
+template <int FORM>
+__global__ void __launch_bounds__(RC_TW)
+eval_downsample_kernel(const void* __restrict__ src, const omt_clip_desc* __restrict__ desc, const int4* __restrict__ tab,
+                       const float* __restrict__ lut_g, const int32_t* __restrict__ sel, uint8_t* __restrict__ out, int F,
+                       int oh, int ow) {
+  __shared__ float lut[256];
+  pdl_sync();
+  const int b = blockIdx.z / F, f = blockIdx.z % F;
+  const omt_clip_desc d = desc[b];
+  if constexpr (FORM == OMT_DS_U8) {
+    const float* t = lut_g + (sel != nullptr ? 256 * __ldg(sel + b) : 0);
+    for (int i = threadIdx.x; i < 256; i += RC_TW) lut[i] = __ldg(t + i);
+    __syncthreads();
+  }
+  const int ox = blockIdx.x * RC_TW + threadIdx.x;
+  if (ox >= ow) return;
+  const int4 ew = __ldg(tab + d.th / 4 + d.cx + ox);
+  const float l0w = __int_as_float(ew.z), l1w = __int_as_float(ew.w);
+  const long long plane = (long long)d.H * d.W;
+  // OMT_DS_U8: frame f of the clip's (F, H, W, 3) bytes; OMT_DS_F32: channel c's frame f at + c F plane
+  const long long frame = d.src + (long long)f * plane * (FORM == OMT_DS_U8 ? 3 : 1);
+  auto value = [&](int y, int x, int c) -> float {
+    if constexpr (FORM == OMT_DS_U8) {
+      return lut[__ldg(static_cast<const uint8_t*>(src) + frame + ((long long)y * d.W + x) * 3 + c)];
+    } else {
+      const float v = __fadd_rn(__ldg(static_cast<const float*>(src) + frame + c * F * plane + (long long)y * d.W + x), 0.5f);
+      return v != v ? v : fminf(fmaxf(v, 0.f), 1.f);        // torch.clamp keeps a NaN
+    }
+  };
+  const int y_end = min(oh, (int)blockIdx.y * RC_TH + RC_TH);
+  for (int oy = blockIdx.y * RC_TH; oy < y_end; ++oy) {
+    const int4 eh = __ldg(tab + d.tv / 4 + d.cy + oy);
+    const float l0h = __int_as_float(eh.z), l1h = __int_as_float(eh.w);
+    const float w00 = __fmul_rn(l0h, l0w), w01 = __fmul_rn(l0h, l1w), w10 = __fmul_rn(l1h, l0w), w11 = __fmul_rn(l1h, l1w);
+    uint8_t* o = out + (((long long)blockIdx.z * oh + oy) * ow + ox) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float x00 = value(eh.x, ew.x, c), x01 = value(eh.x, ew.y, c);
+      const float x10 = value(eh.y, ew.x, c), x11 = value(eh.y, ew.y, c);
+      float v;
+      if (d.form) {
+        v = __fmaf_rn(x11, w11, __fmaf_rn(x10, w10, __fmaf_rn(x00, w00, __fmul_rn(x01, w01))));
+      } else {
+        const float t0 = __fmaf_rn(x00, l0w, __fmul_rn(x01, l1w));
+        const float t1 = __fmaf_rn(x10, l0w, __fmul_rn(x11, l1w));
+        v = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
+      }
+      o[c] = (uint8_t)(__float2int_rz(__fmul_rn(v, 255.f)) & 255);
+    }
+  }
+}
+
 // One axis table of a clip: [n_out][4] entries at word `off` inside the table, every (i0, i1) inside an axis of n_in.
 bool clip_axis_ok(const int32_t* tab_host, long long tab_len, int off, int n_out, int n_in) {
   if (off < 0 || off % 4 != 0 || off + 4LL * n_out > tab_len) return false;
@@ -511,4 +567,35 @@ extern "C" int omt_is_preprocess(const void* src, long long src_elems, int form,
               "omt_is_preprocess: input form %d is neither uint8 (0) nor fp32 (1)", form);
   return suite_preprocess<false>("omt_is_preprocess", src, src_elems, form, 3, desc, desc_host, tab, tab_host, tab_len,
                                  B, F, oh, ow, out, stream);
+}
+
+extern "C" int omt_eval_downsample(const void* src, long long src_elems, int form, const omt_clip_desc* desc,
+                                   const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
+                                   long long tab_len, const float* lut, const int32_t* sel, int B, int F, int oh,
+                                   int ow, uint8_t* out, omt_stream_t stream) {
+  OMT_ENTER();
+  const char* who = "omt_eval_downsample";
+  OMT_REQUIRE(form == OMT_DS_F32 || form == OMT_DS_U8, "%s: input form %d is neither fp32 (0) nor uint8 (1)", who, form);
+  OMT_REQUIRE(form == OMT_DS_F32 || lut, "%s: uint8 clips need a byte table", who);
+  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab}) && aligned_to(4, {lut, sel}) &&
+                  (form == OMT_DS_U8 || aligned_to(4, {src})),
+              "%s: desc must be 8-byte, tab 16-byte and lut / sel / fp32 src 4-byte aligned", who);
+  // check_clips counts a frame as H W 3 elements: true of both forms (3 planes of H W floats, or H W pixels of 3 bytes)
+  int rc = check_clips(who, src, src_elems, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow,
+                       reinterpret_cast<float*>(out), 3);
+  if (rc != OMT_OK) return rc;
+  for (int b = 0; b < B; ++b) {
+    const omt_clip_desc& d = desc_host[b];
+    OMT_REQUIRE(!d.flip && d.y0 == 0 && d.x0 == 0 && d.wh == d.H && d.ww == d.W,
+                "%s: clip %d: the eval downsample has no flip and no window", who, b);
+  }
+  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
+  const int4* t4 = reinterpret_cast<const int4*>(tab);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (form == OMT_DS_U8)
+    OMT_CUDA(launch_k(eval_downsample_kernel<OMT_DS_U8>, grid, dim3(RC_TW), 0, s, src, desc, t4, lut, sel, out, F, oh, ow));
+  else
+    OMT_CUDA(launch_k(eval_downsample_kernel<OMT_DS_F32>, grid, dim3(RC_TW), 0, s, src, desc, t4, lut, sel, out, F, oh, ow));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
 }

@@ -57,7 +57,7 @@ class U8Resize(NamedTuple):
     """An image loader's geometric transform before ToTensor: torchvision Resize(size, filter) on the PIL image (Pillow's
     8-bit resize), then optionally RandomCrop(crop) and RandomHorizontalFlip(0.5), in that order."""
     size: Tuple[int, int]          # (height, width) after the resize
-    filter: str = "bicubic"        # Pillow filter: "bicubic", "bilinear" or "box"
+    filter: str = "bicubic"        # Pillow filter: "bicubic", "bilinear", "box" or "antialias" (LANCZOS)
     crop: int = 0                  # side of the square random crop of the resized image; 0: none
     flip: bool = False
 
@@ -81,6 +81,25 @@ def dit_resize(image_size: int) -> U8Resize:
     """DiT with the OmniTokenizer VAE (Diffusion/DiT/train.py:192-198): Resize((s, s)) -- torchvision's default filter,
     BILINEAR -- then RandomHorizontalFlip."""
     return U8Resize((image_size, image_size), "bilinear", flip=True)
+
+
+def check_infer_downsample(d, what: str = "infer_downsample") -> int:
+    """vqgan_eval.py's --infer_downsample (type=int): an integer factor d >= 1.  Returns it as an int."""
+    if isinstance(d, bool) or not isinstance(d, (int, np.integer)):
+        raise TypeError(f"{what}: infer_downsample must be an integer factor, got {d!r}")
+    if d < 1:
+        raise ValueError(f"{what}: infer_downsample must be >= 1, got {d}")
+    return int(d)
+
+
+def eval_downsample_resize(resolution: int, d: int) -> U8Resize:
+    """vqgan_eval.py's image branch with --infer_downsample d (:207-208, :218-219): img.resize((res // d, res // d),
+    Image.ANTIALIAS), Pillow's LANCZOS, of the saved input and reconstruction."""
+    d = check_infer_downsample(d)
+    side = int(resolution) // d
+    if side < 1:
+        raise ValueError(f"infer_downsample {d} leaves {resolution} // {d} = {side} pixels")
+    return U8Resize((side, side), "antialias")
 
 
 def check_resize(resize: U8Resize):
@@ -110,7 +129,22 @@ def _box(x):
     return np.where((x > -0.5) & (x <= 0.5), 1.0, 0.0)
 
 
-_FILTERS = {"bicubic": (_bicubic, 2.0), "bilinear": (_bilinear, 1.0), "box": (_box, 0.5)}
+def _sinc(x):
+    """Resample.c sinc_filter: sin(pi x) / (pi x), 1 at 0.  sin from the C library, as Pillow calls it (numpy's own
+    vectorised sin may differ in the last bit)."""
+    px = x * math.pi
+    s = np.array([math.sin(v) for v in px.reshape(-1)], dtype=np.float64).reshape(px.shape)
+    return np.where(x == 0.0, 1.0, s / np.where(x == 0.0, 1.0, px))
+
+
+def _lanczos(x):
+    """Resample.c lanczos_filter: the sinc truncated to [-3, 3), windowed by sinc(x / 3)."""
+    x = np.asarray(x, dtype=np.float64)
+    return np.where((x >= -3.0) & (x < 3.0), _sinc(x) * _sinc(x / 3), 0.0)
+
+
+# "antialias": Pillow's LANCZOS under the name vqgan_eval.py resizes with (Image.ANTIALIAS, LANCZOS's old alias)
+_FILTERS = {"bicubic": (_bicubic, 2.0), "bilinear": (_bilinear, 1.0), "box": (_box, 0.5), "antialias": (_lanczos, 3.0)}
 RESAMPLE_BITS = 22       # Resample.c PRECISION_BITS for 8-bit images
 
 
@@ -403,6 +437,47 @@ def resize_clip(clip: torch.Tensor, resize: ClipResize, flip: bool = False, norm
     if norm is not None:
         out = (out - np.asarray(norm.mean, np.float32)) / np.asarray(norm.std, np.float32)
     return torch.from_numpy(np.ascontiguousarray(out.transpose(0, 3, 1, 2)))
+
+
+@functools.lru_cache(maxsize=1024)
+def downsample_geometry(H: int, W: int, d: int) -> ClipGeometry:
+    """vqgan_eval.py's F.interpolate(scale_factor=1 / d, mode="bilinear", align_corners=False) of an H x W frame: the
+    output size from torch's own shape rule (floor of n * (1 / d) in double, so 63 at d = 3 gives 20), and the coordinate
+    scale torch's CPU kernel uses for a given scale_factor, static_cast<float>(1.0 / scale_factor)."""
+    x = torch.empty(1, 1, H, W, device="meta")
+    y = torch.nn.functional.interpolate(x, scale_factor=1 / d, mode="bilinear", align_corners=False)
+    rh, rw = int(y.shape[-2]), int(y.shape[-1])
+    inv = float(np.float32(1.0 / (1 / d)))
+    return ClipGeometry(0, 0, H, W, rh, rw, 0, 0, inv, inv)
+
+
+def downsample_clips(src: torch.Tensor, d: int, one_thread: bool, value_table: torch.Tensor = None,
+                     sel=None) -> torch.Tensor:
+    """Host twin of omt_eval_downsample: (B, T, oh, ow, 3) uint8 = shift_dim(F.interpolate(v, scale_factor=1 / d) * 255,
+    1, -1).byte() in torch's CPU arithmetic (the kernel form clip_interp_form picks for one_thread), of
+    - src fp32 (B, 3, T, H, W), the decoder's reconstruction: v = clamp(src + 0.5, 0, 1) (value_table None);
+    - src uint8 (B, T, H, W, 3), the loader's bytes: v = value_table[sel[b]][byte] (value_table fp32 [n_tab, 256],
+      sel per clip, all 0 when None)."""
+    if value_table is None:
+        v = torch.clamp(src.float() + 0.5, 0, 1).permute(0, 2, 3, 4, 1).numpy()
+    else:
+        B = src.shape[0]
+        sel = np.zeros(B, dtype=np.int64) if sel is None else np.asarray(sel, dtype=np.int64)
+        v = value_table.numpy()[sel.reshape(B, 1, 1, 1, 1), src.numpy()]
+    B, T, H, W, _ = v.shape
+    g = downsample_geometry(H, W, d)
+    th = clip_axis_table(H, g.rh, g.scale_h)
+    tw = clip_axis_table(W, g.rw, g.scale_w)
+    l0h, l1h = (th[:, k].view(np.float32)[None, None, :, None, None] for k in (2, 3))
+    l0w, l1w = (tw[:, k].view(np.float32)[None, None, None, :, None] for k in (2, 3))
+    r0, r1 = v[:, :, th[:, 0]], v[:, :, th[:, 1]]
+    x00, x01, x10, x11 = r0[:, :, :, tw[:, 0]], r0[:, :, :, tw[:, 1]], r1[:, :, :, tw[:, 0]], r1[:, :, :, tw[:, 1]]
+    if clip_interp_form(g, one_thread) == INTERP_WEIGHTS:
+        out = fma32(x11, l1h * l1w, fma32(x10, l1h * l0w, fma32(x00, l0h * l0w, x01 * (l0h * l1w))))
+    else:
+        out = fma32(fma32(x00, l0w, x01 * l1w), l0h, fma32(x10, l0w, x11 * l1w) * l1h)
+    # .byte(): the product truncated to int32, its low byte kept (x86-64)
+    return torch.from_numpy((out * np.float32(255)).astype(np.int32).astype(np.uint8))
 
 
 def peg_neighbour_table(T: int, h: int, w: int, temporal: bool, causal: bool) -> torch.Tensor:

@@ -699,7 +699,8 @@ class OmniTokenizer_VQGAN(nn.Module):
         """forward(x, log_image=True) from uint8 frames, with uint8 out: frames (B, T, H, W, C) or images (B, H, W, C),
         normalised in the patch gather by `norm` (default VIDEO_NORM).  Returns (x_recon, vq_output): x_recon is
         the reconstruction as uint8 'b t h w c' (T = 1 for images) = _to_u8(forward's x_recon, out_affine) byte for byte
-        (default: vqgan_eval.py:139,147-148), vq_output is forward's (None for the VAE).  The CPU RNG is consumed as
+        (default: vqgan_eval.py:139,147-148), vq_output is forward's (None for the VAE).  out_affine None: x_recon is
+        forward's fp32 reconstruction 'b c t h w' on the device instead (T = 1 for images).  The CPU RNG is consumed as
         forward consumes it (VAE noise, then the random frame's randint), so a seeded eval loop stays in step."""
         if self.resolution_scale is not None:
             raise NotImplementedError("resolution_scale resizes the fp32 frames between the / 255 and the shift "
@@ -709,7 +710,8 @@ class OmniTokenizer_VQGAN(nn.Module):
         eng = self.engine()
         with torch.cuda.device(self.device):
             ws, dims = eng.encode_u8(f, "raw" if self.use_vae else "vq", norm)
-            x_recon, vq_output = self._forward_decode(eng, ws, dims, u8=tuple(float(v) for v in out_affine))
+            u8 = None if out_affine is None else tuple(float(v) for v in out_affine)
+            x_recon, vq_output = self._forward_decode(eng, ws, dims, u8=u8)
             if not is_image:
                 torch.randint(0, f.shape[1], [f.shape[0]])                      # forward's random-frame draw (omnitokenizer.py:401)
             return x_recon, vq_output
