@@ -159,218 +159,181 @@ resample_u8_kernel(const uint8_t* __restrict__ src, const omt_resample_desc* __r
   }
 }
 
-// omt_resample_clips: the Latte video loaders' ToTensorVideo -> flip -> bilinear F.interpolate (+ centre crop) ->
-// Normalize, in torch's fp32 CPU arithmetic (either of its two bilinear kernels, per clip: desc.form).  Its own kernel:
-// nothing here is shared with Pillow's integer resize.
-// Each CTA owns RC_TW output columns (one per thread) x RC_TH rows of one frame of one clip; a thread's horizontal table
-// entry is loaded once, and each output row reads exactly two source rows.  Stores run along w within a channel plane.
-// OUT = OUT_FVD (omt_fvd_preprocess): fvd.py's preprocess instead of the loaders' Normalize.  The byte table holds the
-// value each byte stands for (table sel[b] of two when sel is given), the result is 2 y / 255 - 1 in that order, and a
-// frame leaves channels-last as [oh][ow][4] with channel 3 zero (the I3D input layout).
-// OUT = OUT_FID (omt_fid_preprocess): pytorch-fid's ToTensor -> F.interpolate -> 2 x - 1.  The same layout and tables, but
-// the byte table already holds byte / 255 (the division comes before the resize), and the result is 2 y - 1.
+// The bilinear clip kernel of omt_resample_clips, omt_fvd_preprocess, omt_fid_preprocess, omt_fvd_suite_preprocess,
+// omt_is_preprocess and omt_eval_downsample: torch's fp32 CPU F.interpolate(bilinear, align_corners=False) of B clips
+// of F frames, bit for bit, in either of its two kernels per clip (desc.form).  Nothing here is shared with Pillow's
+// integer resize above.  A source policy says what one sample of a frame is worth in fp32; an output policy says what
+// the three resized channel values of a pixel become and where they go.  Each policy keeps the exact intrinsics of the
+// reference it stands for.
+// Each CTA owns RC_TW output columns (one per thread) x RC_TH rows of one frame of one clip (blockIdx.z = b F + f); a
+// thread's horizontal table entry is loaded once, and each output row reads exactly two source rows.  The window origin
+// and the flip apply to every entry point; the host check of those that have neither refuses them.
 constexpr int RC_TW = 128;
 constexpr int RC_TH = 8;
-enum { OUT_NORMALIZE = 0, OUT_FVD = 1, OUT_FID = 2 };
 
-template <int OUT>
-__device__ __forceinline__ void resample_clips_body(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
-                                                    const int4* __restrict__ tab, const float* __restrict__ norm,
-                                                    float* __restrict__ out, int F, int oh, int ow,
-                                                    const int32_t* __restrict__ sel) {
-  constexpr bool FVD = OUT != OUT_NORMALIZE;     // a feature network's input: byte table sel[b], [oh][ow][4] out
-  __shared__ float lut[256];
+// Source policies.  begin() runs once per thread before any thread leaves (a byte table is loaded there) and points
+// the policy at frame f of clip b; then (y, x, c) is channel c of the frame's sample at row y0 + y, column x, as fp32.
+// begin() adds the window's y0 once: added in the row loop, it cost the table instances 8 registers.
+// lut[byte] of (F, H, W, 3) bytes through a 256-entry table in shared memory, table sel[b] of two when sel is given:
+// the loaders (to_tensor's byte / 255), FVD (float(byte) or a byte map), FID (byte / 255) and the eval downsample's
+// real clips (VideoNorm(byte) + 0.5).
+struct ByteTable {
+  static constexpr bool TABLE = true;
+  const uint8_t* src;
+  const float* lut;
+  const int32_t* sel;
+  const float* t = nullptr;
+  const uint8_t* frame = nullptr;
+  int W = 0;
+  __device__ void begin(const omt_clip_desc& d, int b, int f, int) {
+    __shared__ float s[256];
+    const float* g = sel != nullptr ? lut + 256 * __ldg(sel + b) : lut;
+    for (int i = threadIdx.x; i < 256; i += RC_TW) s[i] = __ldg(g + i);
+    __syncthreads();
+    t = s;
+    frame = src + d.src + ((long long)f * d.H + d.y0) * d.W * 3;
+    W = d.W;
+  }
+  __device__ float operator()(int y, int x, int c) const { return t[__ldg(frame + (long long)y * W * 3 + x * 3 + c)]; }
+};
+
+// The video-metric suite's and the Inception Score's frames (desc.src counts elements; the frames of a clip follow each
+// other, so a clip stored with a longer time axis is read as its first F frames):
+//   OMT_FVDS_U8:        (F, H, W, 3) bytes, (float)byte / 255, a true division;
+//   OMT_FVDS_F32:       fp32 (F, C, H, W), C == 1 read by every channel, used as they are (styleganv);
+//   OMT_FVDS_F32_TRUNC: the same through videogpt's (videos * 255).numpy().astype(np.uint8), then .float() / 255.  The
+//                       cast truncates to int32 and keeps the low byte, as the x86-64 conversion does for products
+//                       inside the int32 range.
+__device__ __forceinline__ float suite_u8_value(int b) { return __fdiv_rn((float)b, 255.f); }
+
+template <int FORM>
+struct SuiteFrames {
+  static constexpr bool TABLE = false;
+  const void* src;
+  int C;
+  long long frame = 0;
+  int H = 0, W = 0;
+  __device__ void begin(const omt_clip_desc& d, int, int f, int) {
+    frame = d.src + (FORM == OMT_FVDS_U8 ? 3 * ((long long)f * d.H + d.y0) : (long long)f * C * d.H + d.y0) * d.W;
+    H = d.H;
+    W = d.W;
+  }
+  __device__ float operator()(int y, int x, int c) const {
+    if constexpr (FORM == OMT_FVDS_U8) {
+      return suite_u8_value(__ldg(static_cast<const uint8_t*>(src) + frame + ((long long)y * W + x) * 3 + c));
+    } else {
+      const float v = __ldg(static_cast<const float*>(src) + frame + ((long long)(C == 1 ? 0 : c) * H + y) * W + x);
+      if constexpr (FORM == OMT_FVDS_F32) return v;
+      return suite_u8_value(__float2int_rz(__fmul_rn(v, 255.f)) & 255);
+    }
+  }
+};
+
+// clamp(x + 0.5, 0, 1) of the decoder's fp32 reconstruction, (3, F, H, W) per clip: the eval downsample's other side.
+struct ClampedPlanes {
+  static constexpr bool TABLE = false;
+  const float* src;
+  const float* frame = nullptr;
+  long long cstride = 0;
+  int W = 0;
+  __device__ void begin(const omt_clip_desc& d, int, int f, int F) {
+    const long long plane = (long long)d.H * d.W;
+    frame = src + d.src + f * plane + (long long)d.y0 * d.W;
+    cstride = F * plane;
+    W = d.W;
+  }
+  __device__ float operator()(int y, int x, int c) const {
+    const float v = __fadd_rn(__ldg(frame + c * cstride + (long long)y * W + x), 0.5f);
+    return v != v ? v : fminf(fmaxf(v, 0.f), 1.f);        // torch.clamp keeps a NaN
+  }
+};
+
+// Output policies: (y, b, f, F, oy, ox, oh, ow) writes the resized values y[3] of output pixel (oy, ox) of frame f of
+// clip b.  Each pointer `out` is aligned to the size of what it points to.
+// The loaders' Normalize, (y - mean_c) / std_c with a true division, channel-planar (B, 3, F, oh, ow); norm is the
+// loaders' table: 256 byte values, then mean[3], then std[3].
+struct NormalizePlanes {
+  float* out;
+  const float* norm;
+  __device__ void operator()(const float (&y)[3], int b, int f, int F, int oy, int ox, int oh, int ow) const {
+    const long long plane = (long long)oh * ow;
+    float* o = out + ((long long)b * 3 * F + f) * plane + (long long)oy * ow + ox;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c * F * plane] = __fdiv_rn(__fsub_rn(y[c], __ldg(norm + 256 + c)), __ldg(norm + 259 + c));
+  }
+};
+
+// A feature network's input, channels-last (B, F, oh, ow, 4) with channel 3 zero, one 16-byte store per pixel, after
+// fvd.py's 2 y / 255 - 1 (in that order), pytorch-fid's 2 y - 1, the suite's (y - 0.5) * 2, or the Inception Score's
+// y as it is.
+enum { AFF_FVD, AFF_FID, AFF_SUITE, AFF_NONE };
+template <int AFF>
+struct Float4Pixels {
+  float4* out;
+  __device__ static float affine(float v) {
+    if constexpr (AFF == AFF_FVD) return __fsub_rn(__fdiv_rn(__fmul_rn(2.f, v), 255.f), 1.f);
+    else if constexpr (AFF == AFF_FID) return __fsub_rn(__fmul_rn(2.f, v), 1.f);
+    else if constexpr (AFF == AFF_SUITE) return __fmul_rn(__fsub_rn(v, 0.5f), 2.f);
+    else return v;
+  }
+  __device__ void operator()(const float (&y)[3], int, int, int, int oy, int ox, int oh, int ow) const {
+    out[((long long)blockIdx.z * oh + oy) * ow + ox] = make_float4(affine(y[0]), affine(y[1]), affine(y[2]), 0.f);
+  }
+};
+
+// The eval downsample's * 255 and .byte(): the product truncated to int32 and its low byte kept, as on x86-64, written
+// channels-last as (B, F, oh, ow, 3) uint8.
+struct BytePixels {
+  uint8_t* out;
+  __device__ void operator()(const float (&y)[3], int, int, int, int oy, int ox, int oh, int ow) const {
+    uint8_t* o = out + (((long long)blockIdx.z * oh + oy) * ow + ox) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = (uint8_t)(__float2int_rz(__fmul_rn(y[c], 255.f)) & 255);
+  }
+};
+
+template <class Src, class Out>
+__global__ void __launch_bounds__(RC_TW)
+bilinear_clips_kernel(Src src, const Out out, const omt_clip_desc* __restrict__ desc, const int4* __restrict__ tab,
+                      int F, int oh, int ow) {
   pdl_sync();
   const int b = blockIdx.z / F, f = blockIdx.z % F;
   const omt_clip_desc d = desc[b];
-  if constexpr (FVD) {
-    if (sel != nullptr) norm += 256 * __ldg(sel + b);
-  }
-  for (int i = threadIdx.x; i < 256; i += RC_TW) lut[i] = __ldg(norm + i);
-  __syncthreads();
+  src.begin(d, b, f, F);
   const int ox = blockIdx.x * RC_TW + threadIdx.x;
   if (ox >= ow) return;
-  float mean[3], stdv[3];
-  if constexpr (!FVD) {
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      mean[c] = __ldg(norm + 256 + c);
-      stdv[c] = __ldg(norm + 259 + c);
-    }
-  }
   const int4 ew = __ldg(tab + d.th / 4 + d.cx + ox);
   const int x0 = d.flip ? d.W - 1 - (d.x0 + ew.x) : d.x0 + ew.x;   // the flip comes before the resize: mirror the source
   const int x1 = d.flip ? d.W - 1 - (d.x0 + ew.y) : d.x0 + ew.y;
   const float l0w = __int_as_float(ew.z), l1w = __int_as_float(ew.w);
-  const uint8_t* frame = src + d.src + (long long)f * d.H * d.W * 3;
-  const long long plane = (long long)oh * ow;
-  float* o = out + ((long long)b * 3 * F + f) * plane + ox;        // channel c at + c * F * plane
   const int y_end = min(oh, (int)blockIdx.y * RC_TH + RC_TH);
   for (int oy = blockIdx.y * RC_TH; oy < y_end; ++oy) {
     const int4 eh = __ldg(tab + d.tv / 4 + d.cy + oy);
     const float l0h = __int_as_float(eh.z), l1h = __int_as_float(eh.w);
-    const uint8_t* r0 = frame + (long long)(d.y0 + eh.x) * d.W * 3;
-    const uint8_t* r1 = frame + (long long)(d.y0 + eh.y) * d.W * 3;
     // torch's CPU kernels: each fma rounds once; the products and the division are never contracted or reassociated
     const float w00 = __fmul_rn(l0h, l0w), w01 = __fmul_rn(l0h, l1w), w10 = __fmul_rn(l1h, l0w), w11 = __fmul_rn(l1h, l1w);
-    float y[3];
+    // Direct reads: every sample of the row pair before any arithmetic, so all twelve loads are in flight at once.
+    // Table reads are left to the compiler's order, which measured faster for them.
+    float v[3][4], y[3];
+    if constexpr (!Src::TABLE) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        v[c][0] = src(eh.x, x0, c), v[c][1] = src(eh.x, x1, c), v[c][2] = src(eh.y, x0, c), v[c][3] = src(eh.y, x1, c);
+    }
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float x00 = lut[__ldg(r0 + x0 * 3 + c)], x01 = lut[__ldg(r0 + x1 * 3 + c)];
-      const float x10 = lut[__ldg(r1 + x0 * 3 + c)], x11 = lut[__ldg(r1 + x1 * 3 + c)];
-      float v;
+      if constexpr (Src::TABLE)
+        v[c][0] = src(eh.x, x0, c), v[c][1] = src(eh.x, x1, c), v[c][2] = src(eh.y, x0, c), v[c][3] = src(eh.y, x1, c);
+      const float x00 = v[c][0], x01 = v[c][1], x10 = v[c][2], x11 = v[c][3];
       if (d.form) {
-        v = __fmaf_rn(x11, w11, __fmaf_rn(x10, w10, __fmaf_rn(x00, w00, __fmul_rn(x01, w01))));
+        y[c] = __fmaf_rn(x11, w11, __fmaf_rn(x10, w10, __fmaf_rn(x00, w00, __fmul_rn(x01, w01))));
       } else {
         const float t0 = __fmaf_rn(x00, l0w, __fmul_rn(x01, l1w));
         const float t1 = __fmaf_rn(x10, l0w, __fmul_rn(x11, l1w));
-        v = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
+        y[c] = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
       }
-      if constexpr (OUT == OUT_FID) y[c] = __fsub_rn(__fmul_rn(2.f, v), 1.f);
-      else if constexpr (FVD) y[c] = __fsub_rn(__fdiv_rn(__fmul_rn(2.f, v), 255.f), 1.f);
-      else o[c * F * plane + (long long)oy * ow] = __fdiv_rn(__fsub_rn(v, mean[c]), stdv[c]);
     }
-    if constexpr (FVD)
-      reinterpret_cast<float4*>(out)[((long long)blockIdx.z * oh + oy) * ow + ox] = make_float4(y[0], y[1], y[2], 0.f);
-  }
-}
-
-__global__ void __launch_bounds__(RC_TW)
-resample_clips_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
-                      const int4* __restrict__ tab, const float* __restrict__ norm, float* __restrict__ out, int F,
-                      int oh, int ow) {
-  resample_clips_body<OUT_NORMALIZE>(src, desc, tab, norm, out, F, oh, ow, nullptr);
-}
-
-__global__ void __launch_bounds__(RC_TW)
-fvd_preprocess_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
-                      const int4* __restrict__ tab, const float* __restrict__ lut, const int32_t* __restrict__ sel,
-                      float* __restrict__ out, int F, int oh, int ow) {
-  resample_clips_body<OUT_FVD>(src, desc, tab, lut, out, F, oh, ow, sel);
-}
-
-__global__ void __launch_bounds__(RC_TW)
-fid_preprocess_kernel(const uint8_t* __restrict__ src, const omt_clip_desc* __restrict__ desc,
-                      const int4* __restrict__ tab, const float* __restrict__ lut, const int32_t* __restrict__ sel,
-                      float* __restrict__ out, int oh, int ow) {
-  resample_clips_body<OUT_FID>(src, desc, tab, lut, out, 1, oh, ow, sel);
-}
-
-// omt_fvd_suite_preprocess: evaluation/common_metrics_on_video_quality's FVD preprocess (styleganv / videogpt
-// preprocess_single) from uint8 channels-last or fp32 channel-planar clips.  The same tile walk and bilinear arithmetic
-// as resample_clips_body, but the value of a source sample is read in one of three forms, and the result is
-// (y - 0.5) * 2 in two roundings.  desc.src counts elements of src (bytes or floats); the frames of a clip follow each
-// other, so a clip stored with a longer time axis is read as its first F frames.
-// SUITE = false (omt_is_preprocess): the Inception Score's nn.Upsample alone, y written as it is.
-__device__ __forceinline__ float suite_u8_value(int b) { return __fdiv_rn((float)b, 255.f); }
-
-template <int FORM>
-__device__ __forceinline__ float suite_value(const void* __restrict__ src, long long frame, int C, int H, int W, int y,
-                                             int x, int c) {
-  if constexpr (FORM == OMT_FVDS_U8) {
-    return suite_u8_value(__ldg(static_cast<const uint8_t*>(src) + frame + ((long long)y * W + x) * 3 + c));
-  } else {
-    const float v = __ldg(static_cast<const float*>(src) + frame + ((long long)(C == 1 ? 0 : c) * H + y) * W + x);
-    if constexpr (FORM == OMT_FVDS_F32) return v;
-    // videogpt: (videos * 255).numpy().astype(np.uint8), then .float() / 255.  The cast truncates to int32 and keeps
-    // the low byte, as the x86-64 conversion does for products inside the int32 range.
-    return suite_u8_value(__float2int_rz(__fmul_rn(v, 255.f)) & 255);
-  }
-}
-
-template <int FORM, bool SUITE>
-__global__ void __launch_bounds__(RC_TW)
-fvd_suite_preprocess_kernel(const void* __restrict__ src, const omt_clip_desc* __restrict__ desc,
-                            const int4* __restrict__ tab, int C, float* __restrict__ out, int F, int oh, int ow) {
-  pdl_sync();
-  const int b = blockIdx.z / F, f = blockIdx.z % F;
-  const omt_clip_desc d = desc[b];
-  const int ox = blockIdx.x * RC_TW + threadIdx.x;
-  if (ox >= ow) return;
-  const int4 ew = __ldg(tab + d.th / 4 + d.cx + ox);
-  const int x0 = d.x0 + ew.x, x1 = d.x0 + ew.y;
-  const float l0w = __int_as_float(ew.z), l1w = __int_as_float(ew.w);
-  const long long frame = d.src + (long long)f * (FORM == OMT_FVDS_U8 ? 3 : C) * d.H * d.W;
-  const int y_end = min(oh, (int)blockIdx.y * RC_TH + RC_TH);
-  for (int oy = blockIdx.y * RC_TH; oy < y_end; ++oy) {
-    const int4 eh = __ldg(tab + d.tv / 4 + d.cy + oy);
-    const float l0h = __int_as_float(eh.z), l1h = __int_as_float(eh.w);
-    const int r0 = d.y0 + eh.x, r1 = d.y0 + eh.y;
-    const float w00 = __fmul_rn(l0h, l0w), w01 = __fmul_rn(l0h, l1w), w10 = __fmul_rn(l1h, l0w), w11 = __fmul_rn(l1h, l1w);
-    float y[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      const float x00 = suite_value<FORM>(src, frame, C, d.H, d.W, r0, x0, c);
-      const float x01 = suite_value<FORM>(src, frame, C, d.H, d.W, r0, x1, c);
-      const float x10 = suite_value<FORM>(src, frame, C, d.H, d.W, r1, x0, c);
-      const float x11 = suite_value<FORM>(src, frame, C, d.H, d.W, r1, x1, c);
-      float v;
-      if (d.form) {
-        v = __fmaf_rn(x11, w11, __fmaf_rn(x10, w10, __fmaf_rn(x00, w00, __fmul_rn(x01, w01))));
-      } else {
-        const float t0 = __fmaf_rn(x00, l0w, __fmul_rn(x01, l1w));
-        const float t1 = __fmaf_rn(x10, l0w, __fmul_rn(x11, l1w));
-        v = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
-      }
-      y[c] = SUITE ? __fmul_rn(__fsub_rn(v, 0.5f), 2.f) : v;
-    }
-    reinterpret_cast<float4*>(out)[((long long)blockIdx.z * oh + oy) * ow + ox] = make_float4(y[0], y[1], y[2], 0.f);
-  }
-}
-
-// omt_eval_downsample: vqgan_eval.py's --infer_downsample, F.interpolate(scale_factor = 1 / d) of the clamped
-// reconstruction (OMT_DS_F32) or of the real clip's values (OMT_DS_U8, by byte table), then * 255 and .byte(), written
-// channels-last as uint8.  The tile walk and bilinear arithmetic of resample_clips_body; its own kernel, so the loader
-// and metric preprocess kernels above stay as they are.
-template <int FORM>
-__global__ void __launch_bounds__(RC_TW)
-eval_downsample_kernel(const void* __restrict__ src, const omt_clip_desc* __restrict__ desc, const int4* __restrict__ tab,
-                       const float* __restrict__ lut_g, const int32_t* __restrict__ sel, uint8_t* __restrict__ out, int F,
-                       int oh, int ow) {
-  __shared__ float lut[256];
-  pdl_sync();
-  const int b = blockIdx.z / F, f = blockIdx.z % F;
-  const omt_clip_desc d = desc[b];
-  if constexpr (FORM == OMT_DS_U8) {
-    const float* t = lut_g + (sel != nullptr ? 256 * __ldg(sel + b) : 0);
-    for (int i = threadIdx.x; i < 256; i += RC_TW) lut[i] = __ldg(t + i);
-    __syncthreads();
-  }
-  const int ox = blockIdx.x * RC_TW + threadIdx.x;
-  if (ox >= ow) return;
-  const int4 ew = __ldg(tab + d.th / 4 + d.cx + ox);
-  const float l0w = __int_as_float(ew.z), l1w = __int_as_float(ew.w);
-  const long long plane = (long long)d.H * d.W;
-  // OMT_DS_U8: frame f of the clip's (F, H, W, 3) bytes; OMT_DS_F32: channel c's frame f at + c F plane
-  const long long frame = d.src + (long long)f * plane * (FORM == OMT_DS_U8 ? 3 : 1);
-  auto value = [&](int y, int x, int c) -> float {
-    if constexpr (FORM == OMT_DS_U8) {
-      return lut[__ldg(static_cast<const uint8_t*>(src) + frame + ((long long)y * d.W + x) * 3 + c)];
-    } else {
-      const float v = __fadd_rn(__ldg(static_cast<const float*>(src) + frame + c * F * plane + (long long)y * d.W + x), 0.5f);
-      return v != v ? v : fminf(fmaxf(v, 0.f), 1.f);        // torch.clamp keeps a NaN
-    }
-  };
-  const int y_end = min(oh, (int)blockIdx.y * RC_TH + RC_TH);
-  for (int oy = blockIdx.y * RC_TH; oy < y_end; ++oy) {
-    const int4 eh = __ldg(tab + d.tv / 4 + d.cy + oy);
-    const float l0h = __int_as_float(eh.z), l1h = __int_as_float(eh.w);
-    const float w00 = __fmul_rn(l0h, l0w), w01 = __fmul_rn(l0h, l1w), w10 = __fmul_rn(l1h, l0w), w11 = __fmul_rn(l1h, l1w);
-    uint8_t* o = out + (((long long)blockIdx.z * oh + oy) * ow + ox) * 3;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      const float x00 = value(eh.x, ew.x, c), x01 = value(eh.x, ew.y, c);
-      const float x10 = value(eh.y, ew.x, c), x11 = value(eh.y, ew.y, c);
-      float v;
-      if (d.form) {
-        v = __fmaf_rn(x11, w11, __fmaf_rn(x10, w10, __fmaf_rn(x00, w00, __fmul_rn(x01, w01))));
-      } else {
-        const float t0 = __fmaf_rn(x00, l0w, __fmul_rn(x01, l1w));
-        const float t1 = __fmaf_rn(x10, l0w, __fmul_rn(x11, l1w));
-        v = __fmaf_rn(t0, l0h, __fmul_rn(t1, l1h));
-      }
-      o[c] = (uint8_t)(__float2int_rz(__fmul_rn(v, 255.f)) & 255);
-    }
+    out(y, b, f, F, oy, ox, oh, ow);
   }
 }
 
@@ -433,26 +396,28 @@ extern "C" int omt_resample_u8(const uint8_t* src, long long src_bytes, const om
 }
 
 // The checks the clip entry points make before their launch (`who` names the entry point in the message).  A frame
-// holds H W ch elements of src (src_bytes counts elements).
-static int check_clips(const char* who, const void* src, long long src_bytes, const omt_clip_desc* desc,
-                       const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host, long long tab_len,
-                       int B, int F, int oh, int ow, float* out, int ch = 3) {
+// holds H W ch elements of src (src_elems counts elements); `whole`: the entry point takes no flip and no window.
+static int check_clips(const char* who, const void* src, long long src_elems, int ch, bool whole,
+                       const omt_clip_desc* desc, const omt_clip_desc* desc_host, const int32_t* tab,
+                       const int32_t* tab_host, long long tab_len, int B, int F, int oh, int ow, const void* out) {
   OMT_REQUIRE(src && desc && desc_host && tab && tab_host && out, "%s: null pointer", who);
-  OMT_REQUIRE(B >= 1 && F >= 1 && (long long)B * F <= 65535 && oh >= 1 && ow >= 1 && src_bytes >= 0 && tab_len >= 0,
-              "%s: B=%d, F=%d, output %dx%d, src_bytes=%lld, tab_len=%lld", who, B, F, oh, ow, src_bytes, tab_len);
+  OMT_REQUIRE(B >= 1 && F >= 1 && (long long)B * F <= 65535 && oh >= 1 && ow >= 1 && src_elems >= 0 && tab_len >= 0,
+              "%s: B=%d, F=%d, output %dx%d, src_bytes=%lld, tab_len=%lld", who, B, F, oh, ow, src_elems, tab_len);
   for (int b = 0; b < B; ++b) {
     const omt_clip_desc& d = desc_host[b];
     OMT_REQUIRE(d.H >= 1 && d.W >= 1 && d.wh >= 1 && d.ww >= 1 && d.rh >= 1 && d.rw >= 1,
                 "%s: clip %d: source %dx%d, window %dx%d, resized %dx%d", who, b, d.H, d.W, d.wh, d.ww, d.rh, d.rw);
-    OMT_REQUIRE(d.src >= 0 && d.src + (long long)F * d.H * d.W * ch <= src_bytes,
+    OMT_REQUIRE(d.src >= 0 && d.src + (long long)F * d.H * d.W * ch <= src_elems,
                 "%s: clip %d: bytes [%lld, +%lld) outside the %lld source bytes", who, b, d.src,
-                (long long)F * d.H * d.W * ch, src_bytes);
+                (long long)F * d.H * d.W * ch, src_elems);
     OMT_REQUIRE(d.y0 >= 0 && d.x0 >= 0 && (long long)d.y0 + d.wh <= d.H && (long long)d.x0 + d.ww <= d.W,
                 "%s: clip %d: window %dx%d at (%d, %d) outside the %dx%d frame", who, b, d.wh, d.ww, d.y0, d.x0, d.H, d.W);
     OMT_REQUIRE(d.cy >= 0 && d.cx >= 0 && (long long)d.cy + oh <= d.rh && (long long)d.cx + ow <= d.rw,
                 "%s: clip %d: crop %dx%d at (%d, %d) outside the resized %dx%d frame", who, b, oh, ow, d.cy, d.cx, d.rh,
                 d.rw);
     OMT_REQUIRE((d.flip | d.form) >= 0 && (d.flip | d.form) <= 1, "%s: clip %d: flip / form must be 0 or 1", who, b);
+    OMT_REQUIRE(!whole || (!d.flip && d.y0 == 0 && d.x0 == 0 && d.wh == d.H && d.ww == d.W),
+                "%s: clip %d: this preprocess has no flip and no window", who, b);
     OMT_REQUIRE(clip_axis_ok(tab_host, tab_len, d.tv, d.rh, d.wh),
                 "%s: clip %d: vertical table outside the table or indices outside the window", who, b);
     OMT_REQUIRE(clip_axis_ok(tab_host, tab_len, d.th, d.rw, d.ww),
@@ -461,21 +426,34 @@ static int check_clips(const char* who, const void* src, long long src_bytes, co
   return OMT_OK;
 }
 
+// The alignment checks, check_clips and the launch of one clip entry point.  `words` are its other pointers read as
+// 4-byte words (fp32 sources, byte tables, sel); out is aligned to the size of what its output policy stores.
+template <class Src, class Out>
+static int launch_clips(const char* who, Src s, Out o, std::initializer_list<const void*> words, long long src_elems,
+                        int ch, bool whole, const omt_clip_desc* desc, const omt_clip_desc* desc_host,
+                        const int32_t* tab, const int32_t* tab_host, long long tab_len, int B, int F, int oh, int ow,
+                        omt_stream_t stream) {
+  constexpr int out_align = sizeof(*o.out);
+  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab}) && aligned_to(out_align, {o.out}) && aligned_to(4, words),
+              "%s: desc must be 8-byte, tab 16-byte, out %d-byte and tables, sel and fp32 src 4-byte aligned", who,
+              out_align);
+  int rc = check_clips(who, s.src, src_elems, ch, whole, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, o.out);
+  if (rc != OMT_OK) return rc;
+  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
+  OMT_CUDA(launch_k(bilinear_clips_kernel<Src, Out>, grid, dim3(RC_TW), 0, (cudaStream_t)stream, s, o, desc,
+                    reinterpret_cast<const int4*>(tab), F, oh, ow));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
 extern "C" int omt_resample_clips(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc,
                                   const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
                                   long long tab_len, const float* norm, int B, int F, int oh, int ow, float* out,
                                   omt_stream_t stream) {
   OMT_ENTER();
-  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab}) && aligned_to(4, {norm, out}),
-              "omt_resample_clips: desc must be 8-byte, tab 16-byte and norm / out 4-byte aligned");
   OMT_REQUIRE(norm, "omt_resample_clips: null pointer");
-  int rc = check_clips("omt_resample_clips", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, out);
-  if (rc != OMT_OK) return rc;
-  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
-  OMT_CUDA(launch_k(resample_clips_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
-                    reinterpret_cast<const int4*>(tab), norm, out, F, oh, ow));
-  OMT_LAUNCH_CHECK();
-  return OMT_OK;
+  return launch_clips("omt_resample_clips", ByteTable{src, norm, nullptr}, NormalizePlanes{out, norm}, {norm},
+                      src_bytes, 3, false, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, stream);
 }
 
 extern "C" int omt_fvd_preprocess(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc,
@@ -483,17 +461,10 @@ extern "C" int omt_fvd_preprocess(const uint8_t* src, long long src_bytes, const
                                   long long tab_len, const float* lut, const int32_t* sel, int B, int F, int oh,
                                   int ow, float* out, omt_stream_t stream) {
   OMT_ENTER();
-  OMT_REQUIRE(aligned_to(4, {sel}), "omt_fvd_preprocess: sel must be 4-byte aligned");
-  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && aligned_to(4, {lut}),
-              "omt_fvd_preprocess: desc must be 8-byte, tab / out 16-byte and lut 4-byte aligned");
   OMT_REQUIRE(lut, "omt_fvd_preprocess: null pointer");
-  int rc = check_clips("omt_fvd_preprocess", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, out);
-  if (rc != OMT_OK) return rc;
-  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
-  OMT_CUDA(launch_k(fvd_preprocess_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
-                    reinterpret_cast<const int4*>(tab), lut, sel, out, F, oh, ow));
-  OMT_LAUNCH_CHECK();
-  return OMT_OK;
+  return launch_clips("omt_fvd_preprocess", ByteTable{src, lut, sel},
+                      Float4Pixels<AFF_FVD>{reinterpret_cast<float4*>(out)}, {lut, sel}, src_bytes, 3, false, desc,
+                      desc_host, tab, tab_host, tab_len, B, F, oh, ow, stream);
 }
 
 extern "C" int omt_fid_preprocess(const uint8_t* src, long long src_bytes, const omt_clip_desc* desc,
@@ -501,49 +472,10 @@ extern "C" int omt_fid_preprocess(const uint8_t* src, long long src_bytes, const
                                   long long tab_len, const float* lut, const int32_t* sel, int B, int oh, int ow,
                                   float* out, omt_stream_t stream) {
   OMT_ENTER();
-  OMT_REQUIRE(aligned_to(4, {sel}), "omt_fid_preprocess: sel must be 4-byte aligned");
-  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && aligned_to(4, {lut}),
-              "omt_fid_preprocess: desc must be 8-byte, tab / out 16-byte and lut 4-byte aligned");
   OMT_REQUIRE(lut, "omt_fid_preprocess: null pointer");
-  int rc = check_clips("omt_fid_preprocess", src, src_bytes, desc, desc_host, tab, tab_host, tab_len, B, 1, oh, ow, out);
-  if (rc != OMT_OK) return rc;
-  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B);
-  OMT_CUDA(launch_k(fid_preprocess_kernel, grid, dim3(RC_TW), 0, (cudaStream_t)stream, src, desc,
-                    reinterpret_cast<const int4*>(tab), lut, sel, out, oh, ow));
-  OMT_LAUNCH_CHECK();
-  return OMT_OK;
-}
-
-// The checks and launch of omt_fvd_suite_preprocess (SUITE) and omt_is_preprocess (`who` names the entry point).
-template <bool SUITE>
-static int suite_preprocess(const char* who, const void* src, long long src_elems, int form, int C,
-                            const omt_clip_desc* desc, const omt_clip_desc* desc_host, const int32_t* tab,
-                            const int32_t* tab_host, long long tab_len, int B, int F, int oh, int ow, float* out,
-                            omt_stream_t stream) {
-  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab, out}) && (form == OMT_FVDS_U8 || aligned_to(4, {src})),
-              "%s: desc must be 8-byte, tab / out 16-byte and fp32 src 4-byte aligned", who);
-  int rc = check_clips(who, src, src_elems, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, out,
-                       form == OMT_FVDS_U8 ? 3 : C);
-  if (rc != OMT_OK) return rc;
-  for (int b = 0; b < B; ++b) {
-    const omt_clip_desc& d = desc_host[b];
-    OMT_REQUIRE(!d.flip && d.y0 == 0 && d.x0 == 0 && d.wh == d.H && d.ww == d.W,
-                "%s: clip %d: the suite's preprocess has no flip and no window", who, b);
-  }
-  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
-  const int4* t4 = reinterpret_cast<const int4*>(tab);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (form == OMT_FVDS_U8)
-    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_U8, SUITE>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F,
-                      oh, ow));
-  else if (form == OMT_FVDS_F32)
-    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_F32, SUITE>, grid, dim3(RC_TW), 0, s, src, desc, t4, C, out, F,
-                      oh, ow));
-  else
-    OMT_CUDA(launch_k(fvd_suite_preprocess_kernel<OMT_FVDS_F32_TRUNC, true>, grid, dim3(RC_TW), 0, s, src, desc, t4, C,
-                      out, F, oh, ow));
-  OMT_LAUNCH_CHECK();
-  return OMT_OK;
+  return launch_clips("omt_fid_preprocess", ByteTable{src, lut, sel},
+                      Float4Pixels<AFF_FID>{reinterpret_cast<float4*>(out)}, {lut, sel}, src_bytes, 3, false, desc,
+                      desc_host, tab, tab_host, tab_len, B, 1, oh, ow, stream);
 }
 
 extern "C" int omt_fvd_suite_preprocess(const void* src, long long src_elems, int form, int C,
@@ -551,22 +483,34 @@ extern "C" int omt_fvd_suite_preprocess(const void* src, long long src_elems, in
                                         const int32_t* tab_host, long long tab_len, int B, int F, int oh, int ow,
                                         float* out, omt_stream_t stream) {
   OMT_ENTER();
-  OMT_REQUIRE(form == OMT_FVDS_U8 || form == OMT_FVDS_F32 || form == OMT_FVDS_F32_TRUNC,
-              "omt_fvd_suite_preprocess: unknown input form %d", form);
+  const char* who = "omt_fvd_suite_preprocess";
+  OMT_REQUIRE(form == OMT_FVDS_U8 || form == OMT_FVDS_F32 || form == OMT_FVDS_F32_TRUNC, "%s: unknown input form %d",
+              who, form);
   OMT_REQUIRE(form == OMT_FVDS_U8 ? C == 3 : (C == 1 || C == 3),
-              "omt_fvd_suite_preprocess: C=%d (uint8 clips have 3 channels, fp32 clips 1 or 3)", C);
-  return suite_preprocess<true>("omt_fvd_suite_preprocess", src, src_elems, form, C, desc, desc_host, tab, tab_host,
-                                tab_len, B, F, oh, ow, out, stream);
+              "%s: C=%d (uint8 clips have 3 channels, fp32 clips 1 or 3)", who, C);
+  const Float4Pixels<AFF_SUITE> o{reinterpret_cast<float4*>(out)};
+  auto launch = [&](auto s) {
+    return launch_clips(who, s, o, {form == OMT_FVDS_U8 ? nullptr : src}, src_elems, form == OMT_FVDS_U8 ? 3 : C,
+                        true, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, stream);
+  };
+  if (form == OMT_FVDS_U8) return launch(SuiteFrames<OMT_FVDS_U8>{src, C});
+  if (form == OMT_FVDS_F32) return launch(SuiteFrames<OMT_FVDS_F32>{src, C});
+  return launch(SuiteFrames<OMT_FVDS_F32_TRUNC>{src, C});
 }
 
 extern "C" int omt_is_preprocess(const void* src, long long src_elems, int form, const omt_clip_desc* desc,
                                  const omt_clip_desc* desc_host, const int32_t* tab, const int32_t* tab_host,
                                  long long tab_len, int B, int F, int oh, int ow, float* out, omt_stream_t stream) {
   OMT_ENTER();
-  OMT_REQUIRE(form == OMT_FVDS_U8 || form == OMT_FVDS_F32,
-              "omt_is_preprocess: input form %d is neither uint8 (0) nor fp32 (1)", form);
-  return suite_preprocess<false>("omt_is_preprocess", src, src_elems, form, 3, desc, desc_host, tab, tab_host, tab_len,
-                                 B, F, oh, ow, out, stream);
+  const char* who = "omt_is_preprocess";
+  OMT_REQUIRE(form == OMT_FVDS_U8 || form == OMT_FVDS_F32, "%s: input form %d is neither uint8 (0) nor fp32 (1)", who,
+              form);
+  const Float4Pixels<AFF_NONE> o{reinterpret_cast<float4*>(out)};
+  if (form == OMT_FVDS_U8)
+    return launch_clips(who, SuiteFrames<OMT_FVDS_U8>{src, 3}, o, {}, src_elems, 3, true, desc, desc_host, tab,
+                        tab_host, tab_len, B, F, oh, ow, stream);
+  return launch_clips(who, SuiteFrames<OMT_FVDS_F32>{src, 3}, o, {src}, src_elems, 3, true, desc, desc_host, tab,
+                      tab_host, tab_len, B, F, oh, ow, stream);
 }
 
 extern "C" int omt_eval_downsample(const void* src, long long src_elems, int form, const omt_clip_desc* desc,
@@ -577,25 +521,10 @@ extern "C" int omt_eval_downsample(const void* src, long long src_elems, int for
   const char* who = "omt_eval_downsample";
   OMT_REQUIRE(form == OMT_DS_F32 || form == OMT_DS_U8, "%s: input form %d is neither fp32 (0) nor uint8 (1)", who, form);
   OMT_REQUIRE(form == OMT_DS_F32 || lut, "%s: uint8 clips need a byte table", who);
-  OMT_REQUIRE(aligned_to(8, {desc}) && aligned_to(16, {tab}) && aligned_to(4, {lut, sel}) &&
-                  (form == OMT_DS_U8 || aligned_to(4, {src})),
-              "%s: desc must be 8-byte, tab 16-byte and lut / sel / fp32 src 4-byte aligned", who);
-  // check_clips counts a frame as H W 3 elements: true of both forms (3 planes of H W floats, or H W pixels of 3 bytes)
-  int rc = check_clips(who, src, src_elems, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow,
-                       reinterpret_cast<float*>(out), 3);
-  if (rc != OMT_OK) return rc;
-  for (int b = 0; b < B; ++b) {
-    const omt_clip_desc& d = desc_host[b];
-    OMT_REQUIRE(!d.flip && d.y0 == 0 && d.x0 == 0 && d.wh == d.H && d.ww == d.W,
-                "%s: clip %d: the eval downsample has no flip and no window", who, b);
-  }
-  dim3 grid((ow + RC_TW - 1) / RC_TW, (oh + RC_TH - 1) / RC_TH, B * F);
-  const int4* t4 = reinterpret_cast<const int4*>(tab);
-  cudaStream_t s = (cudaStream_t)stream;
+  // a frame is H W 3 elements in both forms (3 planes of H W floats, or H W pixels of 3 bytes)
   if (form == OMT_DS_U8)
-    OMT_CUDA(launch_k(eval_downsample_kernel<OMT_DS_U8>, grid, dim3(RC_TW), 0, s, src, desc, t4, lut, sel, out, F, oh, ow));
-  else
-    OMT_CUDA(launch_k(eval_downsample_kernel<OMT_DS_F32>, grid, dim3(RC_TW), 0, s, src, desc, t4, lut, sel, out, F, oh, ow));
-  OMT_LAUNCH_CHECK();
-  return OMT_OK;
+    return launch_clips(who, ByteTable{static_cast<const uint8_t*>(src), lut, sel}, BytePixels{out}, {lut, sel},
+                        src_elems, 3, true, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, stream);
+  return launch_clips(who, ClampedPlanes{static_cast<const float*>(src)}, BytePixels{out}, {lut, sel, src}, src_elems,
+                      3, true, desc, desc_host, tab, tab_host, tab_len, B, F, oh, ow, stream);
 }
