@@ -153,11 +153,11 @@ def call(name: str, *args):
     """Invoke an entry point on torch's current CUDA stream; tensors are converted to pointers."""
     global launch_count
     lib = load()
-    launch_count += KERNELS_PER_CALL.get(name, 1)
     conv = [_ptr(a) if (a is None or isinstance(a, torch.Tensor)) else a for a in args]
     rc = getattr(lib, name)(*conv, _stream())
-    if rc != 0:
+    if rc != 0:                     # a refused call launched nothing
         raise RuntimeError(f"{name} failed ({rc}): {lib.omt_last_error().decode()}")
+    launch_count += KERNELS_PER_CALL.get(name, 1)
 
 
 def linear_h(name="omt_linear_h", **kw):

@@ -412,6 +412,10 @@ extern "C" int omt_inception_score(const float* p, int ldp, int N, int n, int sp
   const size_t smem = (size_t)N * sizeof(double);
   OMT_REQUIRE(smem <= 48 * 1024, "omt_inception_score: N=%d classes exceed 48 KiB of fp64 shared memory", N);
   OMT_REQUIRE(aligned_to(4, {p}) && aligned_to(8, {col_mean, kl}), "omt_inception_score: misaligned pointer");
+  // the KL kernel's static red[] comes on top of q[N]: past N = 6128 the two exceed the 48 KiB a launch gets unasked
+  static KernelSetup setup_kl;
+  int rc;
+  if ((rc = setup_kl.smem(quality::is_kl_kernel, 48 * 1024))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   OMT_CUDA(launch_k(quality::is_col_mean_kernel, dim3((N + 255) / 256, splits), dim3(256), 0, st, p, ldp, N, n,
                     col_mean));
