@@ -90,8 +90,9 @@ int omt_layernorm(const float* x, int ldx, float* y, int ldy, const float* w, co
                   int M, int C, float eps, int seg, int seg_stride, int seg_off, omt_stream_t stream);
 
 /* Patch gather + LayerNorm (omnitokenizer.py:806-808 / :814-817: Rearrange + nn.LayerNorm).
- * video (B, Cin, T, H, W) fp32 contiguous.  first=1: frame 0, rows (b,h,w), features (c,p1,p2);
- * first=0: frames 1.., rows (b,t,h,w), features (c,pt,p1,p2).  A is [rows, K] dense.
+ * video (B, Cin, T, H, W) fp32 contiguous, Cin >= 1.  first=1: frame 0, rows (b,h,w), features (c,p1,p2);
+ * first=0: frames 1.., rows (b,t,h,w), features (c,pt,p1,p2), with pt > 0 dividing T - 1.  p > 0 is a multiple of 4
+ * dividing H and W; K = Cin * (1 | pt) * p * p <= 1024.  A is [rows, K] dense.
  * ln_w == ln_b == NULL: plain patch gather (im2col of the strided Conv3d of patch_embed='cnn', omnitokenizer.py:823-838).
  * A_hi != NULL: the rows are written as fp16 hi / lo operand planes [rows, K] instead of A (A may be NULL);
  * A_rs != NULL: in the row-scaled form, inverse row scales to A_rs [rows]. */
@@ -100,7 +101,8 @@ int omt_patchify_ln(const float* video, float* A, uint16_t* A_hi, uint16_t* A_lo
                     omt_stream_t stream);
 
 /* omt_patchify_ln on uint8 frames: the data pipelines' byte -> fp32 normalisation fused into the gather.
- * frames (B, T, H, W, Cin) uint8 contiguous, channels last (decord / PIL / decode_u8 layout), 4-byte aligned; Cin <= 4.
+ * frames (B, T, H, W, Cin) uint8 contiguous, channels last (decord / PIL / decode_u8 layout), 4-byte aligned; 1 <= Cin <= 4.
+ * Patch geometry (p > 0, pt > 0 for the rest frames, K <= 1024) as omt_patchify_ln.
  * lut: fp32 [n_tab][Cin][256], the value byte u of channel c stands for, built on the host with the pipeline's own CPU
  * expression (e.g. (u / 255 - mean_c) / std_c), so the kernel never divides and its values are the pipeline's bits.
  * sel: NULL (n_tab = 1, every sample uses table 0) or int32 [B] table index per sample, 0 or 1 (n_tab = 2; see
@@ -326,14 +328,16 @@ int omt_softmax_rows(const float* x, int ldx, int rows, int N, float* y, int ldy
 int omt_inception_score(const float* p, int ldp, int N, int n, int splits, double* col_mean, double* kl,
                         omt_stream_t stream);
 
-/* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W). */
+/* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W).  Rows, features and
+ * geometry as omt_patchify_ln: Cin >= 1, p > 0 a multiple of 4 dividing H and W, pt > 0 dividing T - 1 for the rest frames. */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,
                    int first, omt_stream_t stream);
 
 /* Un-patchify fused with the consumers' uint8 conversion: u8 = trunc(clamp(x * mul + add, lo, hi) * post), written
  * channels-LAST (B, T, H, W, Cin).  (mul, add, lo, hi, post) = (1, .5, 0, 1, 255) is vqgan_eval.py:139,147-148
  * `(clamp(x_recons + 0.5, 0, 1) * 255).byte()` and Latte's sample_ddp.py:206; (255, 128, 0, 255, 1) is DiT's
- * sample_ddp.py:163.  Each step rounds in fp32 like the torch expression, so the bytes are identical to it. */
+ * sample_ddp.py:163.  Each step rounds in fp32 like the torch expression, so the bytes are identical to it.  Geometry as
+ * omt_unpatchify (Cin >= 1, p > 0, pt > 0 for the rest frames). */
 int omt_unpatchify_u8(const float* P, uint8_t* out, int B, int Cin, int T, int H, int W, int p, int pt,
                       int first, float mul, float add, float lo, float hi, float post, omt_stream_t stream);
 

@@ -8,6 +8,97 @@ namespace omt {
 int g_peg_kernel = 4;   // omt_set_option("peg_kernel", 3|4): 4 = peg_tile4_kernel (cp.async gather + FFMA2, default), 3 = peg_tile_kernel
 
 // ------------------------------------------------------------------------------------------
+// Whole rows in a warp's registers, shared by LayerNorm and both patch gathers.
+// ------------------------------------------------------------------------------------------
+// Column of float4 chunk i of a lane's row.  PAIR (C a multiple of 256, NV = C / 128: 2, 4, 6 or 8): a lane owns 8
+// consecutive columns per 256-column block (two adjacent float4 chunks), so the row-scaled planes leave as 16-byte stores
+// (512 B per warp instruction) instead of 8-byte ones.  Otherwise chunk i of every lane covers 128 consecutive columns.
+template <bool PAIR>
+__device__ __forceinline__ int row_col(int i, int lane) {
+  return PAIR ? ((i >> 1) * 32 + lane) * 8 + (i & 1) * 4 : (i * 32 + lane) * 4;
+}
+
+// LayerNorm of a row of n columns held by the warp, in place: v[i] holds columns row_col<PAIR>(i) .. +3 (zeros past n).
+// Two-pass statistics over the chunk sums (x + y) + (z + w) and fma(x, x, y y) + fma(z, z, w w), then the affine:
+// FUSED_BIAS (the patch gathers, whose b is never NULL) rounds once in fma(v rstd, w, b); otherwise v * rstd * w, then + b
+// when b != NULL, in LayerNorm's own expression (whether that add is contracted is the compiler's choice per instance).
+template <int NV, bool PAIR, bool FUSED_BIAS>
+__device__ __forceinline__ void layernorm_row(float4 (&v)[NV], int n, int lane, const float* __restrict__ w,
+                                              const float* __restrict__ b, float eps) {
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i)
+    if (row_col<PAIR>(i, lane) < n) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+  const float mean = warp_sum(s) / (float)n;
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    if (row_col<PAIR>(i, lane) < n) {
+      v[i].x -= mean; v[i].y -= mean; v[i].z -= mean; v[i].w -= mean;
+      q += fmaf(v[i].x, v[i].x, __fmul_rn(v[i].y, v[i].y)) + fmaf(v[i].z, v[i].z, __fmul_rn(v[i].w, v[i].w));
+    }
+  }
+  const float rstd = 1.0f / sqrtf(warp_sum(q) / (float)n + eps);
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int c = row_col<PAIR>(i, lane);
+    if (c < n) {
+      const float4 g = *reinterpret_cast<const float4*>(w + c);
+      float4 o;
+      if constexpr (FUSED_BIAS) {
+        const float4 bb = *reinterpret_cast<const float4*>(b + c);
+        o.x = fmaf(__fmul_rn(v[i].x, rstd), g.x, bb.x); o.y = fmaf(__fmul_rn(v[i].y, rstd), g.y, bb.y);
+        o.z = fmaf(__fmul_rn(v[i].z, rstd), g.z, bb.z); o.w = fmaf(__fmul_rn(v[i].w, rstd), g.w, bb.w);
+      } else {
+        o.x = v[i].x * rstd * g.x; o.y = v[i].y * rstd * g.y;
+        o.z = v[i].z * rstd * g.z; o.w = v[i].w * rstd * g.w;
+        if (b != nullptr) {
+          const float4 bb = *reinterpret_cast<const float4*>(b + c);
+          o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
+        }
+      }
+      v[i] = o;
+    }
+  }
+}
+
+// Write a finished row of n columns (v as in layernorm_row): fp32 at out + off_f when out != NULL, and fp16 hi / lo
+// planes at hi / lo + off_p when hi != NULL, row-scaled when rs != NULL (the inverse row scale to rs[row]), else 2^11-scaled.
+template <int NV, bool PAIR>
+__device__ __forceinline__ void store_row(const float4 (&v)[NV], int n, int lane, float* out, size_t off_f, uint16_t* hi,
+                                          uint16_t* lo, size_t off_p, float* rs, int row) {
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const int c = row_col<PAIR>(i, lane);
+    if (c < n) {
+      if (out != nullptr) *reinterpret_cast<float4*>(out + off_f + c) = v[i];
+      if (hi != nullptr && rs == nullptr) store_split4(hi, lo, off_p + c, v[i]);
+    }
+  }
+  if (hi != nullptr && rs != nullptr) {
+    float mx = 0.f;                                    // columns past n hold zeros
+#pragma unroll
+    for (int i = 0; i < NV; ++i) mx = fmaxf(mx, max4abs(v[i]));
+    float sc, inv;
+    row_scale(warp_max(mx), sc, inv);
+    if constexpr (PAIR) {
+#pragma unroll
+      for (int i = 0; i < NV; i += 2) {
+        const int c = row_col<true>(i, lane);
+        if (c < n) store_split8u(hi, lo, off_p + c, v[i], v[i + 1], sc);
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < NV; ++i) {
+        const int c = row_col<false>(i, lane);
+        if (c < n) store_split4u(hi, lo, off_p + c, v[i], sc);
+      }
+    }
+    if (lane == 0) rs[row] = inv;
+  }
+}
+
+// ------------------------------------------------------------------------------------------
 // LayerNorm: one warp per row, whole row in registers (C <= 1024), two-pass statistics.
 // ------------------------------------------------------------------------------------------
 struct LnPlanes {          // optional fp16 hi / lo operand planes (omt_layernorm_h), written at the LOGICAL row
@@ -17,9 +108,7 @@ struct LnPlanes {          // optional fp16 hi / lo operand planes (omt_layernor
   float* y_rs; float* x_rs;          // non-NULL: row-scaled planes (omt_common.cuh), the inverse row scale goes here
 };
 
-// PAIR (C a multiple of 256, NV = C / 128: 2, 4, 6 or 8): a lane owns 8 consecutive columns per 256-column block (two adjacent float4 chunks), so
-// the row-scaled planes leave as 16-byte stores (512 B per warp instruction) instead of 8-byte ones.
-template <int NV, bool PAIR>   // float4 chunks per lane
+template <int NV, bool PAIR>   // float4 chunks per lane, column map (row_col)
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, int ldx,
                                                         float* __restrict__ y, int ldy,
                                                         const float* __restrict__ w,
@@ -33,94 +122,21 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
   const long long row = map_row(lrow, seg, seg_stride, seg_off);
   const float* xr = x + (size_t)row * ldx;
   float4 v[NV];
-  float s = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
-    const int c = PAIR ? ((i >> 1) * 32 + lane) * 8 + (i & 1) * 4 : (i * 32 + lane) * 4;
-    if (c < C) {
-      v[i] = *reinterpret_cast<const float4*>(xr + c);
-      s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-      if (pl.x_hi != nullptr && pl.x_rs == nullptr) store_split4(pl.x_hi, pl.x_lo, (size_t)lrow * pl.lds + c, v[i]);
-    } else {
-      v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
+    const int c = row_col<PAIR>(i, lane);
+    v[i] = c < C ? *reinterpret_cast<const float4*>(xr + c) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
-  if (pl.x_hi != nullptr && pl.x_rs != nullptr) {      // row-scaled planes of the raw row
-    float mx = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) mx = fmaxf(mx, max4abs(v[i]));
-    float sc, inv;
-    row_scale(warp_max(mx), sc, inv);
-    if constexpr (PAIR) {
-#pragma unroll
-      for (int i = 0; i < NV; i += 2) {
-        const int c = ((i >> 1) * 32 + lane) * 8;
-        if (c < C) store_split8u(pl.x_hi, pl.x_lo, (size_t)lrow * pl.lds + c, v[i], v[i + 1], sc);
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < NV; ++i) {
-        const int c = (i * 32 + lane) * 4;
-        if (c < C) store_split4u(pl.x_hi, pl.x_lo, (size_t)lrow * pl.lds + c, v[i], sc);
-      }
-    }
-    if (lane == 0) pl.x_rs[lrow] = inv;
-  }
-  const float mean = warp_sum(s) / (float)C;
-  float q = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int c = PAIR ? ((i >> 1) * 32 + lane) * 8 + (i & 1) * 4 : (i * 32 + lane) * 4;
-    if (c < C) {
-      v[i].x -= mean; v[i].y -= mean; v[i].z -= mean; v[i].w -= mean;
-      q += (v[i].x * v[i].x + v[i].y * v[i].y) + (v[i].z * v[i].z + v[i].w * v[i].w);
-    }
-  }
-  const float rstd = 1.0f / sqrtf(warp_sum(q) / (float)C + eps);
-  float* yr = y + (size_t)row * ldy;
-  float omx = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int c = PAIR ? ((i >> 1) * 32 + lane) * 8 + (i & 1) * 4 : (i * 32 + lane) * 4;
-    if (c < C) {
-      const float4 g = *reinterpret_cast<const float4*>(w + c);
-      float4 o;
-      o.x = v[i].x * rstd * g.x; o.y = v[i].y * rstd * g.y;
-      o.z = v[i].z * rstd * g.z; o.w = v[i].w * rstd * g.w;
-      if (b != nullptr) {
-        const float4 bb = *reinterpret_cast<const float4*>(b + c);
-        o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
-      }
-      if (y != nullptr) *reinterpret_cast<float4*>(yr + c) = o;
-      if (pl.y_hi != nullptr && pl.y_rs == nullptr) store_split4(pl.y_hi, pl.y_lo, (size_t)lrow * pl.lds + c, o);
-      v[i] = o;                                        // kept for the row-scaled form below
-      omx = fmaxf(omx, max4abs(o));
-    }
-  }
-  if (pl.y_hi != nullptr && pl.y_rs != nullptr) {      // row-scaled planes of the normalised row
-    float sc, inv;
-    row_scale(warp_max(omx), sc, inv);
-    if constexpr (PAIR) {
-#pragma unroll
-      for (int i = 0; i < NV; i += 2) {
-        const int c = ((i >> 1) * 32 + lane) * 8;
-        if (c < C) store_split8u(pl.y_hi, pl.y_lo, (size_t)lrow * pl.lds + c, v[i], v[i + 1], sc);
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < NV; ++i) {
-        const int c = (i * 32 + lane) * 4;
-        if (c < C) store_split4u(pl.y_hi, pl.y_lo, (size_t)lrow * pl.lds + c, v[i], sc);
-      }
-    }
-    if (lane == 0) pl.y_rs[lrow] = inv;
-  }
+  const size_t poff = (size_t)lrow * pl.lds;
+  store_row<NV, PAIR>(v, C, lane, nullptr, 0, pl.x_hi, pl.x_lo, poff, pl.x_rs, lrow);
+  layernorm_row<NV, PAIR, false>(v, C, lane, w, b, eps);
+  store_row<NV, PAIR>(v, C, lane, y, (size_t)row * ldy, pl.y_hi, pl.y_lo, poff, pl.y_rs, lrow);
 }
 
 // ------------------------------------------------------------------------------------------
 // Patch gather + LayerNorm.  One warp per patch row; K = Cin*p*p (first frame) or Cin*pt*p*p.
 // Feature f = ((c*PT + dt)*p + p1)*p + p2 ; p2 is contiguous in the video (p % 4 == 0).
-// The gather (fp32 video or uint8 frames) fills the lane's v[i] = features f = (i*32 + lane)*4 .. +3 (zeros past K);
+// The gather (fp32 video or uint8 frames) fills the lane's v[i] = features f = row_col<false>(i) .. +3 (zeros past K);
 // patch_ln_emit() is the LayerNorm and output stage both gathers share, so equal v[] give equal bits.
 // ------------------------------------------------------------------------------------------
 struct PatchRow {             // patch row -> (sample, first frame of the row, token row / column)
@@ -140,64 +156,33 @@ __device__ __forceinline__ PatchRow patch_row(int row, int T, int H, int W, int 
   return pr;
 }
 
+struct PatchFeature {         // feature f of a patch row -> (channel, frame in the patch, patch row / column)
+  int c, dt, p1, p2;
+};
+
+__device__ __forceinline__ PatchFeature patch_feature(int f, int p, int PT) {
+  PatchFeature pf;
+  pf.p2 = f % p;
+  pf.p1 = (f / p) % p;
+  pf.dt = (f / (p * p)) % PT;
+  pf.c = f / (p * p * PT);
+  return pf;
+}
+
+// Element of feature pf of patch row pr in the (B, Cin, T, H, W) video.
+__device__ __forceinline__ size_t patch_elem(const PatchRow& pr, const PatchFeature& pf, int Cin, int T, int H, int W, int p) {
+  return ((((size_t)pr.bi * Cin + pf.c) * T + (pr.t0 + pf.dt)) * H + (pr.hi * p + pf.p1)) * W + pr.wi * p + pf.p2;
+}
+
 template <int NV>
 __device__ __forceinline__ void patch_ln_emit(float4 (&v)[NV], int row, int K, int lane, float* __restrict__ A,
                                               uint16_t* __restrict__ A_hi, uint16_t* __restrict__ A_lo,
                                               float* __restrict__ A_rs, const float* __restrict__ lw,
                                               const float* __restrict__ lb, float eps) {
-  float s = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i)
-    if ((i * 32 + lane) * 4 < K) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-  const size_t rbase = (size_t)row * K;
-  // write a finished row: fp32, 2^11-scaled planes, or row-scaled planes (+ the inverse row scale)
-  auto emit = [&](float4 (&o)[NV]) {
-    float sc = 1.f, inv = 1.f;
-    if (A_rs != nullptr) {
-      float mx = 0.f;
-#pragma unroll
-      for (int i = 0; i < NV; ++i) mx = fmaxf(mx, max4abs(o[i]));
-      row_scale(warp_max(mx), sc, inv);
-      if (lane == 0) A_rs[row] = inv;
-    }
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int f = (i * 32 + lane) * 4;
-      if (f < K) {
-        if (A_rs != nullptr) store_split4u(A_hi, A_lo, rbase + f, o[i], sc);
-        else if (A_hi != nullptr) store_split4(A_hi, A_lo, rbase + f, o[i]);
-        else *reinterpret_cast<float4*>(A + rbase + f) = o[i];
-      }
-    }
-  };
-  if (lw == nullptr) {        // plain im2col (patch_embed='cnn': the strided Conv3d is a GEMM on raw patch vectors)
-    emit(v);
-    return;
-  }
-  const float mean = warp_sum(s) / (float)K;
-  float q = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int f = (i * 32 + lane) * 4;
-    if (f < K) {
-      v[i].x -= mean; v[i].y -= mean; v[i].z -= mean; v[i].w -= mean;
-      q += (v[i].x * v[i].x + v[i].y * v[i].y) + (v[i].z * v[i].z + v[i].w * v[i].w);
-    }
-  }
-  const float rstd = 1.0f / sqrtf(warp_sum(q) / (float)K + eps);
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int f = (i * 32 + lane) * 4;
-    if (f < K) {
-      const float4 g = *reinterpret_cast<const float4*>(lw + f);
-      const float4 bb = *reinterpret_cast<const float4*>(lb + f);
-      float4 o;
-      o.x = v[i].x * rstd * g.x + bb.x; o.y = v[i].y * rstd * g.y + bb.y;
-      o.z = v[i].z * rstd * g.z + bb.z; o.w = v[i].w * rstd * g.w + bb.w;
-      v[i] = o;
-    }
-  }
-  emit(v);
+  // lw == NULL: plain im2col (patch_embed='cnn': the strided Conv3d is a GEMM on raw patch vectors)
+  if (lw != nullptr) layernorm_row<NV, false, true>(v, K, lane, lw, lb, eps);
+  const size_t off = (size_t)row * K;
+  store_row<NV, false>(v, K, lane, A_hi != nullptr ? nullptr : A, off, A_hi, A_lo, off, A_rs, row);   // planes replace A
 }
 
 template <int NV>
@@ -218,17 +203,9 @@ __global__ void __launch_bounds__(256) patchify_ln_kernel(const float* __restric
   float4 v[NV];
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
-    const int f = (i * 32 + lane) * 4;
-    if (f < K) {
-      const int p2 = f % p;
-      const int p1 = (f / p) % p;
-      const int dt = (f / (p * p)) % PT;
-      const int c = f / (p * p * PT);
-      const size_t off = ((((size_t)pr.bi * Cin + c) * T + (pr.t0 + dt)) * H + (pr.hi * p + p1)) * W + pr.wi * p + p2;
-      v[i] = *reinterpret_cast<const float4*>(video + off);
-    } else {
-      v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
+    const int f = row_col<false>(i, lane);
+    v[i] = f < K ? *reinterpret_cast<const float4*>(video + patch_elem(pr, patch_feature(f, p, PT), Cin, T, H, W, p))
+                 : make_float4(0.f, 0.f, 0.f, 0.f);
   }
   patch_ln_emit<NV>(v, row, K, lane, A, A_hi, A_lo, A_rs, lw, lb, eps);
 }
@@ -238,7 +215,7 @@ __global__ void __launch_bounds__(256) patchify_ln_kernel(const float* __restric
 // contiguous, 4-byte aligned bytes: each warp stages its row's PT*p lines in shared memory with 32-bit loads, then builds
 // the same v[] as patchify_ln_kernel.  Warps walk rows with a grid stride so the table is loaded once per CTA.
 constexpr int PU8_WARPS = 8;
-constexpr int PU8_MAX_K = 1024;   // = the bytes of one row (K features, one byte each)
+constexpr int PATCH_MAX_K = 1024;   // longest patch vector of both gathers: 8 float4 chunks per lane; the bytes of one staged row
 
 template <int NV>
 __global__ void __launch_bounds__(256) patchify_ln_u8_kernel(const uint8_t* __restrict__ frames,
@@ -249,7 +226,7 @@ __global__ void __launch_bounds__(256) patchify_ln_u8_kernel(const uint8_t* __re
                                                              int rows, int Cin, int T, int H, int W, int p, int pt,
                                                              int first, float eps) {
   __shared__ float tab[2 * 4 * 256];
-  __shared__ uint32_t stage[PU8_WARPS][PU8_MAX_K / 4];
+  __shared__ uint32_t stage[PU8_WARPS][PATCH_MAX_K / 4];
   pdl_sync();
   const int ntab = sel != nullptr ? 2 : 1;
   for (int i = threadIdx.x; i < ntab * Cin * 256; i += blockDim.x) tab[i] = lut[i];
@@ -274,14 +251,11 @@ __global__ void __launch_bounds__(256) patchify_ln_u8_kernel(const uint8_t* __re
     float4 v[NV];
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
-      const int f = (i * 32 + lane) * 4;
+      const int f = row_col<false>(i, lane);
       if (f < K) {
-        const int p2 = f % p;
-        const int p1 = (f / p) % p;
-        const int dt = (f / (p * p)) % PT;
-        const int c = f / (p * p * PT);
-        const uint8_t* px = sb + ((dt * p + p1) * p + p2) * Cin + c;
-        const float* tc = tb + c * 256;
+        const PatchFeature pf = patch_feature(f, p, PT);
+        const uint8_t* px = sb + ((pf.dt * p + pf.p1) * p + pf.p2) * Cin + pf.c;
+        const float* tc = tb + pf.c * 256;
         v[i] = make_float4(tc[px[0]], tc[px[Cin]], tc[px[2 * Cin]], tc[px[3 * Cin]]);
       } else {
         v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -324,25 +298,13 @@ __global__ void __launch_bounds__(256) unpatchify_kernel(const float* __restrict
                                                          int Cin, int T, int H, int W, int p, int pt,
                                                          int first) {
   pdl_sync();
-  const int hh = H / p, ww = W / p;
   const int PT = first ? 1 : pt;
   const int K4 = Cin * PT * p * p / 4;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total4;
        i += (long long)gridDim.x * blockDim.x) {
-    const int f = (int)(i % K4) * 4;
-    int r = (int)(i / K4);
-    const int wi = r % ww; r /= ww;
-    const int hi = r % hh; r /= hh;
-    int ti = 0;
-    if (!first) { const int tn = (T - 1) / pt; ti = r % tn; r /= tn; }
-    const int bi = r;
-    const int t0 = first ? 0 : 1 + ti * pt;
-    const int p2 = f % p;
-    const int p1 = (f / p) % p;
-    const int dt = (f / (p * p)) % PT;
-    const int c = f / (p * p * PT);
-    const size_t off = ((((size_t)bi * Cin + c) * T + (t0 + dt)) * H + (hi * p + p1)) * W + wi * p + p2;
-    *reinterpret_cast<float4*>(video + off) = *reinterpret_cast<const float4*>(P + i * 4);
+    const PatchRow pr = patch_row((int)(i / K4), T, H, W, p, pt, first);
+    const PatchFeature pf = patch_feature((int)(i % K4) * 4, p, PT);
+    *reinterpret_cast<float4*>(video + patch_elem(pr, pf, Cin, T, H, W, p)) = *reinterpret_cast<const float4*>(P + i * 4);
   }
 }
 
@@ -358,25 +320,18 @@ __global__ void __launch_bounds__(256) unpatchify_u8_kernel(const float* __restr
                                                             int pt, int first, float mul, float add, float lo,
                                                             float hi, float post) {
   pdl_sync();
-  const int hh = H / p, ww = W / p;
   const int PT = first ? 1 : pt;
   const int per_row = PT * p * (p / 4);           // (dt, p1, p2-quad) items per patch row
   const int K = Cin * PT * p * p;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     int it = (int)(i % per_row);
-    int r = (int)(i / per_row);
-    const int row = r;
+    const int row = (int)(i / per_row);
     const int q4 = it % (p / 4); it /= (p / 4);
     const int p1 = it % p;
     const int dt = it / p;
-    const int wi = r % ww; r /= ww;
-    const int hi_ = r % hh; r /= hh;
-    int ti = 0;
-    if (!first) { const int tn = (T - 1) / pt; ti = r % tn; r /= tn; }
-    const int bi = r;
-    const int t = first ? 0 : 1 + ti * pt + dt;
-    const size_t pix = (((size_t)bi * T + t) * H + (hi_ * p + p1)) * W + wi * p + q4 * 4;
+    const PatchRow pr = patch_row(row, T, H, W, p, pt, first);
+    const size_t pix = (((size_t)pr.bi * T + (pr.t0 + dt)) * H + (pr.hi * p + p1)) * W + pr.wi * p + q4 * 4;
     uint8_t* o = out + pix * Cin;
     for (int c = 0; c < Cin; ++c) {
       const float4 v = *reinterpret_cast<const float4*>(P + (size_t)row * K + ((c * PT + dt) * p + p1) * p + q4 * 4);
@@ -759,28 +714,14 @@ static int layernorm_impl(const char* who, const float* x, int ldx, float* y, in
   // 8 consecutive columns per lane (16-byte plane stores) when the row splits into whole 256-column blocks and the planes allow it
   const bool pair = C % 256 == 0 && pl.lds % 8 == 0 &&
                     ((uintptr_t)pl.y_hi | (uintptr_t)pl.y_lo | (uintptr_t)pl.x_hi | (uintptr_t)pl.x_lo) % 16 == 0;
-  dim3 grid((M + 7) / 8), block(256);
-  switch (nv) {
-    case 1: OMT_CUDA(launch_k(layernorm_kernel<1, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl)); break;
-    case 2:
-      if (pair) OMT_CUDA(launch_k(layernorm_kernel<2, true>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
-      else OMT_CUDA(launch_k(layernorm_kernel<2, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
-      break;
-    case 3: OMT_CUDA(launch_k(layernorm_kernel<3, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl)); break;
-    case 4:
-      if (pair) OMT_CUDA(launch_k(layernorm_kernel<4, true>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
-      else OMT_CUDA(launch_k(layernorm_kernel<4, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
-      break;
-    case 6:      // C = 768 paired; every other width of 6 chunks takes <8, false>
-      if (pair) OMT_CUDA(launch_k(layernorm_kernel<6, true>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
-      else OMT_CUDA(launch_k(layernorm_kernel<8, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
-      break;
-    case 8:      // C = 1024 paired
-      if (pair) OMT_CUDA(launch_k(layernorm_kernel<8, true>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
-      else OMT_CUDA(launch_k(layernorm_kernel<8, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
-      break;
-    default: OMT_CUDA(launch_k(layernorm_kernel<8, false>, grid, block, 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl)); break;
-  }
+  // PAIR implies C = 128 NV with NV = 2, 4, 6 or 8; unpaired widths of more than 4 chunks take <8, false>
+  using LnKernel = decltype(&layernorm_kernel<1, false>);
+  static const LnKernel paired[] = {layernorm_kernel<2, true>, layernorm_kernel<4, true>, layernorm_kernel<6, true>,
+                                    layernorm_kernel<8, true>};
+  static const LnKernel unpaired[] = {layernorm_kernel<1, false>, layernorm_kernel<2, false>, layernorm_kernel<3, false>,
+                                      layernorm_kernel<4, false>};
+  const LnKernel kernel = pair ? paired[nv / 2 - 1] : (nv <= 4 ? unpaired[nv - 1] : layernorm_kernel<8, false>);
+  OMT_CUDA(launch_k(kernel, dim3((M + 7) / 8), dim3(256), 0, st, x, ldx, y, ldy, w, b, M, C, eps, seg, seg_stride, seg_off, pl));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }
@@ -801,31 +742,57 @@ extern "C" int omt_layernorm_h(const float* x, int ldx, float* y, int ldy, uint1
   return layernorm_impl("omt_layernorm_h", x, ldx, y, ldy, pl, w, b, M, C, eps, seg, seg_stride, seg_off, stream);
 }
 
+// Patch geometry of the four patch entry points: a (B, Cin, T, H, W) video cut into p x p patches of the first frame
+// (first) or of pt frames from frame 1 on.  The checks run in this order so that no division meets an unchecked divisor.
+// *rows = patch rows, *K = features per row.
+static int check_patch_geometry(const char* who, int B, int Cin, int T, int H, int W, int p, int pt, int first,
+                                long long* rows, int* K) {
+  OMT_REQUIRE(B >= 0, "%s: B=%d", who, B);
+  OMT_REQUIRE(Cin >= 1, "%s: Cin=%d must be >= 1", who, Cin);
+  OMT_REQUIRE(p > 0 && p % 4 == 0 && H % p == 0 && W % p == 0, "%s: patch %d must be a positive multiple of 4 dividing %dx%d",
+              who, p, H, W);
+  OMT_REQUIRE(first || (T > 1 && pt > 0 && (T - 1) % pt == 0), "%s: (T-1) %% pt != 0 or pt <= 0 (T=%d, pt=%d)", who, T, pt);
+  *K = Cin * (first ? 1 : pt) * p * p;
+  *rows = (long long)B * (first ? 1 : (T - 1) / pt) * (H / p) * (W / p);
+  return OMT_OK;
+}
+
+// Arguments both gathers check alike: the outputs (A, or hi / lo planes, with row scales only beside planes), LayerNorm
+// weights both or neither, the patch geometry and the patch vector's length.
+static int check_gather(const char* who, const float* A, const uint16_t* A_hi, const uint16_t* A_lo, const float* A_rs,
+                        const float* ln_w, const float* ln_b, int B, int Cin, int T, int H, int W, int p, int pt, int first,
+                        long long* rows, int* K) {
+  OMT_REQUIRE((A || A_hi) && (ln_w == nullptr) == (ln_b == nullptr) && (A_hi == nullptr) == (A_lo == nullptr),
+              "%s: null pointer", who);
+  OMT_REQUIRE(A_rs == nullptr || A_hi != nullptr, "%s: row scales without planes", who);
+  OMT_REQUIRE(aligned_to(16, {A, ln_w, ln_b}), "%s: A, ln_w and ln_b must be 16-byte aligned", who);
+  OMT_REQUIRE(aligned_to(8, {A_hi, A_lo}), "%s: planes must be 8-byte aligned", who);
+  const int rc = check_patch_geometry(who, B, Cin, T, H, W, p, pt, first, rows, K);
+  if (rc != OMT_OK) return rc;
+  OMT_REQUIRE(*K <= PATCH_MAX_K, "%s: patch vector %d > %d", who, *K, PATCH_MAX_K);
+  return OMT_OK;
+}
+
+// float4 chunks per lane of both gathers: 2, 6 or 8 (entry 0, 1 or 2 of their kernel tables)
+static int gather_nv_index(int K) {
+  const int nv = (K / 4 + 31) / 32;
+  return nv <= 2 ? 0 : (nv <= 6 ? 1 : 2);
+}
+
 extern "C" int omt_patchify_ln(const float* video, float* A, uint16_t* A_hi, uint16_t* A_lo, float* A_rs, const float* ln_w,
                                const float* ln_b, int B, int Cin, int T, int H, int W, int p, int pt, int first,
                                float eps, omt_stream_t stream) {
   OMT_ENTER();
-  OMT_REQUIRE(video && (A || A_hi) && ((ln_w == nullptr) == (ln_b == nullptr)) && ((A_hi == nullptr) == (A_lo == nullptr)),
-              "omt_patchify_ln: null pointer");
-  OMT_REQUIRE(aligned_to(16, {video, A, ln_w, ln_b}), "omt_patchify_ln: video, A, ln_w and ln_b must be 16-byte aligned");
-  OMT_REQUIRE(((uintptr_t)A_hi | (uintptr_t)A_lo) % 8 == 0, "omt_patchify_ln: planes must be 8-byte aligned");
-  OMT_REQUIRE(A_rs == nullptr || A_hi != nullptr, "omt_patchify_ln: row scales without planes");
-  OMT_REQUIRE(p % 4 == 0 && H % p == 0 && W % p == 0, "omt_patchify_ln: patch %d must be a multiple of 4 dividing %dx%d", p, H, W);
-  OMT_REQUIRE(first || (T > 1 && (T - 1) % pt == 0), "omt_patchify_ln: (T-1) %% pt != 0");
-  const int PT = first ? 1 : pt;
-  const int K = Cin * PT * p * p;
-  OMT_REQUIRE(K <= 1024, "omt_patchify_ln: patch vector %d > 1024", K);
-  const long long rows = (long long)B * (first ? 1 : (T - 1) / pt) * (H / p) * (W / p);
+  OMT_REQUIRE(video, "omt_patchify_ln: null pointer");
+  OMT_REQUIRE(aligned_to(16, {video}), "omt_patchify_ln: video must be 16-byte aligned");
+  long long rows;
+  int K;
+  const int rc = check_gather("omt_patchify_ln", A, A_hi, A_lo, A_rs, ln_w, ln_b, B, Cin, T, H, W, p, pt, first, &rows, &K);
+  if (rc != OMT_OK) return rc;
   if (rows == 0) return OMT_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  dim3 grid((unsigned)((rows + 7) / 8)), block(256);
-  const int nv = (K / 4 + 31) / 32;
-  if (nv <= 2)
-    OMT_CUDA(launch_k(patchify_ln_kernel<2>, grid, block, 0, st, video, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
-  else if (nv <= 6)
-    OMT_CUDA(launch_k(patchify_ln_kernel<6>, grid, block, 0, st, video, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
-  else
-    OMT_CUDA(launch_k(patchify_ln_kernel<8>, grid, block, 0, st, video, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
+  static decltype(&patchify_ln_kernel<2>) const kernels[] = {patchify_ln_kernel<2>, patchify_ln_kernel<6>, patchify_ln_kernel<8>};
+  OMT_CUDA(launch_k(kernels[gather_nv_index(K)], dim3((unsigned)((rows + 7) / 8)), dim3(256), 0, (cudaStream_t)stream, video,
+                    A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }
@@ -834,31 +801,20 @@ extern "C" int omt_patchify_ln_u8(const uint8_t* frames, const float* lut, const
                                   uint16_t* A_lo, float* A_rs, const float* ln_w, const float* ln_b, int B, int Cin, int T,
                                   int H, int W, int p, int pt, int first, float eps, omt_stream_t stream) {
   OMT_ENTER();
-  OMT_REQUIRE(frames && lut && (A || A_hi) && ((ln_w == nullptr) == (ln_b == nullptr)) && ((A_hi == nullptr) == (A_lo == nullptr)),
-              "omt_patchify_ln_u8: null pointer");
-  OMT_REQUIRE(aligned_to(16, {A, ln_w, ln_b}), "omt_patchify_ln_u8: A, ln_w and ln_b must be 16-byte aligned");
-  OMT_REQUIRE(((uintptr_t)A_hi | (uintptr_t)A_lo) % 8 == 0, "omt_patchify_ln_u8: planes must be 8-byte aligned");
-  OMT_REQUIRE((uintptr_t)frames % 4 == 0, "omt_patchify_ln_u8: frames must be 4-byte aligned");
-  OMT_REQUIRE(A_rs == nullptr || A_hi != nullptr, "omt_patchify_ln_u8: row scales without planes");
-  OMT_REQUIRE(Cin >= 1 && Cin <= 4, "omt_patchify_ln_u8: Cin=%d must be 1..4", Cin);
-  OMT_REQUIRE(p % 4 == 0 && p > 0 && H % p == 0 && W % p == 0, "omt_patchify_ln_u8: patch %d must be a multiple of 4 dividing %dx%d", p, H, W);
-  OMT_REQUIRE(first || (T > 1 && pt > 0 && (T - 1) % pt == 0), "omt_patchify_ln_u8: (T-1) %% pt != 0");
-  const int PT = first ? 1 : pt;
-  const int K = Cin * PT * p * p;
-  OMT_REQUIRE(K <= PU8_MAX_K, "omt_patchify_ln_u8: patch vector %d > %d", K, PU8_MAX_K);
-  const long long rows = (long long)B * (first ? 1 : (T - 1) / pt) * (H / p) * (W / p);
+  OMT_REQUIRE(frames && lut, "omt_patchify_ln_u8: null pointer");
+  OMT_REQUIRE(aligned_to(4, {frames}), "omt_patchify_ln_u8: frames must be 4-byte aligned");
+  OMT_REQUIRE(Cin <= 4, "omt_patchify_ln_u8: Cin=%d must be 1..4", Cin);   // the shared-memory table holds 4 channels
+  long long rows;
+  int K;
+  const int rc = check_gather("omt_patchify_ln_u8", A, A_hi, A_lo, A_rs, ln_w, ln_b, B, Cin, T, H, W, p, pt, first, &rows, &K);
+  if (rc != OMT_OK) return rc;
   if (rows == 0) return OMT_OK;
-  cudaStream_t st = (cudaStream_t)stream;
   long long blocks = (rows + PU8_WARPS - 1) / PU8_WARPS;
   if (blocks > (long long)sm_count() * 8) blocks = (long long)sm_count() * 8;   // 8 CTAs of 256 threads fill an SM
-  dim3 grid((unsigned)blocks), block(32 * PU8_WARPS);
-  const int nv = (K / 4 + 31) / 32;
-  if (nv <= 2)
-    OMT_CUDA(launch_k(patchify_ln_u8_kernel<2>, grid, block, 0, st, frames, lut, sel, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
-  else if (nv <= 6)
-    OMT_CUDA(launch_k(patchify_ln_u8_kernel<6>, grid, block, 0, st, frames, lut, sel, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
-  else
-    OMT_CUDA(launch_k(patchify_ln_u8_kernel<8>, grid, block, 0, st, frames, lut, sel, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
+  static decltype(&patchify_ln_u8_kernel<2>) const kernels[] = {patchify_ln_u8_kernel<2>, patchify_ln_u8_kernel<6>,
+                                                                patchify_ln_u8_kernel<8>};
+  OMT_CUDA(launch_k(kernels[gather_nv_index(K)], dim3((unsigned)blocks), dim3(32 * PU8_WARPS), 0, (cudaStream_t)stream,
+                    frames, lut, sel, A, A_hi, A_lo, A_rs, ln_w, ln_b, (int)rows, Cin, T, H, W, p, pt, first, eps));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }
@@ -881,20 +837,25 @@ extern "C" int omt_u8_norm_select(const uint8_t* frames, int B, long long per_sa
   return OMT_OK;
 }
 
+// Blocks of 256 threads for the un-patchify grid-stride loops over n items: one per 256 items, at most 32 per SM.
+static unsigned unpatchify_blocks(long long n) {
+  const long long blocks = (n + 255) / 256, cap = (long long)sm_count() * 32;
+  return (unsigned)(blocks < cap ? blocks : cap);
+}
+
 extern "C" int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p,
                               int pt, int first, omt_stream_t stream) {
   OMT_ENTER();
   OMT_REQUIRE(P && video, "omt_unpatchify: null pointer");
   OMT_REQUIRE(aligned_to(16, {P, video}), "omt_unpatchify: P and video must be 16-byte aligned");
-  OMT_REQUIRE(p % 4 == 0 && H % p == 0 && W % p == 0, "omt_unpatchify: bad patch size");
-  OMT_REQUIRE(first || (T > 1 && (T - 1) % pt == 0), "omt_unpatchify: (T-1) %% pt != 0");
-  const int PT = first ? 1 : pt;
-  const long long rows = (long long)B * (first ? 1 : (T - 1) / pt) * (H / p) * (W / p);
-  const long long total4 = rows * (Cin * PT * p * p / 4);
+  long long rows;
+  int K;
+  const int rc = check_patch_geometry("omt_unpatchify", B, Cin, T, H, W, p, pt, first, &rows, &K);
+  if (rc != OMT_OK) return rc;
+  const long long total4 = rows * (K / 4);
   if (total4 == 0) return OMT_OK;
-  long long blocks = (total4 + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
-  OMT_CUDA(launch_k(unpatchify_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, P, video, total4, Cin, T, H, W, p, pt, first));
+  OMT_CUDA(launch_k(unpatchify_kernel, dim3(unpatchify_blocks(total4)), dim3(256), 0, (cudaStream_t)stream, P, video, total4,
+                    Cin, T, H, W, p, pt, first));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }
@@ -904,17 +865,15 @@ extern "C" int omt_unpatchify_u8(const float* P, uint8_t* out, int B, int Cin, i
   OMT_ENTER();
   OMT_REQUIRE(P && out, "omt_unpatchify_u8: null pointer");
   OMT_REQUIRE(aligned_to(16, {P}), "omt_unpatchify_u8: P must be 16-byte aligned");
-  OMT_REQUIRE(p % 4 == 0 && H % p == 0 && W % p == 0, "omt_unpatchify_u8: bad patch size");
-  OMT_REQUIRE(first || (T > 1 && (T - 1) % pt == 0), "omt_unpatchify_u8: (T-1) %% pt != 0");
+  long long rows;
+  int K;
+  const int rc = check_patch_geometry("omt_unpatchify_u8", B, Cin, T, H, W, p, pt, first, &rows, &K);
+  if (rc != OMT_OK) return rc;
   OMT_REQUIRE(lo >= 0.f && hi * post < 256.f, "omt_unpatchify_u8: clamp range [%g, %g] x %g does not fit a byte", lo, hi, post);
-  const int PT = first ? 1 : pt;
-  const long long rows = (long long)B * (first ? 1 : (T - 1) / pt) * (H / p) * (W / p);
-  const long long total = rows * PT * p * (p / 4);
+  const long long total = rows * (K / Cin / 4);     // (dt, p1, p2-quad) items
   if (total == 0) return OMT_OK;
-  long long blocks = (total + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
-  OMT_CUDA(launch_k(unpatchify_u8_kernel, dim3((unsigned)blocks), dim3(256), 0, (cudaStream_t)stream, P, out, total, Cin, T, H, W, p,
-                    pt, first, mul, add, lo, hi, post));
+  OMT_CUDA(launch_k(unpatchify_u8_kernel, dim3(unpatchify_blocks(total)), dim3(256), 0, (cudaStream_t)stream, P, out, total,
+                    Cin, T, H, W, p, pt, first, mul, add, lo, hi, post));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

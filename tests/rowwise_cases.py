@@ -16,9 +16,12 @@ import torch
 
 
 def ln_instantiation(C, lds=0, plane_align=16):
-    """(NV, PAIR) of layernorm_kernel, as layernorm_impl (csrc/rowwise.cu) picks it: NV = float4 chunks per lane
-    (1, 2, 3, 4, or 8 for anything larger), PAIR when C is a multiple of 256, NV is 2 or 4, the plane leading dimension
-    is a multiple of 8 and every plane pointer is 16-byte aligned.  A call without planes has lds = 0 and NULL planes."""
+    """(NV, PAIR) of layernorm_kernel, as layernorm_impl (csrc/rowwise.cu) picks it from its kernel tables for every
+    call but the paired ones at C = 768 and 1024: NV = float4 chunks per lane (1, 2, 3, 4, or 8 for anything larger),
+    PAIR when C is a multiple of 256, NV is 2 or 4, the plane leading dimension is a multiple of 8 and every plane
+    pointer is 16-byte aligned.  A call without planes has lds = 0 and NULL planes.  At C = 768 and 1024 this mirror
+    keeps <8, false>, the form of their unpaired calls; test_gpu_width_kernels.ln_instantiation_wide mirrors the paired
+    <6, true> and <8, true> there."""
     nv = (C // 4 + 31) // 32
     pair = C % 256 == 0 and lds % 8 == 0 and plane_align % 16 == 0
     if nv in (2, 4):
@@ -27,7 +30,8 @@ def ln_instantiation(C, lds=0, plane_align=16):
 
 
 def patch_nv(K):
-    """NV of patchify_ln_kernel for a patch vector of K features (omt_patchify_ln: 2, 6 or 8 float4 chunks per lane)."""
+    """NV of patchify_ln_kernel and patchify_ln_u8_kernel for a patch vector of K features, as gather_nv_index
+    (csrc/rowwise.cu) picks it for both gathers: 2, 6 or 8 float4 chunks per lane."""
     nv = (K // 4 + 31) // 32
     return 2 if nv <= 2 else (6 if nv <= 6 else 8)
 

@@ -11,7 +11,8 @@ in tests/rowwise_cases.py):
 Every output lands in a sentinel-filled buffer with guard rows before and after it, and guard columns past C / K where the
 entry point takes a leading dimension; the guards must survive.  Inputs of out-of-place launches stay bit-identical, two
 launches agree bit for bit, and every accuracy check prints its largest error and its bar.  Finally every entry point
-refuses a pointer off the alignment of its vector accesses, naming itself, before anything is launched.
+refuses a pointer off the alignment of its vector accesses, naming itself, before anything is launched, and every patch
+entry point refuses a patch geometry it cannot walk.
 """
 import itertools
 
@@ -572,3 +573,40 @@ def test_misaligned_pointers_raise(cuda):
                 cabi.call(name, *build(bad))
             torch.cuda.synchronize()
             assert bool((o == 7.0).all()) and bool((h16 == 7).all()), f"{name}: a call with misaligned {arg} wrote"
+
+
+# ---------------------------------------------------------------- patch geometry
+
+def test_patch_geometry_refused(cuda):
+    """Every patch entry point refuses a geometry it cannot walk -- p = 0 or not a multiple of 4, H not a multiple of p,
+    rest frames with pt = 0 or (T - 1) % pt != 0, Cin = 0, B < 0 and, for the gathers, a patch vector of more than 1024
+    features -- with a RuntimeError naming itself, and writes nothing; the same call with the valid geometry runs."""
+    f = torch.zeros(1 << 16, device=cuda)
+    u8 = torch.zeros(1 << 16, dtype=torch.uint8, device=cuda)
+    lut = L.u8_norm_table(L.U8Norm("t", (0.5,) * 3, (0.5,) * 3), 3).to(cuda)
+    o = torch.empty(1 << 16, dtype=torch.int32, device=cuda)
+    good = dict(B=1, Cin=3, T=5, H=8, W=8, p=4, pt=2, first=0)
+
+    def geo(g):
+        return tuple(g[k] for k in ("B", "Cin", "T", "H", "W", "p", "pt", "first"))
+
+    # entry point -> argument builder over the geometry
+    calls = {
+        "omt_patchify_ln": lambda g: (f, o, None, None, None, None, None, *geo(g), EPS),
+        "omt_patchify_ln_u8": lambda g: (u8, lut, None, o, None, None, None, None, None, *geo(g), EPS),
+        "omt_unpatchify": lambda g: (f, o, *geo(g)),
+        "omt_unpatchify_u8": lambda g: (f, o, *geo(g), 1.0, 0.5, 0.0, 1.0, 255.0),
+    }
+    bad = {"p = 0": dict(p=0), "p = 6": dict(p=6), "H % p != 0": dict(H=10), "rest frames, pt = 0": dict(pt=0),
+           "(T - 1) % pt != 0": dict(T=4), "Cin = 0": dict(Cin=0), "B = -1": dict(B=-1)}
+    gathers = {"K = 1536 > 1024": dict(p=16, H=16, W=16)}
+    cabi = _cabi()
+    for name, build in calls.items():
+        cabi.call(name, *build(good))
+        torch.cuda.synchronize()
+        for what, change in {**bad, **(gathers if name.startswith("omt_patchify") else {})}.items():
+            o.fill_(SENT32)
+            with pytest.raises(RuntimeError, match=f"{name}: "):
+                cabi.call(name, *build(dict(good, **change)))
+            torch.cuda.synchronize()
+            assert bool((o == SENT32).all()), f"{name}: a call with {what} wrote"
