@@ -328,6 +328,21 @@ int omt_softmax_rows(const float* x, int ldx, int rows, int N, float* y, int ldy
 int omt_inception_score(const float* p, int ldp, int N, int n, int splits, double* col_mean, double* kl,
                         omt_stream_t stream);
 
+/* The pixels vqgan_eval.py's image loop hands pytorch-fid when it saves to a .jpg / .JPEG path (vqgan_eval.py:205-220,
+ * fid_score.py:107): Pillow's img.save(f, "JPEG", quality=q) then Image.open(f).convert("RGB"), byte for byte, as
+ * libjpeg-turbo computes them: baseline 4:2:0, ISLOW forward and inverse DCT, h2v2 fancy upsampling (a chroma plane at
+ * most 2 samples wide is replicated 2 x 2), all in int32 (oracle/jpeg_oracle.py restates the chain).  Entropy coding is
+ * lossless, so no bitstream is made.
+ *   src, dst: (B, H, W, 3) uint8 RGB, contiguous, on the device; dst may not overlap src or scratch.
+ *   qtables: HOST memory, uint16 [2][64] (luminance, chrominance) in natural order, every entry 1..255; copied into the
+ *            launch, so the caller may reuse the array once the call returns.
+ *   scratch: the decoded Y, Cb and Cr planes, B (Hp Wp + 2 (Hp / 2) (Wp / 2)) bytes with Hp = 16 ceil(H / 16) and
+ *            Wp = 16 ceil(W / 16); 8-byte aligned; its contents are overwritten.
+ * B >= 0 (B = 0 launches nothing), H, W >= 1, Hp Wp 3 / 2 < 2^31.  Two launches: one CTA per four MCUs, then a thread
+ * per output pixel. */
+int omt_jpeg_roundtrip_u8(const uint8_t* src, uint8_t* dst, int B, int H, int W, const uint16_t* qtables,
+                          uint8_t* scratch, omt_stream_t stream);
+
 /* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W).  Rows, features and
  * geometry as omt_patchify_ln: Cin >= 1, p > 0 a multiple of 4 dividing H and W, pt > 0 dividing T - 1 for the rest frames. */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,

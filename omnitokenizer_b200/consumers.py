@@ -10,6 +10,7 @@ OmniTokenizer_VQGAN API; with this package's module the uint8 conversions run fu
 """
 from __future__ import annotations
 
+import os
 from typing import Optional, Sequence, Tuple
 
 import torch
@@ -304,25 +305,47 @@ def eval_step_images_u8(vqgan, images: Sequence[torch.Tensor], resize: U8Resize,
     return eval_step_u8(vqgan, _host_transform(images, resize), total_usage, norm)
 
 
+SAVED_FORMATS = ("png", "jpeg")
+_JPEG_EXTENSIONS = (".jpg", ".jpeg", ".jpe", ".jfif")
+
+
+def saved_format(path) -> str:
+    """The format vqgan_eval.py's Image.fromarray(...).save(path) writes (:205-220): Pillow picks it from the lower-cased
+    extension of the dataset's own relative path, batch["path"].  .jpg, .jpeg, .jpe and .jfif -> "jpeg" (ImageNet's
+    .JPEG, CelebA-HQ's .jpg), .png -> "png" (FFHQ); any other extension raises NotImplementedError naming it."""
+    ext = os.path.splitext(os.fspath(path))[1].lower()
+    if ext in _JPEG_EXTENSIONS:
+        return "jpeg"
+    if ext == ".png":
+        return "png"
+    raise NotImplementedError(f"saved_format: vqgan_eval.py would save {os.fspath(path)!r} by its extension {ext!r}; "
+                              f"only PNG and JPEG are reproduced")
+
+
 @torch.no_grad()
 def eval_step_fid(vqgan, images: Sequence[torch.Tensor], resize: U8Resize, inception,
                   total_usage: Optional[torch.Tensor] = None, norm: U8Norm = IMAGE_NORM,
-                  infer_downsample: Optional[int] = None):
+                  infer_downsample: Optional[int] = None, saved_as: str = "png"):
     """The body of vqgan_eval.py's image loop (:185-220) from the decoded ragged host images of ImageDataset, with the
-    PNG round trip and the pytorch-fid run replaced by FID features on the device (fid.FIDInception): forward_images_u8
+    file round trip and the pytorch-fid run replaced by FID features on the device (fid.FIDInception): forward_images_u8
     for the reconstruction's bytes and vq_output, and the pool3 features of both sides.  The real side reads the
     transformed input bytes that call wrote into the encode_u8 slot (the random crop and flip are drawn once) and sees
     the bytes the script saves of the normalised input, ((x + 0.5) * 255).astype(uint8), as a per-byte map.  Returns
     (real_features, fake_features, vq_output), each features (B, 2048) fp32; no image crosses to the host.
     infer_downsample d (:207-208, :218-219): both sides' saved bytes are first resized to (h // d, h // d) with
-    Image.ANTIALIAS (Pillow's LANCZOS, downsample.images_u8); the real side's byte map then comes before the resize."""
+    Image.ANTIALIAS (Pillow's LANCZOS, downsample.images_u8); the real side's byte map then comes before the resize.
+    saved_as: the format the script's img.save(path) writes, saved_format(batch["path"][0]).  "png" is lossless, so
+    the network sees the saved bytes themselves; with "jpeg" both sides' saved bytes (after the resize, if any) go
+    through Pillow's JPEG save at its default quality 75 and reload (jpeg.roundtrip_u8), as pytorch-fid reads them."""
     from .metricnet import real_byte_table
+    if saved_as not in SAVED_FORMATS:
+        raise ValueError(f"eval_step_fid: saved_as {saved_as!r} is not one of {SAVED_FORMATS}")
     images = list(images)
     if not images:
         raise ValueError("eval_step_fid needs at least one image")
     real_byte_table(norm)                    # refuses a per-channel normalisation before the first launch
-    if infer_downsample is not None:
-        return _eval_step_fid_downsample(vqgan, images, resize, inception, total_usage, norm, infer_downsample)
+    if infer_downsample is not None or saved_as != "png":
+        return _eval_step_fid_saved(vqgan, images, resize, inception, total_usage, norm, infer_downsample, saved_as)
     if hasattr(vqgan, "forward_images_u8"):
         fake, vq_output = vqgan.forward_images_u8(images, resize, norm, EVAL_U8)
         if total_usage is not None and vq_output is not None:
@@ -337,13 +360,16 @@ def eval_step_fid(vqgan, images: Sequence[torch.Tensor], resize: U8Resize, incep
     return real_features, fake_features, vq_output
 
 
-def _eval_step_fid_downsample(vqgan, images, resize: U8Resize, inception, total_usage, norm: U8Norm, d):
-    from . import downsample
-    d = L.check_infer_downsample(d, "eval_step_fid")
-    h, w = resize.out_size
-    if h != w:
-        raise ValueError(f"eval_step_fid: infer_downsample resizes square images, the transform makes {h}x{w}")
-    L.eval_downsample_resize(h, d)                       # refuses a factor that leaves no pixel
+def _eval_step_fid_saved(vqgan, images, resize: U8Resize, inception, total_usage, norm: U8Norm, d, saved_as: str):
+    """eval_step_fid on the bytes the script saves, materialised on the device: resized when d is given, then round
+    tripped through JPEG when saved_as is "jpeg"."""
+    from . import downsample, jpeg
+    if d is not None:
+        d = L.check_infer_downsample(d, "eval_step_fid")
+        h, w = resize.out_size
+        if h != w:
+            raise ValueError(f"eval_step_fid: infer_downsample resizes square images, the transform makes {h}x{w}")
+        L.eval_downsample_resize(h, d)                   # refuses a factor that leaves no pixel
     downsample.real_value_table(norm)
     if inception.device.type != "cuda":
         raise ValueError(f"eval_step_fid: the FID network is on {inception.device}, not a CUDA device")
@@ -357,11 +383,16 @@ def _eval_step_fid_downsample(vqgan, images, resize: U8Resize, inception, total_
         fake, vq_output = eval_step_u8(vqgan, real, total_usage, norm)
         real = real.unsqueeze(1)
     # the saved input bytes ((x + 0.5) * 255).astype(uint8): the value map at d = 1 (an identity interpolation)
-    real = downsample.clips_u8(real.contiguous(), 1, real_norm=norm, what="eval_step_fid")
-    real_small = downsample.images_u8(real[:, 0], d, "eval_step_fid")
-    fake_small = downsample.images_u8(fake[:, 0].contiguous(), d, "eval_step_fid")
-    real_features = inception.features(real_small).clone()
-    fake_features = inception.features(fake_small).clone()
+    real = downsample.clips_u8(real.contiguous(), 1, real_norm=norm, what="eval_step_fid")[:, 0]
+    fake = fake[:, 0].contiguous()
+    if d is not None:
+        real = downsample.images_u8(real, d, "eval_step_fid")
+        fake = downsample.images_u8(fake, d, "eval_step_fid")
+    if saved_as == "jpeg":
+        real = jpeg.roundtrip_u8(real, jpeg.DEFAULT_QUALITY)
+        fake = jpeg.roundtrip_u8(fake, jpeg.DEFAULT_QUALITY)
+    real_features = inception.features(real).clone()
+    fake_features = inception.features(fake).clone()
     return real_features, fake_features, vq_output
 
 
