@@ -313,6 +313,30 @@ int omt_lpips_input(const void* x, const float* lut, const int32_t* sel, const f
 int omt_lpips_head(const float* x, int Cs, int C, int P, int h, int w, const float* lin_w, int tap, float* taps_out,
                    float* total, omt_stream_t stream);
 
+/* The per-pixel map of one LPIPS tap (the lpips package's spatial=True, before the upsample): x fp32 [2P][h][w][Cs],
+ * pair p = images p and p + P, C channels; map fp32 [P][h][w] gets, per pixel, exactly the term omt_lpips_head sums:
+ *   sum_c lin_w[c] (x_c / (|x| + 1e-10) - y_c / (|y| + 1e-10))^2,  |x| = sqrt(sum_c x_c^2)  (fp32). */
+int omt_lpips_map(const float* x, int Cs, int C, int P, int h, int w, const float* lin_w, float* map,
+                  omt_stream_t stream);
+
+/* One tap map [P][h][w] fp32 of omt_lpips_upsample_mean (4-byte aligned). */
+typedef struct {
+  const float* map;
+  int h, w;
+} omt_lpips_tap;
+#define OMT_LPIPS_MAX_TAPS 5
+
+/* The lpips package's spatial=True tail (lpips.py upsample and `val += res[kk]`) for P pairs: per output pixel of H x W,
+ *   v = 0; for k in 0 .. n_taps - 1: v += up_k,
+ * up_k = nn.Upsample(size=(H, W), mode='bilinear', align_corners=False) of tap k in torch's fp32 CUDA arithmetic:
+ * scale = (float)h / (float)H, src = max(fmaf(dst + 0.5f, scale, -0.5f), 0), i0 = (int)src, i1 = i0 + (i0 < h - 1),
+ * l1 = src - i0, l0 = 1 - l1 (likewise along w), top = fmaf(w0, a[i0][j0], w1 a[i0][j1]), bottom likewise on row i1,
+ * up = fmaf(h0, top, h1 bottom); a tap of the output's size is copied.  taps: host array of n_taps (1 .. 5) entries.
+ * map_out (NULL: not written): fp32 [P][H][W] of v.  mean_out[p] = (float)(the fp64 sum of pair p's v / (H W)), summed
+ * in a fixed order (no atomics: two runs give the same bits). */
+int omt_lpips_upsample_mean(const omt_lpips_tap* taps, int n_taps, int P, int H, int W, float* map_out,
+                            float* mean_out, omt_stream_t stream);
+
 /* Row softmax of the Inception Score's classifier (calculate_is.py's F.softmax over dim 1), fp32: rows of N logits at
  * x + r * ldx -> y + r * ldy, per row m = max, e_j = exp(x_j - m) (the difference and exp in fp64, rounded once to fp32),
  * s = the fp32 sum of e in a fixed order, y_j = e_j / s (true division).  N >= 1, ldx, ldy >= N, 4-byte aligned. */

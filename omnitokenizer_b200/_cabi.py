@@ -36,6 +36,17 @@ class LinearHArgs(ctypes.Structure):
                 ("a_rs_uniform", c_float), ("u_scale", c_float)]
 
 
+class LpipsTap(ctypes.Structure):
+    """omt_lpips_tap (include/omnitok_b200.h): one tap map of omt_lpips_upsample_mean."""
+    _fields_ = [("map", c_void_p), ("h", c_int), ("w", c_int)]
+
+
+def lpips_taps(maps):
+    """A host omt_lpips_tap array of (map [P][h][w] tensor or address, h, w) entries, for omt_lpips_upsample_mean.
+    The caller keeps the maps alive."""
+    return (LpipsTap * len(maps))(*[LpipsTap(_ptr(m), h, w) for m, h, w in maps])
+
+
 # name -> (restype, argtypes); mirrors include/omnitok_b200.h one to one
 SIGNATURES = {
     "omt_abi_version": (c_int, []),
@@ -77,6 +88,8 @@ SIGNATURES = {
     "omt_psnr_ssim": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_void_p] * 4),
     "omt_lpips_input": (c_int, [c_void_p] * 4 + [c_int] * 4 + [c_void_p, c_void_p]),
     "omt_lpips_head": (c_int, [c_void_p] + [c_int] * 5 + [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "omt_lpips_map": (c_int, [c_void_p] + [c_int] * 5 + [c_void_p, c_void_p, c_void_p]),
+    "omt_lpips_upsample_mean": (c_int, [c_void_p] + [c_int] * 4 + [c_void_p, c_void_p, c_void_p]),
     "omt_softmax_rows": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "omt_inception_score": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "omt_jpeg_roundtrip_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),

@@ -9,6 +9,9 @@
 //                    op order, into the [P][H][W][4] network input of omt_conv3d (channel 3 zero).
 //   omt_lpips_head   normalize_tensor of both images' features at one VGG tap, the squared difference, NetLinLayer's
 //                    1x1 conv and spatial_average: one CTA per pair, a warp per pixel.
+//   omt_lpips_map    the same per-pixel term written as a map (the lpips package's spatial=True AlexNet LPIPS).
+//   omt_lpips_upsample_mean  the five tap maps upsampled to the frame (torch's bilinear, align_corners=False), summed
+//                    in tap order, and each pair's mean over the frame in fp64: one CTA per pair.
 //   omt_softmax_rows  the Inception Score classifier's softmax: one CTA per row.
 //   omt_inception_score  the IS split reduction in fp64: the split's column means (a thread per column), then one CTA
 //                    per split, a warp per row, for the rows' KL divergences from the split's marginal.
@@ -46,6 +49,13 @@ __device__ __forceinline__ double block_sum(double v, double* red) {
   const double r = red[0];
   __syncthreads();
   return r;
+}
+
+// Fixed-order warp sum in fp64: the same butterfly in every lane, so every lane holds the same bits.
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
 }
 
 template <bool F32>
@@ -176,9 +186,28 @@ lpips_input_kernel(const void* __restrict__ x, const float* __restrict__ lut, co
   }
 }
 
-// One VGG tap of P pairs, images i and i + P of x [2P][h][w][Cs]: per pixel
+// One LPIPS pixel of a warp, features pa and pb of C channels:
 //   sum_c w_c (x_c / (|x| + 1e-10) - y_c / (|y| + 1e-10))^2,  |x| = sqrt(sum_c x_c^2)   (fp32, true divisions)
-// summed over the pixels in fp64 (warp partials in pixel order, then the warps in order) and divided by h w.
+// lane partials in channel order, then the warp butterfly: every lane returns the same bits.
+__device__ __forceinline__ float lpips_pixel(const float* pa, const float* pb, int C, const float* __restrict__ lin_w,
+                                             int lane) {
+  float na = 0.f, nb = 0.f;
+  for (int c = lane; c < C; c += 32) {
+    const float u = __ldg(pa + c), v = __ldg(pb + c);
+    na = __fmaf_rn(u, u, na);
+    nb = __fmaf_rn(v, v, nb);
+  }
+  const float da = __fadd_rn(__fsqrt_rn(warp_sum(na)), 1e-10f), db = __fadd_rn(__fsqrt_rn(warp_sum(nb)), 1e-10f);
+  float s = 0.f;
+  for (int c = lane; c < C; c += 32) {
+    const float d = __fsub_rn(__fdiv_rn(__ldg(pa + c), da), __fdiv_rn(__ldg(pb + c), db));
+    s = __fmaf_rn(__ldg(lin_w + c), __fmul_rn(d, d), s);
+  }
+  return warp_sum(s);
+}
+
+// One VGG tap of P pairs, images i and i + P of x [2P][h][w][Cs]: lpips_pixel summed over the pixels in fp64 (warp
+// partials in pixel order, then the warps in order) and divided by h w.
 constexpr int HEAD_THREADS = 512, HEAD_WARPS = HEAD_THREADS / 32;
 __global__ void __launch_bounds__(HEAD_THREADS)
 lpips_head_kernel(const float* __restrict__ x, int Cs, int C, int P, int hw, const float* __restrict__ lin_w, int tap,
@@ -190,21 +219,7 @@ lpips_head_kernel(const float* __restrict__ x, int Cs, int C, int P, int hw, con
   const float* xb = x + (size_t)(p + P) * hw * Cs;
   double acc = 0.0;
   for (int pix = warp; pix < hw; pix += HEAD_WARPS) {
-    const float* pa = xa + (size_t)pix * Cs;
-    const float* pb = xb + (size_t)pix * Cs;
-    float na = 0.f, nb = 0.f;
-    for (int c = lane; c < C; c += 32) {
-      const float u = __ldg(pa + c), v = __ldg(pb + c);
-      na = __fmaf_rn(u, u, na);
-      nb = __fmaf_rn(v, v, nb);
-    }
-    const float da = __fadd_rn(__fsqrt_rn(warp_sum(na)), 1e-10f), db = __fadd_rn(__fsqrt_rn(warp_sum(nb)), 1e-10f);
-    float s = 0.f;
-    for (int c = lane; c < C; c += 32) {
-      const float d = __fsub_rn(__fdiv_rn(__ldg(pa + c), da), __fdiv_rn(__ldg(pb + c), db));
-      s = __fmaf_rn(__ldg(lin_w + c), __fmul_rn(d, d), s);
-    }
-    s = warp_sum(s);
+    const float s = lpips_pixel(xa + (size_t)pix * Cs, xb + (size_t)pix * Cs, C, lin_w, lane);
     acc = __dadd_rn(acc, (double)s);
   }
   if (lane == 0) red[warp] = acc;
@@ -222,11 +237,81 @@ lpips_head_kernel(const float* __restrict__ x, int Cs, int C, int P, int hw, con
   }
 }
 
-// Fixed-order warp sum in fp64: the same butterfly in every lane, so every lane holds the same bits.
-__device__ __forceinline__ double warp_sum_d(double v) {
+// The per-pixel map of one tap: a warp per pixel of the P h w, lane 0 stores lpips_pixel.
+constexpr int MAP_THREADS = 256, MAP_WARPS = MAP_THREADS / 32;
+__global__ void __launch_bounds__(MAP_THREADS)
+lpips_map_kernel(const float* __restrict__ x, int Cs, int C, int P, int hw, const float* __restrict__ lin_w,
+                 float* __restrict__ map) {
+  pdl_sync();
+  const int lane = threadIdx.x & 31;
+  const long long n = (long long)P * hw;
+  for (long long i = blockIdx.x * (long long)MAP_WARPS + (threadIdx.x >> 5); i < n; i += (long long)gridDim.x * MAP_WARPS) {
+    const long long p = i / hw, pix = i - p * hw;
+    const float s = lpips_pixel(x + (size_t)(p * hw + pix) * Cs, x + (size_t)((p + P) * hw + pix) * Cs, C, lin_w, lane);
+    if (lane == 0) map[i] = s;
+  }
+}
+
+// The spatial=True tail: one CTA per pair; thread t takes pixels t, t + UP_THREADS, ... in order, v = 0 + up_0 + ...
+// + up_{n-1} (torch's upsample_bilinear2d_out_frame<float, float> per tap), and the fp64 sum of v over the frame is
+// the per-thread partials, the warp butterfly, then the warps in order.
+constexpr int UP_THREADS = 512, UP_WARPS = UP_THREADS / 32;
+struct UpTaps {
+  omt_lpips_tap t[OMT_LPIPS_MAX_TAPS];
+  float sh[OMT_LPIPS_MAX_TAPS], sw[OMT_LPIPS_MAX_TAPS];   // (float)h / (float)H, (float)w / (float)W, as torch's host
+};
+
+// area_pixel_compute_source_index(scale, dst, align_corners=false, cubic=false) and its two taps and weights
+__device__ __forceinline__ void bilinear_axis(float scale, int dst, int in, int& i0, int& i1, float& l0, float& l1) {
+  float src = __fmaf_rn((float)dst + 0.5f, scale, -0.5f);
+  src = src >= 0.f ? src : 0.f;
+  i0 = (int)src;
+  i1 = i0 + (i0 < in - 1 ? 1 : 0);
+  l1 = __fsub_rn(src, (float)i0);
+  l0 = __fsub_rn(1.f, l1);
+}
+
+__global__ void __launch_bounds__(UP_THREADS)
+lpips_upsample_mean_kernel(UpTaps taps, int n_taps, int H, int W, float* __restrict__ map_out,
+                           float* __restrict__ mean_out) {
+  __shared__ double red[UP_WARPS];
+  pdl_sync();
+  const int p = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int hw = H * W;
+  double acc = 0.0;
+  for (int i = tid; i < hw; i += UP_THREADS) {
+    const int y = i / W, x = i - y * W;
+    float v = 0.f;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
+    for (int k = 0; k < OMT_LPIPS_MAX_TAPS; ++k) {
+      if (k >= n_taps) break;
+      const int h = taps.t[k].h, w = taps.t[k].w;
+      const float* a = taps.t[k].map + (size_t)p * h * w;
+      float up;
+      if (h == H && w == W) {
+        up = __ldg(a + i);
+      } else {
+        int y0, y1, x0, x1;
+        float h0, h1, w0, w1;
+        bilinear_axis(taps.sh[k], y, h, y0, y1, h0, h1);
+        bilinear_axis(taps.sw[k], x, w, x0, x1, w0, w1);
+        const float top = __fmaf_rn(w0, __ldg(a + y0 * w + x0), __fmul_rn(w1, __ldg(a + y0 * w + x1)));
+        const float bot = __fmaf_rn(w0, __ldg(a + y1 * w + x0), __fmul_rn(w1, __ldg(a + y1 * w + x1)));
+        up = __fmaf_rn(h0, top, __fmul_rn(h1, bot));
+      }
+      v = __fadd_rn(v, up);
+    }
+    if (map_out) map_out[(size_t)p * hw + i] = v;
+    acc = __dadd_rn(acc, (double)v);
+  }
+  acc = warp_sum_d(acc);
+  if (lane == 0) red[warp] = acc;
+  __syncthreads();
+  if (tid == 0) {
+    double t = red[0];
+    for (int i = 1; i < UP_WARPS; ++i) t = __dadd_rn(t, red[i]);
+    mean_out[p] = (float)(t / (double)hw);
+  }
 }
 
 // Row r of x -> row r of y: m = max, e = exp(x - m) in fp64 rounded to fp32 (a probability's error then does not grow
@@ -387,6 +472,49 @@ extern "C" int omt_lpips_head(const float* x, int Cs, int C, int P, int h, int w
   OMT_REQUIRE(aligned_to(4, {x, lin_w, taps_out, total}), "omt_lpips_head: misaligned pointer");
   OMT_CUDA(launch_k(quality::lpips_head_kernel, dim3(P), dim3(quality::HEAD_THREADS), 0, (cudaStream_t)stream, x, Cs, C, P,
                     h * w, lin_w, tap, taps_out, total));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_lpips_map(const float* x, int Cs, int C, int P, int h, int w, const float* lin_w, float* map,
+                             omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(x && lin_w && map, "omt_lpips_map: null pointer");
+  OMT_REQUIRE(C >= 1 && Cs >= C && P >= 1 && h >= 1 && w >= 1, "omt_lpips_map: C=%d of stride %d, P=%d, %dx%d", C, Cs,
+              P, h, w);
+  OMT_REQUIRE((long long)h * w <= 0x7fffffffLL, "omt_lpips_map: %dx%d maps are too large", h, w);
+  OMT_REQUIRE(aligned_to(4, {x, lin_w, map}), "omt_lpips_map: misaligned pointer");
+  const long long warps = (long long)P * h * w;
+  const long long blocks = (warps + quality::MAP_WARPS - 1) / quality::MAP_WARPS;
+  const int grid = (int)(blocks < sm_count() * 16LL ? blocks : sm_count() * 16LL);
+  OMT_CUDA(launch_k(quality::lpips_map_kernel, dim3(grid), dim3(quality::MAP_THREADS), 0, (cudaStream_t)stream, x, Cs, C,
+                    P, h * w, lin_w, map));
+  OMT_LAUNCH_CHECK();
+  return OMT_OK;
+}
+
+extern "C" int omt_lpips_upsample_mean(const omt_lpips_tap* taps, int n_taps, int P, int H, int W, float* map_out,
+                                       float* mean_out, omt_stream_t stream) {
+  OMT_ENTER();
+  OMT_REQUIRE(taps && mean_out, "omt_lpips_upsample_mean: null pointer");
+  OMT_REQUIRE(n_taps >= 1 && n_taps <= OMT_LPIPS_MAX_TAPS, "omt_lpips_upsample_mean: %d taps (1 to %d)", n_taps,
+              OMT_LPIPS_MAX_TAPS);
+  OMT_REQUIRE(P >= 1 && H >= 1 && W >= 1 && (long long)H * W <= 0x7fffffffLL, "omt_lpips_upsample_mean: P=%d, %dx%d",
+              P, H, W);
+  OMT_REQUIRE(aligned_to(4, {map_out, mean_out}), "omt_lpips_upsample_mean: misaligned pointer");
+  quality::UpTaps t{};
+  for (int k = 0; k < n_taps; ++k) {
+    const omt_lpips_tap& a = taps[k];
+    OMT_REQUIRE(a.map, "omt_lpips_upsample_mean: tap %d: null map", k);
+    OMT_REQUIRE(a.h >= 1 && a.w >= 1 && (long long)a.h * a.w <= 0x7fffffffLL, "omt_lpips_upsample_mean: tap %d is %dx%d",
+                k, a.h, a.w);
+    OMT_REQUIRE(aligned_to(4, {a.map}), "omt_lpips_upsample_mean: tap %d: misaligned map", k);
+    t.t[k] = a;
+    t.sh[k] = (float)a.h / (float)H;            // area_pixel_compute_scale<float>, align_corners=False, no scale given
+    t.sw[k] = (float)a.w / (float)W;
+  }
+  OMT_CUDA(launch_k(quality::lpips_upsample_mean_kernel, dim3(P), dim3(quality::UP_THREADS), 0, (cudaStream_t)stream, t,
+                    n_taps, H, W, map_out, mean_out));
   OMT_LAUNCH_CHECK();
   return OMT_OK;
 }

@@ -6,15 +6,18 @@ trunk on csrc/i3d.cu's omt_conv3d (3x3, pad 1, ReLU, 3xTF32) and omt_pool2d (2 x
 - frame_metrics(real_u8, fake_u8, lpips=None, real_norm=None): per-frame psnr / ssim (fp64) and lpips (fp32) of device
   uint8 (B, T, H, W, 3) frames;
 - drop-ins with the suite's signatures and result dicts: calculate_psnr, calculate_ssim (videos (B, T, C, H, W) in
-  [0, 1]) and calculate_lpips_vgg (the VGG LPIPS; the suite's calculate_lpips means AlexNet, spatial=True, which is not
-  built here);
+  [0, 1]) and calculate_lpips_vgg (the VGG LPIPS);
+- calculate_lpips(videos1, videos2, device, model): the suite's own calculate_lpips, the lpips package's AlexNet with
+  spatial=True (AlexLPIPS, load_lpips_alex: torchvision's AlexNet file and the package's lin file, taken by path): the
+  five convs on omt_conv3d, the 3 x 3 / 2 max pools on omt_pool2d, each tap's per-pixel map (omt_lpips_map) and the
+  maps upsampled, summed and averaged per frame (omt_lpips_upsample_mean);
 - calculate_fvd(videos1, videos2, device, method, i3d): the suite's FVD at every prefix length, styleganv or videogpt,
   on fvd.I3D.features (csrc/resample.cu's omt_fvd_suite_preprocess and the I3D kernels).
 
 Activations are channels-last fp32 [2P][h][w][C] (the network input [2P][H][W][4]); pair p is images p (real) and
 p + P (reconstruction).  Each VGG tap's LPIPS head runs right after the tap's conv, so only two ping-pong activation
-buffers live.  The frames run in chunks of at most LPIPS_ROWS / (2 H W) pairs; every (chunk, H, W, real_norm) gets its
-own buffers and CUDA graph.
+buffers live; AlexNet writes each tap's map right after the tap's conv in the same way.  The frames run in chunks of at
+most LPIPS_ROWS / (2 H W) pairs; every (chunk, H, W, real_norm) gets its own buffers and CUDA graph.
 """
 from __future__ import annotations
 
@@ -139,11 +142,11 @@ def lpips_state_dict(state_dict: Dict[str, torch.Tensor]) -> Dict[str, torch.Ten
 
 def check_net(net: str = "vgg", spatial: bool = False):
     if net != "vgg":
-        raise NotImplementedError(f"LPIPS net {net!r} is not built: only the tokenizer's VGG16 LPIPS (lpips.py) is; "
-                                  f"the lpips package's AlexNet / SqueezeNet weights are not in the tree")
+        raise NotImplementedError(f"LPIPS net {net!r} is not built here: this class is the tokenizer's VGG16 LPIPS "
+                                  f"(lpips.py); the lpips package's net='alex', spatial=True is quality.AlexLPIPS")
     if spatial:
-        raise NotImplementedError("LPIPS spatial=True (the lpips package's per-pixel map) is not built: the VGG LPIPS "
-                                  "returns the spatial average")
+        raise NotImplementedError("LPIPS spatial=True is not built for the VGG LPIPS, which returns the spatial "
+                                  "average; the lpips package's AlexNet with spatial=True is quality.AlexLPIPS")
 
 
 def input_table(shift: torch.Tensor, scale: torch.Tensor, real_norm: Optional[L.U8Norm] = None) -> torch.Tensor:
@@ -395,6 +398,243 @@ def calculate_lpips_vgg(videos1, videos2, model: LPIPS) -> dict:
     a, b, (B, T), setting = _videos_f32(videos1, videos2, "calculate_lpips_vgg", True, model.device)
     _, _, lp = _run(a, b, FORM_F32, model, None, None)
     return result_dict(lp.view(B, T).cpu().numpy(), setting)
+
+
+# ------------------------------------------------------------------------------------------------ AlexNet LPIPS
+class AlexConv(NamedTuple):
+    """One conv of torchvision's alexnet().features as the lpips package slices it (slice k = the conv and its ReLU,
+    tap k): index, slice, widths, square kernel, stride, padding, and whether MaxPool2d(3, 2) precedes it."""
+    idx: int
+    slice: int
+    cin: int
+    cout: int
+    k: int
+    stride: int
+    pad: int
+    pool: bool
+
+
+# lpips/pretrained_networks.py alexnet: slice1 = features[0:2], slice2 = [2:5], slice3 = [5:8], slice4 = [8:10],
+# slice5 = [10:12]; the taps are relu1 ... relu5
+ALEX = [AlexConv(0, 1, 3, 64, 11, 4, 2, False), AlexConv(3, 2, 64, 192, 5, 1, 2, True),
+        AlexConv(6, 3, 192, 384, 3, 1, 1, True), AlexConv(8, 4, 384, 256, 3, 1, 1, False),
+        AlexConv(10, 5, 256, 256, 3, 1, 1, False)]
+ALEX_CHNS = tuple(c.cout for c in ALEX)
+ALEX_POOL = (3, 2)                 # MaxPool2d(kernel_size=3, stride=2), floor mode
+MIN_ALEX = 31                      # at 30 the second pool gets a 2 x 2 map
+
+
+def alex_tap_sizes(H: int, W: int) -> List[Tuple[int, int]]:
+    """(h, w) of relu1 ... relu5 of an H x W frame: conv1 (H + 4 - 11) // 4 + 1, each pool (n - 3) // 2 + 1, the 3 x 3
+    pad-1 convs keep their size.  Raises ValueError where a pool would get less than its window."""
+    sizes, h, w = [], H, W
+    for c in ALEX:
+        if c.pool:
+            if min(h, w) < ALEX_POOL[0]:
+                raise ValueError(f"AlexNet LPIPS: a {H} x {W} frame leaves a {h} x {w} map for a 3 x 3 pool; H, W >= "
+                                 f"{MIN_ALEX}")
+            h, w = (h - ALEX_POOL[0]) // ALEX_POOL[1] + 1, (w - ALEX_POOL[0]) // ALEX_POOL[1] + 1
+        h, w = (h + 2 * c.pad - c.k) // c.stride + 1, (w + 2 * c.pad - c.k) // c.stride + 1
+        if min(h, w) < 1:
+            raise ValueError(f"AlexNet LPIPS: a {H} x {W} frame is smaller than conv1's 11 x 11 window")
+        sizes.append((h, w))
+    return sizes
+
+
+def alex_expected_keys() -> Dict[str, tuple]:
+    """The keys of the lpips package's LPIPS(net='alex') state_dict."""
+    keys = {}
+    for c in ALEX:
+        keys[f"net.slice{c.slice}.{c.idx}.weight"] = (c.cout, c.cin, c.k, c.k)
+        keys[f"net.slice{c.slice}.{c.idx}.bias"] = (c.cout,)
+    for k, ch in enumerate(ALEX_CHNS):
+        keys[f"lin{k}.model.1.weight"] = (1, ch, 1, 1)
+    keys["scaling_layer.shift"] = (1, 3, 1, 1)
+    keys["scaling_layer.scale"] = (1, 3, 1, 1)
+    return keys
+
+
+def alex_state_dict(state_dict: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """The lpips AlexNet keys of either layout: the lpips module's own state_dict, or torchvision alexnet's
+    `features.{0,3,6,8,10}.*` plus the lpips lin file's `lin{k}.model.1.weight` (`classifier.*` ignored).  Without
+    `scaling_layer.*`, ScalingLayer's constructor values."""
+    sd = {}
+    where = {c.idx: c.slice for c in ALEX}
+    for k, v in state_dict.items():
+        if k.startswith("classifier."):
+            continue
+        if k.startswith("features."):
+            idx, rest = k[len("features."):].split(".", 1)
+            if not idx.isdigit() or int(idx) not in where:
+                raise KeyError(f"AlexNet LPIPS state_dict: unexpected torchvision key {k}")
+            k = f"net.slice{where[int(idx)]}.{idx}.{rest}"
+        sd[k] = v
+    sd.setdefault("scaling_layer.shift", torch.tensor(SHIFT).view(1, 3, 1, 1))
+    sd.setdefault("scaling_layer.scale", torch.tensor(SCALE).view(1, 3, 1, 1))
+    return sd
+
+
+class AlexLPIPS:
+    """The lpips package's LPIPS(net='alex', spatial=True) (v0.1: ScalingLayer, torchvision's AlexNet trunk, five lin
+    layers, each tap's map upsampled to the frame and the maps summed) in eval mode, from a state_dict (see
+    alex_state_dict for the accepted layouts).  A missing or mis-shaped key is named in the error.  The convs are packed
+    once, on `device`.  Only the configuration calculate_lpips.py builds exists: any other net or spatial raises
+    NotImplementedError."""
+
+    def __init__(self, state_dict: Dict[str, torch.Tensor], device="cuda", net: str = "alex", spatial: bool = True):
+        if net != "alex":
+            raise NotImplementedError(f"AlexLPIPS: net {net!r} is not built; only net='alex' (the suite's "
+                                      f"calculate_lpips) is, and quality.LPIPS is the tokenizer's VGG LPIPS")
+        if spatial is not True:
+            raise NotImplementedError(f"AlexLPIPS: spatial={spatial!r} is not built; only spatial=True (the suite's "
+                                      f"calculate_lpips) is")
+        sd = alex_state_dict(state_dict)
+        check_state_dict(sd, alex_expected_keys(), "AlexNet LPIPS")
+        self.device = resolve_device(device)
+        sd = {k: v.detach().float().cpu() for k, v in sd.items()}
+        self.convs = [PackedConv(sd[f"net.slice{c.slice}.{c.idx}.weight"], sd[f"net.slice{c.slice}.{c.idx}.bias"],
+                                 self.device, c, (1, c.stride, c.stride)) for c in ALEX]
+        self.lin = [sd[f"lin{k}.model.1.weight"].reshape(-1).contiguous().to(self.device) for k in range(len(ALEX))]
+        self.shift, self.scale = sd["scaling_layer.shift"].reshape(3), sd["scaling_layer.scale"].reshape(3)
+        self.shift_scale = torch.cat([self.shift, self.scale]).to(self.device)
+        self._ws = {}
+
+
+def load_lpips_alex(device, alexnet_path: str, lin_path: str) -> AlexLPIPS:
+    """AlexLPIPS from the two files lpips.LPIPS(net='alex') reads: torchvision's alexnet-owt-7be5be79.pth and the lpips
+    package's weights/v0.1/alex.pth.  Not shipped; nothing is downloaded."""
+    sd = dict(torch.load(alexnet_path, map_location="cpu", weights_only=True))
+    sd.update(torch.load(lin_path, map_location="cpu", weights_only=True))
+    return AlexLPIPS(sd, device)
+
+
+class _AlexWorkspace:
+    """Buffers, launch list and CUDA graph state of one (form, P, H, W): the network input, the trunk on two ping-pong
+    activation buffers with each tap's map written right after its conv, then the upsampled sum and its per-pair mean."""
+
+    def __init__(self, device, form: int, P: int, H: int, W: int, model: AlexLPIPS):
+        self.graphs = {}
+        f = dict(device=device, dtype=torch.float32)
+        dt = torch.uint8 if form == FORM_U8 else torch.float32
+        self.a = torch.empty(P, H, W, 3, dtype=dt, device=device)
+        self.b = torch.empty(P, H, W, 3, dtype=dt, device=device)
+        self.mean = torch.zeros(P, **f)
+        sizes = alex_tap_sizes(H, W)
+        self.maps = [torch.zeros(P, h, w, **f) for h, w in sizes]
+        x = torch.zeros(2 * P, H, W, 4, **f)
+        big, prev = 0, (H, W)
+        for c, (h, w) in zip(ALEX, sizes):
+            big = max(big, h * w * c.cout, prev[0] * prev[1] * c.cin if c.pool else 0)
+            prev = (h, w)
+        bufs = [torch.zeros(2 * P * big, **f), torch.zeros(2 * P * big, **f)]
+        half = P * H * W * 4
+        self.ops = []
+        if form == FORM_U8:
+            tab = input_table(model.shift, model.scale).to(device)
+            self.ops.append(lambda: _cabi.call("omt_lpips_input", self.a, tab, None, None, form, P, H, W, x))
+            self.ops.append(lambda: _cabi.call("omt_lpips_input", self.b, tab, None, None, form, P, H, W,
+                                               x.data_ptr() + 4 * half))
+        else:
+            ss = model.shift_scale
+            self.ops.append(lambda: _cabi.call("omt_lpips_input", self.a, None, None, ss, form, P, H, W, x))
+            self.ops.append(lambda: _cabi.call("omt_lpips_input", self.b, None, None, ss, form, P, H, W,
+                                               x.data_ptr() + 4 * half))
+        pk, ps = ALEX_POOL
+        cur, c_cur, h, w, nxt = x, 4, H, W, 0
+        for k, (u, (ho, wo)) in enumerate(zip(model.convs, sizes)):
+            c = u.conv
+            if c.pool:
+                ph, pw = (h - pk) // ps + 1, (w - pk) // ps + 1
+                y = bufs[nxt][:2 * P * ph * pw * c_cur].view(2 * P, ph, pw, c_cur)
+                self.ops.append(lambda x_=cur, y_=y, cc=c_cur, h_=h, w_=w, ph_=ph, pw_=pw: _cabi.call(
+                    "omt_pool2d", x_, cc, cc, 2 * P, h_, w_, pk, pk, ps, ps, 0, 0, ph_, pw_, y_, cc, POOL_MAX))
+                cur, h, w, nxt = y, ph, pw, 1 - nxt
+            y = bufs[nxt][:2 * P * ho * wo * c.cout].view(2 * P, ho, wo, c.cout)
+            self.ops.append(u.launch(cur, 2 * P, (1, h, w), (0, c.pad, c.pad), (1, ho, wo), y))
+            cur, c_cur, h, w, nxt = y, c.cout, ho, wo, 1 - nxt
+            self.ops.append(lambda x_=cur, cc=c_cur, h_=h, w_=w, k_=k: _cabi.call(
+                "omt_lpips_map", x_, cc, cc, P, h_, w_, model.lin[k_], self.maps[k_]))
+        taps = _cabi.lpips_taps([(m, m.shape[1], m.shape[2]) for m in self.maps])
+        self.ops.append(lambda: _cabi.call("omt_lpips_upsample_mean", taps, len(ALEX), P, H, W, None, self.mean))
+
+    def run(self):
+        for op in self.ops:
+            op()
+
+
+def _alex_side(v, name: str):
+    """One side of calculate_lpips -> its form, with the dtype and rank refusals."""
+    if not isinstance(v, torch.Tensor):
+        raise TypeError(f"calculate_lpips: {name} must be a torch tensor, got {type(v)}")
+    if v.dtype == torch.uint8:
+        if v.dim() != 5 or v.shape[-1] != 3:
+            raise ValueError(f"calculate_lpips: uint8 {name} must be (B, T, H, W, 3), got {tuple(v.shape)}")
+        return FORM_U8
+    if v.dtype == torch.float32:
+        if v.dim() != 5 or v.shape[2] not in (1, 3):
+            raise ValueError(f"calculate_lpips: fp32 {name} must be (B, T, C, H, W) with C 1 or 3, got "
+                             f"{tuple(v.shape)}")
+        return FORM_F32
+    raise TypeError(f"calculate_lpips: {name} must be fp32 (B, T, C, H, W) in [0, 1] or uint8 (B, T, H, W, 3), got "
+                    f"{v.dtype}")
+
+
+@torch.no_grad()
+def lpips_alex_frames(videos1, videos2, device, model: AlexLPIPS) -> torch.Tensor:
+    """calculate_lpips's per-frame values, (B, T) fp32 on the device, with its refusals (see calculate_lpips)."""
+    if not isinstance(model, AlexLPIPS):
+        raise TypeError(f"calculate_lpips needs the AlexNet LPIPS as model= (quality.load_lpips_alex), got "
+                        f"{type(model)}")
+    forms = [_alex_side(v, n) for v, n in ((videos1, "videos1"), (videos2, "videos2"))]
+    if forms[0] != forms[1]:
+        raise TypeError(f"calculate_lpips: videos1 is {videos1.dtype}, videos2 {videos2.dtype}")
+    if videos1.shape != videos2.shape:
+        raise ValueError(f"calculate_lpips: the two sides differ in shape: {tuple(videos1.shape)} and "
+                         f"{tuple(videos2.shape)}")
+    form = forms[0]
+    if form == FORM_U8:
+        B, T, H, W, C = (int(v) for v in videos1.shape)
+    else:
+        B, T, C, H, W = (int(v) for v in videos1.shape)
+    if min(B, T) < 1:
+        raise ValueError(f"calculate_lpips: empty batch {tuple(videos1.shape)}")
+    if H < MIN_ALEX or W < MIN_ALEX:
+        raise ValueError(f"calculate_lpips: AlexNet's pools need H, W >= {MIN_ALEX}, got {H} x {W}")
+    if 2 * H * W > MAX_CONV_ROWS:
+        raise ValueError(f"calculate_lpips: {H} x {W} frames exceed the conv kernel's {MAX_CONV_ROWS} rows for one pair")
+    if torch.device(device).type != "cuda":
+        raise ValueError(f"calculate_lpips runs on a CUDA device, got {device}")
+    dev = resolve_device(device)
+    if dev != model.device:
+        raise ValueError(f"calculate_lpips: device {dev}, the AlexNet LPIPS network is on {model.device}")
+    P = B * T
+    if form == FORM_U8:
+        a, b = (v.to(dev).contiguous().view(P, H, W, 3) for v in (videos1, videos2))
+    else:
+        a, b = (v.to(dev).permute(0, 1, 3, 4, 2).reshape(P, H, W, C).expand(P, H, W, 3).contiguous()
+                for v in (videos1, videos2))
+    out = torch.empty(P, dtype=torch.float32, device=dev)
+    chunk = chunk_pairs(P, H, W, True)
+    for p0 in range(0, P, chunk):
+        n = min(chunk, P - p0)
+        ws = bounded(model._ws, MAX_WORKSPACES, (dev, form, n, H, W),
+                     lambda: _AlexWorkspace(dev, form, n, H, W, model))
+        ws.a.copy_(a[p0:p0 + n])
+        ws.b.copy_(b[p0:p0 + n])
+        run_graphed(ws.graphs, dev, "lpips_alex", ws.run)
+        out[p0:p0 + n] = ws.mean
+    return out.view(B, T)
+
+
+def calculate_lpips(videos1, videos2, device="cuda", model: Optional[AlexLPIPS] = None) -> dict:
+    """calculate_lpips.py's calculate_lpips: per frame, the mean of the lpips package's AlexNet LPIPS map
+    (model = load_lpips_alex(...)), and the suite's result dict.  videos: fp32 (B, T, C, H, W) in [0, 1] (C 1 or 3; host
+    or device) or uint8 (B, T, H, W, 3) standing for byte / 255 (frames on the device stay there); both sides of one
+    shape and dtype, H, W >= 31.  uint8 frames and fp32 frames of byte / 255 give the same bits, as do grey frames and
+    the same frames repeated to 3 channels.  The frames run in chunks; the values do not depend on the chunking."""
+    per = lpips_alex_frames(videos1, videos2, device, model)
+    H, W = (videos1.shape[2:4] if videos1.dtype == torch.uint8 else videos1.shape[3:5])
+    return result_dict(per.cpu().numpy(), torch.Size([per.shape[1], 3, int(H), int(W)]))
 
 
 # ------------------------------------------------------------------------------------------------ calculate_fvd
