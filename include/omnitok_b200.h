@@ -367,6 +367,58 @@ int omt_inception_score(const float* p, int ldp, int N, int n, int splits, doubl
 int omt_jpeg_roundtrip_u8(const uint8_t* src, uint8_t* dst, int B, int H, int W, const uint16_t* qtables,
                           uint8_t* scratch, omt_stream_t stream);
 
+/* One JPEG file of omt_jpeg_decode_u8, as omnitokenizer_b200/jpeg.py stages it.  Offsets are in bytes. */
+typedef struct {
+  long long scan;         /* blob offset of the entropy-coded data: the bytes after the SOS header */
+  long long scan_bytes;   /* from there to the end of the file, 1 .. 2^27 (the device finds the end marker) */
+  long long tables;       /* blob offset of the file's omt_jpeg_tables, 16-byte aligned */
+  long long out;          /* out offset of the (H, W, 3) uint8 RGB output */
+  long long work;         /* scratch offset of the file's work area, 256-byte aligned, at least 256, after the previous
+                             file's (its size: jpeg.py work_bytes) */
+  int H, W;               /* 1 .. 65535 */
+  int ncomp;              /* 1 (grey) or 3 (YCbCr) */
+  int h[3], v[3];         /* sampling factors in frame order: grey 1x1; luma 1x1, 2x1 or 2x2 with chroma 1x1 */
+  int restart;            /* MCUs per restart interval, 0 without DRI */
+  int nsub;               /* subsequence slots: ceil(8 scan_bytes / 1024) + restart intervals, rounded up to 128 */
+  int reserved;
+} omt_jpeg_desc;
+
+/* A file's tables in the blob: per component c, quantisation table q[c] (natural order) and the libjpeg derived forms
+ * (jpeg_make_d_derived_tbl) of its DC (index 2c) and AC (2c + 1) Huffman tables. */
+typedef struct {
+  int32_t q[3][64];
+  uint16_t lookup[6][256];    /* top 8 bits -> length << 8 | symbol for codes of at most 8 bits, 9 << 8 otherwise */
+  int32_t maxcode[6][18];     /* by code length; -1: no code of that length */
+  int32_t valoffset[6][18];
+  uint8_t values[6][256];
+} omt_jpeg_tables;
+
+/* Image.open(f).convert("RGB") of B baseline JPEG files, byte for byte as Pillow (libjpeg-turbo): the scan's Huffman
+ * decode runs in parallel with Weissenberger & Schmidt's self-synchronising subsequences, then libjpeg-turbo's ISLOW
+ * IDCT, h2v1 / h2v2 fancy upsampling and YCbCr -> RGB as omt_jpeg_roundtrip_u8 (oracle/jpeg_decode_oracle.py restates
+ * every stage).  blob: the staged scans and tables (blob_bytes); desc [B]: device table, desc_host: the same in host
+ * memory, checked before any launch (every scan and table inside the blob, every output inside out, every work area
+ * inside scratch; they must equal the device copy).  scratch: overwritten.  out: each file's pixels at its offset.
+ * status: int32 [B], written: 0, or what made the file undecodable (1 no end marker, 2 restart marker out of order,
+ * 3 wrong number of restart intervals, 4 invalid Huffman code, 5 coefficient index past 63, 6 scan data ends inside an
+ * MCU, 7 the scan is not followed by EOI, 8 extraneous data before a marker); a failed file's output bytes are
+ * unspecified but nothing is written outside out.  libjpeg-turbo decodes all of these files anyway: 5 silently (its
+ * natural-order table has 16 spare entries, so the AC loop just ends), the rest with a warning.  No encoder writes them,
+ * so this decoder refuses them.  The synchronisation reads a 4-byte flag back after each of its
+ * launches (at least two), so the call waits on the stream and cannot be captured in a CUDA graph. */
+int omt_jpeg_decode_u8(const uint8_t* blob, long long blob_bytes, const omt_jpeg_desc* desc,
+                       const omt_jpeg_desc* desc_host, int B, uint8_t* scratch, long long scratch_bytes, uint8_t* out,
+                       long long out_bytes, int32_t* status, omt_stream_t stream);
+
+/* omt_jpeg_decode_u8, also reporting what it ran: stage_ms (NULL, or [5]) the CUDA-event times of destuff,
+ * synchronisation, coefficients (with the prefix sums), IDCT and pixels; sync_launches (NULL, or one int) the
+ * synchronisation's launch count.  A call launches 5 kernels plus those, at least 2 and at most (subsequence CTAs of
+ * the largest file + 2). */
+int omt_jpeg_decode_u8_timed(const uint8_t* blob, long long blob_bytes, const omt_jpeg_desc* desc,
+                             const omt_jpeg_desc* desc_host, int B, uint8_t* scratch, long long scratch_bytes,
+                             uint8_t* out, long long out_bytes, int32_t* status, float* stage_ms, int* sync_launches,
+                             omt_stream_t stream);
+
 /* Inverse Rearrange of to_pixels (omnitokenizer.py:1008 / :1015): P [rows, K] -> video (B,Cin,T,H,W).  Rows, features and
  * geometry as omt_patchify_ln: Cin >= 1, p > 0 a multiple of 4 dividing H and W, pt > 0 dividing T - 1 for the rest frames. */
 int omt_unpatchify(const float* P, float* video, int B, int Cin, int T, int H, int W, int p, int pt,

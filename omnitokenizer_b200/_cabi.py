@@ -93,6 +93,10 @@ SIGNATURES = {
     "omt_softmax_rows": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "omt_inception_score": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "omt_jpeg_roundtrip_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "omt_jpeg_decode_u8": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_void_p, c_int64,
+                                   c_void_p, c_void_p]),
+    "omt_jpeg_decode_u8_timed": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_void_p,
+                                         c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "omt_unpatchify": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_void_p]),
     "omt_unpatchify_u8": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_float] * 5 + [c_void_p]),
     "omt_peg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
@@ -159,6 +163,7 @@ def _stream():
 
 
 # kernels launched per entry point (for bench.py's gpu_launches accounting)
+# (omt_jpeg_decode_u8_timed's count varies with the data: jpeg.decode_into adds what the call reports)
 KERNELS_PER_CALL = {"omt_u8_norm_select": 2, "omt_jpeg_roundtrip_u8": 2}
 launch_count = 0
 

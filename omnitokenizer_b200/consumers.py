@@ -336,7 +336,10 @@ def eval_step_fid(vqgan, images: Sequence[torch.Tensor], resize: U8Resize, incep
     Image.ANTIALIAS (Pillow's LANCZOS, downsample.images_u8); the real side's byte map then comes before the resize.
     saved_as: the format the script's img.save(path) writes, saved_format(batch["path"][0]).  "png" is lossless, so
     the network sees the saved bytes themselves; with "jpeg" both sides' saved bytes (after the resize, if any) go
-    through Pillow's JPEG save at its default quality 75 and reload (jpeg.roundtrip_u8), as pytorch-fid reads them."""
+    through Pillow's JPEG save at its default quality 75 and reload (jpeg.roundtrip_u8), as pytorch-fid reads them.
+    images may also hold JPEG files (bytes-like or paths, as ImageDataset reads them), decoded on the device byte for
+    byte as Image.open(path).convert('RGB') (vqgan.forward_jpeg_u8); the results equal those of Pillow's decoded
+    images, bit for bit."""
     from .metricnet import real_byte_table
     if saved_as not in SAVED_FORMATS:
         raise ValueError(f"eval_step_fid: saved_as {saved_as!r} is not one of {SAVED_FORMATS}")
@@ -347,17 +350,37 @@ def eval_step_fid(vqgan, images: Sequence[torch.Tensor], resize: U8Resize, incep
     if infer_downsample is not None or saved_as != "png":
         return _eval_step_fid_saved(vqgan, images, resize, inception, total_usage, norm, infer_downsample, saved_as)
     if hasattr(vqgan, "forward_images_u8"):
-        fake, vq_output = vqgan.forward_images_u8(images, resize, norm, EVAL_U8)
+        fake, vq_output = _forward_sources(vqgan, images, resize, norm)
         if total_usage is not None and vq_output is not None:
             total_usage += vq_output["batch_usage"]
         real = vqgan.engine().encode_u8_frames(tuple(fake.shape))
     else:
-        real = _host_transform(images, resize).to(inception.device)
+        real = _host_transform(_decoded(images, inception.device), resize).to(inception.device)
         fake, vq_output = eval_step_u8(vqgan, real, total_usage, norm)
         real = real.unsqueeze(1)
     real_features = inception.features(real[:, 0], real_norm=norm).clone()
     fake_features = inception.features(fake[:, 0].contiguous()).clone()
     return real_features, fake_features, vq_output
+
+
+def _forward_sources(vqgan, images, resize: U8Resize, norm: U8Norm):
+    """forward_images_u8, or forward_jpeg_u8 when the list holds JPEG files (anything but a tensor)."""
+    if all(isinstance(im, torch.Tensor) for im in images):
+        return vqgan.forward_images_u8(images, resize, norm, EVAL_U8)
+    return vqgan.forward_jpeg_u8(images, resize, norm, EVAL_U8)
+
+
+def _decoded(images, device):
+    """The list with its JPEG files decoded (jpeg.decode_u8 on device, brought to the host as the model's host path
+    takes them)."""
+    from . import jpeg
+    at = [i for i, im in enumerate(images) if not isinstance(im, torch.Tensor)]
+    if not at:
+        return images
+    out = list(images)
+    for i, t in zip(at, jpeg.decode_u8([images[i] for i in at], device)):
+        out[i] = t.cpu()
+    return out
 
 
 def _eval_step_fid_saved(vqgan, images, resize: U8Resize, inception, total_usage, norm: U8Norm, d, saved_as: str):
@@ -374,12 +397,12 @@ def _eval_step_fid_saved(vqgan, images, resize: U8Resize, inception, total_usage
     if inception.device.type != "cuda":
         raise ValueError(f"eval_step_fid: the FID network is on {inception.device}, not a CUDA device")
     if hasattr(vqgan, "forward_images_u8"):
-        fake, vq_output = vqgan.forward_images_u8(images, resize, norm, EVAL_U8)
+        fake, vq_output = _forward_sources(vqgan, images, resize, norm)
         if total_usage is not None and vq_output is not None:
             total_usage += vq_output["batch_usage"]
         real = vqgan.engine().encode_u8_frames(tuple(fake.shape))
     else:
-        real = _host_transform(images, resize).to(inception.device)
+        real = _host_transform(_decoded(images, inception.device), resize).to(inception.device)
         fake, vq_output = eval_step_u8(vqgan, real, total_usage, norm)
         real = real.unsqueeze(1)
     # the saved input bytes ((x + 0.5) * 255).astype(uint8): the value map at d = 1 (an identity interpolation)

@@ -750,13 +750,14 @@ class Engine:
             raise TypeError(f"encode_u8 takes (B, T, H, W, C) uint8 frames, got {tuple(frames.shape)} {frames.dtype}")
         return self._encode_u8_input(tuple(frames.shape), mode, norm, lambda buf: buf.copy_(frames))
 
-    def encode_images_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params, mode: str, norm: L.U8Norm):
+    def encode_images_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params, mode: str, norm: L.U8Norm,
+                         jpegs=None):
         """encode_u8() of the images the loader's transform `resize` (with params[i] = (top, left, flip)) makes of a ragged
         list of (H_i, W_i, 3) uint8 images in host memory: omt_resample_u8 writes the transformed bytes into encode_u8's
         input buffer (eagerly: the source geometry changes every batch), then encode_u8's body or graph of that shape runs."""
         oh, ow = resize.out_size
         return self._encode_u8_input((len(images), 1, oh, ow, self.cin), mode, norm,
-                                     lambda buf: self.resample_u8(images, resize, params, buf))
+                                     lambda buf: self.resample_u8(images, resize, params, buf, jpegs))
 
     def encode_u8_frames(self, shape) -> torch.Tensor:
         """The encode_u8 slot's static uint8 input buffer for frames of `shape` (B, T, H, W, C): the bytes the last
@@ -795,16 +796,14 @@ class Engine:
         self._run(ws, ("encode_u8", lay.key, mode, norm), body)
         return ws, (B, Tp, h, w)
 
-    def stage_images_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params) -> tuple:
-        """Packs a ragged list of (H_i, W_i, 3) uint8 host images for omt_resample_u8 -- descriptors, the batch's distinct
-        coefficient tables (layout.resample_coeffs), source bytes -- into the grow-only pinned staging buffer and copies it
-        to the device asynchronously on the current stream.  Returns the entry point's arguments up to the output."""
-        if self.cin != 3:
-            raise NotImplementedError(f"omt_resample_u8 resizes RGB images; the model takes {self.cin} channels")
+    def resample_descs(self, shapes, resize: L.U8Resize, params) -> tuple:
+        """omt_resample_u8's descriptors and the batch's distinct coefficient tables (layout.resample_coeffs) for images of
+        sizes shapes[i] = (H_i, W_i): (desc int32 [B, DESC_WORDS] without the source offsets, table parts, tab_len).
+        Needs no source bytes, so an image decoded on the device can be laid out like a host one."""
         rh, rw = resize.size
-        B = len(images)
+        B = len(shapes)
         desc = torch.zeros(B, DESC_WORDS, dtype=torch.int32)
-        tables, parts, tab_len, src_len = {}, [], 0, 0
+        tables, parts, tab_len = {}, [], 0
 
         def axis(n_in, n_out):
             nonlocal tab_len
@@ -816,27 +815,52 @@ class Engine:
                 tab_len += bounds.size + coeffs.size
             return tables[key]
 
-        srcs = []
-        for b, (im, (i, j, flip)) in enumerate(zip(images, params)):
-            H, W = int(im.shape[0]), int(im.shape[1])
+        for b, ((H, W), (i, j, flip)) in enumerate(zip(shapes, params)):
             need_h, need_v = W != rw, H != rh
             hb, hc, hk = axis(W, rw) if need_h else (0, 0, 0)
             vb, vc, vk = axis(H, rh) if need_v else (0, 0, 0)
             desc[b, 2:] = torch.tensor([H, W, rh, rw, i, j, int(flip), int(need_h), int(need_v), hb, hc, hk, vb, vc, vk,
                                         int(L.vertical_first(H, W, rh, rw))], dtype=torch.int32)
-            srcs.append((src_len, im))
-            src_len += H * W * 3
-        dev, host, o_tab, o_src = self._stage_upload(desc, parts, srcs, src_len)
-        return (dev + o_src, src_len, dev, host, dev + o_tab if tab_len else None, host + o_tab if tab_len else None,
-                tab_len, B) + tuple(resize.out_size)
+        return desc, parts, tab_len
 
-    def _stage_upload(self, desc: torch.Tensor, parts, srcs, src_len: int):
+    def stage_images_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params, jpegs=None) -> tuple:
+        """Packs a ragged list of (H_i, W_i, 3) uint8 host images for omt_resample_u8 -- descriptors, the batch's distinct
+        coefficient tables (resample_descs), source bytes -- into the grow-only pinned staging buffer and copies it
+        to the device asynchronously on the current stream.  Returns the entry point's arguments up to the output.
+        jpegs: (staged batch, names) of jpeg.split_sources, whose files stand as jpeg.Pending entries in images; their
+        sources are laid out after the host images' and decoded there on the device (jpeg.decode_into), so only the host
+        images' bytes cross to the device and a corrupt scan raises before the resize launches."""
+        if self.cin != 3:
+            raise NotImplementedError(f"omt_resample_u8 resizes RGB images; the model takes {self.cin} channels")
+        desc, parts, tab_len = self.resample_descs([(int(im.shape[0]), int(im.shape[1])) for im in images], resize,
+                                                   params)
+        offsets, srcs, src_len = [0] * len(images), [], 0
+        for host_side in (True, False):
+            for b, im in enumerate(images):
+                if isinstance(im, torch.Tensor) == host_side:
+                    offsets[b] = src_len
+                    if host_side:
+                        srcs.append((src_len, im))
+                    src_len += int(im.shape[0]) * int(im.shape[1]) * 3
+        host_len = sum(t.numel() for _, t in srcs)
+        dev, host, o_tab, o_src = self._stage_upload(desc, parts, srcs, src_len, offsets, host_len)
+        if jpegs is not None:
+            from . import jpeg
+            staged, names = jpegs
+            pending = sorted((im.index, offsets[b]) for b, im in enumerate(images) if isinstance(im, jpeg.Pending))
+            jpeg.decode_into(staged, names, self._stage_dev[o_src:o_src + src_len], [o for _, o in pending])
+        return (dev + o_src, src_len, dev, host, dev + o_tab if tab_len else None, host + o_tab if tab_len else None,
+                tab_len, len(images)) + tuple(resize.out_size)
+
+    def _stage_upload(self, desc: torch.Tensor, parts, srcs, src_len: int, offsets=None, copy_len=None):
         """Packs descriptors (int32 [B, words], the int64 source offset in words 0-1), int32 table parts and the source
         tensors (srcs: (byte offset, uint8 tensor)) into the grow-only pinned staging buffer, 16-byte aligned sections,
         and copies it to the device asynchronously on the current stream.  An event guards the pinned buffer's reuse.
-        Returns (device base, host base, table offset, source offset) in bytes."""
+        offsets: every sample's source offset (default: those of srcs); copy_len: source bytes to copy (default src_len;
+        the rest is filled on the device).  Returns (device base, host base, table offset, source offset) in bytes."""
         B = desc.shape[0]
-        desc[:, :2] = torch.tensor([s for s, _ in srcs], dtype=torch.int64).view(torch.int32).view(B, 2)
+        offsets = [s for s, _ in srcs] if offsets is None else offsets
+        desc[:, :2] = torch.tensor(offsets, dtype=torch.int64).view(torch.int32).view(B, 2)
         tab_len = sum(p.size for p in parts)
         o_tab = L.round_up(desc.numel() * 4, 16)
         o_src = L.round_up(o_tab + tab_len * 4, 16)
@@ -855,7 +879,8 @@ class Engine:
             st[o_tab:o_tab + tab_len * 4].view(torch.int32).copy_(torch.from_numpy(np.concatenate(parts)))
         for off, t in srcs:
             st[o_src + off:o_src + off + t.numel()].view(t.shape).copy_(t)
-        self._stage_dev[:total].copy_(st[:total], non_blocking=True)
+        n = o_src + (src_len if copy_len is None else copy_len)
+        self._stage_dev[:n].copy_(st[:n], non_blocking=True)
         if self._stage_done is None:
             self._stage_done = torch.cuda.Event()
         self._stage_done.record()
@@ -908,14 +933,15 @@ class Engine:
         _cabi.call("omt_resample_clips", *args, lut, B, F, oh, ow, out)
         return out
 
-    def resample_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params, out: torch.Tensor) -> torch.Tensor:
+    def resample_u8(self, images: Sequence[torch.Tensor], resize: L.U8Resize, params, out: torch.Tensor,
+                    jpegs=None) -> torch.Tensor:
         """The loader's transform `resize` (params[i] = (top, left, flip)) of a ragged list of (H_i, W_i, 3) uint8 host images,
         on the device: out (B, oh, ow, 3) uint8 (any shape of that size), equal byte for byte to layout.resize_u8 / Pillow."""
         oh, ow = resize.out_size
         if out.dtype != torch.uint8 or out.device != self.device or not out.is_contiguous() or out.numel() != len(images) * oh * ow * 3:
             raise ValueError(f"resample_u8 writes {len(images)} x {oh} x {ow} x 3 contiguous uint8 bytes on {self.device}, "
                              f"got {tuple(out.shape)} {out.dtype} on {out.device}")
-        _cabi.call("omt_resample_u8", *self.stage_images_u8(images, resize, params), out)
+        _cabi.call("omt_resample_u8", *self.stage_images_u8(images, resize, params, jpegs), out)
         return out
 
     def z_view(self, ws: Workspace) -> torch.Tensor:

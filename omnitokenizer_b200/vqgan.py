@@ -366,10 +366,15 @@ class OmniTokenizer_VQGAN(nn.Module):
         """Checks a ragged list of decoded uint8 images (H_i, W_i, C) in host memory, the transform and its parameters, and
         the output size against encode's shape rules (with encode's messages) -- all before any launch.  Returns (list,
         params), drawing the parameters from the CPU generator as the loader's transforms would when params is None."""
+        from .jpeg import Pending
         images = list(images)
         L.check_resize(resize)
         C = self.args.image_channels
         for i, im in enumerate(images):
+            if isinstance(im, Pending):             # a JPEG file of encode_jpeg_u8 / forward_jpeg_u8, decoded to RGB
+                if C != 3:
+                    raise ValueError(f"image {i}: a JPEG decodes to 3 channels; the model takes {C}")
+                continue
             if not isinstance(im, torch.Tensor) or im.dtype != torch.uint8:
                 raise TypeError(f"image {i}: expected a uint8 tensor, got {getattr(im, 'dtype', type(im))}")
             if im.ndim != 3 or im.shape[2] != C or im.shape[0] < 1 or im.shape[1] < 1:
@@ -392,6 +397,20 @@ class OmniTokenizer_VQGAN(nn.Module):
         and torchvision do, so the result -- codes, embeddings, VAE latents, usage statistics, CPU RNG draws -- equals
         encode_u8 of the stacked host-transformed images.  params: per image (top, left, flip); None draws them from the
         CPU generator as RandomCrop / RandomHorizontalFlip would (layout.resize_params), before the VAE noise."""
+        return self._encode_images(images, None, resize, norm, include_embeddings, params)
+
+    @torch.no_grad()
+    def encode_jpeg_u8(self, sources, resize, norm=IMAGE_NORM, include_embeddings=False, params=None):
+        """encode_images_u8 of Image.open(f).convert("RGB") of each source, decoded on the device: sources is a list of
+        JPEG files (bytes-like or paths, jpeg.decode_u8's forms) and, where a caller decoded a file itself (e.g. one
+        jpeg.probe refuses), (H, W, 3) uint8 host tensors.  The files are parsed first (a refused or malformed one raises
+        before any launch), then decoded straight into omt_resample_u8's packed source; the result -- codes, embeddings,
+        VAE latents, usage statistics, CPU RNG draws -- equals encode_images_u8 of Pillow's decoded images."""
+        from . import jpeg
+        images, jpegs = jpeg.split_sources(sources)
+        return self._encode_images(images, jpegs, resize, norm, include_embeddings, params)
+
+    def _encode_images(self, images, jpegs, resize, norm, include_embeddings, params):
         images, params = self._images_u8(images, resize, params)
         if not images:
             h, w = resize.out_size
@@ -399,7 +418,7 @@ class OmniTokenizer_VQGAN(nn.Module):
                                   include_embeddings, norm)
         eng = self.engine()
         with torch.cuda.device(self.device):
-            ws, dims = eng.encode_images_u8(images, resize, params, "raw" if self.use_vae else "vq", norm)
+            ws, dims = eng.encode_images_u8(images, resize, params, "raw" if self.use_vae else "vq", norm, jpegs)
             return self._encode_result(eng, ws.idx, eng.z_view(ws), ws.counts, dims, True, include_embeddings)
 
     @torch.no_grad()
@@ -721,6 +740,17 @@ class OmniTokenizer_VQGAN(nn.Module):
         """forward_u8 of the images the loader's transform `resize` makes of a ragged list of decoded (H_i, W_i, C) uint8
         host images (see encode_images_u8): returns (x_recon uint8 (B, 1, h, w, C), vq_output), equal to forward_u8 on the
         stacked host-transformed images, with the same CPU RNG draws (the transform's parameters first when params is None)."""
+        return self._forward_images(images, None, resize, norm, out_affine, params)
+
+    @torch.no_grad()
+    def forward_jpeg_u8(self, sources, resize, norm=IMAGE_NORM, out_affine=EVAL_U8, params=None):
+        """forward_images_u8 of JPEG files decoded on the device, sources as encode_jpeg_u8 takes them; equal to
+        forward_images_u8 of Pillow's decoded images, with the same CPU RNG draws."""
+        from . import jpeg
+        images, jpegs = jpeg.split_sources(sources)
+        return self._forward_images(images, jpegs, resize, norm, out_affine, params)
+
+    def _forward_images(self, images, jpegs, resize, norm, out_affine, params):
         if self.resolution_scale is not None:
             raise NotImplementedError("resolution_scale resizes the fp32 frames between the / 255 and the shift "
                                       "(omnitokenizer.py:334-355); no byte table expresses that -- use forward()")
@@ -729,7 +759,7 @@ class OmniTokenizer_VQGAN(nn.Module):
             raise ValueError("forward_images_u8 needs at least one image")
         eng = self.engine()
         with torch.cuda.device(self.device):
-            ws, dims = eng.encode_images_u8(images, resize, params, "raw" if self.use_vae else "vq", norm)
+            ws, dims = eng.encode_images_u8(images, resize, params, "raw" if self.use_vae else "vq", norm, jpegs)
             return self._forward_decode(eng, ws, dims, u8=tuple(float(v) for v in out_affine))
 
     # ---------------------------------------------------------------- CLI surface
